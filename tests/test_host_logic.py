@@ -49,18 +49,24 @@ def test_canon_shortcut_threshold(make_emu, oracle_mod):
     assert np.array_equal(e.ntt(x), o.ntt_fwd(x))
 
 
-@pytest.mark.parametrize("variant", ["gen", "fast"])
-def test_device_scalar_arithmetic_bounds(make_emu, oracle_mod, variant):
+@pytest.mark.parametrize("variant,moduli", [pytest.param("gen", "60_35_bit", id="gen"), pytest.param("fast", "default", id="fast"),
+                                            pytest.param("gen", "smallest", id="gen-smallest"),
+                                            pytest.param("fast", "fast_mixed", id="fast-fast_mixed")])
+def test_device_scalar_arithmetic_bounds(make_emu, oracle_mod, variant, moduli):
     """modarith.cuh on adversarial inputs: every lazy routine stays inside its documented range (SB = 4: the quotient
     estimates of the Shoup and Barrett products may be up to two short).  Both arithmetic variants: the generic one on a
-    59-bit and a 34-bit modulus, the k * 2^32 + 1 one on the two largest moduli of the default basis."""
+    60-bit and a 35-bit modulus and on the smallest modulus the context accepts (34 bits: bar_shift = 32), the k * 2^32 + 1
+    one on the two largest moduli of the default basis and on the fast_mixed basis of tests/bases.py (37 to 55 bits)."""
+    import bases
     lib = oracle_mod.lib()
     small = (1 << 34) - (1 << 34) % (2 << 12) + 1
     while not lib.dpo_is_prime(small):
         small += 2 << 12
     defaults = oracle_mod.Oracle(12, 2).moduli
     assert all(q & 0xFFFFFFFF == 1 for q in defaults)
-    e = make_emu(12, 2, defaults if variant == "fast" else [defaults[0] - 0, small], variant=variant)
+    mods = {"60_35_bit": [defaults[0] - 0, small], "default": defaults, "smallest": [bases.SMALLEST_GENERIC],
+            "fast_mixed": bases.catalogue(oracle_mod)["fast_mixed"]}[moduli]
+    e = make_emu(12, len(mods), mods, variant=variant)
     SB = 4
     rng = np.random.default_rng(2)
     for l, q in enumerate(e.moduli):
