@@ -325,6 +325,8 @@ void dpfhe_context_destroy(dpfhe_ctx *ctx) {
     cudaFree(ctx->hoist_delta);
     cudaFree(ctx->hoist_zero);
     cudaFree(ctx->hoistg_buf);
+    cudaFree(ctx->ckks_tab);
+    cudaFree(ctx->ckks_work);
     cudaFree(ctx->lc.ks_hyb);
     for (int k = 0; k < PIPE_DEPTH; ++k) {
         cudaFree(ctx->stage_in[k]);
@@ -365,6 +367,7 @@ size_t dpfhe_context_device_bytes(const dpfhe_ctx *ctx) {
     n += ctx->hoist_chunk * (L * P8 + sizeof(u32));                                  // hoisted rotations: shared transforms + zero flags
     if (ctx->hoist_M) n += 3 * P8 + L * L * 8;                                       //   per-rotation constants
     n += ctx->hoistg_bytes;                                                          //   grouped hybrid keys: lifted digits + accumulators
+    n += ctx->ckks_tab_bytes + ctx->ckks_work_bytes;                                 // CKKS encoding tables and scratch
     if (ctx->lc.ks_prof) n += ctx->lc.ks_slots * 16 * sizeof(unsigned long long);
     return n;
 }
@@ -379,6 +382,9 @@ int dpfhe_context_trim(dpfhe_ctx *ctx) {
     ctx->hoist_U = nullptr; ctx->hoist_zero = nullptr; ctx->hoist_chunk = 0;
     cudaFree(ctx->hoistg_buf);
     ctx->hoistg_buf = nullptr; ctx->hoistg_bytes = 0;
+    cudaFree(ctx->ckks_tab); cudaFree(ctx->ckks_work);
+    ctx->ckks_tab = nullptr; ctx->ckks_tab_bytes = 0; ctx->ckks = CkksTables();
+    ctx->ckks_work = nullptr; ctx->ckks_work_bytes = 0;
     ctx->ms_tau = nullptr; ctx->ms_tau_bytes = 0;
     ctx->stage_key = nullptr; ctx->stage_key_bytes = 0;
     for (int k = 0; k < PIPE_DEPTH; ++k) {
@@ -982,6 +988,107 @@ int dpfhe_ct_mul_plain_host(dpfhe_ctx *ctx, const uint64_t *h_ct, const uint64_t
                             CU_TRY(VCALL(launch_ct_mul_plain, ctx->lc, dc, ctx->stage_key, dout, cnt, st));
                             note_launch(ctx, 1);
                             return DPFHE_OK;
+                        });
+}
+
+// ---------------------------------------------------------------- CKKS slot encoding (DESIGN.md §2.12)
+
+// the context's encoding tables (built and uploaded once) and `need` bytes of scratch
+static int ckks_prepare(dpfhe_ctx *ctx, size_t need, cudaStream_t st) {
+    if (!ctx->ckks_tab) {
+        std::vector<Cplx> tw;
+        std::vector<uint32_t> tj;
+        std::vector<uint64_t> pow2;
+        build_ckks_tables(ctx->hp, tw, tj, pow2);
+        const size_t b_tw = tw.size() * sizeof(Cplx), b_tj = tj.size() * 4, b_p2 = pow2.size() * 8;
+        void *p = nullptr;
+        CU_TRY(cudaMalloc(&p, b_tw + b_tj + b_p2));
+        unsigned char *base = (unsigned char *)p;
+        if (cudaMemcpy(base, tw.data(), b_tw, cudaMemcpyHostToDevice) != cudaSuccess ||
+            cudaMemcpy(base + b_tw, pow2.data(), b_p2, cudaMemcpyHostToDevice) != cudaSuccess ||
+            cudaMemcpy(base + b_tw + b_p2, tj.data(), b_tj, cudaMemcpyHostToDevice) != cudaSuccess) {
+            cudaFree(p);
+            return fail(DPFHE_ERR_CUDA, "CUDA error at %s:%d: uploading the CKKS tables failed", __FILE__, __LINE__);
+        }
+        ctx->ckks_tab = p;
+        ctx->ckks_tab_bytes = b_tw + b_tj + b_p2;
+        ctx->ckks.tw = (const Cplx *)base;
+        ctx->ckks.pow2 = (const u64 *)(base + b_tw);
+        ctx->ckks.tj = (const u32 *)(base + b_tw + b_p2);
+    }
+    if (need > ctx->ckks_work_bytes) {
+        CU_TRY(cudaStreamSynchronize(st));   // the old scratch may still be in use on this stream
+        if (ctx->ckks_work) cudaFree(ctx->ckks_work);
+        ctx->ckks_work = nullptr;
+        ctx->ckks_work_bytes = 0;
+        CU_TRY(cudaMalloc(&ctx->ckks_work, need));
+        ctx->ckks_work_bytes = need;
+    }
+    return DPFHE_OK;
+}
+
+static bool valid_scale(double scale) { return scale > 0.0 && scale <= 1.7976931348623157e308; }   // finite and positive (NaN fails both)
+
+int dpfhe_ckks_encode(dpfhe_ctx *ctx, const double *d_slots, uint64_t *d_pt, size_t n_vec, double scale, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
+    if (n_vec == 0) return DPFHE_OK;
+    CHECK_PTR(d_slots); CHECK_PTR(d_pt);
+    cudaStream_t st = pick(ctx, stream);
+    rc = ckks_prepare(ctx, n_vec * ctx->N() * sizeof(double), st);
+    if (rc) return rc;
+    const double sc = scale * (2.0 / (double)ctx->N());
+    CU_TRY(VCALL(launch_ckks_encode, ctx->lc, (const Cplx *)d_slots, (double *)ctx->ckks_work, d_pt, ctx->ckks, sc, n_vec, st));
+    note_launch(ctx, 2);   // ckks_enc_fft_kernel + ckks_enc_ntt(_pair)_kernel
+    return DPFHE_OK;
+}
+
+int dpfhe_ckks_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, double *d_slots, size_t n_vec, double scale, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
+    if (n_vec == 0) return DPFHE_OK;
+    CHECK_PTR(d_pt); CHECK_PTR(d_slots);
+    cudaStream_t st = pick(ctx, stream);
+    const size_t bytes = n_vec * ctx->P() * 8;
+    rc = ckks_prepare(ctx, bytes, st);
+    if (rc) return rc;
+    u64 *work = (u64 *)ctx->ckks_work;
+    CU_TRY(cudaMemcpyAsync(work, d_pt, bytes, cudaMemcpyDeviceToDevice, st));   // the caller's plaintexts stay unchanged
+    CU_TRY(VCALL(launch_ntt, ctx->lc, work, n_vec, true, st));
+    CkksConsts K;
+    build_ckks_consts(ctx->hp, scale, K);
+    CU_TRY(VCALL(launch_ckks_decode, ctx->lc, work, (Cplx *)d_slots, ctx->ckks, K, n_vec, st));
+    note_launch(ctx, 2);   // inverse transform + ckks_dec_kernel
+    return DPFHE_OK;
+}
+
+int dpfhe_ckks_encode_host(dpfhe_ctx *ctx, const double *h_slots, uint64_t *h_pt, size_t n_vec, double scale) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
+    if (n_vec == 0) return DPFHE_OK;
+    if (!h_slots || !h_pt) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const size_t P = ctx->P(), S = ctx->N();   // words of a plaintext, and of a slot vector (N/2 complex doubles)
+    const size_t chunk = pick_chunk(ctx, P * 8, n_vec);
+    return run_pipeline(ctx, (const u64 *)h_slots, nullptr, h_pt, n_vec, S, P, chunk,
+                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                            return dpfhe_ckks_encode(ctx, (const double *)din, dout, cnt, scale, st);
+                        });
+}
+
+int dpfhe_ckks_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, double *h_slots, size_t n_vec, double scale) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
+    if (n_vec == 0) return DPFHE_OK;
+    if (!h_slots || !h_pt) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const size_t P = ctx->P(), S = ctx->N();
+    const size_t chunk = pick_chunk(ctx, P * 8, n_vec);
+    return run_pipeline(ctx, h_pt, nullptr, (u64 *)h_slots, n_vec, P, S, chunk,
+                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                            return dpfhe_ckks_decode(ctx, din, (double *)dout, cnt, scale, st);
                         });
 }
 

@@ -35,6 +35,13 @@ struct dpfhe_ctx {
     size_t hoist_chunk = 0;                  // ciphertexts the current U / zero buffers hold
     dpfhe::u64 *hoistg_buf = nullptr;        // hoisted rotations with grouped hybrid keys: lifted digits, accumulators and tau' rows of a chunk
     size_t hoistg_bytes = 0;
+    // CKKS slot encoding (allocated on first use): twiddles, slot permutation and 2^e mod q tables in one allocation, and a
+    // scratch row set (encode: [n_vec][N] rounded coefficients; decode: [n_vec][L][N] inverse transforms)
+    void *ckks_tab = nullptr;
+    size_t ckks_tab_bytes = 0;
+    dpfhe::CkksTables ckks;
+    void *ckks_work = nullptr;
+    size_t ckks_work_bytes = 0;
     dpfhe::u64 *stage_in[DPFHE_PIPE_DEPTH] = {}, *stage_out[DPFHE_PIPE_DEPTH] = {}, *stage_key = nullptr;
     size_t stage_in_bytes = 0, stage_out_bytes = 0, stage_key_bytes = 0;
     cudaEvent_t ev_h2d[DPFHE_PIPE_DEPTH] = {}, ev_comp[DPFHE_PIPE_DEPTH] = {}, ev_d2h[DPFHE_PIPE_DEPTH] = {};

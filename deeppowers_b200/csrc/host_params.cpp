@@ -231,4 +231,83 @@ void build_group_consts(const HostParams &hp, unsigned K, uint64_t t_plain, Grou
     }
 }
 
+// ---- CKKS slot encoding (DESIGN.md §2.12) ----------------------------------------------------------------------
+// cos and sin of pi k / N in fixed point with 126 fractional bits (Taylor series, error below 2^-120), rounded once to double.
+namespace {
+// floor(a * b / 2^126) for a, b <= 2^127
+u128 fx126_mul(u128 a, u128 b) {
+    const uint64_t a0 = (uint64_t)a, a1 = (uint64_t)(a >> 64), b0 = (uint64_t)b, b1 = (uint64_t)(b >> 64);
+    const u128 p00 = (u128)a0 * b0, p01 = (u128)a0 * b1, p10 = (u128)a1 * b0, p11 = (u128)a1 * b1;
+    const u128 mid = (p00 >> 64) + (uint64_t)p01 + (uint64_t)p10;
+    const u128 hi = p11 + (p01 >> 64) + (p10 >> 64) + (mid >> 64);
+    return (hi << 2) | ((uint64_t)mid >> 62);
+}
+// v / 2^126 (v <= 2^126) rounded to the nearest double, ties to even
+double fx126_to_double(u128 v) {
+    if (v == 0) return 0.0;
+    int msb = 127;
+    while (!((v >> msb) & 1)) --msb;
+    if (msb <= 52) return (double)(uint64_t)v * 0x1p-126;   // exact
+    const int sh = msb - 52;
+    uint64_t m = (uint64_t)(v >> sh);
+    const u128 rem = v & (((u128)1 << sh) - 1), half = (u128)1 << (sh - 1);
+    if (rem > half || (rem == half && (m & 1))) ++m;
+    return (double)m * 0x1p-126 * (double)((u128)1 << sh);   // m < 2^54 and a power of two: both products exact
+}
+// (cos, sin) of pi k / N for 0 <= k <= N/4 (the first octant)
+Cplx cos_sin_octant(uint64_t k, unsigned log_n) {
+    const u128 pi126 = ((u128)0xC90FDAA22168C234ull << 64) | 0xC4C6628B80DC1CD1ull;   // floor(pi * 2^126)
+    const u128 x = (pi126 >> log_n) * k + (((pi126 & (((u128)1 << log_n) - 1)) * k) >> log_n);
+    u128 c_pos = 0, c_neg = 0, s_pos = 0, s_neg = 0;
+    u128 t = (u128)1 << 126;   // x^n / n!
+    for (unsigned n = 0; t; ++n) {
+        if (n % 2 == 0) ((n / 2) % 2 ? c_neg : c_pos) += t;
+        else ((n / 2) % 2 ? s_neg : s_pos) += t;
+        t = fx126_mul(t, x) / (n + 1);
+    }
+    return Cplx{fx126_to_double(c_pos - c_neg), fx126_to_double(s_pos - s_neg)};
+}
+}  // namespace
+
+void build_ckks_tables(const HostParams &hp, std::vector<Cplx> &tw, std::vector<uint32_t> &tj, std::vector<uint64_t> &pow2) {
+    const unsigned log_n = hp.log_n;
+    const uint64_t N = (uint64_t)1 << log_n, quarter = N / 4, half = N / 2;
+    tw.resize(N);
+    for (uint64_t k = 0; k < N; ++k) {
+        const uint64_t r = k % half;   // angle pi r / N in [0, pi/2)
+        Cplx v = r <= quarter ? cos_sin_octant(r, log_n) : cos_sin_octant(half - r, log_n);
+        if (r > quarter) v = Cplx{v.im, v.re};
+        if (k >= half) v = Cplx{0.0 - v.im, v.re};   // (cos, sin)(a + pi/2) = (-sin a, cos a); cos(pi/2) is +0
+        tw[k] = v;
+    }
+    tj.resize(half);
+    uint64_t e = 1;
+    for (uint64_t j = 0; j < half; ++j, e = e * 5 % (2 * N)) tj[j] = (uint32_t)((e - 1) / 4);
+    pow2.resize((size_t)hp.L * CKKS_POW2_E);
+    for (unsigned l = 0; l < hp.L; ++l) {
+        const uint64_t q = hp.limbs[l].lp.q;
+        uint64_t p = 1;
+        for (int x = 0; x < CKKS_POW2_E; ++x, p = host_mulmod(p, 2, q)) pow2[(size_t)l * CKKS_POW2_E + x] = p;
+    }
+}
+
+void build_ckks_consts(const HostParams &hp, double scale, CkksConsts &K) {
+    K = CkksConsts();
+    const unsigned L = hp.L;
+    for (unsigned i = 0; i < L; ++i) {
+        const uint64_t qi = hp.limbs[i].lp.q;
+        K.qd[i] = (double)qi;
+        for (unsigned j = 0; j < i; ++j) K.ginv[j][i] = host_powmod(hp.limbs[j].lp.q % qi, qi - 2, qi);
+    }
+    // (Q - 1) / 2 from the digits q_i - 1 of Q - 1, halved from the most significant digit
+    uint64_t r = 0;
+    for (unsigned i = L; i-- > 0;) {
+        const uint64_t qi = hp.limbs[i].lp.q;
+        const u128 v = (u128)r * qi + (qi - 1);
+        K.half[i] = (uint64_t)(v >> 1);
+        r = (uint64_t)(v & 1);
+    }
+    K.scale = scale;
+}
+
 }  // namespace dpfhe

@@ -34,6 +34,12 @@ void build_ms_consts(const HostParams &hp, uint64_t t_plain, MsConsts &K);
 // receives the constants of the division by P.  Requires 1 <= K <= KS_MAX_SPECIAL, K < hp.L, t_plain < every special prime.
 void build_group_consts(const HostParams &hp, unsigned K, uint64_t t_plain, GroupConsts &G, MsConsts &Km);
 
+// CKKS slot encoding (DESIGN.md §2.12): the twiddles (cos, sin)(pi k / N), k < N, each correctly rounded; the slot
+// permutation t_j, j < N/2; and 2^e mod q_l, [L][CKKS_POW2_E]
+void build_ckks_tables(const HostParams &hp, std::vector<Cplx> &tw, std::vector<uint32_t> &tj, std::vector<uint64_t> &pow2);
+// decoding constants (Garner inverses, the digits of (Q-1)/2, the moduli as doubles) with the divisor `scale`
+void build_ckks_consts(const HostParams &hp, double scale, CkksConsts &K);
+
 uint64_t host_mulmod(uint64_t a, uint64_t b, uint64_t q);
 uint64_t host_powmod(uint64_t a, uint64_t e, uint64_t q);
 bool host_is_prime(uint64_t n);

@@ -93,12 +93,10 @@ DPFHE_HD U64x2 ld_keep(const U64x2 *p) {
 
 // ---- standalone transforms (one limb per call) ----------------------------------------
 // data: [N] coefficients of limb `p`, in place.  buf: N words of shared memory.
-template <int LOGN, int NT, class CTA>
-DPFHE_HD void ntt_fwd_body(CTA &cta, u64 *buf, u64 *data, const Twiddle *tw, const LimbParams &p) {
-    const U64x2 *src = reinterpret_cast<const U64x2 *>(data);
-    cta.par([&](int tid) {
-        fwd_load_stage<LOGN, NT, false>(buf, tw, p, tid, [&](int c) { return ld_stream(src + c); });
-    });
+// SRC(chunk) -> U64x2: the canonical input chunk (a limb in memory, or values reduced into the limb as they are loaded)
+template <int LOGN, int NT, class CTA, class SRC>
+DPFHE_HD void ntt_fwd_src_body(CTA &cta, u64 *buf, SRC src, u64 *data, const Twiddle *tw, const LimbParams &p) {
+    cta.par([&](int tid) { fwd_load_stage<LOGN, NT, false>(buf, tw, p, tid, src); });
     fwd_passes<LOGN, NT, 1>(cta, buf, tw, p);
     U64x2 *dst = reinterpret_cast<U64x2 *>(data);
     cta.par([&](int tid) {
@@ -109,6 +107,11 @@ DPFHE_HD void ntt_fwd_body(CTA &cta, u64 *buf, u64 *data, const Twiddle *tw, con
             st_stream(dst + c, v);
         }
     });
+}
+template <int LOGN, int NT, class CTA>
+DPFHE_HD void ntt_fwd_body(CTA &cta, u64 *buf, u64 *data, const Twiddle *tw, const LimbParams &p) {
+    const U64x2 *src = reinterpret_cast<const U64x2 *>(data);
+    ntt_fwd_src_body<LOGN, NT>(cta, buf, [&](int c) { return ld_stream(src + c); }, data, tw, p);
 }
 
 // the limb already sits in shared memory in the swizzled layout (copied by the threads below, or by the TMA unit:
@@ -142,12 +145,14 @@ DPFHE_HD void ntt_inv_body(CTA &cta, u64 *buf, u64 *data, const Twiddle *itw, co
 //            shared memory and two from the partner's (distributed shared memory), each CTA finishing half of the columns.
 constexpr int NTT_PAIR_LOGN = 14;
 
+template <int NT, class CTA, class SRC>
+DPFHE_HD void ntt_fwd_half_load_src(CTA &cta, u64 *buf, SRC src, const Twiddle *tw, const LimbParams &p, int h) {
+    cta.par([&](int tid) { fwd_load_stage_half<NTT_PAIR_LOGN, NT, false>(buf, tw, p, tid, src, h); });
+}
 template <int NT, class CTA>
 DPFHE_HD void ntt_fwd_half_load(CTA &cta, u64 *buf, const u64 *data, const Twiddle *tw, const LimbParams &p, int h) {
     const U64x2 *src = reinterpret_cast<const U64x2 *>(data);
-    cta.par([&](int tid) {
-        fwd_load_stage_half<NTT_PAIR_LOGN, NT, false>(buf, tw, p, tid, [&](int c) { return ld_stream(src + c); }, h);
-    });
+    ntt_fwd_half_load_src<NT>(cta, buf, [&](int c) { return ld_stream(src + c); }, tw, p, h);
 }
 template <int NT, class CTA>
 DPFHE_HD void ntt_fwd_half_finish(CTA &cta, u64 *buf, u64 *data, const Twiddle *tw, const LimbParams &p, int h) {
@@ -1249,6 +1254,166 @@ DPFHE_HD void pt_inner_tile(CTA &cta, u64 *smem, const PtInnerArgs &A, const Lim
             }
         });
     }
+}
+
+// ---- CKKS slot encoding (DESIGN.md §2.12) ------------------------------------------------------------------------
+// Floating point with one fixed operation order: every product and sum is rounded on its own.  nvcc never contracts the
+// __d*_rn intrinsics into FMAs; host builds of these bodies (tests/emu) compile with -ffp-contract=off.
+DPFHE_HD double f_add(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+DPFHE_HD double f_sub(double a, double b) { return f_add(a, -b); }
+DPFHE_HD double f_mul(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+DPFHE_HD double f_div(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __ddiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
+DPFHE_HD double f_rint(double a) {   // nearest integer, ties to even
+#if defined(__CUDA_ARCH__)
+    return rint(a);
+#else
+    return __builtin_rint(a);
+#endif
+}
+DPFHE_HD double f_from_u64(u64 a) {
+#if defined(__CUDA_ARCH__)
+    return __ull2double_rn(a);
+#else
+    return (double)a;
+#endif
+}
+DPFHE_HD u64 f_bits(double a) {
+#if defined(__CUDA_ARCH__)
+    return (u64)__double_as_longlong(a);
+#else
+    u64 b;
+    __builtin_memcpy(&b, &a, 8);
+    return b;
+#endif
+}
+// (ar br - ai bi, ar bi + ai br)
+DPFHE_HD Cplx c_mul(const Cplx &a, const Cplx &b) {
+    return Cplx{f_sub(f_mul(a.re, b.re), f_mul(a.im, b.im)), f_add(f_mul(a.re, b.im), f_mul(a.im, b.re))};
+}
+DPFHE_HD Cplx c_conj(const Cplx &a) { return Cplx{a.re, -a.im}; }
+
+// Radix-2 decimation in time over S = N/2 points in bit-reversed order: Y[t] = sum_k a[k] W^(+-tk), W = exp(2 pi i / S) = tw[4].
+// The twiddle of butterfly j at stage s (span h = 2^s) is W^(j S / 2h) = tw[j N / h]; `inverse` conjugates it.
+template <int LOGN, int NT, class CTA>
+DPFHE_HD void ckks_fft_stages(CTA &cta, Cplx *a, const Cplx *tw, bool inverse) {
+    constexpr int S = 1 << (LOGN - 1);
+#pragma unroll 1
+    for (int s = 0; s < LOGN - 1; ++s) {
+        cta.par([&](int tid) {
+#pragma unroll 1
+            for (int b = tid; b < S / 2; b += NT) {
+                const int j = b & ((1 << s) - 1), i0 = ((b >> s) << (s + 1)) + j, i1 = i0 + (1 << s);
+                Cplx w = tw[j << (LOGN - s)];
+                if (inverse) w = c_conj(w);
+                const Cplx x = a[i0], y = c_mul(a[i1], w);
+                a[i0] = Cplx{f_add(x.re, y.re), f_add(x.im, y.im)};
+                a[i1] = Cplx{f_sub(x.re, y.re), f_sub(x.im, y.im)};
+            }
+        });
+    }
+}
+
+// encode, one vector: z [N/2] slots -> x [N] rounded coefficients rint(sc * m_k), sc = scale * 2/N.  a: N/2 complex of
+// shared memory.
+template <int LOGN, int NT, class CTA>
+DPFHE_HD void ckks_enc_fft_body(CTA &cta, Cplx *a, const Cplx *z, double *x, const Cplx *tw, const u32 *tj, double sc) {
+    constexpr int S = 1 << (LOGN - 1);
+    cta.par([&](int tid) {
+        for (int j = tid; j < S; j += NT) a[bitrev_n(tj[j], LOGN - 1)] = z[j];
+    });
+    ckks_fft_stages<LOGN, NT>(cta, a, tw, true);
+    cta.par([&](int tid) {
+        for (int k = tid; k < S; k += NT) {
+            const Cplx u = c_mul(a[k], c_conj(tw[k]));
+            x[k] = f_rint(f_mul(sc, u.re));
+            x[k + S] = f_rint(f_mul(sc, u.im));
+        }
+    });
+}
+
+// the exact residue of an integral double x modulo q_l: x = +-M 2^e, M < 2^53, so x mod q = +-(M mod q)(2^e mod q).
+// pow2: the limb's 2^e mod q table.  Non-finite values give some residue (the table index stays in range).
+DPFHE_HD u64 ckks_reduce(double x, const LimbParams &p, const u64 *pow2) {
+    const u64 b = f_bits(x);
+    const int ex = (int)((b >> 52) & 0x7ff);
+    const u64 m = (b & ((1ull << 52) - 1)) | (ex ? 1ull << 52 : 0);
+    const int e = (ex ? ex : 1) - 1075;
+    const u64 v = e >= 0 ? m : (e > -64 ? m >> -e : 0);
+    const int pe = e < 0 ? 0 : (e < CKKS_POW2_E ? e : CKKS_POW2_E - 1);
+    const u64 r = mulmod(canon(v, p), pow2[pe], p);
+    return (b >> 63) && r ? p.q - r : r;
+}
+
+// decode, one coefficient: the residues col[l * stride], l < L (canonical), are overwritten by the mixed-radix digits of X
+// (Garner); returns centred(X) / scale as a double: Horner from the most significant digit, then one division.
+DPFHE_HD double ckks_crt_double(u64 *col, size_t stride, u32 L, const LimbParams *lp, const CkksConsts &K) {
+#pragma unroll 1
+    for (u32 i = 1; i < L; ++i) {
+        const LimbParams &p = lp[i];
+        u64 t = col[i * stride];
+#pragma unroll 1
+        for (u32 j = 0; j < i; ++j) {
+            const u64 d = canon(col[j * stride], p);
+            t = mulmod(t >= d ? t - d : t + p.q - d, K.ginv[j][i], p);
+        }
+        col[i * stride] = t;
+    }
+    // X > (Q-1)/2 ?  (lexicographic from the most significant digit)
+    int cmp = 0;
+#pragma unroll 1
+    for (u32 i = L; i-- > 0 && cmp == 0;) {
+        const u64 d = col[i * stride];
+        cmp = d > K.half[i] ? 1 : (d < K.half[i] ? -1 : 0);
+    }
+    const bool neg = cmp > 0;
+    // digits of Q - X: 0 below the lowest non-zero digit p of X, q_p - d_p at p, q_i - 1 - d_i above
+    u32 low = 0;
+    if (neg)
+        while (col[low * stride] == 0) ++low;
+    double r = 0.0;
+#pragma unroll 1
+    for (u32 i = L; i-- > 0;) {
+        const u64 d = col[i * stride], q = lp[i].q;
+        const u64 f = !neg ? d : (i > low ? q - 1 - d : (i == low ? q - d : 0));
+        r = i == L - 1 ? f_from_u64(f) : f_add(f_mul(r, K.qd[i]), f_from_u64(f));
+    }
+    return f_div(neg ? -r : r, K.scale);
+}
+
+// decode, one vector: col [L][N] coefficients (inverse-transformed, canonical; overwritten) -> z [N/2] slots
+template <int LOGN, int NT, class CTA>
+DPFHE_HD void ckks_dec_fft_body(CTA &cta, Cplx *a, u64 *col, Cplx *z, const Cplx *tw, const u32 *tj, const LimbParams *lp, const CkksConsts &K,
+                                u32 L) {
+    constexpr int S = 1 << (LOGN - 1);
+    constexpr size_t N = (size_t)1 << LOGN;
+    cta.par([&](int tid) {
+        for (int k = tid; k < S; k += NT) {
+            const Cplx u{ckks_crt_double(col + k, N, L, lp, K), ckks_crt_double(col + k + S, N, L, lp, K)};
+            a[bitrev_n((u32)k, LOGN - 1)] = c_mul(u, tw[k]);
+        }
+    });
+    ckks_fft_stages<LOGN, NT>(cta, a, tw, false);
+    cta.par([&](int tid) {
+        for (int j = tid; j < S; j += NT) z[j] = a[tj[j]];
+    });
 }
 
 }  // namespace DPFHE_VNS

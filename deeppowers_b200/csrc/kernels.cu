@@ -224,6 +224,77 @@ __global__ void __launch_bounds__(NT, MINB) md_limb_kernel(const u64 *in, const 
     }
 }
 
+// ------------------------------------------------------------------ CKKS slot encoding (DESIGN.md §2.12, §4.8)
+// One CTA per vector: its N/2 complex values (64 KiB at N = 8192, 128 KiB at N = 16384) stay in shared memory for all stages.
+template <int LOGN, int NT>
+__global__ void __launch_bounds__(NT, 1) ckks_enc_fft_kernel(const Cplx *slots, double *coeffs, const Cplx *__restrict__ tw,
+                                                              const u32 *__restrict__ tj, double sc) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    constexpr size_t N = (size_t)1 << LOGN;
+    DevCta<NT> cta;
+    const size_t v = blockIdx.x;
+    ckks_enc_fft_body<LOGN, NT>(cta, reinterpret_cast<Cplx *>(smem_raw), slots + v * (N / 2), coeffs + v * N, tw, tj, sc);
+}
+
+// forward transform of one limb of one encoded vector, the coefficients reduced into the limb by the load stage
+template <int LOGN, int NT, int MINB>
+__global__ void __launch_bounds__(NT, MINB) ckks_enc_ntt_kernel(const double *coeffs, u64 *pt, const Twiddle *__restrict__ tw,
+                                                                 const u64 *__restrict__ pow2, const __grid_constant__ LimbTable lt, u32 L) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    u64 *buf = reinterpret_cast<u64 *>(smem_raw);
+    constexpr size_t N = (size_t)1 << LOGN;
+    DevCta<NT> cta;
+    const size_t w = blockIdx.x;
+    const u32 l = (u32)(w % L);
+    const LimbParams &p = lt.lp[l];
+    const double *x = coeffs + (w / L) * N;
+    const u64 *p2 = pow2 + (size_t)l * CKKS_POW2_E;
+    auto src = [&](int c) {
+        U64x2 r;
+        r.x = ckks_reduce(x[2 * c], p, p2);
+        r.y = ckks_reduce(x[2 * c + 1], p, p2);
+        return r;
+    };
+    ntt_fwd_src_body<LOGN, NT>(cta, buf, src, pt + w * N, tw + (size_t)l * N, p);
+}
+
+// N = 16384: two CTAs per limb, each keeping half of the outer radix-4 step (as ntt_pair_kernel's forward half; the input is
+// not overwritten, so the two CTAs need no cluster barrier)
+template <int NT, int MINB>
+__global__ void __launch_bounds__(NT, MINB) ckks_enc_ntt_pair_kernel(const double *coeffs, u64 *pt, const Twiddle *__restrict__ tw,
+                                                                      const u64 *__restrict__ pow2, const __grid_constant__ LimbTable lt, u32 L) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    u64 *buf = reinterpret_cast<u64 *>(smem_raw);
+    constexpr size_t N = (size_t)1 << NTT_PAIR_LOGN;
+    DevCta<NT> cta;
+    const size_t w = blockIdx.x / 2;
+    const int h = (int)(blockIdx.x & 1);
+    const u32 l = (u32)(w % L);
+    const LimbParams &p = lt.lp[l];
+    const double *x = coeffs + (w / L) * N;
+    const u64 *p2 = pow2 + (size_t)l * CKKS_POW2_E;
+    auto src = [&](int c) {
+        U64x2 r;
+        r.x = ckks_reduce(x[2 * c], p, p2);
+        r.y = ckks_reduce(x[2 * c + 1], p, p2);
+        return r;
+    };
+    ntt_fwd_half_load_src<NT>(cta, buf, src, tw + (size_t)l * N, p, h);
+    ntt_fwd_half_finish<NT>(cta, buf, pt + w * N, tw + (size_t)l * N, p, h);
+}
+
+// decode: Garner, centring, Horner, scaling and the forward special FFT of one vector; work [n_vec][L][N] holds the inverse
+// transforms (overwritten by the mixed-radix digits)
+template <int LOGN, int NT>
+__global__ void __launch_bounds__(NT, 1) ckks_dec_kernel(u64 *work, Cplx *slots, const Cplx *__restrict__ tw, const u32 *__restrict__ tj,
+                                                          const __grid_constant__ LimbTable lt, const __grid_constant__ CkksConsts K, u32 L) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    constexpr size_t N = (size_t)1 << LOGN;
+    DevCta<NT> cta;
+    const size_t v = blockIdx.x;
+    ckks_dec_fft_body<LOGN, NT>(cta, reinterpret_cast<Cplx *>(smem_raw), work + v * L * N, slots + v * (N / 2), tw, tj, lt.lp, K, L);
+}
+
 #endif
 // ------------------------------------------------------------------ fused key-switch family
 __device__ __forceinline__ u32 ld_acquire_u32(const u32 *p) {
@@ -1029,6 +1100,82 @@ cudaError_t launch_mod_down_special(const LaunchCtx &lc, const u64 *in, u64 *tau
         case 12: return launch_md_t<12, 256, 2>(lc, in, tau, out, K, G, n_polys, st);
         case 13: return launch_md_t<13, 256, 3>(lc, in, tau, out, K, G, n_polys, st);
         case 14: return launch_md_t<14, 512, 1>(lc, in, tau, out, K, G, n_polys, st);
+    }
+    return cudaErrorInvalidValue;
+}
+
+// ---- CKKS slot encoding
+constexpr int CKKS_FFT_NT = 512;
+
+template <class K>
+static cudaError_t set_smem_once(K kern, size_t smem, ConfiguredMask &configured, int device) {
+    if (configured.has(device)) return cudaSuccess;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) configured.set(device);
+    return e;
+}
+
+template <int LOGN>
+static cudaError_t launch_ckks_encode_t(const LaunchCtx &lc, const Cplx *slots, double *coeffs, u64 *pt, const CkksTables &T, double sc,
+                                        size_t n_vec, cudaStream_t st) {
+    auto kf = ckks_enc_fft_kernel<LOGN, CKKS_FFT_NT>;
+    const size_t smem_fft = ((size_t)1 << (LOGN - 1)) * sizeof(Cplx);
+    static ConfiguredMask conf_fft, conf_ntt;
+    cudaError_t e = set_smem_once(kf, smem_fft, conf_fft, lc.device);
+    if (e != cudaSuccess) return e;
+    kf<<<(unsigned)n_vec, CKKS_FFT_NT, smem_fft, st>>>(slots, coeffs, T.tw, T.tj, sc);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    const size_t n_limbs = n_vec * lc.L;
+    if constexpr (LOGN == NTT_PAIR_LOGN) {
+        auto kn = ckks_enc_ntt_pair_kernel<256, 2>;   // at 3 CTAs per SM (80 registers) the reducing load stage spills
+        const size_t smem = Geometry<13>::LIMB_BYTES;   // half a limb
+        e = set_smem_once(kn, smem, conf_ntt, lc.device);
+        if (e != cudaSuccess) return e;
+        kn<<<(unsigned)(2 * n_limbs), 256, smem, st>>>(coeffs, pt, lc.tw, T.pow2, lc.lt, lc.L);
+    } else {
+        constexpr int MINB = LOGN == 12 ? 2 : 3;
+        auto kn = ckks_enc_ntt_kernel<LOGN, 256, MINB>;
+        const size_t smem = Geometry<LOGN>::LIMB_BYTES;
+        e = set_smem_once(kn, smem, conf_ntt, lc.device);
+        if (e != cudaSuccess) return e;
+        kn<<<(unsigned)n_limbs, 256, smem, st>>>(coeffs, pt, lc.tw, T.pow2, lc.lt, lc.L);
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ckks_encode(const LaunchCtx &lc, const Cplx *slots, double *coeffs, u64 *pt, const CkksTables &T, double sc, size_t n_vec,
+                               cudaStream_t st) {
+    if (n_vec == 0) return cudaSuccess;
+    if (n_vec * lc.L * 2 > 0x7fffffffull) return cudaErrorInvalidValue;
+    switch (lc.log_n) {
+        case 12: return launch_ckks_encode_t<12>(lc, slots, coeffs, pt, T, sc, n_vec, st);
+        case 13: return launch_ckks_encode_t<13>(lc, slots, coeffs, pt, T, sc, n_vec, st);
+        case 14: return launch_ckks_encode_t<14>(lc, slots, coeffs, pt, T, sc, n_vec, st);
+    }
+    return cudaErrorInvalidValue;
+}
+
+template <int LOGN>
+static cudaError_t launch_ckks_decode_t(const LaunchCtx &lc, u64 *work, Cplx *slots, const CkksTables &T, const CkksConsts &K, size_t n_vec,
+                                        cudaStream_t st) {
+    auto kd = ckks_dec_kernel<LOGN, CKKS_FFT_NT>;
+    const size_t smem = ((size_t)1 << (LOGN - 1)) * sizeof(Cplx);
+    static ConfiguredMask conf;
+    cudaError_t e = set_smem_once(kd, smem, conf, lc.device);
+    if (e != cudaSuccess) return e;
+    kd<<<(unsigned)n_vec, CKKS_FFT_NT, smem, st>>>(work, slots, T.tw, T.tj, lc.lt, K, lc.L);
+    return cudaGetLastError();
+}
+
+// work: [n_vec][L][N] inverse transforms of the plaintexts (overwritten)
+cudaError_t launch_ckks_decode(const LaunchCtx &lc, u64 *work, Cplx *slots, const CkksTables &T, const CkksConsts &K, size_t n_vec, cudaStream_t st) {
+    if (n_vec == 0) return cudaSuccess;
+    if (n_vec > 0x7fffffffull) return cudaErrorInvalidValue;
+    switch (lc.log_n) {
+        case 12: return launch_ckks_decode_t<12>(lc, work, slots, T, K, n_vec, st);
+        case 13: return launch_ckks_decode_t<13>(lc, work, slots, T, K, n_vec, st);
+        case 14: return launch_ckks_decode_t<14>(lc, work, slots, T, K, n_vec, st);
     }
     return cudaErrorInvalidValue;
 }

@@ -72,7 +72,11 @@ struct LaunchCtx {
     cudaError_t launch_ct_mul_plain(const LaunchCtx &lc, const u64 *ct, const u64 *pt, u64 *out, size_t batch, cudaStream_t st); \
     cudaError_t launch_ct_mul_plain_acc(const LaunchCtx &lc, const u64 *ct, const u64 *pt, u64 *acc, size_t batch, cudaStream_t st); \
     cudaError_t launch_ct_tensor(const LaunchCtx &lc, const u64 *a, const u64 *b, u64 *d, size_t batch, cudaStream_t st); \
-    cudaError_t launch_fill_uniform(const LaunchCtx &lc, u64 seed, u64 first_poly, u64 *data, size_t n_polys, cudaStream_t st);
+    cudaError_t launch_fill_uniform(const LaunchCtx &lc, u64 seed, u64 first_poly, u64 *data, size_t n_polys, cudaStream_t st); \
+    cudaError_t launch_ckks_encode(const LaunchCtx &lc, const Cplx *slots, double *coeffs, u64 *pt, const CkksTables &T, double sc, size_t n_vec, \
+                                   cudaStream_t st); \
+    cudaError_t launch_ckks_decode(const LaunchCtx &lc, u64 *work, Cplx *slots, const CkksTables &T, const CkksConsts &K, size_t n_vec, \
+                                   cudaStream_t st);
 
 namespace gen {
 DPFHE_DECLARE_LAUNCHERS

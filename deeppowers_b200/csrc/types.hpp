@@ -112,6 +112,25 @@ DPFHE_HD int tw_pos(int s, int i) {
     return (1 << s) + j * (1 << (LOGN - 4)) + row;
 }
 
+// CKKS slot encoding (DESIGN.md §2.12).  A complex double, laid out as the (re, im) pairs of the slot arrays.
+struct alignas(16) Cplx {
+    double re, im;
+};
+constexpr int CKKS_POW2_E = 1024;   // 2^e mod q_l is tabulated for 0 <= e < 1024, every exponent a finite double can carry
+// device tables of one context, built on first use (host_params.cpp:build_ckks_tables)
+struct CkksTables {
+    const Cplx *tw = nullptr;       // [N]   (cos, sin)(pi k / N), correctly rounded
+    const u32 *tj = nullptr;        // [N/2] t_j = (5^j mod 2N - 1) / 4: slot j is the DFT output t_j
+    const u64 *pow2 = nullptr;      // [L][CKKS_POW2_E] 2^e mod q_l
+};
+// decoding constants of one context (host_params.cpp:build_ckks_consts), passed by value in the kernel parameter block
+struct CkksConsts {
+    u64 ginv[16][16];   // [j][i] q_j^-1 mod q_i (j < i): Garner's mixed-radix digits
+    u64 half[16];       // mixed-radix digits of (Q - 1) / 2, Q = q_0 ... q_{L-1}
+    double qd[16];      // q_l rounded to double
+    double scale;       // the divisor of the decoded coefficients
+};
+
 enum KsMode { KS_MUL_RELIN = 0, KS_PLAIN = 1, KS_ROTATE = 2 };
 // tau' rows of a hybrid key-switching group are double-buffered by round parity (the division step runs one round late)
 constexpr int KS_HYB_ROWS = 6;

@@ -29,6 +29,24 @@ def _ptr(x):
     raise TypeError("unsupported buffer type %r" % type(x))
 
 
+def _cptr(x):
+    """device pointer of a contiguous complex128 CUDA tensor (CKKS slots, N/2 per vector)"""
+    import torch
+    if not hasattr(x, "data_ptr") or x.dtype != torch.complex128 or not x.is_contiguous():
+        raise ValueError("CKKS slots must be contiguous complex128 tensors")
+    if not x.is_cuda:
+        raise ValueError("expected a CUDA tensor (use the *_host entry points for host arrays)")
+    return C.c_void_p(x.data_ptr())
+
+
+def _chptr(a, writable=False):
+    if not isinstance(a, np.ndarray) or a.dtype != np.complex128 or not a.flags["C_CONTIGUOUS"]:
+        raise ValueError("CKKS slots must be C-contiguous numpy complex128 arrays")
+    if writable and not a.flags["WRITEABLE"]:
+        raise ValueError("output array is read-only")
+    return C.c_void_p(a.ctypes.data)
+
+
 def _hptr(a, writable=False):
     if not isinstance(a, np.ndarray) or a.dtype != np.uint64 or not a.flags["C_CONTIGUOUS"]:
         raise ValueError("host buffers must be C-contiguous numpy uint64 arrays")
@@ -275,6 +293,22 @@ class Context:
 
     def rotate_hybrid(self, ct, galois_elt, gk, out, batch, t_plain=0, stream=None):
         self._chk(self._l.dpfhe_rotate_hybrid(self._h, _ptr(ct), int(galois_elt), _ptr(gk), _ptr(out), batch, int(t_plain), _stream(stream)))
+
+    # CKKS slot encoding (DESIGN.md section 2.12): slots [n_vec][N/2] complex128, plaintexts [n_vec][L][N] in evaluation form;
+    # bit-exact against the oracle's restatement.  Plaintexts for a context with special primes: encode with the context
+    # over the ciphertext moduli.
+    def ckks_encode(self, slots, pt, n_vec, scale, stream=None):
+        self._chk(self._l.dpfhe_ckks_encode(self._h, _cptr(slots), _ptr(pt), n_vec, float(scale), _stream(stream)))
+
+    def ckks_decode(self, pt, slots, n_vec, scale, stream=None):
+        """pt is not modified (the inverse transform runs into the context's scratch)"""
+        self._chk(self._l.dpfhe_ckks_decode(self._h, _ptr(pt), _cptr(slots), n_vec, float(scale), _stream(stream)))
+
+    def ckks_encode_host(self, slots, pt, scale):
+        self._chk(self._l.dpfhe_ckks_encode_host(self._h, _chptr(slots), _hptr(pt, True), slots.size // (self.N // 2), float(scale)))
+
+    def ckks_decode_host(self, pt, slots, scale):
+        self._chk(self._l.dpfhe_ckks_decode_host(self._h, _hptr(pt), _chptr(slots, True), pt.size // self.P, float(scale)))
 
     def fill_uniform(self, seed, data, n_polys, first_poly=0, stream=None):
         self._chk(self._l.dpfhe_fill_uniform(self._h, int(seed), int(first_poly), _ptr(data), n_polys, _stream(stream)))

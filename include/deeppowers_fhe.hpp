@@ -13,6 +13,7 @@
 // Header-only over the extern "C" library (include/dpfhe.h, libdpfhe.so); no CUDA headers needed.
 #pragma once
 
+#include <complex>
 #include <cstddef>
 #include <cstdint>
 #include <stdexcept>
@@ -77,6 +78,16 @@ public:
         for (; e; e >>= 1, b = b * b % two_n)
             if (e & 1) g = g * b % two_n;
         return g;
+    }
+
+    // ---- CKKS slot encoding (DESIGN.md §2.12): `count` vectors of slot_count() slots <-> `count` plaintexts of poly_words()
+    //      words in evaluation form; synchronous host-buffer calls ----
+    std::size_t slot_count() const { return poly_degree() / 2; }
+    void encode_ckks(const std::complex<double> *slots, std::size_t count, double scale, std::uint64_t *plain_eval) {
+        check(dpfhe_ckks_encode_host(ctx_, reinterpret_cast<const double *>(slots), plain_eval, count, scale));
+    }
+    void decode_ckks(const std::uint64_t *plain_eval, std::size_t count, double scale, std::complex<double> *slots) {
+        check(dpfhe_ckks_decode_host(ctx_, plain_eval, reinterpret_cast<double *>(slots), count, scale));
     }
 
     // ---- host-buffer calls: synchronous; H2D / compute / D2H are pipelined inside the library ----

@@ -222,6 +222,20 @@ int dpfhe_ct_mul_relin_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const ui
 int dpfhe_rotate_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_ct, uint64_t galois_elt,
                               const uint64_t *h_gk, uint64_t *h_out, size_t batch, uint64_t t_plain);
 
+/* ---- CKKS slot encoding (DESIGN.md §2.12).  Slots are N/2 complex doubles stored as interleaved (re, im) pairs,
+ *      [n_vec][N/2][2]; plaintexts are [n_vec][L][N] in evaluation form.  Slot j is the value of the plaintext polynomial at
+ *      exp(i pi (5^j mod 2N) / N) divided by `scale`, so dpfhe_galois_element(k) moves slot j+k to slot j and 2N-1 conjugates.
+ *      encode: coefficients rint(scale * m_k), reduced exactly into every limb, then the forward transform.
+ *      decode: inverse transform (into scratch: d_pt is not modified), centred CRT value / scale, then the special FFT.
+ *      The results are bit-exact: the floating-point operation order is fixed by the specification.  `scale` must be finite and
+ *      positive; non-finite slots, or coefficients beyond the double range, give unspecified (but memory-safe) results.
+ *      A plaintext for ciphertexts under a context with special primes is encoded with the context over the ciphertext moduli.
+ *      The *_host forms take host buffers and pipeline them in chunks (synchronous). ---- */
+int dpfhe_ckks_encode(dpfhe_ctx *ctx, const double *d_slots, uint64_t *d_pt, size_t n_vec, double scale, void *stream);
+int dpfhe_ckks_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, double *d_slots, size_t n_vec, double scale, void *stream);
+int dpfhe_ckks_encode_host(dpfhe_ctx *ctx, const double *h_slots, uint64_t *h_pt, size_t n_vec, double scale);
+int dpfhe_ckks_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, double *h_slots, size_t n_vec, double scale);
+
 /* ---- synthetic data (DESIGN.md §5): x[k] = mulhi64(splitmix64(seed + k), q_limb),
  *      k = (first_poly + p)*L*N + l*N + n.  Fills [n_polys][L][N]. ---- */
 int dpfhe_fill_uniform(dpfhe_ctx *ctx, uint64_t seed, uint64_t first_poly, uint64_t *d_data,
