@@ -461,8 +461,12 @@ class LinearLayer:
             raise DpfheError(self._l.dpfhe_last_error().decode())
 
     def close(self):
+        """Close the layer before its context.  dpfhe_linear_destroy reads the context, so once the context is closed (for example
+        when the garbage collector finalizes both in the wrong order) the layer is dropped without it and its device buffers go
+        with the process."""
         if getattr(self, "_h", None) and self._h.value:
-            self._l.dpfhe_linear_destroy(self._h)
+            if self.ctx._h.value:
+                self._l.dpfhe_linear_destroy(self._h)
             self._h = C.c_void_p()
 
     __del__ = close
