@@ -83,6 +83,8 @@ SYMBOLS = {
     "dpfhe_multi_rotate_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t]),
     "dpfhe_multi_ct_mul_relin_gather": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.c_int, C.c_size_t]),
     "dpfhe_linear_create": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "dpfhe_linear_create_grouped": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint64,
+                                              C.POINTER(C.c_void_p)]),
     "dpfhe_linear_destroy": (None, [C.c_void_p]),
     "dpfhe_linear_apply": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "dpfhe_linear_apply_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),

@@ -494,6 +494,18 @@ static int check_special(const dpfhe_ctx *ctx, unsigned n_special) {
     return DPFHE_OK;
 }
 
+// the special-prime accumulator and tau' rows of the hybrid / grouped key-switch kernels, allocated at the first call that needs them
+static int ensure_hyb(dpfhe_ctx *ctx) {
+    if (ctx->lc.ks_hyb) return DPFHE_OK;
+    u64 *hyb = nullptr;
+    const size_t hyb_bytes = (ctx->lc.ks_slots / 2 + 1) * KS_HYB_ROWS * ctx->N() * sizeof(u64), acc_bytes = ctx->lc.ks_slots * 4 * ctx->N() * sizeof(u64);
+    CU_TRY(cudaMalloc(&hyb, hyb_bytes));
+    ctx->lc.ks_hyb = hyb;
+    CU_TRY(cudaMalloc(&ctx->lc.ks_acc_hyb, acc_bytes));
+    ctx->device_bytes += hyb_bytes + acc_bytes;
+    return DPFHE_OK;
+}
+
 static int ks_hybrid_common(dpfhe_ctx *ctx, int mode, const uint64_t *a, const uint64_t *b, const uint64_t *key, uint64_t *out,
                             size_t batch, uint64_t galois, uint64_t t_plain, void *stream, unsigned n_special = 1) {
     int rc = enter(ctx);
@@ -515,14 +527,8 @@ static int ks_hybrid_common(dpfhe_ctx *ctx, int mode, const uint64_t *a, const u
         if (overlaps(out, batch * ct_bytes, a, in_bytes) || overlaps(out, batch * ct_bytes, b, in_bytes))
             return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
     }
-    if (!ctx->lc.ks_hyb) {
-        u64 *hyb = nullptr;
-        const size_t hyb_bytes = (ctx->lc.ks_slots / 2 + 1) * KS_HYB_ROWS * ctx->N() * sizeof(u64), acc_bytes = ctx->lc.ks_slots * 4 * ctx->N() * sizeof(u64);
-        CU_TRY(cudaMalloc(&hyb, hyb_bytes));
-        ctx->lc.ks_hyb = hyb;
-        CU_TRY(cudaMalloc(&ctx->lc.ks_acc_hyb, acc_bytes));
-        ctx->device_bytes += hyb_bytes + acc_bytes;
-    }
+    rc = ensure_hyb(ctx);
+    if (rc) return rc;
     MsConsts K;
     if (n_special == 1) {
         build_ms_consts(ctx->hp, t_plain, K);
@@ -658,8 +664,11 @@ int dpfhe_rotate_hoisted(dpfhe_ctx *ctx, const uint64_t *d_ct, size_t n_rot, con
 // Hoisted rotations with grouped hybrid keys (DESIGN.md §2.11b): the mod-up of c1 is done once per ciphertext
 // (ks_hoistg_kernel), every rotation is then gathers + multiply-accumulates over all L limbs (rot_apply_grouped_kernel) and
 // the division by P (md_tau / md_limb kernels).  Same plaintexts as n_rot calls of dpfhe_rotate_grouped, not the same bits.
-int dpfhe_rotate_hoisted_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_ct, size_t n_rot, const uint64_t *galois_elts,
-                                 const uint64_t *const *d_gks, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+// key_s: optional Shoup companions of every key, kept by the caller (a linear layer applies the same rotations to every batch);
+// nullptr = built per rotation into the context's scratch (one more launch each).
+static int rotate_hoisted_grouped_impl(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_ct, size_t n_rot, const uint64_t *galois_elts,
+                                       const uint64_t *const *d_gks, const uint64_t *const *key_s, uint64_t *d_out, size_t batch, uint64_t t_plain,
+                                       void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (batch == 0 || n_rot == 0) return DPFHE_OK;
@@ -707,12 +716,17 @@ int dpfhe_rotate_hoisted_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint6
         note_launch(ctx, 1);
         for (size_t r = 0; r < n_rot; ++r) {
             u64 *out = d_out + (r * batch + first) * 2 * Pq;
-            CU_TRY(VCALL(launch_rot_apply_grouped, ctx->lc, in, U, d_gks[r], nullptr, (u32)galois_elts[r], acc, K, G, cnt, st));
+            CU_TRY(VCALL(launch_rot_apply_grouped, ctx->lc, in, U, d_gks[r], key_s ? key_s[r] : nullptr, (u32)galois_elts[r], acc, K, G, cnt, st));
             CU_TRY(VCALL(launch_mod_down_special, ctx->lc, acc, tau, out, K, G, 2 * cnt, st));
-            note_launch(ctx, 4);   // key_prepare, rot_apply_grouped, md_tau, md_limb
+            note_launch(ctx, key_s ? 3 : 4);   // (key_prepare,) rot_apply_grouped, md_tau, md_limb
         }
     }
     return DPFHE_OK;
+}
+
+int dpfhe_rotate_hoisted_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_ct, size_t n_rot, const uint64_t *galois_elts,
+                                 const uint64_t *const *d_gks, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+    return rotate_hoisted_grouped_impl(ctx, n_special, d_ct, n_rot, galois_elts, d_gks, nullptr, d_out, batch, t_plain, stream);
 }
 
 int dpfhe_ct_mul_plain(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch, void *stream) {
@@ -1205,17 +1219,28 @@ int dpfhe_debug_phase_cycles(dpfhe_ctx *ctx, uint64_t *out16) {
 //   all giant-step inner sums in one pass over the baby steps               -> dpfhe_ct_mul_plain_inner
 //   Horner over the giant steps: acc = rot_baby(acc) + inner[g]              -> dpfhe_rotate + dpfhe_poly_add
 // and the host-buffer form pipelines chunks of the batch through it (upload / compute / download overlapped).
+// With grouped special-prime keys (dpfhe_linear_create_grouped, ciphertexts of Lq = L - K limbs) the baby steps are hoisted
+// grouped rotations with companions prepared at creation, the inner sums run on an Lq-limb view of the context, and every
+// Horner step is ONE launch: the grouped rotation adds inner[g] in its final store (ks_grouped_kernel<..., ADD>).
 struct dpfhe_linear {
     dpfhe_ctx *ctx = nullptr;
     size_t n = 0, baby = 0, giant = 0;
-    u64 *d_diags = nullptr;                 // [n][L][N]
-    u64 *d_keys = nullptr;                  // [baby-1 + 1][L][2][L][N]: baby-step keys, then the giant-step key
+    unsigned n_special = 0;                 // 0: per-limb-digit keys; K > 0: grouped keys with K special primes
+    size_t Lq = 0;                          // limbs of a ciphertext polynomial: L, or L - K with grouped keys
+    u64 *d_diags = nullptr;                 // [n][Lq][N]
+    u64 *d_keys = nullptr;                  // [baby-1 + 1][key]: baby-step keys, then the giant-step key; key [L][2][L][N] or grouped [dnum][2][L][N]
     std::vector<uint64_t> g_baby;           // Galois elements 5^b, b = 1 .. baby-1
     std::vector<const uint64_t *> k_baby;   // device pointers of the baby-step keys
-    u64 *d_prep = nullptr;                  // per baby step: Shoup companions of its key [L][2][L][N] + kprime [2][L][N], built once
-    std::vector<const uint64_t *> prep;     // {companions, kprime} pointers per baby step (rotate_hoisted_impl)
+    u64 *d_prep = nullptr;                  // per baby step: Shoup companions of its key [L][2][L][N] + kprime [2][L][N], built once;
+                                            //   grouped: the companions of every key [baby-1 + 1][dnum][2][L][N]
+    std::vector<const uint64_t *> prep;     // {companions, kprime} pointers per baby step (rotate_hoisted_impl); grouped: companions per
+                                            //   baby step (rotate_hoisted_grouped_impl)
+    const u64 *prep_giant = nullptr;        // grouped: companions of the giant-step key
     uint64_t g_giant = 0;
-    u64 *scratch = nullptr;                 // [baby + giant + 1][cap][2][L][N]
+    uint64_t t_plain = 0;                   // grouped: plaintext modulus of the divisions by P (0: plain rounding)
+    MsConsts K;                             // grouped: constants of the division by P
+    GroupConsts G;
+    u64 *scratch = nullptr;                 // [baby + giant + 1][cap][2][Lq][N]
     size_t cap = 0;                         // ciphertexts the scratch holds
 };
 
@@ -1227,8 +1252,16 @@ static int linear_reserve(dpfhe_linear *lin, size_t batch) {
     cudaFree(lin->scratch);
     lin->scratch = nullptr;
     lin->cap = 0;
-    CU_TRY(cudaMalloc(&lin->scratch, (lin->baby + lin->giant + 1) * batch * 2 * ctx->P() * 8));
+    CU_TRY(cudaMalloc(&lin->scratch, (lin->baby + lin->giant + 1) * batch * 2 * lin->Lq * ctx->N() * 8));
     lin->cap = batch;
+    return DPFHE_OK;
+}
+
+static int linear_check_shape(size_t n_diags, size_t baby, const uint64_t *h_gk_baby, const uint64_t *h_gk_giant) {
+    if (baby == 0 || baby > 128 || n_diags == 0 || n_diags % baby) return fail(DPFHE_ERR_INVALID, "need 1 <= baby <= 128 and a multiple of baby diagonals");
+    const size_t giant = n_diags / baby;
+    if (giant > 65535) return fail(DPFHE_ERR_INVALID, "too many giant steps");
+    if ((baby > 1 && !h_gk_baby) || (giant > 1 && !h_gk_giant)) return fail(DPFHE_ERR_INVALID, "missing Galois keys");
     return DPFHE_OK;
 }
 
@@ -1238,13 +1271,12 @@ int dpfhe_linear_create(dpfhe_ctx *ctx, const uint64_t *h_diags, size_t n_diags,
     if (rc) return rc;
     if (!out || !h_diags) return fail(DPFHE_ERR_INVALID, "null argument");
     *out = nullptr;
-    if (baby == 0 || baby > 128 || n_diags == 0 || n_diags % baby) return fail(DPFHE_ERR_INVALID, "need 1 <= baby <= 128 and a multiple of baby diagonals");
+    rc = linear_check_shape(n_diags, baby, h_gk_baby, h_gk_giant);
+    if (rc) return rc;
     const size_t giant = n_diags / baby;
-    if (giant > 65535) return fail(DPFHE_ERR_INVALID, "too many giant steps");
-    if ((baby > 1 && !h_gk_baby) || (giant > 1 && !h_gk_giant)) return fail(DPFHE_ERR_INVALID, "missing Galois keys");
     dpfhe_linear *lin = new (std::nothrow) dpfhe_linear();
     if (!lin) return fail(DPFHE_ERR_NOMEM, "out of host memory");
-    lin->ctx = ctx; lin->n = n_diags; lin->baby = baby; lin->giant = giant;
+    lin->ctx = ctx; lin->n = n_diags; lin->baby = baby; lin->giant = giant; lin->Lq = ctx->hp.L;
     const size_t P8 = ctx->P() * 8, key_bytes = 2 * ctx->hp.L * P8;
     cudaError_t e = cudaMalloc(&lin->d_diags, n_diags * P8);
     if (e == cudaSuccess) e = cudaMalloc(&lin->d_keys, baby * key_bytes);
@@ -1286,6 +1318,65 @@ int dpfhe_linear_create(dpfhe_ctx *ctx, const uint64_t *h_diags, size_t n_diags,
     return DPFHE_OK;
 }
 
+int dpfhe_linear_create_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_diags, size_t n_diags, size_t baby,
+                                const uint64_t *h_gk_baby, const uint64_t *h_gk_giant, uint64_t t_plain, dpfhe_linear **out) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!out || !h_diags) return fail(DPFHE_ERR_INVALID, "null argument");
+    *out = nullptr;
+    rc = check_special(ctx, n_special);
+    if (rc) return rc;
+    const unsigned L = ctx->hp.L;
+    for (unsigned k = 0; k < n_special; ++k)
+        if (t_plain >= ctx->hp.limbs[L - 1 - k].lp.q) return fail(DPFHE_ERR_INVALID, "plaintext modulus must be below the special prime");
+    rc = linear_check_shape(n_diags, baby, h_gk_baby, h_gk_giant);
+    if (rc) return rc;
+    dpfhe_linear *lin = new (std::nothrow) dpfhe_linear();
+    if (!lin) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    const size_t N = ctx->N(), Lq = L - n_special, dnum = (Lq + n_special - 1) / n_special, key_bytes = dnum * 2 * L * N * 8;
+    lin->ctx = ctx; lin->n = n_diags; lin->baby = baby; lin->giant = n_diags / baby; lin->n_special = n_special; lin->Lq = Lq; lin->t_plain = t_plain;
+    build_group_consts(ctx->hp, n_special, t_plain, lin->G, lin->K);
+    cudaError_t e = cudaMalloc(&lin->d_diags, n_diags * Lq * N * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&lin->d_keys, baby * key_bytes);
+    if (e == cudaSuccess) e = cudaMalloc(&lin->d_prep, baby * key_bytes);
+    if (e == cudaSuccess) e = cudaMemcpy(lin->d_diags, h_diags, n_diags * Lq * N * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && baby > 1) e = cudaMemcpy(lin->d_keys, h_gk_baby, (baby - 1) * key_bytes, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && lin->giant > 1) e = cudaMemcpy(lin->d_keys + (baby - 1) * key_bytes / 8, h_gk_giant, key_bytes, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        dpfhe_linear_destroy(lin);
+        return fail(DPFHE_ERR_CUDA, "linear layer upload: %s", cudaGetErrorString(e));
+    }
+    for (size_t b = 1; b < baby; ++b) {
+        uint64_t g = 0;
+        dpfhe_galois_element(ctx, (int)b, &g);
+        lin->g_baby.push_back(g);
+        lin->k_baby.push_back(lin->d_keys + (b - 1) * key_bytes / 8);
+        lin->prep.push_back(lin->d_prep + (b - 1) * key_bytes / 8);
+    }
+    dpfhe_galois_element(ctx, (int)baby, &lin->g_giant);
+    lin->prep_giant = lin->d_prep + (baby - 1) * key_bytes / 8;
+    // the Shoup companions of every key, once: each application would otherwise rebuild them for every rotation
+    rc = lin->giant > 1 ? ensure_hyb(ctx) : DPFHE_OK;   // the special-prime rows of the giant steps' kernel
+    if (rc) {
+        dpfhe_linear_destroy(lin);
+        return rc;
+    }
+    cudaStream_t st = pick(ctx, nullptr);
+    for (size_t b = 0; b < baby && e == cudaSuccess; ++b) {
+        if (b + 1 < baby || lin->giant > 1) {
+            e = VCALL(launch_key_prepare_grouped, ctx->lc, lin->d_keys + b * key_bytes / 8, lin->d_prep + b * key_bytes / 8, (u32)dnum, st);
+            note_launch(ctx, 1);
+        }
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) {
+        dpfhe_linear_destroy(lin);
+        return fail(DPFHE_ERR_CUDA, "linear layer constants: %s", cudaGetErrorString(e));
+    }
+    *out = lin;
+    return DPFHE_OK;
+}
+
 void dpfhe_linear_destroy(dpfhe_linear *lin) {
     if (!lin) return;
     if (lin->ctx) {
@@ -1299,7 +1390,48 @@ void dpfhe_linear_destroy(dpfhe_linear *lin) {
     delete lin;
 }
 
+// grouped keys: hoisted baby steps, the inner sums on the ciphertext moduli, giant - 1 fused Horner steps.  Launches per application
+// (a batch within one chunk of the hoisted-rotation scratch): [baby > 1] * (1 + 3 (baby-1)) + ceil(giant / gmax(baby)) + (giant - 1),
+// gmax = the giant steps one inner-product launch holds.
+static int linear_apply_grouped_on(dpfhe_linear *lin, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
+    dpfhe_ctx *ctx = lin->ctx;
+    const size_t ctb = batch * 2 * lin->Lq * ctx->N();          // words of one ciphertext batch
+    u64 *steps = lin->scratch, *inner = steps + lin->baby * ctb, *tmp = inner + lin->giant * ctb;
+    cudaStream_t st = pick(ctx, stream);
+    CU_TRY(cudaMemcpyAsync(steps, d_ct, ctb * 8, cudaMemcpyDeviceToDevice, st));
+    int rc = DPFHE_OK;
+    if (lin->baby > 1)
+        rc = rotate_hoisted_grouped_impl(ctx, lin->n_special, steps, lin->baby - 1, lin->g_baby.data(), lin->k_baby.data(), lin->prep.data(),
+                                         steps + ctb, batch, lin->t_plain, stream);
+    if (rc) return rc;
+    // every inner sum in one pass, on the first Lq limbs: a view of the context's launch state (its tables of those limbs come
+    // first), driven on the stream of this call, so it costs no device memory and keeps the calls' order
+    st = pick(ctx, stream);
+    LaunchCtx lcq = ctx->lc;
+    lcq.L = (u32)lin->Lq;
+    unsigned launches = 0;
+    CU_TRY(VCALL(launch_pt_inner, lcq, steps, (u32)lin->baby, lin->d_diags, (u32)lin->giant, inner, batch, st, &launches));
+    note_launch(ctx, launches);
+    if (lin->giant == 1) {
+        CU_TRY(cudaMemcpyAsync(d_out, inner, ctb * 8, cudaMemcpyDeviceToDevice, st));
+        return DPFHE_OK;
+    }
+    // Horner: acc = rot_baby(acc) + inner[g], one launch per step.  The output may not alias the rotated input or the addend: the
+    // steps alternate between tmp and d_out so that the last one (g = 0) writes d_out.
+    const u64 *gk_giant = lin->d_keys + (lin->prep_giant - lin->d_prep);   // same position in the key array as its companions
+    const u64 *acc = inner + (lin->giant - 1) * ctb;
+    for (size_t g = lin->giant - 1; g-- > 0;) {
+        u64 *dst = g % 2 == 0 ? d_out : tmp;
+        CU_TRY(VCALL(launch_ks_grouped, ctx->lc, KS_ROTATE, acc, nullptr, gk_giant, dst, batch, (u32)lin->g_giant, lin->K, lin->G, st, inner + g * ctb,
+                     lin->prep_giant));
+        note_launch(ctx, 1);
+        acc = dst;
+    }
+    return DPFHE_OK;
+}
+
 static int linear_apply_on(dpfhe_linear *lin, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
+    if (lin->n_special) return linear_apply_grouped_on(lin, d_ct, d_out, batch, stream);
     dpfhe_ctx *ctx = lin->ctx;
     const size_t ctb = batch * 2 * ctx->P();                 // words of one ciphertext batch
     u64 *steps = lin->scratch, *inner = steps + lin->baby * ctb, *tmp = inner + lin->giant * ctb;
@@ -1329,7 +1461,8 @@ int dpfhe_linear_apply(dpfhe_linear *lin, const uint64_t *d_ct, uint64_t *d_out,
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
     CHECK_PTR(d_ct); CHECK_PTR(d_out);
-    if (overlaps(d_out, batch * 2 * lin->ctx->P() * 8, d_ct, batch * 2 * lin->ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    const size_t ct_bytes = batch * 2 * lin->Lq * lin->ctx->N() * 8;   // Lq = L - K limbs with grouped keys
+    if (overlaps(d_out, ct_bytes, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
     rc = linear_reserve(lin, batch);
     if (rc) return rc;
     return linear_apply_on(lin, d_ct, d_out, batch, stream);
@@ -1343,7 +1476,8 @@ int dpfhe_linear_apply_host(dpfhe_linear *lin, const uint64_t *h_ct, uint64_t *h
     if (batch == 0) return DPFHE_OK;
     if (!h_ct || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
     // Chunks of about a fifth of the batch, rounded to whole rounds of the persistent key-switch grid (3 CTAs per SM, L CTAs
-    // per ciphertext): a chunk that leaves the grid's last round mostly empty costs more than the transfers it hides.  The
+    // per ciphertext: with grouped keys L = Lq + K, every limb of the context): a chunk that leaves the grid's last round mostly
+    // empty costs more than the transfers it hides.  The
     // first upload and the last download are the only transfers not overlapped with a neighbouring chunk's compute.
     const size_t groups = std::max<size_t>(1, (size_t)ctx->lc.num_sms * 3 / ctx->hp.L);
     size_t rounds = (batch / 5 + groups / 2) / groups;
@@ -1354,7 +1488,7 @@ int dpfhe_linear_apply_host(dpfhe_linear *lin, const uint64_t *h_ct, uint64_t *h
     if (chunk > batch) chunk = batch;
     rc = linear_reserve(lin, chunk);
     if (rc) return rc;
-    const size_t ct_words = 2 * ctx->P();
+    const size_t ct_words = 2 * lin->Lq * ctx->N();
     return run_pipeline(ctx, h_ct, nullptr, h_out, batch, ct_words, ct_words, chunk,
                         [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int { return linear_apply_on(lin, din, dout, cnt, st); });
 }

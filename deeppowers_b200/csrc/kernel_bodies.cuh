@@ -665,11 +665,14 @@ DPFHE_HD void ms_tau_body(CTA &cta, u64 *buf, const u64 *row, u64 *work, const T
 // step 2, one (polynomial, kept limb i): out = (c[i] - s * NTT_i(centred(tau') mod q_i)) * q_last^-1 mod q_i.
 // COHERENT: c[i] is an L2-resident lazy accumulator written in this launch (any 64-bit value; may be `out_limb`).
 // LIFT(chunk): the residue mod q_i of the (centred) value to subtract, lazy below 4q.
-template <int LOGN, int NT, bool COHERENT, class CTA, class LIFT>
+// ADD: add_limb (canonical, N words) is added to the result before the store, one csub(q) keeping it canonical: a Horner step
+// rot(acc) + inner_g of a linear layer in the store that writes the rotation anyway (bit-identical to a separate poly_add).
+template <int LOGN, int NT, bool COHERENT, bool ADD = false, class CTA, class LIFT>
 DPFHE_HD void ms_limb_core(CTA &cta, u64 *buf, LIFT lift, const u64 *c_limb, u64 *out_limb, const Twiddle *tw, const LimbParams &p,
-                           const MsConsts &K, u32 i) {
+                           const MsConsts &K, u32 i, const u64 *add_limb = nullptr) {
     constexpr int NC = 1 << (LOGN - 1);
     const U64x2 *cin = reinterpret_cast<const U64x2 *>(c_limb);
+    const U64x2 *addend = reinterpret_cast<const U64x2 *>(add_limb);
     U64x2 *dst = reinterpret_cast<U64x2 *>(out_limb);
     const u64 inv = K.inv[i], inv_s = K.inv_s[i], sinv = K.sinv[i], sinv_s = K.sinv_s[i];
     // c: chunk of the limb; c_buf: where its transform output sits in shared memory
@@ -678,6 +681,11 @@ DPFHE_HD void ms_limb_core(CTA &cta, u64 *buf, LIFT lift, const u64 *c_limb, u64
         U64x2 r;   // c*inv - u*(s*inv): both Shoup products below 2q, difference kept positive with + 2q
         r.x = canon4(shoup_exact(cv.x, inv, inv_s, p) + p.q2 - shoup_exact(u.x, sinv, sinv_s, p), p);
         r.y = canon4(shoup_exact(cv.y, inv, inv_s, p) + p.q2 - shoup_exact(u.y, sinv, sinv_s, p), p);
+        if constexpr (ADD) {   // both canonical: the sum is below 2q
+            const U64x2 a = ld_stream(addend + c);
+            r.x = csub(r.x + a.x, p.q);
+            r.y = csub(r.y + a.y, p.q);
+        }
         st_stream(dst + c, r);
     };
     if constexpr (LOGN <= 13 || NT >= 512) {
@@ -714,10 +722,10 @@ DPFHE_HD void ms_limb_body(CTA &cta, u64 *buf, const u64 *tau, const u64 *c_limb
 }
 
 // division by the product P of K special primes (DESIGN.md §2.11): tau_rows + k * tau_stride is y_k = tau'_k * Phat_k^-1 of
-// special prime k; the value to subtract is sum_k centred(y_k) * Phat_k, converted term by term.
-template <int LOGN, int NT, bool COHERENT = true, class CTA>
+// special prime k; the value to subtract is sum_k centred(y_k) * Phat_k, converted term by term.  ADD / add_limb: as ms_limb_core.
+template <int LOGN, int NT, bool COHERENT = true, bool ADD = false, class CTA>
 DPFHE_HD void ms_limb_group(CTA &cta, u64 *buf, const u64 *tau_rows, size_t tau_stride, const u64 *c_limb, u64 *out_limb, const Twiddle *tw,
-                            const LimbParams &p, const MsConsts &K, const GroupConsts &G, u32 i) {
+                            const LimbParams &p, const MsConsts &K, const GroupConsts &G, u32 i, const u64 *add_limb = nullptr) {
     const u64 neg_p = G.neg_p[i];
     auto lift = [&](int c) {
         U64x2 r;
@@ -737,7 +745,7 @@ DPFHE_HD void ms_limb_group(CTA &cta, u64 *buf, const u64 *tau_rows, size_t tau_
         r.y = csub(csub(r.y, p.q8), p.q4);
         return r;
     };
-    ms_limb_core<LOGN, NT, COHERENT>(cta, buf, lift, c_limb, out_limb, tw, p, K, i);
+    ms_limb_core<LOGN, NT, COHERENT, ADD>(cta, buf, lift, c_limb, out_limb, tw, p, K, i, add_limb);
 }
 
 // ---- hoisted rotations (DESIGN.md §2.8b, §4.4d) ---------------------------------------------------

@@ -621,10 +621,13 @@ __global__ void __launch_bounds__(NT, MINB) ks_hybrid_kernel(KsArgs A, const __g
 //               2 x [basis conversion of the K tau' rows + NTT], out = (acc - s*u) / P     (one round late, as above)
 //   special CTA dnum x [basis conversion + NTT + MAC into its scratch rows]; 2 x INTT (* (t Phat)^-1) -> tau', publish
 // With Lq = 4, K = 2 every CTA runs four transforms per ciphertext (24 in all, against 30 for one special prime).
-template <int LOGN, int NT, int MINB, int MODE>
+// ADD (KS_ROTATE only): the division step adds addend [batch][2][Lq][N] (canonical) to the result before its one store, so that a
+// Horner step of a linear layer, out = rot(acc) + inner_g, is one launch (DESIGN.md §4.4b′).  out must not alias a or addend.
+template <int LOGN, int NT, int MINB, int MODE, bool ADD = false>
 __global__ void __launch_bounds__(NT, MINB) ks_grouped_kernel(KsArgs A, const __grid_constant__ LimbTable lt, const __grid_constant__ MsConsts K,
                                                               const __grid_constant__ GroupConsts G, size_t batch, u32 *flags, u32 epoch,
-                                                              u32 *ticket, u64 *mail) {
+                                                              u32 *ticket, u64 *mail, const u64 *addend) {
+    static_assert(!ADD || MODE == KS_ROTATE, "the fused addition is a Horner step of rotations");
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     constexpr size_t N = (size_t)1 << LOGN;
     u64 *buf = reinterpret_cast<u64 *>(smem_raw);
@@ -653,8 +656,10 @@ __global__ void __launch_bounds__(NT, MINB) ks_grouped_kernel(KsArgs A, const __
         const size_t P = (size_t)Lq * N;
         for (u32 c = 0; c < 2; ++c) {
             u64 *row = A.out + ct * 2 * P + c * P + (size_t)i * N;
-            ms_limb_group<LOGN, NT>(cta, buf, hyb_of(0) + ks_hyb_tau_row(parity, c) * N, (size_t)KS_HYB_ROWS * N, acc_of(parity) + c * N, row,
-                                    A.tw + (size_t)i * N, p, K, G, i);
+            const u64 *add_row = nullptr;
+            if constexpr (ADD) add_row = addend + ct * 2 * P + c * P + (size_t)i * N;
+            ms_limb_group<LOGN, NT, true, ADD>(cta, buf, hyb_of(0) + ks_hyb_tau_row(parity, c) * N, (size_t)KS_HYB_ROWS * N, acc_of(parity) + c * N, row,
+                                               A.tw + (size_t)i * N, p, K, G, i, add_row);
         }
     };
     bool pending = false;
@@ -1352,10 +1357,11 @@ cudaError_t launch_ks_hybrid(LaunchCtx &lc, int mode, const u64 *a, const u64 *b
 
 #endif
 #if DPFHE_PART_GROUPED
-template <int LOGN, int MODE>
-static cudaError_t launch_ks_grouped_t(LaunchCtx &lc, const KsArgs &A, const MsConsts &K, const GroupConsts &Gc, size_t batch, cudaStream_t st) {
+template <int LOGN, int MODE, bool ADD = false>
+static cudaError_t launch_ks_grouped_t(LaunchCtx &lc, const KsArgs &A, const MsConsts &K, const GroupConsts &Gc, size_t batch, cudaStream_t st,
+                                       const u64 *addend) {
     constexpr int NT = 256, MINB = 3;
-    auto kern = ks_grouped_kernel<LOGN, NT, MINB, MODE>;
+    auto kern = ks_grouped_kernel<LOGN, NT, MINB, MODE, ADD>;
     const size_t smem = LOGN <= 13 ? Geometry<LOGN>::LIMB_BYTES : Geometry<13>::LIMB_BYTES;
     static ConfiguredMask configured;
     if (!configured.has(lc.device)) {
@@ -1388,19 +1394,22 @@ static cudaError_t launch_ks_grouped_t(LaunchCtx &lc, const KsArgs &A, const MsC
     u32 epoch = lc.ks_epoch;
     u32 *ticket = lc.ks_ticket;
     u64 *mail = lc.ks_mail;
-    void *params[] = {&args, &lt, &consts, &gc, &batch_arg, &flags, &epoch, &ticket, &mail};
+    const u64 *add = addend;
+    void *params[] = {&args, &lt, &consts, &gc, &batch_arg, &flags, &epoch, &ticket, &mail, &add};
     e = cudaLaunchCooperativeKernel((void *)kern, dim3((unsigned)G), dim3(NT), params, smem, st);
     lc.ks_epoch += rounds;
     return e;
 }
 
 // data has Lq = L - K limbs, the key [dnum][2][L][N]; scratch requirements as launch_ks_hybrid (K <= Lq keeps the special
-// CTAs' rows within lc.ks_hyb)
+// CTAs' rows within lc.ks_hyb).  addend (KS_ROTATE only): out = rotation + addend, one launch.  key_s: the key's Shoup companions,
+// built by the caller once (a linear layer); nullptr = built here into lc.ks_key_s (one more launch).
 cudaError_t launch_ks_grouped(LaunchCtx &lc, int mode, const u64 *a, const u64 *b, const u64 *key, u64 *out, size_t batch, u32 galois,
-                              const MsConsts &K, const GroupConsts &Gc, cudaStream_t st) {
+                              const MsConsts &K, const GroupConsts &Gc, cudaStream_t st, const u64 *addend, const u64 *key_s) {
     if (batch == 0) return cudaSuccess;
     if (lc.L < 2 || !lc.ks_hyb || !lc.ks_acc_hyb || Gc.Lq + Gc.K != lc.L || Gc.K > Gc.Lq || Gc.K > (u32)KS_MAX_SPECIAL) return cudaErrorInvalidValue;
-    {
+    if (addend && mode != KS_ROTATE) return cudaErrorInvalidValue;
+    if (!key_s) {
         const size_t n = (size_t)2 * Gc.dnum * lc.L << lc.log_n;
         const unsigned grid = ew_grid(lc, n);
         if (lc.log_n == 12) key_prepare_kernel<12><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
@@ -1408,17 +1417,20 @@ cudaError_t launch_ks_grouped(LaunchCtx &lc, int mode, const u64 *a, const u64 *
         else key_prepare_kernel<14><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
+        key_s = lc.ks_key_s;
     }
     KsArgs A;
-    A.a = a; A.b = b; A.key = key; A.key_s = lc.ks_key_s; A.out = out; A.scratch = lc.ks_scratch;
+    A.a = a; A.b = b; A.key = key; A.key_s = key_s; A.out = out; A.scratch = lc.ks_scratch;
     A.tw = lc.tw; A.itw = lc.itw; A.L = Gc.Lq; A.galois = galois; A.Lk = lc.L; A.hyb = lc.ks_hyb; A.only = nullptr;
     A.acc = lc.ks_acc_hyb; A.acc_par = 2; A.lift_reduce = 0u;
-#define KS_GRP_DISPATCH(LOGN)                                                                        \
-    switch (mode) {                                                                                  \
-        case KS_MUL_RELIN: return launch_ks_grouped_t<LOGN, KS_MUL_RELIN>(lc, A, K, Gc, batch, st);   \
-        case KS_PLAIN: return launch_ks_grouped_t<LOGN, KS_PLAIN>(lc, A, K, Gc, batch, st);           \
-        case KS_ROTATE: return launch_ks_grouped_t<LOGN, KS_ROTATE>(lc, A, K, Gc, batch, st);         \
-    }                                                                                                \
+#define KS_GRP_DISPATCH(LOGN)                                                                                          \
+    switch (mode) {                                                                                                    \
+        case KS_MUL_RELIN: return launch_ks_grouped_t<LOGN, KS_MUL_RELIN>(lc, A, K, Gc, batch, st, nullptr);            \
+        case KS_PLAIN: return launch_ks_grouped_t<LOGN, KS_PLAIN>(lc, A, K, Gc, batch, st, nullptr);                    \
+        case KS_ROTATE:                                                                                                \
+            if (addend) return launch_ks_grouped_t<LOGN, KS_ROTATE, true>(lc, A, K, Gc, batch, st, addend);            \
+            return launch_ks_grouped_t<LOGN, KS_ROTATE>(lc, A, K, Gc, batch, st, nullptr);                              \
+    }                                                                                                                  \
     return cudaErrorInvalidValue;
     switch (lc.log_n) {
         case 12: KS_GRP_DISPATCH(12)
@@ -1583,6 +1595,20 @@ cudaError_t launch_hoist_grouped(LaunchCtx &lc, const u64 *ct, u64 *U, const Gro
         case 14: return launch_hoistg_t<14>(lc, A, G, batch, st);
     }
     return cudaErrorInvalidValue;
+}
+
+// Shoup companions of a grouped key [dnum][2][L][N] into key_s (same layout): what launch_ks_grouped and launch_rot_apply_grouped
+// build per call when they are not given them
+cudaError_t launch_key_prepare_grouped(const LaunchCtx &lc, const u64 *key, u64 *key_s, u32 dnum, cudaStream_t st) {
+    const size_t n = (size_t)2 * dnum * lc.L << lc.log_n;
+    const unsigned grid = ew_grid(lc, n);
+    switch (lc.log_n) {
+        case 12: key_prepare_kernel<12><<<grid, 256, 0, st>>>(key, key_s, lc.lp, lc.L, n); break;
+        case 13: key_prepare_kernel<13><<<grid, 256, 0, st>>>(key, key_s, lc.lp, lc.L, n); break;
+        case 14: key_prepare_kernel<14><<<grid, 256, 0, st>>>(key, key_s, lc.lp, lc.L, n); break;
+        default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
 }
 
 // step 2: acc [batch][2][L][N] of one rotation (key companions built here into lc.ks_key_s unless the caller supplies them)

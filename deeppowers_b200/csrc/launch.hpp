@@ -58,8 +58,10 @@ struct LaunchCtx {
     cudaError_t launch_ks_hybrid(LaunchCtx &lc, int mode, const u64 *a, const u64 *b, const u64 *key, u64 *out, size_t batch, u32 galois, \
                                  const MsConsts &K, cudaStream_t st); \
     cudaError_t launch_ks_grouped(LaunchCtx &lc, int mode, const u64 *a, const u64 *b, const u64 *key, u64 *out, size_t batch, u32 galois, \
-                                  const MsConsts &K, const GroupConsts &G, cudaStream_t st); \
+                                  const MsConsts &K, const GroupConsts &G, cudaStream_t st, const u64 *addend = nullptr, \
+                                  const u64 *key_s = nullptr); \
     cudaError_t launch_hoist_grouped(LaunchCtx &lc, const u64 *ct, u64 *U, const GroupConsts &G, size_t batch, cudaStream_t st); \
+    cudaError_t launch_key_prepare_grouped(const LaunchCtx &lc, const u64 *key, u64 *key_s, u32 dnum, cudaStream_t st); \
     cudaError_t launch_rot_apply_grouped(LaunchCtx &lc, const u64 *ct, const u64 *U, const u64 *key, const u64 *key_s, u32 galois, u64 *acc, \
                                          const MsConsts &K, const GroupConsts &G, size_t batch, cudaStream_t st); \
     cudaError_t launch_pt_inner(const LaunchCtx &lc, const u64 *steps, u32 nb, const u64 *pts, u32 ng, u64 *out, size_t batch, cudaStream_t st, \
@@ -87,5 +89,7 @@ DPFHE_DECLARE_LAUNCHERS
 #undef DPFHE_DECLARE_LAUNCHERS
 // launch_ks: `only` = optional [batch] filter (non-zero = process); key_ready: the key's Shoup companions are already in key_s
 // (or, with key_s == nullptr, in lc.ks_key_s).  launch_rot_prepare / launch_rot_apply: key_s(_out) == nullptr means lc.ks_key_s.
+// launch_ks_grouped: key_s == nullptr builds the companions into lc.ks_key_s (two launches), otherwise one launch; addend (KS_ROTATE
+// only) is added to the result in the kernel's final store.
 
 }  // namespace dpfhe

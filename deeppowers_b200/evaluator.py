@@ -448,17 +448,33 @@ def linear_bsgs_grouped(ctx, ctx_q, n_special, ct, diags, gk_baby, gk_giant, bab
 class LinearLayer:
     """Encrypted linear layer as a library object (dpfhe_linear_*): diagonal plaintexts and Galois keys live on the device; apply()
     takes device buffers, apply_host() host buffers (pipelined in chunks).  diags [n][L][N], gk_baby [baby-1][L][2][L][N] (keys of the
-    rotations by 1 .. baby-1), gk_giant [L][2][L][N] (rotation by `baby`): C-contiguous numpy uint64 arrays."""
+    rotations by 1 .. baby-1), gk_giant [L][2][L][N] (rotation by `baby`): C-contiguous numpy uint64 arrays.
+    LinearLayer.grouped(...) builds the same layer with grouped special-prime keys."""
 
-    def __init__(self, ctx, diags, baby, gk_baby, gk_giant):
+    def __init__(self, ctx, diags, baby, gk_baby, gk_giant, _n_special=0, _t_plain=0):
         self._l, self.ctx = ctx._l, ctx
         self._h = C.c_void_p()
+        self.n_special = int(_n_special)
+        self.Lq = ctx.L - self.n_special                     # limbs of a ciphertext polynomial
         n = diags.shape[0]
-        rc = self._l.dpfhe_linear_create(ctx._h, _hptr(diags), n, int(baby), _hptr(gk_baby) if gk_baby is not None else None,
-                                         _hptr(gk_giant) if gk_giant is not None else None, C.byref(self._h))
+        kb = _hptr(gk_baby) if gk_baby is not None else None
+        kg = _hptr(gk_giant) if gk_giant is not None else None
+        if self.n_special:
+            rc = self._l.dpfhe_linear_create_grouped(ctx._h, self.n_special, _hptr(diags), n, int(baby), kb, kg, int(_t_plain), C.byref(self._h))
+        else:
+            rc = self._l.dpfhe_linear_create(ctx._h, _hptr(diags), n, int(baby), kb, kg, C.byref(self._h))
         if rc != 0:
             self._h = C.c_void_p()
             raise DpfheError(self._l.dpfhe_last_error().decode())
+
+    @classmethod
+    def grouped(cls, ctx, n_special, diags, baby, gk_baby, gk_giant, t_plain=0):
+        """The layer with grouped special-prime Galois keys (dpfhe_linear_create_grouped): ctx's last n_special limbs are special primes,
+        Lq = L - n_special.  diags [n][Lq][N] (pre-rotated as for linear_bsgs_grouped), gk_baby [baby-1][dnum][2][L][N], gk_giant
+        [dnum][2][L][N]; apply / apply_host take ciphertexts [batch][2][Lq][N].  Bit-identical to linear_bsgs_grouped."""
+        if int(n_special) < 1:
+            raise ValueError("n_special must be at least 1")
+        return cls(ctx, diags, baby, gk_baby, gk_giant, _n_special=n_special, _t_plain=t_plain)
 
     def close(self):
         """Close the layer before its context.  dpfhe_linear_destroy reads the context, so once the context is closed (for example
@@ -475,7 +491,7 @@ class LinearLayer:
         self.ctx._chk(self._l.dpfhe_linear_apply(self._h, _ptr(ct), _ptr(out), batch, _stream(stream)))
 
     def apply_host(self, ct, out):
-        self.ctx._chk(self._l.dpfhe_linear_apply_host(self._h, _hptr(ct), _hptr(out, True), ct.size // (2 * self.ctx.P)))
+        self.ctx._chk(self._l.dpfhe_linear_apply_host(self._h, _hptr(ct), _hptr(out, True), ct.size // (2 * self.Lq * self.ctx.N)))
 
 
 class MultiContext:

@@ -248,6 +248,13 @@ public:
                 const std::uint64_t *giant_key) {
         Evaluator::check(dpfhe_linear_create(ev.native_handle(), diagonals, n_diagonals, baby, baby_keys, giant_key, &h_));
     }
+    // with grouped special-prime keys: the evaluator's last `special` limbs are special primes, ciphertexts and diagonals carry
+    // limbs()-special limbs, keys are [dnum][2][limbs()][N] (dpfhe_linear_create_grouped)
+    LinearLayer(Evaluator &ev, unsigned special, const std::uint64_t *diagonals, std::size_t n_diagonals, std::size_t baby,
+                const std::uint64_t *baby_keys, const std::uint64_t *giant_key, std::uint64_t plain_modulus) {
+        Evaluator::check(dpfhe_linear_create_grouped(ev.native_handle(), special, diagonals, n_diagonals, baby, baby_keys, giant_key, plain_modulus,
+                                                     &h_));
+    }
     ~LinearLayer() { dpfhe_linear_destroy(h_); }
     LinearLayer(const LinearLayer &) = delete;
     LinearLayer &operator=(const LinearLayer &) = delete;

@@ -156,6 +156,14 @@ int dpfhe_ct_mul_plain_inner(dpfhe_ctx *ctx, const uint64_t *d_steps, size_t n_s
 typedef struct dpfhe_linear dpfhe_linear;
 int dpfhe_linear_create(dpfhe_ctx *ctx, const uint64_t *h_diags, size_t n_diags, size_t baby, const uint64_t *h_gk_baby,
                         const uint64_t *h_gk_giant, dpfhe_linear **out);
+/*      The same layer with grouped special-prime Galois keys (DESIGN.md §2.11; the context's last n_special limbs are special
+ *      primes, ciphertexts carry Lq = L - n_special limbs, dnum = ceil(Lq / n_special)): h_diags [n_diags][Lq][N],
+ *      h_gk_baby [baby-1][dnum][2][L][N], h_gk_giant [dnum][2][L][N]; t_plain as dpfhe_rotate_hoisted_grouped (below every
+ *      special prime, 0 = plain rounding).  apply / apply_host / destroy serve both kinds; their buffers are [batch][2][Lq][N].
+ *      Bit-identical to the composition of dpfhe_rotate_hoisted_grouped, dpfhe_ct_mul_plain_inner on the ciphertext moduli,
+ *      dpfhe_rotate_grouped and dpfhe_poly_add; each giant step is one launch (the addition rides on the rotation's store). */
+int dpfhe_linear_create_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_diags, size_t n_diags, size_t baby,
+                                const uint64_t *h_gk_baby, const uint64_t *h_gk_giant, uint64_t t_plain, dpfhe_linear **out);
 void dpfhe_linear_destroy(dpfhe_linear *layer);
 int dpfhe_linear_apply(dpfhe_linear *layer, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream);
 int dpfhe_linear_apply_host(dpfhe_linear *layer, const uint64_t *h_ct, uint64_t *h_out, size_t batch);
