@@ -267,11 +267,12 @@ int dpfhe_context_create(const dpfhe_params *p, int device_id, dpfhe_ctx **out) 
     lc.itw = ctx->d_itw;
     // digit-exchange scratch for the fused key-switch kernel: one slot per resident CTA, two parities
     lc.ks_slots = (size_t)lc.num_sms * 4;
-    // digit slots and accumulator rows: ONE allocation, so that a single L2 access-policy window can cover the whole
-    // cross-phase working set of the fused kernel (launch_ks_t)
-    CTX_TRY(cudaMalloc(&lc.ks_scratch, 2 * lc.ks_slots * 2 * N * 8));
-    lc.ks_acc = lc.ks_scratch + lc.ks_slots * 2 * N;
-    lc.ks_window_bytes = 2 * lc.ks_slots * 2 * N * 8;
+    // digit slots and, at N = 16384, accumulator rows: ONE allocation, so that a single L2 access-policy window can cover the
+    // whole cross-phase working set of the fused kernel (launch_ks_t).  At N <= 8192 the accumulators live in shared memory.
+    const size_t ks_parts = ctx->hp.log_n > 13 ? 2 : 1;
+    CTX_TRY(cudaMalloc(&lc.ks_scratch, ks_parts * lc.ks_slots * 2 * N * 8));
+    lc.ks_acc = ks_parts > 1 ? lc.ks_scratch + lc.ks_slots * 2 * N : nullptr;
+    lc.ks_window_bytes = ks_parts * lc.ks_slots * 2 * N * 8;
     {
         int max_persist = 0, max_window = 0;
         cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, device_id);
@@ -291,7 +292,7 @@ int dpfhe_context_create(const dpfhe_params *p, int device_id, dpfhe_ctx **out) 
     CTX_TRY(cudaMalloc(&lc.ks_ticket, 64));
     CTX_TRY(cudaMalloc(&lc.ks_mail, lc.ks_slots * sizeof(u64)));
     CTX_TRY(cudaMemset(lc.ks_mail, 0, lc.ks_slots * sizeof(u64)));
-    ctx->device_bytes += 2 * lc.ks_slots * 2 * N * 8 + lc.ks_slots * (2 * sizeof(u32) + sizeof(u64)) + 64;
+    ctx->device_bytes += ks_parts * lc.ks_slots * 2 * N * 8 + lc.ks_slots * (2 * sizeof(u32) + sizeof(u64)) + 64;
     if (getenv("DPFHE_KS_PROF")) {   // diagnostics: per-phase cycle counters of the fused kernel
         CTX_TRY(cudaMalloc(&lc.ks_prof, lc.ks_slots * 16 * sizeof(unsigned long long)));
         CTX_TRY(cudaMemset(lc.ks_prof, 0, lc.ks_slots * 16 * sizeof(unsigned long long)));
@@ -1202,10 +1203,11 @@ int dpfhe_debug_phase_cycles(dpfhe_ctx *ctx, uint64_t *out16) {
     for (int k = 0; k < 16; ++k) out16[k] = 0;
     for (size_t s = 0; s < ctx->lc.ks_slots; ++s)
         for (int k = 0; k < 16; ++k) out16[k] += h[s * 16 + k];
-    out16[12] = out16[13] = 0;   // [12] = min, [13] = max CTA lifetime (ns) over the CTAs that ran
+    out16[11] = out16[12] = out16[13] = 0;   // [11] = CTAs that ran (the launched grid); [12] = min, [13] = max CTA lifetime (ns)
     for (size_t s = 0; s < ctx->lc.ks_slots; ++s) {
         const uint64_t ns = h[s * 16 + 14];
         if (!ns) continue;
+        ++out16[11];
         if (ns > out16[13]) out16[13] = ns;
         if (!out16[12] || ns < out16[12]) out16[12] = ns;
     }
@@ -1499,8 +1501,9 @@ int dpfhe_describe(const dpfhe_ctx *ctx, char *buf, size_t buf_len) {
     int n = snprintf(buf, buf_len,
                      "{\"log_n\": %u, \"n_limbs\": %u, \"num_sms\": %d, \"ntt_kernel\": {\"threads\": %u, \"smem_bytes\": %zu, "
                      "\"grid\": \"one CTA per limb\"}, \"ks_fused_kernel\": {\"threads\": %u, \"smem_bytes\": %zu, "
-                     "\"grid\": \"persistent cooperative, multiple of L, <= %zu slots\"}}",
-                     ctx->hp.log_n, ctx->hp.L, ctx->lc.num_sms, nt, ctx->N() * 8, 256u, ctx->hp.log_n <= 13 ? ctx->N() * 8 : ctx->N() * 4, ctx->lc.ks_slots);
+                     "\"grid\": \"persistent cooperative, multiple of %s, <= %zu slots\"}}",
+                     ctx->hp.log_n, ctx->hp.L, ctx->lc.num_sms, nt, ctx->N() * 8, 256u, ctx->hp.log_n <= 13 ? (size_t)3 * 4096 * 8 : ctx->N() * 4,
+                     ctx->hp.log_n == 13 ? "2L (a cluster of two CTAs per limb)" : "L", ctx->lc.ks_slots);
     return n;
 }
 

@@ -580,6 +580,185 @@ DPFHE_HD void ks_phase2_digit(CTA &cta, u64 *buf, const KsArgs &A, const LimbPar
     ks_phase2_core<LOGN, NT, HYB, SPECIAL, 3>(cta, buf, A, p, ct, i, j, jj, A.L, load, acc_rows);
 }
 
+// ---- fused key switch at N <= 8192: one 4096-point block per CTA (DESIGN.md §4.4) -----------------------------------------
+// Work item = (ciphertext ct, limb i, half h).  At N = 8192 the two halves of a limb are a CTA pair (a thread-block cluster of
+// two); at N = 4096 the limb is one block and h = 0.  Shared memory holds the CTA's 4096-point transform buffer buf (32 KiB) and
+// its two lazy accumulator half-rows acc[0, HC) and acc[HC, 2 HC) (64 KiB), so the accumulators never leave the SM.  The output
+// rows are written once, with the final canonical values, by the last digit, so `out` may still be peer memory.
+//   phase 1: ks_blk_phase1_local: digit + own key terms, inverse register passes on the block;
+//            (pair barrier) ks_blk_phase1_outer: the outermost inverse stage over the pair -> t_i, half of the columns per CTA.
+//   phase 2: ks_blk_phase2 for every other digit j: lift of all of t_j and the first forward stage for the CTA's own block,
+//            the three forward passes, multiply-accumulate with the key half-row.
+// Every lazy value is the one ks_phase1 / ks_phase2_digit compute for the same coefficient, so the results are bit-identical.
+constexpr int KS_BLK_LOGN = 12;                  // the block a CTA owns
+constexpr int KS_BLK_HC = 1 << (KS_BLK_LOGN - 1);   // its 16-byte chunks
+template <int LOGN>
+DPFHE_HD constexpr int ks_blk_pair() {   // CTAs per limb
+    return 1 << (LOGN - KS_BLK_LOGN);
+}
+
+// Phase-1 operands and start values of one chunk, as ks_phase1 / ks_p1_chunk compute them (non-hybrid).  They are restated here
+// rather than factored out of those two: ks_phase1 also serves the hybrid, grouped and N = 16384 kernels, which compile to the
+// same SASS as before this body existed only while its code is left as it is.
+template <int MODE>
+DPFHE_HD KsP1Pointers ks_blk_p1_pointers(const KsArgs &A, size_t ct, u32 i, size_t N) {
+    const size_t P = (size_t)A.L * N;
+    const size_t koff_b = ((size_t)i * 2 + 0) * P + (size_t)i * N, koff_a = ((size_t)i * 2 + 1) * P + (size_t)i * N;
+    const size_t in_off = (MODE == KS_PLAIN ? ct * P : ct * 2 * P) + (size_t)i * N;
+    KsP1Pointers ptr;
+    ptr.kb = reinterpret_cast<const U64x2 *>(A.key + koff_b);
+    ptr.ka = reinterpret_cast<const U64x2 *>(A.key + koff_a);
+    ptr.kbs = reinterpret_cast<const U64x2 *>(A.key_s + koff_b);
+    ptr.kas = reinterpret_cast<const U64x2 *>(A.key_s + koff_a);
+    ptr.a0 = reinterpret_cast<const U64x2 *>(A.a + in_off);
+    ptr.a1 = reinterpret_cast<const U64x2 *>(A.a + in_off + P);
+    ptr.b0 = reinterpret_cast<const U64x2 *>((MODE == KS_MUL_RELIN ? A.b : A.a) + in_off);
+    ptr.b1 = reinterpret_cast<const U64x2 *>((MODE == KS_MUL_RELIN ? A.b : A.a) + in_off + P);
+    ptr.c0 = A.a + in_off;
+    ptr.c1 = A.a + in_off + P;
+    return ptr;
+}
+// d: the digit (< SB*q); r0, r1: accumulator start values (< (2 SB + 1) q)
+template <int MODE>
+DPFHE_HD void ks_blk_p1_terms(const KsP1Operands &o, const LimbParams &p, U64x2 &d, U64x2 &r0, U64x2 &r1) {
+    U64x2 s0, s1;   // own contributions to acc0 (< SB*q) / acc1 (< (SB+1) q)
+    if (MODE == KS_MUL_RELIN) {
+        tensor_coeff(o.a0.x, o.a1.x, o.b0.x, o.b1.x, p, s0.x, s1.x, d.x);
+        tensor_coeff(o.a0.y, o.a1.y, o.b0.y, o.b1.y, p, s0.y, s1.y, d.y);
+    } else if (MODE == KS_PLAIN) {
+        d = o.a0;
+        s0.x = s0.y = s1.x = s1.y = 0;
+    } else {
+        d = o.a1;
+        s0 = o.a0;
+        s1.x = s1.y = 0;
+    }
+    r0.x = s0.x + shoup_lazy(d.x, o.kb.x, o.kbs.x, p);
+    r0.y = s0.y + shoup_lazy(d.y, o.kb.y, o.kbs.y, p);
+    r1.x = s1.x + shoup_lazy(d.x, o.ka.x, o.kas.x, p);
+    r1.y = s1.y + shoup_lazy(d.y, o.ka.y, o.kas.y, p);
+}
+
+template <int LOGN, int NT, int MODE, class CTA>
+DPFHE_HD void ks_blk_phase1_local(CTA &cta, u64 *buf, U64x2 *acc, const KsArgs &A, const LimbParams &p, size_t ct, u32 i, int h) {
+    static_assert(LOGN == 12 || LOGN == 13, "one or two 4096-point blocks per limb");
+    constexpr int N = 1 << LOGN, HC = KS_BLK_HC;
+    const size_t P = (size_t)A.L * N;
+    const int c0 = h * HC;   // first chunk of the block in the limb
+    U64x2 *out0 = reinterpret_cast<U64x2 *>(A.out + ct * 2 * P + (size_t)i * N) + c0;
+    U64x2 *out1 = reinterpret_cast<U64x2 *>(A.out + ct * 2 * P + P + (size_t)i * N) + c0;
+    const bool only = A.L == 1;   // a single digit: no phase 2, write the canonical result here
+    const KsP1Pointers ptr = ks_blk_p1_pointers<MODE>(A, ct, i, N);
+    const u32 galois = A.galois;
+    cta.par([&](int tid) {
+        // operands one chunk ahead: the 128-register budget of two CTAs per SM has room for a second operand set
+        KsP1Operands nxt = ks_p1_fetch<LOGN, MODE>(ptr, galois, c0 + tid);
+#pragma unroll 1
+        for (int lc = tid; lc < HC; lc += NT) {
+            const KsP1Operands o = nxt;
+            if (lc + NT < HC) nxt = ks_p1_fetch<LOGN, MODE>(ptr, galois, c0 + lc + NT);
+            U64x2 d, r0, r1;
+            ks_blk_p1_terms<MODE>(o, p, d, r0, r1);
+            reinterpret_cast<U64x2 *>(buf)[swz_chunk(lc)] = d;
+            if (only) {
+                r0.x = canon(r0.x, p); r0.y = canon(r0.y, p);
+                r1.x = canon(r1.x, p); r1.y = canon(r1.y, p);
+                st_stream(out0 + lc, r0);
+                st_stream(out1 + lc, r1);
+            } else {
+                acc[lc] = r0;
+                acc[HC + lc] = r1;
+            }
+        }
+    });
+    cta.mark(0);   // tensor / digit build + own key terms
+    if (only) return;
+    inv_passes_blk<LOGN, NT, 1>(cta, buf, A.itw + (size_t)i * N, p, h);
+    cta.mark(1);   // inverse register passes
+}
+
+// peer: the partner's transform buffer (distributed shared memory at N = 8192; unused at N = 4096; a plain second buffer in the
+// emulator).  CTA h finishes chunk columns [h, h + 1) * HC / pair of both blocks and stores them to t_slot (the limb's digit slot).
+template <int LOGN, int NT, class CTA>
+DPFHE_HD void ks_blk_phase1_outer(CTA &cta, const u64 *buf, const u64 *peer, const KsArgs &A, const LimbParams &p, u32 i, int h, u64 *t_slot) {
+    constexpr int HC = KS_BLK_HC, CW = HC / ks_blk_pair<LOGN>();
+    U64x2 *dst = reinterpret_cast<U64x2 *>(t_slot);
+    cta.par([&](int tid) {
+        inv_outer_stage<LOGN, NT>(
+            A.itw + ((size_t)i << LOGN), p, tid,
+            [&](int c) {
+                const int b = c / HC;
+                return reinterpret_cast<const U64x2 *>(b == h ? buf : peer)[swz_chunk(c - b * HC)];
+            },
+            [&](int c, const U64x2 &v) { st_cg(dst + c, v); }, h * CW, (h + 1) * CW);
+    });
+    cta.mark(2);   // outer inverse stage + digit publish
+}
+
+// t_src: the published t of digit j (N words, natural order, canonical mod q_j)
+template <int LOGN, int NT, class CTA>
+DPFHE_HD void ks_blk_phase2(CTA &cta, u64 *buf, U64x2 *acc, const KsArgs &A, const LimbParams &p, size_t ct, u32 i, u32 j, u32 jj, int h,
+                            const u64 *t_src) {
+    constexpr int N = 1 << LOGN, HC = KS_BLK_HC, BIN = 3;
+    const size_t P = (size_t)A.L * N;
+    const int c0 = h * HC;
+    const Twiddle *tw = A.tw + (size_t)i * N;
+    const U64x2 *src = reinterpret_cast<const U64x2 *>(t_src);
+    // lift of the digit into Z_{q_i}, as ks_phase2_digit
+    const bool lift = A.lift_reduce != 0u;
+    auto get = [&](int c) { return ld_cg(src + c); };
+    cta.par([&](int tid) {
+        if (lift) fwd_load_stage_blk<LOGN, NT, true>(buf, tw, p, tid, get, h);
+        else fwd_load_stage_blk<LOGN, NT, false>(buf, tw, p, tid, get, h);
+    });
+    cta.mark(4);   // digit fetch + lift + outer forward stage
+    fwd_passes_blk<LOGN, NT, BIN, 1>(cta, buf, tw, p, h);
+    cta.mark(5);   // forward register passes
+    const size_t koff_b = ((size_t)j * 2 + 0) * P + (size_t)i * N, koff_a = ((size_t)j * 2 + 1) * P + (size_t)i * N;
+    const U64x2 *kb = reinterpret_cast<const U64x2 *>(A.key + koff_b) + c0, *ka = reinterpret_cast<const U64x2 *>(A.key + koff_a) + c0;
+    const U64x2 *kbs = reinterpret_cast<const U64x2 *>(A.key_s + koff_b) + c0, *kas = reinterpret_cast<const U64x2 *>(A.key_s + koff_a) + c0;
+    U64x2 *out0 = reinterpret_cast<U64x2 *>(A.out + ct * 2 * P + (size_t)i * N) + c0;
+    U64x2 *out1 = reinterpret_cast<U64x2 *>(A.out + ct * 2 * P + P + (size_t)i * N) + c0;
+    // lazy accumulator bound and trims as ks_phase2_core: below (2 SB + 1) q after phase 1, + SB*q per digit
+    constexpr int B0 = 2 * SB + 1;
+    const bool last = jj + 1 == A.L;
+    const bool trim = !last && acc_trim_after(B0, (int)jj - 1);
+    cta.par([&](int tid) {
+        U64x2 vb = ld_keep(kb + tid), va = ld_keep(ka + tid), vbs = ld_keep(kbs + tid), vas = ld_keep(kas + tid);
+#pragma unroll 1
+        for (int lc = tid; lc < HC; lc += NT) {
+            const U64x2 b = vb, a = va, bs = vbs, as = vas;
+            if (lc + NT < HC) {   // the next chunk's key loads fly during this chunk's math
+                vb = ld_keep(kb + lc + NT);
+                va = ld_keep(ka + lc + NT);
+                vbs = ld_keep(kbs + lc + NT);
+                vas = ld_keep(kas + lc + NT);
+            }
+            // u < 16q straight from the transform: Shoup multiplication accepts any 64-bit operand
+            const U64x2 u = reinterpret_cast<const U64x2 *>(buf)[swz_chunk(lc)];
+            U64x2 r0 = acc[lc], r1 = acc[HC + lc];
+            r0.x += shoup_lazy(u.x, b.x, bs.x, p);
+            r0.y += shoup_lazy(u.y, b.y, bs.y, p);
+            r1.x += shoup_lazy(u.x, a.x, as.x, p);
+            r1.y += shoup_lazy(u.y, a.y, as.y, p);
+            if (trim) {
+                r0.x = csub(r0.x, p.q8); r0.y = csub(r0.y, p.q8);
+                r1.x = csub(r1.x, p.q8); r1.y = csub(r1.y, p.q8);
+            }
+            if (last) {
+                r0.x = canon(r0.x, p); r0.y = canon(r0.y, p);
+                r1.x = canon(r1.x, p); r1.y = canon(r1.y, p);
+                st_stream(out0 + lc, r0);
+                st_stream(out1 + lc, r1);
+            } else {
+                acc[lc] = r0;
+                acc[HC + lc] = r1;
+            }
+        }
+    });
+    cta.mark(6);   // multiply-accumulate with the key half-row (the last digit also canonicalises and stores)
+}
+
 // a digit of several limbs (grouped hybrid key switching, DESIGN.md §2.11): the lift of group g into limb i is the fast basis
 // conversion sum_{j in g} y_j * (Qhat_j mod q_i), y_j = the scaled inverse transforms the members published.
 // t_rows + j * t_stride: the published row of limb j.

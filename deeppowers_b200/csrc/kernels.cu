@@ -320,20 +320,24 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void *p, u32 bytes) {
 }
 
 #if DPFHE_PART_MAIN
-// grid = G CTAs, G a multiple of L, all co-resident (cooperative launch).  The L CTAs of slots
-// [g*L, (g+1)*L) form a group that processes one ciphertext at a time: CTA `slot` owns output limb
-// i = slot % L.  The group leader (i == 0) draws the next ciphertext index from a global ticket counter
-// and posts it in the group's mailbox (dynamic balancing: groups that run ahead take more work);
-// the members exchange their INTT'd digits through `scratch` (double-buffered by round parity,
-// L2 resident) under release/acquire flags.
+// grid = G CTAs, G a multiple of the group size, all co-resident (cooperative launch).  A group processes one ciphertext at a
+// time; its leader draws the next ciphertext index from a global ticket counter and posts it in the group's mailbox (dynamic
+// balancing: groups that run ahead take more work); the members exchange their INTT'd digits through `scratch`
+// (double-buffered by round parity, L2 resident) under release/acquire flags.
 // FILTER (hoisted-rotation fallback): only the ciphertexts flagged in A.only are processed; the digit slots then
 // alternate over the rounds that actually run.
-template <int LOGN, int NT, int MINB, int MODE, bool PROF, bool FILTER = false>
-__global__ void __launch_bounds__(NT, MINB) ks_fused_kernel(KsArgs A, const __grid_constant__ LimbTable lt, size_t batch, u32 *flags, u32 epoch,
-                                                            u32 *ticket, u64 *mail, unsigned long long *prof, u32 pf_dist, u32 *consumed) {
+//   N <= 8192 (ks_fused_blk): one 4096-point block per CTA, accumulators in shared memory; a group is L pairs (N = 8192, each
+//             pair a cluster of two CTAs) or L CTAs (N = 4096); pair `slot` owns limb i = slot % L and digit slot `slot`.
+//   N = 16384 (else branch of ks_fused_kernel): one limb per CTA in two halves, accumulators in L2-resident scratch rows; a group is L CTAs.
+
+template <int LOGN, int NT, int MODE, bool PROF, bool FILTER>
+__device__ __forceinline__ void ks_fused_blk(const KsArgs &A, const LimbTable &lt, size_t batch, u32 *flags, u32 epoch, u32 *ticket, u64 *mail,
+                                             unsigned long long *prof, u32 pf_dist) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     constexpr size_t N = (size_t)1 << LOGN;
+    constexpr u32 PAIR = (u32)ks_blk_pair<LOGN>();
     u64 *buf = reinterpret_cast<u64 *>(smem_raw);
+    U64x2 *acc = reinterpret_cast<U64x2 *>(smem_raw + ((size_t)8 << KS_BLK_LOGN));
     DevCta<NT, PROF> cta;
     unsigned long long t_start = 0, c_start = 0;
     if (PROF) {
@@ -342,25 +346,23 @@ __global__ void __launch_bounds__(NT, MINB) ks_fused_kernel(KsArgs A, const __gr
         c_start = (unsigned long long)cta.last;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_start));
     }
+    namespace cg = cooperative_groups;
     __shared__ u32 s_ct;
-    const u32 L = A.L, slot = blockIdx.x, i = slot % L, group = slot / L;
+    const u32 L = A.L, h = blockIdx.x % PAIR, slot = blockIdx.x / PAIR, i = slot % L, group = slot / L;
+    const u64 *peer = buf;
+    if constexpr (PAIR == 2) peer = cg::this_cluster().map_shared_rank(buf, (int)h ^ 1);
+    auto pair_sync = [&]() {
+        if constexpr (PAIR == 2) cg::this_cluster().sync();
+        else __syncthreads();
+    };
     const LimbParams &p = lt.lp[i];
     u32 executed = 0;
-    // Single-buffered digit slots (consumed != nullptr): slot s holds ONE digit; its owner may overwrite it only after the L-1
-    // siblings that read the previous digit have signalled.  The counters are monotone across launches: the value found at
-    // kernel start is the base (no reader of an earlier launch is still running).  One slot per CTA instead of two keeps
-    // 26 MB (N = 8192, 396 CTAs: 3 on each of 132 SMs) of the kernel's cross-phase working set out of the L2.
-    __shared__ u32 s_base;
-    if (consumed && threadIdx.x == 0) s_base = ld_acquire_u32(consumed + slot);
-    __syncthreads();
-    const u32 consumed_base = consumed ? s_base : 0u;
-    u32 published = 0;   // digits this CTA has published in this launch
     for (u32 round = 0;; ++round) {
         if (!FILTER && threadIdx.x == 0) {
             const u32 tag = epoch + round + 1;
-            if (i == 0) {
+            if (i == 0 && h == 0) {
                 const u32 t = atomicAdd(ticket, 1u);
-                if (L > 1) st_release_u64(mail + group, ((u64)tag << 32) | t);
+                if (L * PAIR > 1) st_release_u64(mail + group, ((u64)tag << 32) | t);
                 s_ct = t;
             } else {
                 u64 m;
@@ -370,38 +372,35 @@ __global__ void __launch_bounds__(NT, MINB) ks_fused_kernel(KsArgs A, const __gr
             }
         }
         __syncthreads();
-        // FILTER: static assignment computed by every thread.  Skipped rounds involve no exchange between the members of
-        // a group, so a leader handing out tickets could run ahead and overwrite a mailbox tag (or s_ct) before it was read.
-        const size_t ct = FILTER ? (size_t)round * (gridDim.x / L) + group : (size_t)s_ct;
+        // FILTER: static assignment computed by every thread (see the N = 16384 branch below)
+        const size_t ct = FILTER ? (size_t)round * (gridDim.x / (L * PAIR)) + group : (size_t)s_ct;
         if (ct >= batch) break;   // every member of the group reads the same ticket, so they leave together
         if (FILTER && A.only[ct] == 0u) continue;
-        // Tickets are drawn in order, so ciphertext ct + pf_dist will be started by some group a few microseconds
-        // from now: pull this CTA's limb of its inputs from HBM into L2 with the TMA unit's bulk prefetch, so the
-        // tensor phase that consumes them is L2- rather than HBM-latency bound.
+        // bulk prefetch of this CTA's block of the inputs of ciphertext ct + pf_dist (see the N = 16384 branch below)
         if (pf_dist && threadIdx.x == 0 && ct + pf_dist < batch) {
-            const size_t nc = ct + pf_dist, P = (size_t)L * N;
-            constexpr u32 LB = (u32)(N * 8);
+            const size_t nc = ct + pf_dist, P = (size_t)L * N, off = (size_t)i * N + ((size_t)h << KS_BLK_LOGN);
+            constexpr u32 BB = 8u << KS_BLK_LOGN;
             if (MODE == KS_PLAIN) {
-                bulk_prefetch_l2(A.a + nc * P + (size_t)i * N, LB);
+                bulk_prefetch_l2(A.a + nc * P + off, BB);
             } else {
-                bulk_prefetch_l2(A.a + nc * 2 * P + (size_t)i * N, LB);
-                bulk_prefetch_l2(A.a + nc * 2 * P + P + (size_t)i * N, LB);
+                bulk_prefetch_l2(A.a + nc * 2 * P + off, BB);
+                bulk_prefetch_l2(A.a + nc * 2 * P + P + off, BB);
                 if (MODE == KS_MUL_RELIN) {
-                    bulk_prefetch_l2(A.b + nc * 2 * P + (size_t)i * N, LB);
-                    bulk_prefetch_l2(A.b + nc * 2 * P + P + (size_t)i * N, LB);
+                    bulk_prefetch_l2(A.b + nc * 2 * P + off, BB);
+                    bulk_prefetch_l2(A.b + nc * 2 * P + P + off, BB);
                 }
             }
         }
-        const u32 parity = consumed ? 0u : (FILTER ? executed++ : round) & 1u;
-        const size_t slot_stride = consumed ? 1 : 2;      // digit slots per CTA
-        u64 *acc_rows = A.acc + (size_t)slot * 2 * N;   // this CTA's two lazy accumulator rows (L2 resident, reused every round)
-        ks_phase1<LOGN, NT, MODE>(cta, buf, A, p, ct, i, A.scratch + ((size_t)slot * slot_stride + parity) * N, acc_rows, 0, 0,
-                                  consumed && L > 1 ? consumed + slot : nullptr, consumed_base + published * (L - 1));
-        ++published;
+        const u32 parity = (FILTER ? executed++ : round) & 1u;
+        ks_blk_phase1_local<LOGN, NT, MODE>(cta, buf, acc, A, p, ct, i, (int)h);
+        // the partner's block has been through the inverse passes, and the partner has read this round's mailbox (with L = 1 this
+        // barrier is what keeps a leader from posting the next ticket before its partner has read the current one)
+        pair_sync();
         if (L > 1) {
+            ks_blk_phase1_outer<LOGN, NT>(cta, buf, peer, A, p, i, (int)h, A.scratch + ((size_t)slot * 2 + parity) * N);
             __threadfence();
-            __syncthreads();
-            if (threadIdx.x == 0) st_release_u32(flags + slot, epoch + round + 1);
+            pair_sync();   // both halves of t_i are stored, and the partner has finished reading this CTA's buffer
+            if (h == 0 && threadIdx.x == 0) st_release_u32(flags + slot, epoch + round + 1);
             for (u32 jj = 1; jj < L; ++jj) {
                 const u32 j = (i + jj) % L, sib = slot - i + j;
                 if (threadIdx.x == 0) {
@@ -410,12 +409,7 @@ __global__ void __launch_bounds__(NT, MINB) ks_fused_kernel(KsArgs A, const __gr
                 }
                 __syncthreads();
                 cta.mark(3);   // waiting for the sibling's digit
-                ks_phase2_digit<LOGN, NT>(cta, buf, A, p, ct, i, j, jj, A.scratch + ((size_t)sib * slot_stride + parity) * N, acc_rows);
-                // every thread is past its last read of the sibling's digit (the body ends with a CTA barrier): hand the slot back
-                if (consumed && threadIdx.x == 0) {
-                    __threadfence();
-                    atomicAdd(consumed + sib, 1u);
-                }
+                ks_blk_phase2<LOGN, NT>(cta, buf, acc, A, p, ct, i, j, jj, (int)h, A.scratch + ((size_t)sib * 2 + parity) * N);
             }
         }
     }
@@ -424,6 +418,111 @@ __global__ void __launch_bounds__(NT, MINB) ks_fused_kernel(KsArgs A, const __gr
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_end));
         cta.prof[14] += t_end - t_start;
         cta.prof[15] += (unsigned long long)clock64() - c_start;
+    }
+}
+
+template <int LOGN, int NT, int MINB, int MODE, bool PROF, bool FILTER = false>
+__global__ void __launch_bounds__(NT, MINB) ks_fused_kernel(KsArgs A, const __grid_constant__ LimbTable lt, size_t batch, u32 *flags, u32 epoch,
+                                                            u32 *ticket, u64 *mail, unsigned long long *prof, u32 pf_dist, u32 *consumed) {
+    if constexpr (LOGN <= 13) {
+        ks_fused_blk<LOGN, NT, MODE, PROF, FILTER>(A, lt, batch, flags, epoch, ticket, mail, prof, pf_dist);
+    } else {
+        // the L CTAs of slots [g*L, (g+1)*L) form group g: CTA `slot` owns output limb i = slot % L; the leader is i == 0
+        extern __shared__ __align__(1024) unsigned char smem_raw[];
+        constexpr size_t N = (size_t)1 << LOGN;
+        u64 *buf = reinterpret_cast<u64 *>(smem_raw);
+        DevCta<NT, PROF> cta;
+        unsigned long long t_start = 0, c_start = 0;
+        if (PROF) {
+            cta.prof = prof + (size_t)blockIdx.x * 16;
+            cta.last = clock64();
+            c_start = (unsigned long long)cta.last;
+            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_start));
+        }
+        __shared__ u32 s_ct;
+        const u32 L = A.L, slot = blockIdx.x, i = slot % L, group = slot / L;
+        const LimbParams &p = lt.lp[i];
+        u32 executed = 0;
+        // Single-buffered digit slots (consumed != nullptr): slot s holds ONE digit; its owner may overwrite it only after the L-1
+        // siblings that read the previous digit have signalled.  The counters are monotone across launches: the value found at
+        // kernel start is the base (no reader of an earlier launch is still running).  One slot per CTA instead of two keeps
+        // half of the digit slots out of the kernel's cross-phase working set in the L2.
+        __shared__ u32 s_base;
+        if (consumed && threadIdx.x == 0) s_base = ld_acquire_u32(consumed + slot);
+        __syncthreads();
+        const u32 consumed_base = consumed ? s_base : 0u;
+        u32 published = 0;   // digits this CTA has published in this launch
+        for (u32 round = 0;; ++round) {
+            if (!FILTER && threadIdx.x == 0) {
+                const u32 tag = epoch + round + 1;
+                if (i == 0) {
+                    const u32 t = atomicAdd(ticket, 1u);
+                    if (L > 1) st_release_u64(mail + group, ((u64)tag << 32) | t);
+                    s_ct = t;
+                } else {
+                    u64 m;
+                    do m = ld_acquire_u64(mail + group);
+                    while ((u32)(m >> 32) != tag);
+                    s_ct = (u32)m;
+                }
+            }
+            __syncthreads();
+            // FILTER: static assignment computed by every thread.  Skipped rounds involve no exchange between the members of
+            // a group, so a leader handing out tickets could run ahead and overwrite a mailbox tag (or s_ct) before it was read.
+            const size_t ct = FILTER ? (size_t)round * (gridDim.x / L) + group : (size_t)s_ct;
+            if (ct >= batch) break;   // every member of the group reads the same ticket, so they leave together
+            if (FILTER && A.only[ct] == 0u) continue;
+            // Tickets are drawn in order, so ciphertext ct + pf_dist will be started by some group a few microseconds
+            // from now: pull this CTA's limb of its inputs from HBM into L2 with the TMA unit's bulk prefetch, so the
+            // tensor phase that consumes them is L2- rather than HBM-latency bound.
+            if (pf_dist && threadIdx.x == 0 && ct + pf_dist < batch) {
+                const size_t nc = ct + pf_dist, P = (size_t)L * N;
+                constexpr u32 LB = (u32)(N * 8);
+                if (MODE == KS_PLAIN) {
+                    bulk_prefetch_l2(A.a + nc * P + (size_t)i * N, LB);
+                } else {
+                    bulk_prefetch_l2(A.a + nc * 2 * P + (size_t)i * N, LB);
+                    bulk_prefetch_l2(A.a + nc * 2 * P + P + (size_t)i * N, LB);
+                    if (MODE == KS_MUL_RELIN) {
+                        bulk_prefetch_l2(A.b + nc * 2 * P + (size_t)i * N, LB);
+                        bulk_prefetch_l2(A.b + nc * 2 * P + P + (size_t)i * N, LB);
+                    }
+                }
+            }
+            const u32 parity = consumed ? 0u : (FILTER ? executed++ : round) & 1u;
+            const size_t slot_stride = consumed ? 1 : 2;      // digit slots per CTA
+            u64 *acc_rows = A.acc + (size_t)slot * 2 * N;   // this CTA's two lazy accumulator rows (L2 resident, reused every round)
+            ks_phase1<LOGN, NT, MODE>(cta, buf, A, p, ct, i, A.scratch + ((size_t)slot * slot_stride + parity) * N, acc_rows, 0, 0,
+                                      consumed && L > 1 ? consumed + slot : nullptr, consumed_base + published * (L - 1));
+            ++published;
+            if (L > 1) {
+                __threadfence();
+                __syncthreads();
+                if (threadIdx.x == 0) st_release_u32(flags + slot, epoch + round + 1);
+                for (u32 jj = 1; jj < L; ++jj) {
+                    const u32 j = (i + jj) % L, sib = slot - i + j;
+                    if (threadIdx.x == 0) {
+                        while ((int)(ld_acquire_u32(flags + sib) - (epoch + round + 1)) < 0) {
+                        }
+                    }
+                    __syncthreads();
+                    cta.mark(3);   // waiting for the sibling's digit
+                    ks_phase2_digit<LOGN, NT>(cta, buf, A, p, ct, i, j, jj, A.scratch + ((size_t)sib * slot_stride + parity) * N, acc_rows);
+                    // every thread is past its last read of the sibling's digit (the body ends with a CTA barrier): hand the slot back
+                    if (consumed && threadIdx.x == 0) {
+                        __threadfence();
+                        atomicAdd(consumed + sib, 1u);
+                    }
+                }
+            }
+        }
+        if (PROF && threadIdx.x == 0) {   // CTA lifetime in nanoseconds (globaltimer) and in SM cycles
+            unsigned long long t_end;
+            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_end));
+            cta.prof[14] += t_end - t_start;
+            cta.prof[15] += (unsigned long long)clock64() - c_start;
+        }
+
     }
 }
 
@@ -1205,8 +1304,10 @@ static cudaError_t epoch_guard(LaunchCtx &lc, size_t batch, cudaStream_t st) {
 #if DPFHE_PART_MAIN
 template <int LOGN, int MODE>
 static cudaError_t launch_ks_t(LaunchCtx &lc, const KsArgs &A, size_t batch, cudaStream_t st) {
-    // at most 64 KiB of shared memory per CTA (N = 16384 is processed as two half-limbs) -> three CTAs per SM
-    constexpr int NT = 256, MINB = 3;
+    // N <= 8192: a 4096-point block and two accumulator half-rows, 96 KiB of shared memory -> two CTAs per SM, CTA pairs of a
+    // cluster at N = 8192.  N = 16384: 64 KiB (two half-limbs in turn) -> three CTAs per SM.
+    constexpr bool BLK = LOGN <= 13;
+    constexpr int NT = 256, MINB = BLK ? 2 : 3, PAIR = BLK ? ks_blk_pair<LOGN>() : 1;
     const bool filter = A.only != nullptr;
     if (filter && MODE != KS_ROTATE) return cudaErrorInvalidValue;
     auto kern = ks_fused_kernel<LOGN, NT, MINB, MODE, false>;
@@ -1214,7 +1315,7 @@ static cudaError_t launch_ks_t(LaunchCtx &lc, const KsArgs &A, size_t batch, cud
         if (lc.ks_prof) kern = ks_fused_kernel<LOGN, NT, MINB, MODE, true>;
     }
     if (filter) kern = ks_fused_kernel<LOGN, NT, MINB, MODE == KS_ROTATE ? MODE : KS_ROTATE, false, MODE == KS_ROTATE>;
-    const size_t smem = LOGN <= 13 ? Geometry<LOGN>::LIMB_BYTES : Geometry<13>::LIMB_BYTES;
+    const size_t smem = BLK ? 3 * Geometry<KS_BLK_LOGN>::LIMB_BYTES : Geometry<13>::LIMB_BYTES;
     static ConfiguredMask configured[3];
     const int variant = filter ? 2 : (lc.ks_prof && MODE == KS_MUL_RELIN ? 1 : 0);
     if (!configured[variant].has(lc.device)) {
@@ -1222,16 +1323,40 @@ static cudaError_t launch_ks_t(LaunchCtx &lc, const KsArgs &A, size_t batch, cud
         if (e != cudaSuccess) return e;
         configured[variant].set(lc.device);
     }
-    int occ = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, NT, smem);
-    if (e != cudaSuccess) return e;
-    if (occ < 1) return cudaErrorLaunchOutOfResources;
-    if (lc.ks_occ_cap > 0 && occ > lc.ks_occ_cap) occ = lc.ks_occ_cap;
-    size_t G = (size_t)lc.num_sms * occ;
+    cudaLaunchConfig_t cfg = {};
+    cfg.blockDim = dim3(NT);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[3];
+    attr[0].id = cudaLaunchAttributeCooperative;   // the spin-waits need every CTA of the grid resident
+    attr[0].val.cooperative = 1;
+    attr[1].id = cudaLaunchAttributeClusterDimension;
+    attr[1].val.clusterDim.x = PAIR;
+    attr[1].val.clusterDim.y = 1;
+    attr[1].val.clusterDim.z = 1;
+    int n_attr = PAIR > 1 ? 2 : 1;
+    size_t G = 0;   // resident CTAs
+    cudaError_t e;
+    if (PAIR > 1) {
+        cfg.gridDim = dim3(PAIR);
+        cfg.attrs = attr + 1;
+        cfg.numAttrs = 1;
+        int clusters = 0;
+        e = cudaOccupancyMaxActiveClusters(&clusters, (const void *)kern, &cfg);
+        if (e != cudaSuccess) return e;
+        G = (size_t)clusters * PAIR;
+    } else {
+        int occ = 0;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, NT, smem);
+        if (e != cudaSuccess) return e;
+        G = (size_t)lc.num_sms * occ;
+    }
+    if (G == 0) return cudaErrorLaunchOutOfResources;
+    if (lc.ks_occ_cap > 0 && G > (size_t)lc.num_sms * lc.ks_occ_cap) G = (size_t)lc.num_sms * lc.ks_occ_cap;
     if (G > lc.ks_slots) G = lc.ks_slots;
-    G = (G / lc.L) * lc.L;
-    const size_t n_work = batch * lc.L;
-    if (G > n_work) G = n_work;
+    const size_t GS = (size_t)lc.L * PAIR;   // CTAs of a group
+    G = (G / GS) * GS;
+    if (G > batch * GS) G = batch * GS;
     if (G == 0) return cudaErrorInvalidConfiguration;
     // flag / mailbox tags this launch may consume: one per round, and a group runs at most batch + 1 rounds
     const u32 rounds = (u32)(batch + 1);
@@ -1248,32 +1373,26 @@ static cudaError_t launch_ks_t(LaunchCtx &lc, const KsArgs &A, size_t batch, cud
     u32 *ticket = lc.ks_ticket;
     u64 *mail = lc.ks_mail;
     u32 pf_dist = (u32)lc.ks_prefetch;
-    u32 *consumed = lc.ks_single ? lc.ks_consumed : nullptr;
+    u32 *consumed = !BLK && lc.ks_single ? lc.ks_consumed : nullptr;   // single-buffered digit slots: N = 16384 only
     void *params[] = {&args, &lt, &batch_arg, &flags, &epoch, &ticket, &mail, &prof, &pf_dist, &consumed};
     if (lc.l2_persist && lc.l2_persist_max && lc.ks_window_bytes) {
-        // tuning (DPFHE_L2_PERSIST): the digit slots and accumulator rows are re-read within microseconds, the ciphertext
-        // streams never; a persisting access-policy window over the scratch keeps the streams from evicting it
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)G);
-        cfg.blockDim = dim3(NT);
-        cfg.dynamicSmemBytes = smem;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[2];
-        attr[0].id = cudaLaunchAttributeCooperative;
-        attr[0].val.cooperative = 1;
-        attr[1].id = cudaLaunchAttributeAccessPolicyWindow;
-        attr[1].val.accessPolicyWindow.base_ptr = lc.ks_scratch;
-        attr[1].val.accessPolicyWindow.num_bytes = lc.ks_window_bytes;
+        // tuning (DPFHE_L2_PERSIST): the digit slots (and at N = 16384 the accumulator rows) are re-read within microseconds,
+        // the ciphertext streams never; a persisting access-policy window over the scratch keeps the streams from evicting it
+        attr[n_attr].id = cudaLaunchAttributeAccessPolicyWindow;
+        attr[n_attr].val.accessPolicyWindow.base_ptr = lc.ks_scratch;
+        attr[n_attr].val.accessPolicyWindow.num_bytes = lc.ks_window_bytes;
         const double ratio = (double)lc.l2_persist_max / (double)lc.ks_window_bytes;
-        attr[1].val.accessPolicyWindow.hitRatio = (float)(ratio > 1.0 ? 1.0 : ratio);
-        attr[1].val.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-        attr[1].val.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-        cfg.attrs = attr;
-        cfg.numAttrs = 2;
-        e = cudaLaunchKernelExC(&cfg, (const void *)kern, params);
-    } else {
-        e = cudaLaunchCooperativeKernel((void *)kern, dim3((unsigned)G), dim3(NT), params, smem, st);
+        attr[n_attr].val.accessPolicyWindow.hitRatio = (float)(ratio > 1.0 ? 1.0 : ratio);
+        attr[n_attr].val.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
+        attr[n_attr].val.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
+        ++n_attr;
     }
+    // Cooperative and, at N = 8192, a cluster dimension of two.  Never launched without the co-residency guarantee: if the
+    // runtime refuses the combination, the call returns its error.
+    cfg.gridDim = dim3((unsigned)G);
+    cfg.attrs = attr;
+    cfg.numAttrs = (unsigned)n_attr;
+    e = cudaLaunchKernelExC(&cfg, (const void *)kern, params);
     lc.ks_epoch += rounds;
     return e;
 }

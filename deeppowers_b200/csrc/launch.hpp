@@ -23,8 +23,8 @@ struct LaunchCtx {
     const Twiddle *itw = nullptr;     // [L][N] inverse twiddles
     // fused key-switch pipeline
     u64 *ks_scratch = nullptr;        // [ks_slots][2][N] digit exchange buffers
-    u64 *ks_acc = nullptr;            // [ks_slots][2][N] lazy accumulator rows of the resident work items (second half of ks_scratch's allocation)
-    size_t ks_window_bytes = 0;       // bytes of ks_scratch + ks_acc an L2 access-policy window may cover
+    u64 *ks_acc = nullptr;            // N = 16384 only: [ks_slots][2][N] lazy accumulator rows of the resident work items (second half of ks_scratch's allocation)
+    size_t ks_window_bytes = 0;       // bytes of ks_scratch (+ ks_acc) an L2 access-policy window may cover
     size_t l2_persist_max = 0;        // cudaDevAttrMaxPersistingL2CacheSize
     int l2_persist = 0;               // DPFHE_L2_PERSIST: 1 = mark the fused kernel's scratch as persisting in L2
     u64 *ks_acc_hyb = nullptr;        // hybrid key switching: [ks_slots][2 parities][2][N], allocated at the first hybrid call

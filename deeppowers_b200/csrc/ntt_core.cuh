@@ -344,6 +344,38 @@ DPFHE_HD void fwd_load_stage_half(u64 *buf, const Twiddle *__restrict__ tw, cons
     }
 }
 
+// Block variant of fwd_load_stage (fused key switch at N <= 8192, one 4096-point block per CTA): at N = 8192 (K = 1) it reads
+// both input blocks and keeps output block h of the outer radix-2 step (the same products as the whole stage); at N = 4096 the
+// block is the limb.
+template <int LOGN, int NT, bool IN_REDUCE, class SRC>
+DPFHE_HD void fwd_load_stage_blk(u64 *buf, const Twiddle *__restrict__ tw, const LimbParams &p, int tid, SRC src, int h) {
+    if constexpr (LOGN == 12) {
+        fwd_load_stage<LOGN, NT, IN_REDUCE>(buf, tw, p, tid, src);
+    } else {
+        static_assert(LOGN == 13, "the block load stage is written for K <= 1");
+        constexpr int CPB = 1 << (LOGN - 2);   // chunks per block
+        const Twiddle w = tw[tw_pos<LOGN>(0, 0)];
+        U64x2 nx = src(tid), ny = src(CPB + tid);   // loads of the next iteration are issued before this iteration's butterflies
+#pragma unroll 1
+        for (int c = tid; c < CPB; c += NT) {
+            const U64x2 vx = nx, vy = ny;
+            if (c + NT < CPB) {
+                nx = src(c + NT);
+                ny = src(CPB + c + NT);
+            }
+            U64x2 o;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const u64 x = IN_REDUCE ? word_reduce(e ? vx.y : vx.x, p) : (e ? vx.y : vx.x);
+                const u64 y = IN_REDUCE ? word_reduce(e ? vy.y : vy.x, p) : (e ? vy.y : vy.x);
+                const u64 t = shoup_lazy(y, w.x, w.y, p);
+                (e ? o.y : o.x) = h == 0 ? x + t : x + p.qsb - t;
+            }
+            reinterpret_cast<U64x2 *>(buf)[swz_chunk(c)] = o;
+        }
+    }
+}
+
 // ---- whole-limb drivers --------------------------------------------------------------
 // The CTA policy provides three barrier scopes (all of them "run f(tid) for every thread, then sync"):
 //   cta.par(f)       whole CTA                     (__syncthreads)

@@ -31,5 +31,8 @@ for _ in range(reps):
 e1.record(); torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / reps
 cyc = c.phase_cycles()
+grid = int(cyc[11])   # CTAs of the launched grid (the same in every launch of this shape)
 smi = subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm,power.draw,clocks_event_reasons.sw_power_cap", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-print(json.dumps({"cta_ns_min_max": [float(cyc[12]) / reps, float(cyc[13]) / reps], "cta_ns_avg": float(cyc[14]) / reps / 444, "cta_cycles_avg": float(cyc[15]) / reps / 444, "eff_mhz": float(cyc[15]) / float(cyc[14]) * 1e3, "ms_per_launch": ms, "ct_per_s": B / ms * 1e3, "sum_cta_cycles_per_launch": float(cyc[:8].sum()) / reps, "smi_after": smi}))
+print(json.dumps({"grid_ctas": grid, "cta_ns_min_max": [float(cyc[12]) / reps, float(cyc[13]) / reps], "cta_ns_avg": float(cyc[14]) / reps / grid,
+                  "cta_cycles_avg": float(cyc[15]) / reps / grid, "eff_mhz": float(cyc[15]) / float(cyc[14]) * 1e3, "ms_per_launch": ms,
+                  "ct_per_s": B / ms * 1e3, "sum_cta_cycles_per_launch": float(cyc[:8].sum()) / reps, "smi_after": smi}))
