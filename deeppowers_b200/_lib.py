@@ -53,6 +53,10 @@ SYMBOLS = {
     "dpfhe_ckks_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_double, C.c_void_p]),
     "dpfhe_ckks_encode_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_double]),
     "dpfhe_ckks_decode_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_double]),
+    "dpfhe_bgv_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p]),
+    "dpfhe_bgv_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p]),
+    "dpfhe_bgv_encode_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64]),
+    "dpfhe_bgv_decode_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64]),
     "dpfhe_fill_uniform": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_size_t, C.c_void_p]),
     "dpfhe_ntt_fwd_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "dpfhe_ntt_inv_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),

@@ -327,7 +327,8 @@ void dpfhe_context_destroy(dpfhe_ctx *ctx) {
     cudaFree(ctx->hoist_zero);
     cudaFree(ctx->hoistg_buf);
     cudaFree(ctx->ckks_tab);
-    cudaFree(ctx->ckks_work);
+    cudaFree(ctx->bgv_tab);
+    cudaFree(ctx->enc_work);
     cudaFree(ctx->lc.ks_hyb);
     for (int k = 0; k < PIPE_DEPTH; ++k) {
         cudaFree(ctx->stage_in[k]);
@@ -368,7 +369,7 @@ size_t dpfhe_context_device_bytes(const dpfhe_ctx *ctx) {
     n += ctx->hoist_chunk * (L * P8 + sizeof(u32));                                  // hoisted rotations: shared transforms + zero flags
     if (ctx->hoist_M) n += 3 * P8 + L * L * 8;                                       //   per-rotation constants
     n += ctx->hoistg_bytes;                                                          //   grouped hybrid keys: lifted digits + accumulators
-    n += ctx->ckks_tab_bytes + ctx->ckks_work_bytes;                                 // CKKS encoding tables and scratch
+    n += ctx->ckks_tab_bytes + ctx->bgv_tab_bytes + ctx->enc_work_bytes;             // CKKS and BGV encoding tables, their scratch
     if (ctx->lc.ks_prof) n += ctx->lc.ks_slots * 16 * sizeof(unsigned long long);
     return n;
 }
@@ -383,9 +384,10 @@ int dpfhe_context_trim(dpfhe_ctx *ctx) {
     ctx->hoist_U = nullptr; ctx->hoist_zero = nullptr; ctx->hoist_chunk = 0;
     cudaFree(ctx->hoistg_buf);
     ctx->hoistg_buf = nullptr; ctx->hoistg_bytes = 0;
-    cudaFree(ctx->ckks_tab); cudaFree(ctx->ckks_work);
+    cudaFree(ctx->ckks_tab); cudaFree(ctx->bgv_tab); cudaFree(ctx->enc_work);
     ctx->ckks_tab = nullptr; ctx->ckks_tab_bytes = 0; ctx->ckks = CkksTables();
-    ctx->ckks_work = nullptr; ctx->ckks_work_bytes = 0;
+    ctx->bgv_tab = nullptr; ctx->bgv_tab_bytes = 0; ctx->bgv_t = 0; ctx->bgv = BgvTables();
+    ctx->enc_work = nullptr; ctx->enc_work_bytes = 0;
     ctx->ms_tau = nullptr; ctx->ms_tau_bytes = 0;
     ctx->stage_key = nullptr; ctx->stage_key_bytes = 0;
     for (int k = 0; k < PIPE_DEPTH; ++k) {
@@ -1008,6 +1010,19 @@ int dpfhe_ct_mul_plain_host(dpfhe_ctx *ctx, const uint64_t *h_ct, const uint64_t
 
 // ---------------------------------------------------------------- CKKS slot encoding (DESIGN.md §2.12)
 
+// `need` bytes of the slot encoders' scratch
+static int enc_work_prepare(dpfhe_ctx *ctx, size_t need, cudaStream_t st) {
+    if (need > ctx->enc_work_bytes) {
+        CU_TRY(cudaStreamSynchronize(st));   // the old scratch may still be in use on this stream
+        if (ctx->enc_work) cudaFree(ctx->enc_work);
+        ctx->enc_work = nullptr;
+        ctx->enc_work_bytes = 0;
+        CU_TRY(cudaMalloc(&ctx->enc_work, need));
+        ctx->enc_work_bytes = need;
+    }
+    return DPFHE_OK;
+}
+
 // the context's encoding tables (built and uploaded once) and `need` bytes of scratch
 static int ckks_prepare(dpfhe_ctx *ctx, size_t need, cudaStream_t st) {
     if (!ctx->ckks_tab) {
@@ -1031,15 +1046,7 @@ static int ckks_prepare(dpfhe_ctx *ctx, size_t need, cudaStream_t st) {
         ctx->ckks.pow2 = (const u64 *)(base + b_tw);
         ctx->ckks.tj = (const u32 *)(base + b_tw + b_p2);
     }
-    if (need > ctx->ckks_work_bytes) {
-        CU_TRY(cudaStreamSynchronize(st));   // the old scratch may still be in use on this stream
-        if (ctx->ckks_work) cudaFree(ctx->ckks_work);
-        ctx->ckks_work = nullptr;
-        ctx->ckks_work_bytes = 0;
-        CU_TRY(cudaMalloc(&ctx->ckks_work, need));
-        ctx->ckks_work_bytes = need;
-    }
-    return DPFHE_OK;
+    return enc_work_prepare(ctx, need, st);
 }
 
 static bool valid_scale(double scale) { return scale > 0.0 && scale <= 1.7976931348623157e308; }   // finite and positive (NaN fails both)
@@ -1054,7 +1061,7 @@ int dpfhe_ckks_encode(dpfhe_ctx *ctx, const double *d_slots, uint64_t *d_pt, siz
     rc = ckks_prepare(ctx, n_vec * ctx->N() * sizeof(double), st);
     if (rc) return rc;
     const double sc = scale * (2.0 / (double)ctx->N());
-    CU_TRY(VCALL(launch_ckks_encode, ctx->lc, (const Cplx *)d_slots, (double *)ctx->ckks_work, d_pt, ctx->ckks, sc, n_vec, st));
+    CU_TRY(VCALL(launch_ckks_encode, ctx->lc, (const Cplx *)d_slots, (double *)ctx->enc_work, d_pt, ctx->ckks, sc, n_vec, st));
     note_launch(ctx, 2);   // ckks_enc_fft_kernel + ckks_enc_ntt(_pair)_kernel
     return DPFHE_OK;
 }
@@ -1069,7 +1076,7 @@ int dpfhe_ckks_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, double *d_slots, siz
     const size_t bytes = n_vec * ctx->P() * 8;
     rc = ckks_prepare(ctx, bytes, st);
     if (rc) return rc;
-    u64 *work = (u64 *)ctx->ckks_work;
+    u64 *work = (u64 *)ctx->enc_work;
     CU_TRY(cudaMemcpyAsync(work, d_pt, bytes, cudaMemcpyDeviceToDevice, st));   // the caller's plaintexts stay unchanged
     CU_TRY(VCALL(launch_ntt, ctx->lc, work, n_vec, true, st));
     CkksConsts K;
@@ -1106,6 +1113,112 @@ int dpfhe_ckks_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, double *h_slots
                             return dpfhe_ckks_decode(ctx, din, (double *)dout, cnt, scale, st);
                         });
 }
+
+// ---------------------------------------------------------------- BGV slot encoding (DESIGN.md §2.13)
+
+#define CHECK_T(t)                                                                                                \
+    do {                                                                                                          \
+        if (!bgv_plain_modulus_valid(ctx->hp.log_n, (t)))                                                         \
+            return fail(DPFHE_ERR_INVALID, "plaintext modulus %llu is not a prime below 2^31 that is 1 mod 2N",  \
+                        (unsigned long long)(t));                                                                 \
+    } while (0)
+
+// the tables of plaintext modulus t (kept for the last t used: built and uploaded on first use and whenever t changes) and
+// `need` bytes of scratch
+static int bgv_prepare(dpfhe_ctx *ctx, uint64_t t, size_t need, cudaStream_t st) {
+    if (ctx->bgv_t != t) {
+        std::vector<uint32_t> tab;
+        BgvTables T;
+        if (!build_bgv_tables(ctx->hp, t, tab, T)) return fail(DPFHE_ERR_INVALID, "invalid plaintext modulus");
+        if (ctx->bgv_tab) {
+            // earlier calls may still read the old tables; st already waits for the last of them, whatever its stream (§4.7)
+            CU_TRY(cudaStreamSynchronize(st));
+            cudaFree(ctx->bgv_tab);
+            ctx->bgv_tab = nullptr;
+            ctx->bgv_tab_bytes = 0;
+            ctx->bgv_t = 0;
+            ctx->bgv = BgvTables();
+        }
+        const size_t bytes = tab.size() * sizeof(uint32_t);
+        void *p = nullptr;
+        CU_TRY(cudaMalloc(&p, bytes));
+        if (cudaMemcpy(p, tab.data(), bytes, cudaMemcpyHostToDevice) != cudaSuccess) {
+            cudaFree(p);
+            return fail(DPFHE_ERR_CUDA, "CUDA error at %s:%d: uploading the BGV tables failed", __FILE__, __LINE__);
+        }
+        const size_t N = ctx->N();
+        T.tw = (const u32 *)p;
+        T.pos = (const u32 *)p + 4 * N;
+        ctx->bgv_tab = p;
+        ctx->bgv_tab_bytes = bytes;
+        ctx->bgv = T;
+        ctx->bgv_t = t;
+    }
+    return enc_work_prepare(ctx, need, st);
+}
+
+int dpfhe_bgv_encode(dpfhe_ctx *ctx, const int64_t *d_slots, uint64_t *d_pt, size_t n_vec, uint64_t t_plain, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_T(t_plain);
+    if (n_vec == 0) return DPFHE_OK;
+    CHECK_PTR(d_slots); CHECK_PTR(d_pt);
+    cudaStream_t st = pick(ctx, stream);
+    rc = bgv_prepare(ctx, t_plain, n_vec * ctx->N() * sizeof(u32), st);
+    if (rc) return rc;
+    CU_TRY(VCALL(launch_bgv_encode, ctx->lc, d_slots, (u32 *)ctx->enc_work, d_pt, ctx->bgv, n_vec, st));
+    note_launch(ctx, 2);   // bgv_enc_kernel + bgv_enc_ntt(_pair)_kernel
+    return DPFHE_OK;
+}
+
+int dpfhe_bgv_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, uint64_t *d_slots, size_t n_vec, uint64_t t_plain, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_T(t_plain);
+    if (n_vec == 0) return DPFHE_OK;
+    CHECK_PTR(d_pt); CHECK_PTR(d_slots);
+    cudaStream_t st = pick(ctx, stream);
+    const size_t bytes = n_vec * ctx->P() * 8;
+    rc = bgv_prepare(ctx, t_plain, bytes, st);
+    if (rc) return rc;
+    u64 *work = (u64 *)ctx->enc_work;
+    CU_TRY(cudaMemcpyAsync(work, d_pt, bytes, cudaMemcpyDeviceToDevice, st));   // the caller's plaintexts stay unchanged
+    CU_TRY(VCALL(launch_ntt, ctx->lc, work, n_vec, true, st));
+    BgvConsts K;
+    build_bgv_consts(ctx->hp, t_plain, K);
+    CU_TRY(VCALL(launch_bgv_decode, ctx->lc, work, d_slots, ctx->bgv, K, n_vec, st));
+    note_launch(ctx, 2);   // inverse transform + bgv_dec_kernel
+    return DPFHE_OK;
+}
+
+int dpfhe_bgv_encode_host(dpfhe_ctx *ctx, const int64_t *h_slots, uint64_t *h_pt, size_t n_vec, uint64_t t_plain) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_T(t_plain);
+    if (n_vec == 0) return DPFHE_OK;
+    if (!h_slots || !h_pt) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const size_t P = ctx->P(), S = ctx->N();   // words of a plaintext, and of a slot vector
+    const size_t chunk = pick_chunk(ctx, P * 8, n_vec);
+    return run_pipeline(ctx, (const u64 *)h_slots, nullptr, h_pt, n_vec, S, P, chunk,
+                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                            return dpfhe_bgv_encode(ctx, (const int64_t *)din, dout, cnt, t_plain, st);
+                        });
+}
+
+int dpfhe_bgv_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, uint64_t *h_slots, size_t n_vec, uint64_t t_plain) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_T(t_plain);
+    if (n_vec == 0) return DPFHE_OK;
+    if (!h_slots || !h_pt) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const size_t P = ctx->P(), S = ctx->N();
+    const size_t chunk = pick_chunk(ctx, P * 8, n_vec);
+    return run_pipeline(ctx, h_pt, nullptr, h_slots, n_vec, P, S, chunk,
+                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                            return dpfhe_bgv_decode(ctx, din, dout, cnt, t_plain, st);
+                        });
+}
+#undef CHECK_T
 
 // waits for everything this context has in flight, whatever stream it was issued on
 int dpfhe_synchronize(dpfhe_ctx *ctx) {

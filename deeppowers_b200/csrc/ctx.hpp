@@ -35,13 +35,19 @@ struct dpfhe_ctx {
     size_t hoist_chunk = 0;                  // ciphertexts the current U / zero buffers hold
     dpfhe::u64 *hoistg_buf = nullptr;        // hoisted rotations with grouped hybrid keys: lifted digits, accumulators and tau' rows of a chunk
     size_t hoistg_bytes = 0;
-    // CKKS slot encoding (allocated on first use): twiddles, slot permutation and 2^e mod q tables in one allocation, and a
-    // scratch row set (encode: [n_vec][N] rounded coefficients; decode: [n_vec][L][N] inverse transforms)
+    // CKKS slot encoding (allocated on first use): twiddles, slot permutation and 2^e mod q tables in one allocation
     void *ckks_tab = nullptr;
     size_t ckks_tab_bytes = 0;
     dpfhe::CkksTables ckks;
-    void *ckks_work = nullptr;
-    size_t ckks_work_bytes = 0;
+    // BGV slot encoding: the twiddles mod t and slot positions of the plaintext modulus bgv_t last used (0: none), in one
+    // allocation, replaced when t changes
+    void *bgv_tab = nullptr;
+    size_t bgv_tab_bytes = 0;
+    uint64_t bgv_t = 0;
+    dpfhe::BgvTables bgv;
+    // scratch rows of both slot encoders (encode: [n_vec][N] coefficients; decode: [n_vec][L][N] inverse transforms)
+    void *enc_work = nullptr;
+    size_t enc_work_bytes = 0;
     dpfhe::u64 *stage_in[DPFHE_PIPE_DEPTH] = {}, *stage_out[DPFHE_PIPE_DEPTH] = {}, *stage_key = nullptr;
     size_t stage_in_bytes = 0, stage_out_bytes = 0, stage_key_bytes = 0;
     cudaEvent_t ev_h2d[DPFHE_PIPE_DEPTH] = {}, ev_comp[DPFHE_PIPE_DEPTH] = {}, ev_d2h[DPFHE_PIPE_DEPTH] = {};

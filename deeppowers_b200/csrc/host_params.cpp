@@ -310,4 +310,71 @@ void build_ckks_consts(const HostParams &hp, double scale, CkksConsts &K) {
     K.scale = scale;
 }
 
+// ---- BGV slot encoding (DESIGN.md §2.13) ----------------------------------------------------------------------
+static uint32_t shoup32_of(uint64_t w, uint64_t t) { return (uint32_t)((w << 32) / t); }
+
+static Mod32 make_mod32(uint64_t t) {
+    const uint64_t r32 = ((uint64_t)1 << 32) % t;
+    return Mod32{(uint32_t)t, (uint32_t)r32, shoup32_of(r32, t), shoup32_of(1, t)};
+}
+
+bool bgv_plain_modulus_valid(unsigned log_n, uint64_t t) {
+    const uint64_t two_n = (uint64_t)2 << log_n;
+    return t < ((uint64_t)1 << 31) && t > two_n && (t - 1) % two_n == 0 && host_is_prime(t);
+}
+
+uint64_t bgv_zeta(unsigned log_n, uint64_t t) {
+    const uint64_t two_n = (uint64_t)2 << log_n;
+    uint64_t g = 2;
+    while (host_powmod(g, (t - 1) / 2, t) != t - 1) ++g;   // the least quadratic non-residue
+    return host_powmod(g, (t - 1) / two_n, t);             // zeta^N = g^((t-1)/2) = -1: a primitive 2N-th root of unity
+}
+
+bool build_bgv_tables(const HostParams &hp, uint64_t t, std::vector<uint32_t> &tab, BgvTables &T) {
+    const unsigned log_n = hp.log_n;
+    if (!bgv_plain_modulus_valid(log_n, t)) return false;
+    const uint64_t N = (uint64_t)1 << log_n, two_n = 2 * N, zeta = bgv_zeta(log_n, t);
+    std::vector<uint64_t> zp(two_n);   // zeta^k
+    zp[0] = 1;
+    for (uint64_t k = 1; k < two_n; ++k) zp[k] = zp[k - 1] * zeta % t;
+    tab.assign(5 * N, 0);
+    for (uint64_t k = 0; k < N; ++k) {
+        const uint64_t e = rev_bits((uint32_t)k, log_n), w = zp[e], wi = zp[(two_n - e) % two_n];
+        tab[k] = (uint32_t)w;
+        tab[N + k] = shoup32_of(w, t);
+        tab[2 * N + k] = (uint32_t)wi;
+        tab[3 * N + k] = shoup32_of(wi, t);
+    }
+    // slot (0, c) holds m(zeta^e), slot (1, c) m(zeta^(2N - e)), e = 5^c mod 2N; the forward transform's output br(i) is m(zeta^(2i+1))
+    uint64_t e = 1;
+    for (uint64_t c = 0; c < N / 2; ++c, e = e * 5 % two_n) {
+        tab[4 * N + c] = rev_bits((uint32_t)((e - 1) / 2), log_n);
+        tab[4 * N + N / 2 + c] = rev_bits((uint32_t)((two_n - e - 1) / 2), log_n);
+    }
+    T = BgvTables();
+    T.m = make_mod32(t);
+    T.ninv = (uint32_t)host_powmod(N, t - 2, t);
+    T.ninv_s = shoup32_of(T.ninv, t);
+    return true;
+}
+
+void build_bgv_consts(const HostParams &hp, uint64_t t, BgvConsts &K) {
+    K = BgvConsts();
+    CkksConsts C;
+    build_ckks_consts(hp, 1.0, C);
+    for (unsigned i = 0; i < 16; ++i) {
+        for (unsigned j = 0; j < 16; ++j) K.ginv[i][j] = C.ginv[i][j];
+        K.half[i] = C.half[i];
+    }
+    uint64_t Qt = 1;
+    for (unsigned i = 0; i < hp.L; ++i) {
+        const uint64_t r = hp.limbs[i].lp.q % t;
+        K.qt[i] = (uint32_t)r;
+        K.qt_s[i] = shoup32_of(r, t);
+        Qt = Qt * r % t;
+    }
+    K.Qt = (uint32_t)Qt;
+    K.m = make_mod32(t);
+}
+
 }  // namespace dpfhe

@@ -40,6 +40,16 @@ void build_ckks_tables(const HostParams &hp, std::vector<Cplx> &tw, std::vector<
 // decoding constants (Garner inverses, the digits of (Q-1)/2, the moduli as doubles) with the divisor `scale`
 void build_ckks_consts(const HostParams &hp, double scale, CkksConsts &K);
 
+// BGV slot encoding (DESIGN.md §2.13).  A valid plaintext modulus is a prime t < 2^31 with t = 1 (mod 2N).
+bool bgv_plain_modulus_valid(unsigned log_n, uint64_t t);
+// zeta = g^((t-1)/2N), g the least quadratic non-residue mod t (requires a valid t)
+uint64_t bgv_zeta(unsigned log_n, uint64_t t);
+// tab receives [5][N] words: the four twiddle rows of BgvTables::tw, then the slot positions; T the constants of t (its
+// pointers stay null: the caller places tab).  Returns false, building nothing, for an invalid t.
+bool build_bgv_tables(const HostParams &hp, uint64_t t, std::vector<uint32_t> &tab, BgvTables &T);
+// decoding constants: CKKS's Garner inverses and digits of (Q-1)/2, q_i mod t and Q mod t (requires a valid t)
+void build_bgv_consts(const HostParams &hp, uint64_t t, BgvConsts &K);
+
 uint64_t host_mulmod(uint64_t a, uint64_t b, uint64_t q);
 uint64_t host_powmod(uint64_t a, uint64_t e, uint64_t q);
 bool host_is_prime(uint64_t n);

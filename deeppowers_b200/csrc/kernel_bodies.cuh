@@ -1549,9 +1549,10 @@ DPFHE_HD u64 ckks_reduce(double x, const LimbParams &p, const u64 *pow2) {
     return (b >> 63) && r ? p.q - r : r;
 }
 
-// decode, one coefficient: the residues col[l * stride], l < L (canonical), are overwritten by the mixed-radix digits of X
-// (Garner); returns centred(X) / scale as a double: Horner from the most significant digit, then one division.
-DPFHE_HD double ckks_crt_double(u64 *col, size_t stride, u32 L, const LimbParams *lp, const CkksConsts &K) {
+// Garner, shared by the CKKS and BGV decoders: the residues col[l * stride], l < L (canonical), are overwritten by the
+// mixed-radix digits of X = d_0 + d_1 q_0 + d_2 q_0 q_1 + ...; returns X > (Q-1)/2 (the digits of (Q-1)/2 in `half`, compared
+// lexicographically from the most significant one)
+DPFHE_HD bool garner_digits(u64 *col, size_t stride, u32 L, const LimbParams *lp, const u64 (&ginv)[16][16], const u64 *half) {
 #pragma unroll 1
     for (u32 i = 1; i < L; ++i) {
         const LimbParams &p = lp[i];
@@ -1559,18 +1560,23 @@ DPFHE_HD double ckks_crt_double(u64 *col, size_t stride, u32 L, const LimbParams
 #pragma unroll 1
         for (u32 j = 0; j < i; ++j) {
             const u64 d = canon(col[j * stride], p);
-            t = mulmod(t >= d ? t - d : t + p.q - d, K.ginv[j][i], p);
+            t = mulmod(t >= d ? t - d : t + p.q - d, ginv[j][i], p);
         }
         col[i * stride] = t;
     }
-    // X > (Q-1)/2 ?  (lexicographic from the most significant digit)
     int cmp = 0;
 #pragma unroll 1
     for (u32 i = L; i-- > 0 && cmp == 0;) {
         const u64 d = col[i * stride];
-        cmp = d > K.half[i] ? 1 : (d < K.half[i] ? -1 : 0);
+        cmp = d > half[i] ? 1 : (d < half[i] ? -1 : 0);
     }
-    const bool neg = cmp > 0;
+    return cmp > 0;
+}
+
+// decode, one coefficient: the residues col[l * stride], l < L (canonical), are overwritten by the mixed-radix digits of X
+// (Garner); returns centred(X) / scale as a double: Horner from the most significant digit, then one division.
+DPFHE_HD double ckks_crt_double(u64 *col, size_t stride, u32 L, const LimbParams *lp, const CkksConsts &K) {
+    const bool neg = garner_digits(col, stride, L, lp, K.ginv, K.half);
     // digits of Q - X: 0 below the lowest non-zero digit p of X, q_p - d_p at p, q_i - 1 - d_i above
     u32 low = 0;
     if (neg)
@@ -1600,6 +1606,83 @@ DPFHE_HD void ckks_dec_fft_body(CTA &cta, Cplx *a, u64 *col, Cplx *z, const Cplx
     ckks_fft_stages<LOGN, NT>(cta, a, tw, false);
     cta.par([&](int tid) {
         for (int j = tid; j < S; j += NT) z[j] = a[tj[j]];
+    });
+}
+
+// ---- BGV slot encoding (DESIGN.md §2.13) ---------------------------------------------------------------------------
+// The negacyclic transform of N values mod t (32-bit arithmetic) in shared memory, radix-2 stages with CTA barriers and the
+// conventions of §2.3 with psi = zeta: stage s has 2^s groups of span N / 2^(s+1), the twiddle of group i is tw[2^s + i].
+// Forward: Cooley-Tukey, natural in, bit-reversed out, a[i] -> m(zeta^(2 br(i) + 1)).  Inverse: Gentleman-Sande, bit-reversed
+// in, natural out, WITHOUT the factor N^-1.  Every value stays canonical, so the result is an exact integer.
+template <int LOGN, int NT, class CTA>
+DPFHE_HD void bgv_ntt_stages(CTA &cta, u32 *a, const u32 *tw, u32 t, bool inverse) {
+    constexpr int N = 1 << LOGN;
+#pragma unroll 1
+    for (int k = 0; k < LOGN; ++k) {
+        const int s = inverse ? LOGN - 1 - k : k, hs = LOGN - 1 - s;   // 2^s groups of span 2^hs
+        const u32 *w = tw + (inverse ? 2 * N : 0), *ws = w + N;
+        cta.par([&](int tid) {
+#pragma unroll 1
+            for (int b = tid; b < N / 2; b += NT) {
+                const int g = (1 << s) + (b >> hs), i0 = ((b >> hs) << (hs + 1)) + (b & ((1 << hs) - 1)), i1 = i0 + (1 << hs);
+                const u32 x = a[i0], y = a[i1];
+                if (!inverse) {
+                    const u32 v = shoup32(y, w[g], ws[g], t);
+                    a[i0] = add32(x, v, t);
+                    a[i1] = sub32(x, v, t);
+                } else {
+                    a[i0] = add32(x, y, t);
+                    a[i1] = shoup32(x + t - y, w[g], ws[g], t);   // x + t - y < 2t < 2^32: shoup32 takes any 32-bit word
+                }
+            }
+        });
+    }
+}
+
+// floor-mod of any int64 by t (numpy's %).  INT64_MIN included: the magnitude 0 - (u64)v of a negative v is exact.
+DPFHE_HD u32 bgv_reduce_slot(int64_t v, const Mod32 &m) {
+    if (v >= 0) return reduce64_32((u64)v, m);
+    const u32 r = reduce64_32(0 - (u64)v, m);
+    return r ? m.t - r : 0u;
+}
+
+// the centred lift of a coefficient c in [0, t) into a limb: c <= floor(t/2) stays, above it is c - t, i.e. q - (t - c)
+DPFHE_HD u64 bgv_lift(u32 c, u32 t, const LimbParams &p) { return c > (t >> 1) ? p.q - (t - c) : (u64)c; }
+
+// encode, one vector: z [2][N/2] slots -> x [N] coefficients in [0, t).  a: N words of shared memory.
+template <int LOGN, int NT, class CTA>
+DPFHE_HD void bgv_enc_body(CTA &cta, u32 *a, const int64_t *z, u32 *x, const BgvTables &T) {
+    constexpr int N = 1 << LOGN;
+    cta.par([&](int tid) {
+        for (int j = tid; j < N; j += NT) a[T.pos[j]] = bgv_reduce_slot(z[j], T.m);
+    });
+    bgv_ntt_stages<LOGN, NT>(cta, a, T.tw, T.m.t, true);
+    cta.par([&](int tid) {
+        for (int k = tid; k < N; k += NT) x[k] = shoup32(a[k], T.ninv, T.ninv_s, T.m.t);
+    });
+}
+
+// decode, one coefficient: Garner digits of X (written over the residues col[l * stride]), then centred(X) mod t by Horner from
+// the most significant digit, r = r (q_i mod t) + (d_i mod t), minus Q mod t when X > (Q-1)/2
+DPFHE_HD u32 bgv_crt_mod_t(u64 *col, size_t stride, u32 L, const LimbParams *lp, const BgvConsts &K) {
+    const bool neg = garner_digits(col, stride, L, lp, K.ginv, K.half);
+    const u32 t = K.m.t;
+    u32 r = reduce64_32(col[(L - 1) * stride], K.m);
+#pragma unroll 1
+    for (u32 i = L - 1; i-- > 0;) r = add32(shoup32(r, K.qt[i], K.qt_s[i], t), reduce64_32(col[i * stride], K.m), t);
+    return neg ? sub32(r, K.Qt, t) : r;
+}
+
+// decode, one vector: col [L][N] coefficients (inverse-transformed, canonical; overwritten) -> z [2][N/2] slots in [0, t)
+template <int LOGN, int NT, class CTA>
+DPFHE_HD void bgv_dec_body(CTA &cta, u32 *a, u64 *col, u64 *z, const BgvTables &T, const LimbParams *lp, const BgvConsts &K, u32 L) {
+    constexpr int N = 1 << LOGN;
+    cta.par([&](int tid) {
+        for (int k = tid; k < N; k += NT) a[k] = bgv_crt_mod_t(col + k, N, L, lp, K);
+    });
+    bgv_ntt_stages<LOGN, NT>(cta, a, T.tw, T.m.t, false);
+    cta.par([&](int tid) {
+        for (int j = tid; j < N; j += NT) z[j] = a[T.pos[j]];
     });
 }
 

@@ -295,6 +295,75 @@ __global__ void __launch_bounds__(NT, 1) ckks_dec_kernel(u64 *work, Cplx *slots,
     ckks_dec_fft_body<LOGN, NT>(cta, reinterpret_cast<Cplx *>(smem_raw), work + v * L * N, slots + v * (N / 2), tw, tj, lt.lp, K, L);
 }
 
+// ------------------------------------------------------------------ BGV slot encoding (DESIGN.md §2.13, §4.9)
+// One CTA per vector: its N words mod t (16 / 32 / 64 KiB at N = 4096 / 8192 / 16384) stay in shared memory for all stages.
+template <int LOGN, int NT>
+__global__ void __launch_bounds__(NT, 1) bgv_enc_kernel(const int64_t *slots, u32 *coeffs, const __grid_constant__ BgvTables T) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    constexpr size_t N = (size_t)1 << LOGN;
+    DevCta<NT> cta;
+    const size_t v = blockIdx.x;
+    bgv_enc_body<LOGN, NT>(cta, reinterpret_cast<u32 *>(smem_raw), slots + v * N, coeffs + v * N, T);
+}
+
+// forward transform of one limb of one encoded vector, the coefficients lifted (centred) into the limb by the load stage
+template <int LOGN, int NT, int MINB>
+__global__ void __launch_bounds__(NT, MINB) bgv_enc_ntt_kernel(const u32 *coeffs, u64 *pt, const Twiddle *__restrict__ tw, u32 t,
+                                                                const __grid_constant__ LimbTable lt, u32 L) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    u64 *buf = reinterpret_cast<u64 *>(smem_raw);
+    constexpr size_t N = (size_t)1 << LOGN;
+    DevCta<NT> cta;
+    const size_t w = blockIdx.x;
+    const u32 l = (u32)(w % L);
+    const LimbParams &p = lt.lp[l];
+    const uint2 *x = reinterpret_cast<const uint2 *>(coeffs + (w / L) * N);
+    auto src = [&](int c) {
+        const uint2 v = x[c];
+        U64x2 r;
+        r.x = bgv_lift(v.x, t, p);
+        r.y = bgv_lift(v.y, t, p);
+        return r;
+    };
+    ntt_fwd_src_body<LOGN, NT>(cta, buf, src, pt + w * N, tw + (size_t)l * N, p);
+}
+
+// N = 16384: two CTAs per limb, as ckks_enc_ntt_pair_kernel
+template <int NT, int MINB>
+__global__ void __launch_bounds__(NT, MINB) bgv_enc_ntt_pair_kernel(const u32 *coeffs, u64 *pt, const Twiddle *__restrict__ tw, u32 t,
+                                                                     const __grid_constant__ LimbTable lt, u32 L) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    u64 *buf = reinterpret_cast<u64 *>(smem_raw);
+    constexpr size_t N = (size_t)1 << NTT_PAIR_LOGN;
+    DevCta<NT> cta;
+    const size_t w = blockIdx.x / 2;
+    const int h = (int)(blockIdx.x & 1);
+    const u32 l = (u32)(w % L);
+    const LimbParams &p = lt.lp[l];
+    const uint2 *x = reinterpret_cast<const uint2 *>(coeffs + (w / L) * N);
+    auto src = [&](int c) {
+        const uint2 v = x[c];
+        U64x2 r;
+        r.x = bgv_lift(v.x, t, p);
+        r.y = bgv_lift(v.y, t, p);
+        return r;
+    };
+    ntt_fwd_half_load_src<NT>(cta, buf, src, tw + (size_t)l * N, p, h);
+    ntt_fwd_half_finish<NT>(cta, buf, pt + w * N, tw + (size_t)l * N, p, h);
+}
+
+// decode: Garner, centring, reduction mod t, the forward transform mod t and the slot gather of one vector; work [n_vec][L][N]
+// holds the inverse transforms (overwritten by the mixed-radix digits)
+template <int LOGN, int NT>
+__global__ void __launch_bounds__(NT, 1) bgv_dec_kernel(u64 *work, u64 *slots, const __grid_constant__ BgvTables T, const __grid_constant__ LimbTable lt,
+                                                         const __grid_constant__ BgvConsts K, u32 L) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    constexpr size_t N = (size_t)1 << LOGN;
+    DevCta<NT> cta;
+    const size_t v = blockIdx.x;
+    bgv_dec_body<LOGN, NT>(cta, reinterpret_cast<u32 *>(smem_raw), work + v * L * N, slots + v * N, T, lt.lp, K, L);
+}
+
 #endif
 // ------------------------------------------------------------------ fused key-switch family
 __device__ __forceinline__ u32 ld_acquire_u32(const u32 *p) {
@@ -1280,6 +1349,74 @@ cudaError_t launch_ckks_decode(const LaunchCtx &lc, u64 *work, Cplx *slots, cons
         case 12: return launch_ckks_decode_t<12>(lc, work, slots, T, K, n_vec, st);
         case 13: return launch_ckks_decode_t<13>(lc, work, slots, T, K, n_vec, st);
         case 14: return launch_ckks_decode_t<14>(lc, work, slots, T, K, n_vec, st);
+    }
+    return cudaErrorInvalidValue;
+}
+
+// ---- BGV slot encoding
+constexpr int BGV_NT = 512;
+
+template <int LOGN>
+static cudaError_t launch_bgv_encode_t(const LaunchCtx &lc, const int64_t *slots, u32 *coeffs, u64 *pt, const BgvTables &T, size_t n_vec,
+                                       cudaStream_t st) {
+    auto ke = bgv_enc_kernel<LOGN, BGV_NT>;
+    const size_t smem_t = ((size_t)1 << LOGN) * sizeof(u32);
+    static ConfiguredMask conf_enc, conf_ntt;
+    cudaError_t e = set_smem_once(ke, smem_t, conf_enc, lc.device);
+    if (e != cudaSuccess) return e;
+    ke<<<(unsigned)n_vec, BGV_NT, smem_t, st>>>(slots, coeffs, T);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    const size_t n_limbs = n_vec * lc.L;
+    if constexpr (LOGN == NTT_PAIR_LOGN) {
+        auto kn = bgv_enc_ntt_pair_kernel<256, 2>;
+        const size_t smem = Geometry<13>::LIMB_BYTES;   // half a limb
+        e = set_smem_once(kn, smem, conf_ntt, lc.device);
+        if (e != cudaSuccess) return e;
+        kn<<<(unsigned)(2 * n_limbs), 256, smem, st>>>(coeffs, pt, lc.tw, T.m.t, lc.lt, lc.L);
+    } else {
+        constexpr int MINB = LOGN == 12 ? 2 : 3;
+        auto kn = bgv_enc_ntt_kernel<LOGN, 256, MINB>;
+        const size_t smem = Geometry<LOGN>::LIMB_BYTES;
+        e = set_smem_once(kn, smem, conf_ntt, lc.device);
+        if (e != cudaSuccess) return e;
+        kn<<<(unsigned)n_limbs, 256, smem, st>>>(coeffs, pt, lc.tw, T.m.t, lc.lt, lc.L);
+    }
+    return cudaGetLastError();
+}
+
+// coeffs: [n_vec][N] words of scratch
+cudaError_t launch_bgv_encode(const LaunchCtx &lc, const int64_t *slots, u32 *coeffs, u64 *pt, const BgvTables &T, size_t n_vec, cudaStream_t st) {
+    if (n_vec == 0) return cudaSuccess;
+    if (n_vec * lc.L * 2 > 0x7fffffffull) return cudaErrorInvalidValue;
+    switch (lc.log_n) {
+        case 12: return launch_bgv_encode_t<12>(lc, slots, coeffs, pt, T, n_vec, st);
+        case 13: return launch_bgv_encode_t<13>(lc, slots, coeffs, pt, T, n_vec, st);
+        case 14: return launch_bgv_encode_t<14>(lc, slots, coeffs, pt, T, n_vec, st);
+    }
+    return cudaErrorInvalidValue;
+}
+
+template <int LOGN>
+static cudaError_t launch_bgv_decode_t(const LaunchCtx &lc, u64 *work, u64 *slots, const BgvTables &T, const BgvConsts &K, size_t n_vec,
+                                       cudaStream_t st) {
+    auto kd = bgv_dec_kernel<LOGN, BGV_NT>;
+    const size_t smem = ((size_t)1 << LOGN) * sizeof(u32);
+    static ConfiguredMask conf;
+    cudaError_t e = set_smem_once(kd, smem, conf, lc.device);
+    if (e != cudaSuccess) return e;
+    kd<<<(unsigned)n_vec, BGV_NT, smem, st>>>(work, slots, T, lc.lt, K, lc.L);
+    return cudaGetLastError();
+}
+
+// work: [n_vec][L][N] inverse transforms of the plaintexts (overwritten)
+cudaError_t launch_bgv_decode(const LaunchCtx &lc, u64 *work, u64 *slots, const BgvTables &T, const BgvConsts &K, size_t n_vec, cudaStream_t st) {
+    if (n_vec == 0) return cudaSuccess;
+    if (n_vec > 0x7fffffffull) return cudaErrorInvalidValue;
+    switch (lc.log_n) {
+        case 12: return launch_bgv_decode_t<12>(lc, work, slots, T, K, n_vec, st);
+        case 13: return launch_bgv_decode_t<13>(lc, work, slots, T, K, n_vec, st);
+        case 14: return launch_bgv_decode_t<14>(lc, work, slots, T, K, n_vec, st);
     }
     return cudaErrorInvalidValue;
 }

@@ -78,7 +78,11 @@ struct LaunchCtx {
     cudaError_t launch_ckks_encode(const LaunchCtx &lc, const Cplx *slots, double *coeffs, u64 *pt, const CkksTables &T, double sc, size_t n_vec, \
                                    cudaStream_t st); \
     cudaError_t launch_ckks_decode(const LaunchCtx &lc, u64 *work, Cplx *slots, const CkksTables &T, const CkksConsts &K, size_t n_vec, \
-                                   cudaStream_t st);
+                                   cudaStream_t st); \
+    cudaError_t launch_bgv_encode(const LaunchCtx &lc, const int64_t *slots, u32 *coeffs, u64 *pt, const BgvTables &T, size_t n_vec, \
+                                  cudaStream_t st); \
+    cudaError_t launch_bgv_decode(const LaunchCtx &lc, u64 *work, u64 *slots, const BgvTables &T, const BgvConsts &K, size_t n_vec, \
+                                  cudaStream_t st);
 
 namespace gen {
 DPFHE_DECLARE_LAUNCHERS

@@ -278,5 +278,24 @@ DPFHE_HD u64 canon4(u64 x, const LimbParams &p) { return csub(csub(x, p.q2), p.q
 // canonical factors -> canonical product
 DPFHE_HD u64 mulmod(u64 a, u64 b, const LimbParams &p) { return canon4(mulmod_lazy(a, b, p), p); }
 
+// ---- 32-bit arithmetic modulo a prime t < 2^31 (the BGV plaintext modulus, DESIGN.md §2.13) ----
+DPFHE_HD u32 mulhi32(u32 a, u32 b) {
+#if defined(__CUDA_ARCH__)
+    return __umulhi(a, b);   // IMAD.HI
+#else
+    return (u32)(((u64)a * b) >> 32);
+#endif
+}
+DPFHE_HD u32 csub32(u32 x, u32 t) { return x >= t ? x - t : x; }
+// Shoup multiplication by a fixed w < t with ws = floor(w * 2^32 / t), canonical result for ANY 32-bit x: h = hi32(x * ws) is
+// floor(x w / t) or one less, so x w - h t lies in [0, 2t) and 2t < 2^32: the low words give it exactly (one IMAD.HI, two IMAD)
+DPFHE_HD u32 shoup32(u32 x, u32 w, u32 ws, u32 t) { return csub32(x * w - mulhi32(x, ws) * t, t); }
+DPFHE_HD u32 add32(u32 a, u32 b, u32 t) { return csub32(a + b, t); }   // canonical operands
+DPFHE_HD u32 sub32(u32 a, u32 b, u32 t) { return a >= b ? a - b : a + t - b; }
+// any 64-bit x -> x mod t: x = xh 2^32 + xl, reduced as xh (2^32 mod t) + xl * 1 with two Shoup products
+DPFHE_HD u32 reduce64_32(u64 x, const Mod32 &m) {
+    return add32(shoup32((u32)(x >> 32), m.r32, m.r32_s, m.t), shoup32((u32)x, 1u, m.one_s, m.t), m.t);
+}
+
 }  // namespace DPFHE_VNS
 }  // namespace dpfhe

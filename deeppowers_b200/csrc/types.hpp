@@ -131,6 +131,29 @@ struct CkksConsts {
     double scale;       // the divisor of the decoded coefficients
 };
 
+// BGV slot encoding (DESIGN.md §2.13).  A prime plaintext modulus t < 2^31 and the constants of its 32-bit arithmetic
+// (modarith.cuh: shoup32, reduce64_32)
+struct Mod32 {
+    u32 t;
+    u32 r32, r32_s;   // 2^32 mod t and its Shoup companion floor(r32 * 2^32 / t)
+    u32 one_s;        // floor(2^32 / t), the Shoup companion of 1
+};
+// device tables of the plaintext modulus last used (host_params.cpp:build_bgv_tables), cached by the context
+struct BgvTables {
+    const u32 *tw = nullptr;    // [4][N] zeta^br(k), their Shoup companions, zeta^-br(k), their companions (br over log2 N bits)
+    const u32 *pos = nullptr;   // [2][N/2] slot (r, c) -> position of its value in the bit-reversed evaluation order
+    Mod32 m{};
+    u32 ninv = 0, ninv_s = 0;   // N^-1 mod t and its Shoup companion
+};
+// decoding constants of one context and t (host_params.cpp:build_bgv_consts), passed by value in the kernel parameter block
+struct BgvConsts {
+    u64 ginv[16][16];       // Garner's inverses, as CkksConsts
+    u64 half[16];           // mixed-radix digits of (Q - 1) / 2
+    u32 qt[16], qt_s[16];   // q_i mod t and its Shoup companion
+    u32 Qt;                 // Q mod t
+    Mod32 m;
+};
+
 enum KsMode { KS_MUL_RELIN = 0, KS_PLAIN = 1, KS_ROTATE = 2 };
 // tau' rows of a hybrid key-switching group are double-buffered by round parity (the division step runs one round late)
 constexpr int KS_HYB_ROWS = 6;

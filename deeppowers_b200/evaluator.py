@@ -47,6 +47,14 @@ def _chptr(a, writable=False):
     return C.c_void_p(a.ctypes.data)
 
 
+def _ihptr(a, writable=False):
+    if not isinstance(a, np.ndarray) or a.dtype not in (np.int64, np.uint64) or not a.flags["C_CONTIGUOUS"]:
+        raise ValueError("BGV slots must be C-contiguous numpy int64 arrays")
+    if writable and not a.flags["WRITEABLE"]:
+        raise ValueError("output array is read-only")
+    return C.c_void_p(a.ctypes.data)
+
+
 def _hptr(a, writable=False):
     if not isinstance(a, np.ndarray) or a.dtype != np.uint64 or not a.flags["C_CONTIGUOUS"]:
         raise ValueError("host buffers must be C-contiguous numpy uint64 arrays")
@@ -309,6 +317,22 @@ class Context:
 
     def ckks_decode_host(self, pt, slots, scale):
         self._chk(self._l.dpfhe_ckks_decode_host(self._h, _hptr(pt), _chptr(slots, True), pt.size // self.P, float(scale)))
+
+    # BGV slot encoding (DESIGN.md section 2.13): slots [n_vec][2][N/2] int64 (encode: any value, reduced mod t; decode: values in
+    # [0, t)), plaintexts [n_vec][L][N] in evaluation form; exact.  t_plain: a prime below 2^31 that is 1 mod 2N.  Device forms take
+    # 8-byte integer CUDA tensors, host forms C-contiguous numpy int64 (slots) and uint64 (plaintexts) arrays.
+    def bgv_encode(self, slots, pt, n_vec, t_plain, stream=None):
+        self._chk(self._l.dpfhe_bgv_encode(self._h, _ptr(slots), _ptr(pt), n_vec, int(t_plain), _stream(stream)))
+
+    def bgv_decode(self, pt, slots, n_vec, t_plain, stream=None):
+        """pt is not modified (the inverse transform runs into the context's scratch)"""
+        self._chk(self._l.dpfhe_bgv_decode(self._h, _ptr(pt), _ptr(slots), n_vec, int(t_plain), _stream(stream)))
+
+    def bgv_encode_host(self, slots, pt, t_plain):
+        self._chk(self._l.dpfhe_bgv_encode_host(self._h, _ihptr(slots), _hptr(pt, True), slots.size // self.N, int(t_plain)))
+
+    def bgv_decode_host(self, pt, slots, t_plain):
+        self._chk(self._l.dpfhe_bgv_decode_host(self._h, _hptr(pt), _ihptr(slots, True), pt.size // self.P, int(t_plain)))
 
     def fill_uniform(self, seed, data, n_polys, first_poly=0, stream=None):
         self._chk(self._l.dpfhe_fill_uniform(self._h, int(seed), int(first_poly), _ptr(data), n_polys, _stream(stream)))

@@ -90,6 +90,15 @@ public:
         check(dpfhe_ckks_decode_host(ctx_, plain_eval, reinterpret_cast<double *>(slots), count, scale));
     }
 
+    // ---- BGV slot encoding (DESIGN.md §2.13): `count` vectors of poly_degree() slots ([2][N/2], int64 in, values in
+    //      [0, plain_modulus) out) <-> `count` plaintexts of poly_words() words in evaluation form; synchronous host-buffer calls ----
+    void encode_bgv(const std::int64_t *slots, std::size_t count, std::uint64_t plain_modulus, std::uint64_t *plain_eval) {
+        check(dpfhe_bgv_encode_host(ctx_, slots, plain_eval, count, plain_modulus));
+    }
+    void decode_bgv(const std::uint64_t *plain_eval, std::size_t count, std::uint64_t plain_modulus, std::uint64_t *slots) {
+        check(dpfhe_bgv_decode_host(ctx_, plain_eval, slots, count, plain_modulus));
+    }
+
     // ---- host-buffer calls: synchronous; H2D / compute / D2H are pipelined inside the library ----
     void multiply_relin(ConstCiphertextBatch a, ConstCiphertextBatch b, const std::uint64_t *relin_key, CiphertextBatch out) {
         same(a.count, b.count, out.count);

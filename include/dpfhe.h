@@ -244,6 +244,21 @@ int dpfhe_ckks_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, double *d_slots, siz
 int dpfhe_ckks_encode_host(dpfhe_ctx *ctx, const double *h_slots, uint64_t *h_pt, size_t n_vec, double scale);
 int dpfhe_ckks_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, double *h_slots, size_t n_vec, double scale);
 
+/* ---- BGV slot encoding (DESIGN.md §2.13).  The plaintext modulus t_plain must be a prime below 2^31 with t_plain = 1 (mod 2N);
+ *      any other value returns DPFHE_ERR_INVALID.  Slots are [n_vec][2][N/2]: slot (0, c) is m(zeta^e) and slot (1, c) is
+ *      m(zeta^(2N-e)), e = 5^c mod 2N, zeta = g^((t-1)/2N) with g the least quadratic non-residue mod t; so
+ *      dpfhe_galois_element(k) rolls each row left by k and 2N-1 swaps the rows.  Plaintexts are [n_vec][L][N] in evaluation form.
+ *      encode: int64 slots (any value, reduced by floor-mod into [0, t)) -> the polynomial m mod t with those slots, each
+ *      coefficient lifted centred (above floor(t/2) it is m_k - t) into every limb, then the forward transform.
+ *      decode: inverse transform (into scratch: d_pt is not modified), the centred CRT value mod t, its slots in [0, t).
+ *      The results are exact.  The context keeps the tables of the last t_plain used; a call with another t replaces them after
+ *      the earlier calls have finished.  A plaintext for ciphertexts under a context with special primes is encoded with the
+ *      context over the ciphertext moduli.  The *_host forms take host buffers and pipeline them in chunks (synchronous). ---- */
+int dpfhe_bgv_encode(dpfhe_ctx *ctx, const int64_t *d_slots, uint64_t *d_pt, size_t n_vec, uint64_t t_plain, void *stream);
+int dpfhe_bgv_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, uint64_t *d_slots, size_t n_vec, uint64_t t_plain, void *stream);
+int dpfhe_bgv_encode_host(dpfhe_ctx *ctx, const int64_t *h_slots, uint64_t *h_pt, size_t n_vec, uint64_t t_plain);
+int dpfhe_bgv_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, uint64_t *h_slots, size_t n_vec, uint64_t t_plain);
+
 /* ---- synthetic data (DESIGN.md §5): x[k] = mulhi64(splitmix64(seed + k), q_limb),
  *      k = (first_poly + p)*L*N + l*N + n.  Fills [n_polys][L][N]. ---- */
 int dpfhe_fill_uniform(dpfhe_ctx *ctx, uint64_t seed, uint64_t first_poly, uint64_t *d_data,
