@@ -313,7 +313,7 @@ void build_ckks_consts(const HostParams &hp, double scale, CkksConsts &K) {
 // ---- BGV slot encoding (DESIGN.md §2.13) ----------------------------------------------------------------------
 static uint32_t shoup32_of(uint64_t w, uint64_t t) { return (uint32_t)((w << 32) / t); }
 
-static Mod32 make_mod32(uint64_t t) {
+Mod32 make_mod32(uint64_t t) {
     const uint64_t r32 = ((uint64_t)1 << 32) % t;
     return Mod32{(uint32_t)t, (uint32_t)r32, shoup32_of(r32, t), shoup32_of(1, t)};
 }

@@ -42,6 +42,8 @@ void build_ckks_consts(const HostParams &hp, double scale, CkksConsts &K);
 
 // BGV slot encoding (DESIGN.md §2.13).  A valid plaintext modulus is a prime t < 2^31 with t = 1 (mod 2N).
 bool bgv_plain_modulus_valid(unsigned log_n, uint64_t t);
+// the constants of the 32-bit arithmetic modulo a prime t < 2^31 (modarith.cuh: shoup32, reduce64_32)
+Mod32 make_mod32(uint64_t t);
 // zeta = g^((t-1)/2N), g the least quadratic non-residue mod t (requires a valid t)
 uint64_t bgv_zeta(unsigned log_n, uint64_t t);
 // tab receives [5][N] words: the four twiddle rows of BgvTables::tw, then the slot positions; T the constants of t (its
