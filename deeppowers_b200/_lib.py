@@ -57,6 +57,17 @@ SYMBOLS = {
     "dpfhe_bgv_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p]),
     "dpfhe_bgv_encode_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64]),
     "dpfhe_bgv_decode_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64]),
+    "dpfhe_random_seed": (C.c_int, [C.c_char_p]),
+    "dpfhe_secret_keygen": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p]),
+    "dpfhe_relin_keygen": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint64, C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p]),
+    "dpfhe_galois_keygen": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint64, C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p]),
+    "dpfhe_encrypt": (C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_decrypt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_secret_keygen_host": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p]),
+    "dpfhe_relin_keygen_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint64, C.c_void_p, C.c_char_p, C.c_void_p]),
+    "dpfhe_galois_keygen_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint64, C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_void_p]),
+    "dpfhe_encrypt_host": (C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "dpfhe_decrypt_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint, C.c_void_p, C.c_size_t]),
     "dpfhe_fill_uniform": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_size_t, C.c_void_p]),
     "dpfhe_ntt_fwd_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "dpfhe_ntt_inv_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),

@@ -5,8 +5,10 @@
 // are reported with file:line (as hal::CUDADevice::check_cuda_error does) — but as a status
 // code plus thread-local message, because exceptions cannot cross a C ABI.
 #include <cuda_runtime.h>
+#include <sys/random.h>
 
 #include <algorithm>
+#include <cerrno>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -1219,6 +1221,225 @@ int dpfhe_bgv_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, uint64_t *h_slot
                         });
 }
 #undef CHECK_T
+
+// ---------------------------------------------------------------- key generation, encryption, decryption (DESIGN.md §2.14)
+
+int dpfhe_random_seed(uint8_t seed[32]) {
+    if (!seed) return fail(DPFHE_ERR_INVALID, "null seed");
+    size_t got = 0;
+    while (got < 32) {
+        const ssize_t r = getrandom(seed + got, 32 - got, 0);
+        if (r < 0) {
+            if (errno == EINTR) continue;
+            return fail(DPFHE_ERR_OS, "getrandom failed: %s", strerror(errno));
+        }
+        got += (size_t)r;
+    }
+    return DPFHE_OK;
+}
+
+#define CHECK_SEED(s) \
+    do { if (!(s)) return fail(DPFHE_ERR_INVALID, "null seed"); } while (0)
+
+int dpfhe_secret_keygen(dpfhe_ctx *ctx, const uint8_t seed[32], uint64_t *d_sk, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    CHECK_PTR(d_sk);
+    KeyArgs A = build_key_args(ctx->hp, seed, 0, 1);
+    A.out = d_sk;
+    CU_TRY(VCALL(launch_keys, ctx->lc, KM_SECRET, A, 1, pick(ctx, stream)));
+    note_launch(ctx, 1);
+    return DPFHE_OK;
+}
+
+static int check_key_special(const dpfhe_ctx *ctx, unsigned n_special) { return n_special ? check_special(ctx, n_special) : DPFHE_OK; }
+
+int dpfhe_relin_keygen(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32], uint64_t *d_key,
+                       void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    rc = check_key_special(ctx, n_special);
+    if (rc) return rc;
+    CHECK_PTR(d_sk); CHECK_PTR(d_key);
+    KeyArgs A = build_key_args(ctx->hp, seed, n_special, t_plain);
+    if (overlaps(d_key, (size_t)A.ndig * 2 * ctx->P() * 8, d_sk, ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the secret");
+    A.s = d_sk;
+    A.out = d_key;
+    CU_TRY(VCALL(launch_keys, ctx->lc, KM_RELIN, A, A.ndig, pick(ctx, stream)));
+    note_launch(ctx, 1);
+    return DPFHE_OK;
+}
+
+int dpfhe_galois_keygen(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *d_sk, size_t n_elts, const uint64_t *galois_elts,
+                        const uint8_t seed[32], uint64_t *d_keys, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    rc = check_key_special(ctx, n_special);
+    if (rc) return rc;
+    if (n_elts == 0) return DPFHE_OK;
+    if (!galois_elts) return fail(DPFHE_ERR_INVALID, "null galois_elts");
+    const uint64_t two_n = (uint64_t)2 << ctx->hp.log_n;
+    for (size_t e = 0; e < n_elts; ++e)
+        if (!(galois_elts[e] & 1) || galois_elts[e] >= two_n) return fail(DPFHE_ERR_INVALID, "galois element must be odd and < 2N");
+    CHECK_PTR(d_sk); CHECK_PTR(d_keys);
+    KeyArgs A = build_key_args(ctx->hp, seed, n_special, t_plain);
+    A.s = d_sk;
+    const size_t key_words = (size_t)A.ndig * 2 * ctx->P();
+    if (overlaps(d_keys, n_elts * key_words * 8, d_sk, ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the secret");
+    cudaStream_t st = pick(ctx, stream);
+    uint64_t launches = 0;
+    for (size_t e0 = 0; e0 < n_elts; e0 += KEYS_MAX_ELTS) {
+        const size_t cnt = std::min<size_t>(KEYS_MAX_ELTS, n_elts - e0);
+        for (size_t e = 0; e < cnt; ++e) A.galois[e] = galois_elts[e0 + e];
+        A.out = d_keys + e0 * key_words;
+        CU_TRY(VCALL(launch_keys, ctx->lc, KM_GALOIS, A, cnt * A.ndig, st));
+        ++launches;
+    }
+    note_launch(ctx, launches);
+    return DPFHE_OK;
+}
+
+int dpfhe_encrypt(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32], uint64_t first_index, const uint64_t *d_pt,
+                  uint64_t *d_ct, size_t n, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    if (n == 0) return DPFHE_OK;
+    CHECK_PTR(d_sk); CHECK_PTR(d_pt); CHECK_PTR(d_ct);
+    if (overlaps(d_ct, n * 2 * ctx->P() * 8, d_pt, n * ctx->P() * 8) || overlaps(d_ct, n * 2 * ctx->P() * 8, d_sk, ctx->P() * 8))
+        return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+    KeyArgs A = build_key_args(ctx->hp, seed, 0, t_plain);
+    A.s = d_sk;
+    A.pt = d_pt;
+    A.out = d_ct;
+    A.item0 = first_index;
+    CU_TRY(VCALL(launch_keys, ctx->lc, KM_ENC, A, n, pick(ctx, stream)));
+    note_launch(ctx, 1);
+    return DPFHE_OK;
+}
+
+int dpfhe_decrypt(dpfhe_ctx *ctx, const uint64_t *d_sk, const uint64_t *d_ct, unsigned n_comp, uint64_t *d_pt, size_t n, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (n_comp != 2 && n_comp != 3) return fail(DPFHE_ERR_INVALID, "n_comp must be 2 or 3");
+    if (n == 0) return DPFHE_OK;
+    CHECK_PTR(d_sk); CHECK_PTR(d_ct); CHECK_PTR(d_pt);
+    CU_TRY(VCALL(launch_decrypt, ctx->lc, d_ct, d_sk, d_pt, n_comp, n, pick(ctx, stream)));
+    note_launch(ctx, 1);
+    return DPFHE_OK;
+}
+
+// host forms of the key generators: a device buffer of their own, the call, a copy out (synchronous)
+static int keygen_host(dpfhe_ctx *ctx, const uint64_t *h_sk, size_t out_words, uint64_t *h_out,
+                       int (*call)(dpfhe_ctx *, const uint64_t *, uint64_t *, const void *), const void *arg) {
+    if (!h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const size_t sk_words = h_sk ? ctx->P() : 0;
+    u64 *d = nullptr;
+    CU_TRY(cudaMalloc(&d, (sk_words + out_words) * 8));
+    cudaStream_t st = pick(ctx, nullptr);
+    int rc = DPFHE_OK;
+    if (h_sk && cudaMemcpyAsync(d, h_sk, sk_words * 8, cudaMemcpyHostToDevice, st) != cudaSuccess)
+        rc = fail(DPFHE_ERR_CUDA, "CUDA error at %s:%d: uploading the secret failed", __FILE__, __LINE__);
+    if (!rc) rc = call(ctx, h_sk ? d : nullptr, d + sk_words, arg);
+    if (!rc && cudaMemcpyAsync(h_out, d + sk_words, out_words * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess)
+        rc = fail(DPFHE_ERR_CUDA, "CUDA error at %s:%d: copying the result out failed", __FILE__, __LINE__);
+    const cudaError_t e = cudaStreamSynchronize(st);
+    cudaFree(d);
+    if (!rc && e != cudaSuccess) rc = fail(DPFHE_ERR_CUDA, "CUDA error at %s:%d: %s", __FILE__, __LINE__, cudaGetErrorString(e));
+    return rc;
+}
+
+struct KeygenHostArgs {
+    unsigned n_special;
+    uint64_t t_plain;
+    const uint8_t *seed;
+    size_t n_elts;
+    const uint64_t *galois_elts;
+};
+
+int dpfhe_secret_keygen_host(dpfhe_ctx *ctx, const uint8_t seed[32], uint64_t *h_sk) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    return keygen_host(ctx, nullptr, ctx->P(), h_sk,
+                       [](dpfhe_ctx *c, const uint64_t *, uint64_t *out, const void *a) {
+                           return dpfhe_secret_keygen(c, (const uint8_t *)a, out, nullptr);
+                       }, seed);
+}
+
+int dpfhe_relin_keygen_host(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t *h_key) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    rc = check_key_special(ctx, n_special);
+    if (rc) return rc;
+    if (!h_sk) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const unsigned L = ctx->hp.L, ndig = n_special ? (L - n_special + n_special - 1) / n_special : L;
+    const KeygenHostArgs args{n_special, t_plain, seed, 0, nullptr};
+    return keygen_host(ctx, h_sk, (size_t)ndig * 2 * ctx->P(), h_key,
+                       [](dpfhe_ctx *c, const uint64_t *sk, uint64_t *out, const void *a) {
+                           const KeygenHostArgs &k = *(const KeygenHostArgs *)a;
+                           return dpfhe_relin_keygen(c, k.n_special, k.t_plain, sk, k.seed, out, nullptr);
+                       }, &args);
+}
+
+int dpfhe_galois_keygen_host(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *h_sk, size_t n_elts, const uint64_t *galois_elts,
+                             const uint8_t seed[32], uint64_t *h_keys) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    rc = check_key_special(ctx, n_special);
+    if (rc) return rc;
+    if (n_elts == 0) return DPFHE_OK;
+    if (!h_sk) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const unsigned L = ctx->hp.L, ndig = n_special ? (L - n_special + n_special - 1) / n_special : L;
+    const KeygenHostArgs args{n_special, t_plain, seed, n_elts, galois_elts};
+    return keygen_host(ctx, h_sk, n_elts * ndig * 2 * ctx->P(), h_keys,
+                       [](dpfhe_ctx *c, const uint64_t *sk, uint64_t *out, const void *a) {
+                           const KeygenHostArgs &k = *(const KeygenHostArgs *)a;
+                           return dpfhe_galois_keygen(c, k.n_special, k.t_plain, sk, k.n_elts, k.galois_elts, k.seed, out, nullptr);
+                       }, &args);
+}
+
+int dpfhe_encrypt_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t first_index, const uint64_t *h_pt,
+                       uint64_t *h_ct, size_t n) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    if (n == 0) return DPFHE_OK;
+    if (!h_sk || !h_pt || !h_ct) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const size_t P = ctx->P();
+    rc = upload_key(ctx, h_sk, P);
+    if (rc) return rc;
+    const size_t chunk = pick_chunk(ctx, 2 * P * 8, n);
+    uint64_t next = first_index;   // the chunks run in order: ciphertext k keeps item number first_index + k
+    return run_pipeline(ctx, h_pt, nullptr, h_ct, n, P, 2 * P, chunk,
+                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                            const int r = dpfhe_encrypt(ctx, t_plain, ctx->stage_key, seed, next, din, dout, cnt, st);
+                            next += cnt;
+                            return r;
+                        });
+}
+
+int dpfhe_decrypt_host(dpfhe_ctx *ctx, const uint64_t *h_sk, const uint64_t *h_ct, unsigned n_comp, uint64_t *h_pt, size_t n) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (n_comp != 2 && n_comp != 3) return fail(DPFHE_ERR_INVALID, "n_comp must be 2 or 3");
+    if (n == 0) return DPFHE_OK;
+    if (!h_sk || !h_ct || !h_pt) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const size_t P = ctx->P();
+    rc = upload_key(ctx, h_sk, P);
+    if (rc) return rc;
+    const size_t chunk = pick_chunk(ctx, n_comp * P * 8, n);
+    return run_pipeline(ctx, h_ct, nullptr, h_pt, n, n_comp * P, P, chunk,
+                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                            return dpfhe_decrypt(ctx, ctx->stage_key, din, n_comp, dout, cnt, st);
+                        });
+}
+#undef CHECK_SEED
 
 // waits for everything this context has in flight, whatever stream it was issued on
 int dpfhe_synchronize(dpfhe_ctx *ctx) {

@@ -7,6 +7,29 @@ typedef unsigned __int128 u128;
 
 uint64_t host_mulmod(uint64_t a, uint64_t b, uint64_t q) { return (uint64_t)((u128)a * b % q); }
 
+// seed words, the exact uniform reduction (2^64 mod q and its Shoup companion), the noise factor t (1 for t = 0) and the gadget
+// factor of the digits (P mod q_l, the product of the last K limbs; 1 for per-limb digits)
+KeyArgs build_key_args(const HostParams &hp, const uint8_t seed[32], unsigned K, uint64_t t_plain) {
+    KeyArgs A = {};
+    for (int i = 0; i < 8; ++i)
+        A.seed[i] = (uint32_t)seed[4 * i] | (uint32_t)seed[4 * i + 1] << 8 | (uint32_t)seed[4 * i + 2] << 16 | (uint32_t)seed[4 * i + 3] << 24;
+    const unsigned L = hp.L;
+    A.K = K;
+    A.Lq = L - K;
+    A.ndig = K ? (A.Lq + K - 1) / K : L;
+    for (unsigned l = 0; l < L; ++l) {
+        const uint64_t q = hp.limbs[l].lp.q;
+        const uint64_t r64 = (uint64_t)(((u128)1 << 64) % q);
+        A.r64[l] = r64;
+        A.r64_s[l] = (uint64_t)(((u128)r64 << 64) / q);
+        A.tq[l] = t_plain ? t_plain % q : 1;
+        uint64_t f = 1 % q;
+        for (unsigned k = L - K; k < L; ++k) f = host_mulmod(f, hp.limbs[k].lp.q % q, q);
+        A.fac[l] = f;
+    }
+    return A;
+}
+
 uint64_t host_powmod(uint64_t a, uint64_t e, uint64_t q) {
     uint64_t r = 1 % q, base = a % q;
     for (; e; e >>= 1) {

@@ -52,6 +52,10 @@ bool build_bgv_tables(const HostParams &hp, uint64_t t, std::vector<uint32_t> &t
 // decoding constants: CKKS's Garner inverses and digits of (Q-1)/2, q_i mod t and Q mod t (requires a valid t)
 void build_bgv_consts(const HostParams &hp, uint64_t t, BgvConsts &K);
 
+// key generation and encryption (DESIGN.md §2.14): the constants of one launch of the key / encryption kernels for the 32-byte seed,
+// K special primes (0: per-limb digits) and the noise factor t (t = 0: unscaled); the pointers and item numbers stay unset
+KeyArgs build_key_args(const HostParams &hp, const uint8_t seed[32], unsigned K, uint64_t t_plain);
+
 uint64_t host_mulmod(uint64_t a, uint64_t b, uint64_t q);
 uint64_t host_powmod(uint64_t a, uint64_t e, uint64_t q);
 bool host_is_prime(uint64_t n);

@@ -1,0 +1,156 @@
+// keys.cu — sm_90a kernels and launchers of key generation, encryption and decryption (DESIGN.md §2.14, §4.10).
+//
+// Compiled once per arithmetic variant (-DDPFHE_FAST=0 / 1, namespace dpfhe::gen / dpfhe::fast), like kernels.cu.  A separate
+// compilation unit: no kernel of kernels.cu shares a body with these.
+#include <cuda_runtime.h>
+
+#include <atomic>
+
+#include "keys.cuh"
+#include "launch.hpp"
+
+namespace dpfhe {
+namespace DPFHE_VNS {
+
+template <int NT>
+struct KeyCta {
+    template <class F>
+    __device__ __forceinline__ void par(F f) {
+        f((int)threadIdx.x);
+        __syncthreads();
+    }
+    template <class F>
+    __device__ __forceinline__ void par_dom(F f) {
+        f((int)threadIdx.x);
+        if (NT <= 256) __syncthreads();
+        else asm volatile("bar.sync %0, 256;" ::"r"(1 + ((int)threadIdx.x >> 8)) : "memory");
+    }
+    template <class F>
+    __device__ __forceinline__ void par_warp(F f) {
+        f((int)threadIdx.x);
+        __syncwarp();
+    }
+};
+
+// one CTA per (item, limb): the limb's transform in shared memory, followed by the item's small row (N int8)
+template <int LOGN, int NT, int MINB, int MODE>
+__global__ void __launch_bounds__(NT, MINB) keys_ntt_kernel(const __grid_constant__ KeyArgs A, const Twiddle *__restrict__ tw,
+                                                            const __grid_constant__ LimbTable lt, u32 L) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    constexpr size_t N = (size_t)1 << LOGN;
+    u64 *buf = reinterpret_cast<u64 *>(smem_raw);
+    signed char *small = reinterpret_cast<signed char *>(smem_raw + N * 8);
+    KeyCta<NT> cta;
+    const size_t w = blockIdx.x;
+    const u32 l = (u32)(w % L);
+    keys_limb_body<LOGN, NT, MODE>(cta, buf, small, A, tw + (size_t)l * N, lt.lp[l], l, L, w / L);
+}
+
+// N = 16384: two CTAs per (item, limb), each keeping half of the outer radix-4 step
+template <int NT, int MINB, int MODE>
+__global__ void __launch_bounds__(NT, MINB) keys_ntt_pair_kernel(const __grid_constant__ KeyArgs A, const Twiddle *__restrict__ tw,
+                                                                 const __grid_constant__ LimbTable lt, u32 L) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    constexpr size_t N = (size_t)1 << NTT_PAIR_LOGN;
+    u64 *buf = reinterpret_cast<u64 *>(smem_raw);
+    signed char *small = reinterpret_cast<signed char *>(smem_raw + N * 4);   // after half a limb
+    KeyCta<NT> cta;
+    const size_t w = blockIdx.x / 2;
+    const int h = (int)(blockIdx.x & 1);
+    const u32 l = (u32)(w % L);
+    keys_half_body<NT, MODE>(cta, buf, small, A, tw + (size_t)l * N, lt.lp[l], l, L, w / L, h);
+}
+
+// pt [n][L][N] = c0 + c1 s (+ c2 s^2), ct [n][n_comp][L][N], s [L][N]
+template <int LOGN>
+__global__ void __launch_bounds__(256) decrypt_kernel(const U64x2 *__restrict__ ct, const U64x2 *__restrict__ s, U64x2 *__restrict__ pt,
+                                                      const LimbParams *__restrict__ lps, u32 L, u32 n_comp, size_t n_chunks) {
+    constexpr size_t NC = (size_t)1 << (LOGN - 1);
+    const size_t pc = NC * L;
+    for (size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x; c < n_chunks; c += (size_t)gridDim.x * blockDim.x) {
+        const size_t k = c / pc, in_poly = c % pc;
+        st_stream(pt + c, decrypt_chunk(ct + k * n_comp * pc + in_poly, s + in_poly, pc, n_comp, lps[in_poly / NC]));
+    }
+}
+
+namespace {
+
+struct ConfiguredMask {
+    std::atomic<unsigned long long> bits{0};
+    bool has(int device) const { return (bits.load(std::memory_order_acquire) >> (device & 63)) & 1ull; }
+    void set(int device) { bits.fetch_or(1ull << (device & 63), std::memory_order_release); }
+};
+
+template <class Kern>
+cudaError_t set_smem_once(Kern kern, size_t smem, ConfiguredMask &configured, int device) {
+    if (configured.has(device)) return cudaSuccess;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) configured.set(device);
+    return e;
+}
+
+template <int LOGN, int MODE>
+cudaError_t launch_keys_mode(const LaunchCtx &lc, const KeyArgs &A, size_t n_items, cudaStream_t st) {
+    constexpr size_t N = (size_t)1 << LOGN;
+    const size_t n_limbs = n_items * lc.L;
+    static ConfiguredMask conf;
+    if constexpr (LOGN == NTT_PAIR_LOGN) {
+        auto k = keys_ntt_pair_kernel<256, 2, MODE>;
+        const size_t smem = N * 4 + N;   // half a limb + the small row
+        cudaError_t e = set_smem_once(k, smem, conf, lc.device);
+        if (e != cudaSuccess) return e;
+        k<<<(unsigned)(2 * n_limbs), 256, smem, st>>>(A, lc.tw, lc.lt, lc.L);
+    } else {
+        auto k = keys_ntt_kernel<LOGN, 256, 2, MODE>;   // at 3 CTAs per SM (80 registers) the generic variant's store stage spills
+        const size_t smem = N * 8 + N;
+        cudaError_t e = set_smem_once(k, smem, conf, lc.device);
+        if (e != cudaSuccess) return e;
+        k<<<(unsigned)n_limbs, 256, smem, st>>>(A, lc.tw, lc.lt, lc.L);
+    }
+    return cudaGetLastError();
+}
+
+template <int LOGN>
+cudaError_t launch_keys_n(const LaunchCtx &lc, int mode, const KeyArgs &A, size_t n_items, cudaStream_t st) {
+    switch (mode) {
+        case KM_SECRET: return launch_keys_mode<LOGN, KM_SECRET>(lc, A, n_items, st);
+        case KM_ENC: return launch_keys_mode<LOGN, KM_ENC>(lc, A, n_items, st);
+        case KM_RELIN: return launch_keys_mode<LOGN, KM_RELIN>(lc, A, n_items, st);
+        case KM_GALOIS: return launch_keys_mode<LOGN, KM_GALOIS>(lc, A, n_items, st);
+    }
+    return cudaErrorInvalidValue;
+}
+
+}  // namespace
+
+// n_items: 1 (secret), ciphertexts (encryption), n_elts * ndig (keys); one launch
+cudaError_t launch_keys(const LaunchCtx &lc, int mode, const KeyArgs &A, size_t n_items, cudaStream_t st) {
+    if (n_items == 0) return cudaSuccess;
+    if (n_items * lc.L * 2 > 0x7fffffffull) return cudaErrorInvalidValue;
+    switch (lc.log_n) {
+        case 12: return launch_keys_n<12>(lc, mode, A, n_items, st);
+        case 13: return launch_keys_n<13>(lc, mode, A, n_items, st);
+        case 14: return launch_keys_n<14>(lc, mode, A, n_items, st);
+    }
+    return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_decrypt(const LaunchCtx &lc, const u64 *ct, const u64 *s, u64 *pt, u32 n_comp, size_t n, cudaStream_t st) {
+    const size_t n_chunks = n * lc.L * ((size_t)1 << (lc.log_n - 1));
+    if (!n_chunks) return cudaSuccess;
+    size_t blocks = (n_chunks + 255) / 256;
+    const size_t cap = (size_t)lc.num_sms * 32;   // as the element-wise kernels of kernels.cu
+    if (blocks > cap) blocks = cap;
+    auto C = reinterpret_cast<const U64x2 *>(ct), S = reinterpret_cast<const U64x2 *>(s);
+    auto O = reinterpret_cast<U64x2 *>(pt);
+    switch (lc.log_n) {
+        case 12: decrypt_kernel<12><<<(unsigned)blocks, 256, 0, st>>>(C, S, O, lc.lp, lc.L, n_comp, n_chunks); break;
+        case 13: decrypt_kernel<13><<<(unsigned)blocks, 256, 0, st>>>(C, S, O, lc.lp, lc.L, n_comp, n_chunks); break;
+        case 14: decrypt_kernel<14><<<(unsigned)blocks, 256, 0, st>>>(C, S, O, lc.lp, lc.L, n_comp, n_chunks); break;
+        default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
+}
+
+}  // namespace DPFHE_VNS
+}  // namespace dpfhe

@@ -63,6 +63,15 @@ def _hptr(a, writable=False):
     return C.c_void_p(a.ctypes.data)
 
 
+def _seed(s):
+    """a 32-byte seed (bytes); None passes a null pointer, which the library rejects"""
+    if s is None:
+        return None
+    if not isinstance(s, (bytes, bytearray)) or len(s) != 32:
+        raise ValueError("a seed is 32 bytes")
+    return bytes(s)
+
+
 _CUDA_STREAM_LEGACY = 1   # cudaStreamLegacy: the ABI reserves NULL for "the context's own stream"
 
 
@@ -333,6 +342,53 @@ class Context:
 
     def bgv_decode_host(self, pt, slots, t_plain):
         self._chk(self._l.dpfhe_bgv_decode_host(self._h, _hptr(pt), _ihptr(slots, True), pt.size // self.P, int(t_plain)))
+
+    # key generation, encryption and decryption (DESIGN.md section 2.14), drawn from the ChaCha20 stream of a 32-byte seed (bytes;
+    # random_seed() draws one from the operating system).  secret [L][N]; keys [digits][2][L][N] (n_special = 0: L digits, else
+    # grouped_digits(n_special)), Galois keys [n_elts][digits][2][L][N]; ciphertexts [n][2][L][N] (decrypt: [n][n_comp][L][N]).
+    # Device forms take 8-byte integer CUDA tensors, host forms C-contiguous numpy uint64 arrays.
+    def random_seed(self):
+        buf = C.create_string_buffer(32)
+        self._chk(self._l.dpfhe_random_seed(buf))
+        return buf.raw
+
+    def key_digits(self, n_special):
+        return self.grouped_digits(n_special) if n_special else self.L
+
+    def generate_secret(self, seed, sk, stream=None):
+        self._chk(self._l.dpfhe_secret_keygen(self._h, _seed(seed), _ptr(sk), _stream(stream)))
+
+    def generate_relin_key(self, n_special, t_plain, sk, seed, key, stream=None):
+        self._chk(self._l.dpfhe_relin_keygen(self._h, int(n_special), int(t_plain), _ptr(sk), _seed(seed), _ptr(key), _stream(stream)))
+
+    def generate_galois_keys(self, n_special, t_plain, sk, galois_elts, seed, keys, stream=None):
+        n = len(galois_elts)
+        ge = (C.c_uint64 * max(n, 1))(*[int(g) for g in galois_elts])
+        self._chk(self._l.dpfhe_galois_keygen(self._h, int(n_special), int(t_plain), _ptr(sk), n, ge, _seed(seed), _ptr(keys), _stream(stream)))
+
+    def encrypt(self, t_plain, sk, seed, first_index, pt, ct, n, stream=None):
+        self._chk(self._l.dpfhe_encrypt(self._h, int(t_plain), _ptr(sk), _seed(seed), int(first_index), _ptr(pt), _ptr(ct), n, _stream(stream)))
+
+    def decrypt(self, sk, ct, n_comp, pt, n, stream=None):
+        self._chk(self._l.dpfhe_decrypt(self._h, _ptr(sk), _ptr(ct), int(n_comp), _ptr(pt), n, _stream(stream)))
+
+    def generate_secret_host(self, seed, sk):
+        self._chk(self._l.dpfhe_secret_keygen_host(self._h, _seed(seed), _hptr(sk, True)))
+
+    def generate_relin_key_host(self, n_special, t_plain, sk, seed, key):
+        self._chk(self._l.dpfhe_relin_keygen_host(self._h, int(n_special), int(t_plain), _hptr(sk), _seed(seed), _hptr(key, True)))
+
+    def generate_galois_keys_host(self, n_special, t_plain, sk, galois_elts, seed, keys):
+        n = len(galois_elts)
+        ge = (C.c_uint64 * max(n, 1))(*[int(g) for g in galois_elts])
+        self._chk(self._l.dpfhe_galois_keygen_host(self._h, int(n_special), int(t_plain), _hptr(sk), n, ge, _seed(seed), _hptr(keys, True)))
+
+    def encrypt_host(self, t_plain, sk, seed, first_index, pt, ct):
+        self._chk(self._l.dpfhe_encrypt_host(self._h, int(t_plain), _hptr(sk), _seed(seed), int(first_index), _hptr(pt), _hptr(ct, True),
+                                             pt.size // self.P))
+
+    def decrypt_host(self, sk, ct, n_comp, pt):
+        self._chk(self._l.dpfhe_decrypt_host(self._h, _hptr(sk), _hptr(ct), int(n_comp), _hptr(pt, True), pt.size // self.P))
 
     def fill_uniform(self, seed, data, n_polys, first_poly=0, stream=None):
         self._chk(self._l.dpfhe_fill_uniform(self._h, int(seed), int(first_poly), _ptr(data), n_polys, _stream(stream)))

@@ -13,6 +13,7 @@
 // Header-only over the extern "C" library (include/dpfhe.h, libdpfhe.so); no CUDA headers needed.
 #pragma once
 
+#include <array>
 #include <complex>
 #include <cstddef>
 #include <cstdint>
@@ -97,6 +98,68 @@ public:
     }
     void decode_bgv(const std::uint64_t *plain_eval, std::size_t count, std::uint64_t plain_modulus, std::uint64_t *slots) {
         check(dpfhe_bgv_decode_host(ctx_, plain_eval, slots, count, plain_modulus));
+    }
+
+    // ---- keys, encryption, decryption (DESIGN.md §2.14), drawn from the ChaCha20 stream of a 32-byte seed.  The seed is the
+    //      storage form of the secret.  special = 0: per-limb-digit keys (switch_key_words()), else grouped keys of
+    //      grouped_digits(special) digits; plain_modulus = 0 leaves the noise unscaled (CKKS).  Host forms are synchronous. ----
+    typedef std::array<std::uint8_t, 32> Seed;
+    static Seed random_seed() {
+        Seed s;
+        check(dpfhe_random_seed(s.data()));
+        return s;
+    }
+    std::size_t key_words(unsigned special) const { return (special ? grouped_digits(special) : limbs_) * 2 * poly_words(); }
+    void generate_secret(const Seed &seed, std::uint64_t *secret) { check(dpfhe_secret_keygen_host(ctx_, seed.data(), secret)); }
+    void generate_relin_key(unsigned special, std::uint64_t plain_modulus, const std::uint64_t *secret, const Seed &seed, std::uint64_t *key) {
+        check(dpfhe_relin_keygen_host(ctx_, special, plain_modulus, secret, seed.data(), key));
+    }
+    // keys [steps.size()][key_words(special)] for rotations by steps[i] slots
+    void generate_galois_keys(unsigned special, std::uint64_t plain_modulus, const std::uint64_t *secret, const std::vector<long> &steps,
+                              const Seed &seed, std::uint64_t *keys) {
+        generate_galois_keys_for_elements(special, plain_modulus, secret, galois_elements(steps), seed, keys);
+    }
+    // the same for Galois elements (odd, < 2N), e.g. the conjugation 2N - 1
+    void generate_galois_keys_for_elements(unsigned special, std::uint64_t plain_modulus, const std::uint64_t *secret,
+                                           const std::vector<std::uint64_t> &elements, const Seed &seed, std::uint64_t *keys) {
+        check(dpfhe_galois_keygen_host(ctx_, special, plain_modulus, secret, elements.size(), elements.data(), seed.data(), keys));
+    }
+    void encrypt(std::uint64_t plain_modulus, const std::uint64_t *secret, const Seed &seed, std::uint64_t first_index,
+                 const std::uint64_t *plain_eval, CiphertextBatch out) {
+        check(dpfhe_encrypt_host(ctx_, plain_modulus, secret, seed.data(), first_index, plain_eval, out.data, out.count));
+    }
+    // ct holds ct.count ciphertexts of n_comp (2 or 3: before relinearisation) polynomials each
+    void decrypt(const std::uint64_t *secret, ConstCiphertextBatch ct, std::uint64_t *plain_eval, unsigned n_comp = 2) {
+        check(dpfhe_decrypt_host(ctx_, secret, ct.data, n_comp, plain_eval, ct.count));
+    }
+    void generate_secret_device(const Seed &seed, std::uint64_t *secret, void *stream = nullptr) {
+        check(dpfhe_secret_keygen(ctx_, seed.data(), secret, stream));
+    }
+    void generate_relin_key_device(unsigned special, std::uint64_t plain_modulus, const std::uint64_t *secret, const Seed &seed,
+                                   std::uint64_t *key, void *stream = nullptr) {
+        check(dpfhe_relin_keygen(ctx_, special, plain_modulus, secret, seed.data(), key, stream));
+    }
+    void generate_galois_keys_device(unsigned special, std::uint64_t plain_modulus, const std::uint64_t *secret, const std::vector<long> &steps,
+                                     const Seed &seed, std::uint64_t *keys, void *stream = nullptr) {
+        generate_galois_keys_for_elements_device(special, plain_modulus, secret, galois_elements(steps), seed, keys, stream);
+    }
+    void generate_galois_keys_for_elements_device(unsigned special, std::uint64_t plain_modulus, const std::uint64_t *secret,
+                                                  const std::vector<std::uint64_t> &elements, const Seed &seed, std::uint64_t *keys,
+                                                  void *stream = nullptr) {
+        check(dpfhe_galois_keygen(ctx_, special, plain_modulus, secret, elements.size(), elements.data(), seed.data(), keys, stream));
+    }
+    void encrypt_device(std::uint64_t plain_modulus, const std::uint64_t *secret, const Seed &seed, std::uint64_t first_index,
+                        const std::uint64_t *plain_eval, CiphertextBatch out, void *stream = nullptr) {
+        check(dpfhe_encrypt(ctx_, plain_modulus, secret, seed.data(), first_index, plain_eval, out.data, out.count, stream));
+    }
+    void decrypt_device(const std::uint64_t *secret, ConstCiphertextBatch ct, std::uint64_t *plain_eval, unsigned n_comp = 2,
+                        void *stream = nullptr) {
+        check(dpfhe_decrypt(ctx_, secret, ct.data, n_comp, plain_eval, ct.count, stream));
+    }
+    std::vector<std::uint64_t> galois_elements(const std::vector<long> &steps) const {
+        std::vector<std::uint64_t> elts;
+        for (long k : steps) elts.push_back(galois_element(k));
+        return elts;
     }
 
     // ---- host-buffer calls: synchronous; H2D / compute / D2H are pipelined inside the library ----
@@ -246,6 +309,30 @@ private:
     }
     dpfhe_ctx *ctx_ = nullptr;
     unsigned log_n_, limbs_;
+};
+
+// Encrypts under one secret with one seed, numbering the ciphertexts itself: every call continues where the previous one stopped,
+// so no (seed, index) pair repeats within one Encryptor.  The secret is in host memory (Memory::host: encrypt takes host buffers) or
+// in device memory (Memory::device: encrypt takes device buffers, asynchronous on `stream`).
+class Encryptor {
+public:
+    enum class Memory { host, device };
+    Encryptor(Evaluator &ev, Memory where, const std::uint64_t *secret, const Evaluator::Seed &seed, std::uint64_t plain_modulus,
+              std::uint64_t first_index = 0)
+        : ev_(ev), where_(where), secret_(secret), seed_(seed), t_(plain_modulus), next_(first_index) {}
+    void encrypt(const std::uint64_t *plain_eval, CiphertextBatch out, void *stream = nullptr) {
+        if (where_ == Memory::host) ev_.encrypt(t_, secret_, seed_, next_, plain_eval, out);
+        else ev_.encrypt_device(t_, secret_, seed_, next_, plain_eval, out, stream);
+        next_ += out.count;
+    }
+    std::uint64_t next_index() const { return next_; }
+
+private:
+    Evaluator &ev_;
+    Memory where_;
+    const std::uint64_t *secret_;
+    Evaluator::Seed seed_;
+    std::uint64_t t_, next_;
 };
 
 // An encrypted linear layer y = W x (baby-step/giant-step diagonals) whose weights and Galois keys live on the device.

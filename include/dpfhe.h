@@ -64,7 +64,8 @@ enum {
     DPFHE_OK = 0,
     DPFHE_ERR_INVALID = -1,    /* bad argument / unsupported parameter set */
     DPFHE_ERR_CUDA = -2,       /* CUDA runtime error (message has file:line) */
-    DPFHE_ERR_NOMEM = -3
+    DPFHE_ERR_NOMEM = -3,
+    DPFHE_ERR_OS = -4          /* the operating system failed a request (dpfhe_random_seed: getrandom) */
 };
 
 /* thread-local message of the last failing call on this thread */
@@ -258,6 +259,42 @@ int dpfhe_bgv_encode(dpfhe_ctx *ctx, const int64_t *d_slots, uint64_t *d_pt, siz
 int dpfhe_bgv_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, uint64_t *d_slots, size_t n_vec, uint64_t t_plain, void *stream);
 int dpfhe_bgv_encode_host(dpfhe_ctx *ctx, const int64_t *h_slots, uint64_t *h_pt, size_t n_vec, uint64_t t_plain);
 int dpfhe_bgv_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, uint64_t *h_slots, size_t n_vec, uint64_t t_plain);
+
+/* ---- key generation, encryption and decryption (DESIGN.md §2.14).  Every random value is drawn from a ChaCha20 stream keyed by a
+ *      caller-supplied 32-byte seed, one stream per sampled row (its nonce names the row), so the results are reproducible from the
+ *      seed.  The seed is the storage form of the secret: keep it as secret as the key.  Encrypting two plaintexts with the same
+ *      (seed, index) leaks their difference.  No constant-time or side-channel claim is made.  All results are canonical, in
+ *      evaluation form.  t_plain >= 2 scales the noise by t (BGV), t_plain = 0 leaves it unscaled (CKKS).
+ *      secret_keygen: d_sk [L][N] over all of the context's limbs, special primes included; its first l rows are the secret of
+ *        the context over the first l moduli.
+ *      relin_keygen / galois_keygen: switch keys for s o s / sigma_g(s) under d_sk.  n_special = 0: per-limb digits [L][2][L][N]
+ *        (dpfhe_ct_mul_relin, dpfhe_rotate); n_special = K in 1 .. 4 with 2K <= L: the grouped key [dnum][2][L][N] of the
+ *        *_grouped calls (K = 1: the *_hybrid calls).  galois_keygen writes n_elts keys back to back; every element odd, < 2N.
+ *      encrypt: d_pt [n][L][N] plaintexts (as dpfhe_bgv_encode / dpfhe_ckks_encode produce them) -> d_ct [n][2][L][N]; ciphertext
+ *        k is drawn with index first_index + k.  Under a context with special primes, encrypt and decrypt with the context over
+ *        the ciphertext moduli and the first rows of the secret.
+ *      decrypt: d_ct [n][n_comp][L][N], n_comp 2 or 3 -> d_pt [n][L][N] = c0 + c1 o s (+ c2 o s^2), ready for the decoders.
+ *      The *_host forms take host buffers (encrypt / decrypt pipelined in chunks; synchronous).
+ *      dpfhe_random_seed fills 32 bytes from the operating system (getrandom; DPFHE_ERR_OS if that fails).
+ *      Outputs must not overlap the secret, the plaintexts or each other's inputs. ---- */
+int dpfhe_random_seed(uint8_t seed[32]);
+int dpfhe_secret_keygen(dpfhe_ctx *ctx, const uint8_t seed[32], uint64_t *d_sk, void *stream);
+int dpfhe_relin_keygen(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32],
+                       uint64_t *d_key, void *stream);
+int dpfhe_galois_keygen(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *d_sk, size_t n_elts,
+                        const uint64_t *galois_elts, const uint8_t seed[32], uint64_t *d_keys, void *stream);
+int dpfhe_encrypt(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32], uint64_t first_index,
+                  const uint64_t *d_pt, uint64_t *d_ct, size_t n, void *stream);
+int dpfhe_decrypt(dpfhe_ctx *ctx, const uint64_t *d_sk, const uint64_t *d_ct, unsigned n_comp, uint64_t *d_pt, size_t n,
+                  void *stream);
+int dpfhe_secret_keygen_host(dpfhe_ctx *ctx, const uint8_t seed[32], uint64_t *h_sk);
+int dpfhe_relin_keygen_host(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32],
+                            uint64_t *h_key);
+int dpfhe_galois_keygen_host(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *h_sk, size_t n_elts,
+                             const uint64_t *galois_elts, const uint8_t seed[32], uint64_t *h_keys);
+int dpfhe_encrypt_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t first_index,
+                       const uint64_t *h_pt, uint64_t *h_ct, size_t n);
+int dpfhe_decrypt_host(dpfhe_ctx *ctx, const uint64_t *h_sk, const uint64_t *h_ct, unsigned n_comp, uint64_t *h_pt, size_t n);
 
 /* ---- synthetic data (DESIGN.md §5): x[k] = mulhi64(splitmix64(seed + k), q_limb),
  *      k = (first_poly + p)*L*N + l*N + n.  Fills [n_polys][L][N]. ---- */
