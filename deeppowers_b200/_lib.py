@@ -103,6 +103,14 @@ SYMBOLS = {
     "dpfhe_linear_destroy": (None, [C.c_void_p]),
     "dpfhe_linear_apply": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "dpfhe_linear_apply_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "dpfhe_ct_lincomb": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_ct_add_plain": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_ct_add_plain_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "dpfhe_polyeval_create_grouped": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint64, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "dpfhe_polyeval_result_limbs": (C.c_uint, [C.c_void_p]),
+    "dpfhe_polyeval_apply": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_polyeval_apply_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "dpfhe_polyeval_destroy": (None, [C.c_void_p]),
     "dpfhe_host_alloc": (C.c_int, [C.POINTER(C.c_void_p), C.c_size_t]),
     "dpfhe_host_free": (C.c_int, [C.c_void_p]),
     "dpfhe_launch_count": (C.c_uint64, [C.c_void_p]),

@@ -13,12 +13,14 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <new>
 #include <string>
 #include <vector>
 
 #include "../../include/dpfhe.h"
 #include "ctx.hpp"
+#include "eval.cuh"
 
 using namespace dpfhe;
 
@@ -373,6 +375,7 @@ size_t dpfhe_context_device_bytes(const dpfhe_ctx *ctx) {
     n += ctx->hoistg_bytes;                                                          //   grouped hybrid keys: lifted digits + accumulators
     n += ctx->ckks_tab_bytes + ctx->bgv_tab_bytes + ctx->enc_work_bytes;             // CKKS and BGV encoding tables, their scratch
     if (ctx->lc.ks_prof) n += ctx->lc.ks_slots * 16 * sizeof(unsigned long long);
+    n += ctx->object_bytes;                                                          // polynomial evaluators: level tables, keys, scratch
     return n;
 }
 
@@ -1827,6 +1830,465 @@ int dpfhe_linear_apply_host(dpfhe_linear *lin, const uint64_t *h_ct, uint64_t *h
     const size_t ct_words = 2 * lin->Lq * ctx->N();
     return run_pipeline(ctx, h_ct, nullptr, h_out, batch, ct_words, ct_words, chunk,
                         [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int { return linear_apply_on(lin, din, dout, cnt, st); });
+}
+
+// ---------------------------------------------------------------- scalar linear combinations, BGV polynomial evaluation (DESIGN.md §2.15)
+int dpfhe_ct_lincomb(dpfhe_ctx *ctx, size_t n_terms, const uint64_t *const *d_cts, const int64_t *coeffs, int64_t constant, uint64_t *d_out,
+                     size_t batch, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (n_terms < 1 || n_terms > (size_t)LINCOMB_MAX_TERMS) return fail(DPFHE_ERR_INVALID, "n_terms must be in [1, %d]", LINCOMB_MAX_TERMS);
+    if (!d_cts || !coeffs) return fail(DPFHE_ERR_INVALID, "null argument");
+    for (size_t i = 0; i < n_terms; ++i)
+        if (!d_cts[i] || !aligned16(d_cts[i])) return fail(DPFHE_ERR_INVALID, "null or misaligned input ciphertext %zu", i);
+    CHECK_PTR(d_out);
+    if (batch == 0) return DPFHE_OK;
+    // the output may BE an input (a thread reads chunk c of every input, then writes chunk c), but not overlap one at another offset
+    const size_t ct_bytes = batch * 2 * ctx->P() * 8;
+    for (size_t i = 0; i < n_terms; ++i)
+        if (d_out != d_cts[i] && overlaps(d_out, ct_bytes, d_cts[i], ct_bytes))
+            return fail(DPFHE_ERR_INVALID, "output must be an input or not overlap it (input %zu)", i);
+    CU_TRY(VCALL(launch_lincomb, ctx->lc, d_cts, coeffs, (u32)n_terms, constant, nullptr, d_out, batch, pick(ctx, stream)));
+    note_launch(ctx, 1);
+    return DPFHE_OK;
+}
+
+// the linear-combination body with one term of coefficient 1 and the plaintext as the c0 addend
+int dpfhe_ct_add_plain(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_PTR(d_ct); CHECK_PTR(d_pt); CHECK_PTR(d_out);
+    if (batch == 0) return DPFHE_OK;
+    if (overlaps(d_out, batch * 2 * ctx->P() * 8, d_pt, ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the plaintext");
+    const int64_t one = 1;
+    CU_TRY(VCALL(launch_lincomb, ctx->lc, &d_ct, &one, 1u, (int64_t)0, d_pt, d_out, batch, pick(ctx, stream)));
+    note_launch(ctx, 1);
+    return DPFHE_OK;
+}
+
+// host buffers: the plaintext uploaded once, the batch pipelined in chunks (as dpfhe_ct_mul_plain_host)
+int dpfhe_ct_add_plain_host(dpfhe_ctx *ctx, const uint64_t *h_ct, const uint64_t *h_pt, uint64_t *h_out, size_t batch) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (batch == 0) return DPFHE_OK;
+    if (!h_ct || !h_pt || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const size_t P = ctx->P();
+    rc = upload_key(ctx, h_pt, P);
+    if (rc) return rc;
+    const size_t chunk = pick_chunk(ctx, 2 * P * 8, batch);
+    const int64_t one = 1;
+    return run_pipeline(ctx, h_ct, nullptr, h_out, batch, 2 * P, 2 * P, chunk,
+                        [&](u64 *dc, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                            const u64 *in = dc;
+                            CU_TRY(VCALL(launch_lincomb, ctx->lc, &in, &one, 1u, (int64_t)0, ctx->stage_key, dout, cnt, st));
+                            note_launch(ctx, 1);
+                            return DPFHE_OK;
+                        });
+}
+
+namespace {
+
+// x^-1 mod m for gcd(x, m) = 1 (m < 2^31)
+uint64_t inv_mod(uint64_t x, uint64_t m) {
+    int64_t a = (int64_t)(x % m), b = (int64_t)m, u = 1, v = 0;
+    while (b) {
+        const int64_t q = a / b;
+        a -= q * b; std::swap(a, b);
+        u -= q * v; std::swap(u, v);
+    }
+    return (uint64_t)((u % (int64_t)m + (int64_t)m) % (int64_t)m);
+}
+int64_t centred(uint64_t x, uint64_t t) { return x <= t / 2 ? (int64_t)x : (int64_t)x - (int64_t)t; }
+unsigned ceil_log2(size_t k) {
+    unsigned j = 0;
+    while (((size_t)1 << j) < k) ++j;
+    return j;
+}
+
+// key switching at level l: the basis {q_0 .. q_{l-1}, p_0 .. p_{K-1}}, its device tables (the context's own at the top level), the
+// level's key restricted from the top-level key and its Shoup companions
+struct PeLevel {
+    unsigned l = 0;
+    HostParams hp;
+    LimbParams *d_lp = nullptr;
+    Twiddle *d_tw = nullptr, *d_itw = nullptr;
+    LimbTable lt;
+    bool lift_reduce = true;
+    MsConsts K;
+    GroupConsts G;
+    u64 *key = nullptr, *key_s = nullptr;
+};
+
+// one step of an application.  Buffers: >= 0 an entry of bufs, IN the input, OUT the output
+enum PeOpKind { PE_MUL = 0, PE_SWITCH = 1, PE_LINCOMB = 2 };
+constexpr int PE_IN = -1, PE_OUT = -2;
+struct PeOp {
+    int kind;
+    unsigned level;           // PE_MUL: level of the product; PE_SWITCH: level of the input (drops q_{level-1}); PE_LINCOMB: its level
+    int a, b, out;
+    std::vector<int> terms;   // PE_LINCOMB
+    std::vector<int64_t> coeffs;
+    int64_t constant = 0;
+};
+
+}  // namespace
+
+struct dpfhe_polyeval {
+    dpfhe_ctx *ctx = nullptr;
+    unsigned K = 0, Lq = 0, Lf = 0;
+    uint64_t t = 0;
+    std::vector<PeLevel> lev;            // by level: lev[l - lev_lo]
+    unsigned lev_lo = 0;
+    std::vector<MsConsts> ms;            // BGV modulus switch dropping q_{l-1}: ms[l]
+    std::vector<PeOp> ops;
+    std::vector<unsigned> bufs;          // level of every scratch buffer
+    size_t fixed_bytes = 0;              // level tables and keys
+    u64 *scratch = nullptr;              // the buffers back to back, then the switch's tau rows [2 cap][N]
+    size_t cap = 0, scratch_bytes = 0;
+};
+
+namespace {
+
+size_t pe_scratch_words(const dpfhe_polyeval *pe, size_t batch) {
+    size_t w = 0;
+    for (unsigned l : pe->bufs) w += batch * 2 * l * pe->ctx->N();
+    return w + (pe->bufs.empty() ? 0 : 2 * batch * pe->ctx->N());
+}
+
+void pe_free(dpfhe_polyeval *pe) {
+    for (auto &v : pe->lev) {
+        if (v.l != pe->Lq) {
+            cudaFree(v.d_lp);
+            cudaFree(v.d_tw);
+            cudaFree(v.d_itw);
+        }
+        cudaFree(v.key);
+        cudaFree(v.key_s);
+    }
+    cudaFree(pe->scratch);
+    if (pe->ctx) pe->ctx->object_bytes -= pe->fixed_bytes + pe->scratch_bytes;
+    delete pe;
+}
+
+int pe_reserve(dpfhe_polyeval *pe, size_t batch) {
+    if (batch <= pe->cap || pe->bufs.empty()) return DPFHE_OK;
+    dpfhe_ctx *ctx = pe->ctx;
+    int rc = dpfhe_synchronize(ctx);
+    if (rc) return rc;
+    cudaFree(pe->scratch);
+    pe->scratch = nullptr;
+    ctx->object_bytes -= pe->scratch_bytes;
+    pe->scratch_bytes = 0;
+    pe->cap = 0;
+    const size_t bytes = pe_scratch_words(pe, batch) * 8;
+    CU_TRY(cudaMalloc(&pe->scratch, bytes));
+    pe->scratch_bytes = bytes;
+    ctx->object_bytes += bytes;
+    pe->cap = batch;
+    return DPFHE_OK;
+}
+
+// the schedule of DESIGN.md §2.15: powers in increasing order, each operand brought to the product's level by single-limb switches
+// (each copy made once, from the copy one level above), the combination one level above the last switch
+int pe_plan(dpfhe_polyeval *pe, const int64_t *coeffs, size_t d) {
+    const unsigned Lq = pe->Lq, D = ceil_log2(d);
+    const uint64_t t = pe->t;
+    std::vector<uint64_t> a(d + 1), qinv(Lq);
+    for (size_t k = 0; k <= d; ++k) a[k] = floor_mod(coeffs[k], t);
+    for (unsigned i = 0; i < Lq; ++i) qinv[i] = inv_mod(pe->ctx->hp.limbs[i].lp.q % t, t);
+    if (D == 0) {
+        PeOp op{PE_LINCOMB, Lq, 0, 0, PE_OUT};
+        op.terms = {PE_IN};
+        op.coeffs = {centred(a[1], t)};
+        op.constant = centred(a[0], t);
+        pe->ops.push_back(op);
+        return DPFHE_OK;
+    }
+    const unsigned Lf = Lq - D;
+    // powers needed: every k with a_k != 0 and, recursively, the operands of their products (x alone if every a_k, k >= 1, is 0)
+    std::vector<char> need(d + 1, 0);
+    bool any = false;
+    for (size_t k = 1; k <= d; ++k) any |= (need[k] = a[k] != 0);
+    if (!any) need[1] = 1;
+    auto split = [](size_t k, size_t &u, size_t &v) {
+        size_t p = 1;
+        while (2 * p < k) p *= 2;
+        u = p;
+        v = k - p;   // = p when k is a power of two
+    };
+    for (size_t k = d; k >= 2; --k)
+        if (need[k]) {
+            size_t u, v;
+            split(k, u, v);
+            need[u] = need[v] = 1;
+        }
+    // copies of the powers by level, with their factors
+    std::vector<std::vector<int>> at(d + 1, std::vector<int>(Lq + 1, -3));
+    std::vector<std::vector<uint64_t>> fac(d + 1, std::vector<uint64_t>(Lq + 1, 0));
+    std::vector<int> ybuf(d + 1, -3);
+    std::vector<uint64_t> yfac(d + 1, 0);
+    at[1][Lq] = PE_IN;
+    fac[1][Lq] = 1;
+    auto new_buf = [&](unsigned l) {
+        pe->bufs.push_back(l);
+        return (int)pe->bufs.size() - 1;
+    };
+    int tmp = -3;   // the product of a power that is switched right away: one buffer at the top level, reused
+    std::function<void(size_t, unsigned)> get = [&](size_t k, unsigned l) {
+        if (at[k][l] != -3) return;
+        get(k, l + 1);
+        const int b = new_buf(l);
+        pe->ops.push_back(PeOp{PE_SWITCH, l + 1, at[k][l + 1], 0, b});
+        at[k][l] = b;
+        fac[k][l] = fac[k][l + 1] * qinv[l] % t;
+    };
+    for (size_t k = 2; k <= d; ++k) {
+        if (!need[k]) continue;
+        size_t u, v;
+        split(k, u, v);
+        const unsigned ck = ceil_log2(k), l = Lq - ck + 1;
+        get(u, l);
+        get(v, l);
+        const uint64_t f = fac[u][l] * fac[v][l] % t;
+        if (ck == D) {
+            ybuf[k] = new_buf(l);
+            yfac[k] = f;
+            pe->ops.push_back(PeOp{PE_MUL, l, at[u][l], at[v][l], ybuf[k]});
+        } else {
+            if (tmp == -3) tmp = new_buf(Lq);
+            pe->ops.push_back(PeOp{PE_MUL, l, at[u][l], at[v][l], tmp});
+            const int b = new_buf(l - 1);
+            pe->ops.push_back(PeOp{PE_SWITCH, l, tmp, 0, b});
+            at[k][l - 1] = b;
+            fac[k][l - 1] = f * qinv[l - 1] % t;
+        }
+    }
+    const uint64_t G = pe->ctx->hp.limbs[Lf].lp.q % t;
+    if (tmp == -3) tmp = new_buf(Lf + 1);
+    PeOp lc{PE_LINCOMB, Lf + 1, 0, 0, tmp};
+    for (size_t k = 1; k <= d; ++k) {
+        if (any ? a[k] == 0 : k != 1) continue;
+        uint64_t g;
+        if (ceil_log2(k) == D) {   // the pre-switch product, at Lf + 1 already
+            lc.terms.push_back(ybuf[k]);
+            g = yfac[k];
+        } else {
+            get(k, Lf + 1);
+            lc.terms.push_back(at[k][Lf + 1]);
+            g = fac[k][Lf + 1];
+        }
+        lc.coeffs.push_back(centred(a[k] * inv_mod(g, t) % t * G % t, t));
+    }
+    lc.constant = centred(a[0] * G % t, t);
+    pe->ops.push_back(lc);
+    pe->ops.push_back(PeOp{PE_SWITCH, Lf + 1, tmp, 0, PE_OUT});
+    return DPFHE_OK;
+}
+
+// the launch state of key switching at level l: the context's, with the level's limb tables (DESIGN.md §4.11)
+LaunchCtx pe_view(const dpfhe_polyeval *pe, const PeLevel &v) {
+    LaunchCtx lc = pe->ctx->lc;
+    lc.L = v.l + pe->K;
+    lc.lp = v.d_lp;
+    lc.lt = v.lt;
+    lc.tw = v.d_tw;
+    lc.itw = v.d_itw;
+    lc.lift_reduce = v.lift_reduce;
+    return lc;
+}
+
+// builds level l's tables, key and companions (st: the context's stream)
+int pe_level(dpfhe_polyeval *pe, PeLevel &v, unsigned l, const uint64_t *h_key, cudaStream_t st) {
+    dpfhe_ctx *ctx = pe->ctx;
+    const unsigned K = pe->K, Lq = pe->Lq, L = ctx->hp.L, Ll = l + K;
+    const size_t N = ctx->N(), dl = (l + K - 1) / K;
+    v.l = l;
+    std::vector<uint64_t> mod(Ll);
+    for (unsigned i = 0; i < l; ++i) mod[i] = ctx->hp.limbs[i].lp.q;
+    for (unsigned k = 0; k < K; ++k) mod[l + k] = ctx->hp.limbs[Lq + k].lp.q;
+    std::string msg = build_host_params(ctx->hp.log_n, Ll, mod.data(), v.hp);
+    if (!msg.empty()) return fail(DPFHE_ERR_INVALID, "%s", msg.c_str());
+    build_group_consts(v.hp, K, pe->t, v.G, v.K);
+    memset(&v.lt, 0, sizeof(v.lt));
+    uint64_t qmin = ~0ull, qmax = 0;
+    for (unsigned i = 0; i < Ll; ++i) {
+        v.lt.lp[i] = v.hp.limbs[i].lp;
+        qmin = std::min(qmin, mod[i]);
+        qmax = std::max(qmax, mod[i]);
+    }
+    v.lift_reduce = !(qmax < 2 * qmin) || getenv("DPFHE_LIFT_REDUCE") != nullptr;   // as dpfhe_context_create
+    if (l == Lq) {
+        v.d_lp = ctx->d_lp;
+        v.d_tw = ctx->d_tw;
+        v.d_itw = ctx->d_itw;
+    } else {
+        CU_TRY(cudaMalloc(&v.d_lp, Ll * sizeof(LimbParams)));
+        CU_TRY(cudaMalloc(&v.d_tw, Ll * N * sizeof(Twiddle)));
+        CU_TRY(cudaMalloc(&v.d_itw, Ll * N * sizeof(Twiddle)));
+        pe->fixed_bytes += Ll * sizeof(LimbParams) + 2 * Ll * N * sizeof(Twiddle);
+        for (unsigned i = 0; i < Ll; ++i) {
+            CU_TRY(cudaMemcpy(v.d_tw + i * N, v.hp.limbs[i].tw.data(), N * sizeof(Twiddle), cudaMemcpyHostToDevice));
+            CU_TRY(cudaMemcpy(v.d_itw + i * N, v.hp.limbs[i].itw.data(), N * sizeof(Twiddle), cudaMemcpyHostToDevice));
+        }
+        CU_TRY(cudaMemcpy(v.d_lp, v.lt.lp, Ll * sizeof(LimbParams), cudaMemcpyHostToDevice));
+    }
+    // the key of level l: digits g < ceil(l / K), limb rows 0 .. l-1 and the special rows Lq .. Lq+K-1 of the top-level key
+    const size_t key_words = dl * 2 * Ll * N;
+    CU_TRY(cudaMalloc(&v.key, key_words * 8));
+    CU_TRY(cudaMalloc(&v.key_s, key_words * 8));
+    pe->fixed_bytes += 2 * key_words * 8;
+    for (size_t g = 0; g < dl; ++g)
+        for (size_t c = 0; c < 2; ++c) {
+            const uint64_t *src = h_key + (g * 2 + c) * L * N;
+            u64 *dst = v.key + (g * 2 + c) * Ll * N;
+            CU_TRY(cudaMemcpy(dst, src, l * N * 8, cudaMemcpyHostToDevice));
+            CU_TRY(cudaMemcpy(dst + l * N, src + Lq * N, K * N * 8, cudaMemcpyHostToDevice));
+        }
+    const LaunchCtx lc = pe_view(pe, v);
+    CU_TRY(VCALL(launch_key_prepare_grouped, lc, v.key, v.key_s, (u32)dl, st));
+    note_launch(ctx, 1);
+    return DPFHE_OK;
+}
+
+int pe_apply_on(dpfhe_polyeval *pe, const u64 *d_ct, u64 *d_out, size_t batch, void *stream) {
+    dpfhe_ctx *ctx = pe->ctx;
+    const size_t N = ctx->N();
+    std::vector<u64 *> ptr(pe->bufs.size());
+    u64 *p = pe->scratch;
+    for (size_t i = 0; i < pe->bufs.size(); ++i) {
+        ptr[i] = p;
+        p += batch * 2 * pe->bufs[i] * N;
+    }
+    u64 *tau = p;
+    auto buf = [&](int b) -> u64 * { return b == PE_IN ? const_cast<u64 *>(d_ct) : b == PE_OUT ? d_out : ptr[b]; };
+    cudaStream_t st = pick(ctx, stream);
+    for (const PeOp &op : pe->ops) {
+        if (op.kind == PE_MUL) {
+            const PeLevel &v = pe->lev[op.level - pe->lev_lo];
+            LaunchCtx lc = pe_view(pe, v);
+            lc.ks_epoch = ctx->lc.ks_epoch;
+            const cudaError_t e = VCALL(launch_ks_grouped, lc, KS_MUL_RELIN, buf(op.a), buf(op.b), v.key, buf(op.out), batch, 0u, v.K, v.G, st, nullptr,
+                                        v.key_s);
+            // the round numbering is the context's: the next key switch on any view must continue from here
+            ctx->lc.ks_epoch = lc.ks_epoch;
+            ctx->lc.ks_epoch_restarts = lc.ks_epoch_restarts;
+            CU_TRY(e);
+            note_launch(ctx, 1);
+        } else if (op.kind == PE_SWITCH) {
+            LaunchCtx lc = ctx->lc;   // the ciphertext moduli q_0 .. q_{l-1} are the first l limbs of the context
+            lc.L = op.level;
+            CU_TRY(VCALL(launch_mod_switch, lc, buf(op.a), tau, buf(op.out), pe->ms[op.level], 2 * batch, st));
+            note_launch(ctx, 2);
+        } else {
+            LaunchCtx lc = ctx->lc;
+            lc.L = op.level;
+            std::vector<const u64 *> in;
+            for (int b : op.terms) in.push_back(buf(b));
+            CU_TRY(VCALL(launch_lincomb, lc, in.data(), op.coeffs.data(), (u32)in.size(), op.constant, nullptr, buf(op.out), batch, st));
+            note_launch(ctx, 1);
+        }
+    }
+    return DPFHE_OK;
+}
+
+}  // namespace
+
+int dpfhe_polyeval_create_grouped(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const int64_t *coeffs, size_t degree,
+                                  const uint64_t *h_relin_key, dpfhe_polyeval **out) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!out || !coeffs || !h_relin_key) return fail(DPFHE_ERR_INVALID, "null argument");
+    *out = nullptr;
+    rc = check_special(ctx, n_special);
+    if (rc) return rc;
+    if (t_plain < 2 || t_plain >= ((uint64_t)1 << 31)) return fail(DPFHE_ERR_INVALID, "the plaintext modulus must be in [2, 2^31)");
+    if (degree < 1 || degree > 64) return fail(DPFHE_ERR_INVALID, "the degree must be in [1, 64]");
+    const unsigned L = ctx->hp.L, K = n_special, Lq = L - K, D = ceil_log2(degree);
+    if (D > Lq - 1 || D > Lq - K + 1)
+        return fail(DPFHE_ERR_INVALID, "degree %zu needs %u levels: at most min(Lq - 1, Lq - K + 1) = %u with Lq = %u, K = %u", degree, D,
+                    std::min(Lq - 1, Lq - K + 1), Lq, K);
+    dpfhe_polyeval *pe = new (std::nothrow) dpfhe_polyeval();
+    if (!pe) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    pe->ctx = ctx; pe->K = K; pe->Lq = Lq; pe->Lf = Lq - D; pe->t = t_plain;
+    rc = pe_plan(pe, coeffs, degree);
+    // the levels of the products, and the BGV switch constants of every level a switch starts from
+    unsigned lo = Lq + 1;
+    for (const PeOp &op : pe->ops)
+        if (op.kind == PE_MUL) lo = std::min(lo, op.level);
+    pe->ms.resize(Lq + 1);
+    for (unsigned l = pe->Lf + 1; l <= Lq && rc == DPFHE_OK && D > 0; ++l) {
+        HostParams hp;
+        std::vector<uint64_t> mod(l);
+        for (unsigned i = 0; i < l; ++i) mod[i] = ctx->hp.limbs[i].lp.q;
+        std::string msg = build_host_params(ctx->hp.log_n, l, mod.data(), hp);
+        if (!msg.empty()) rc = fail(DPFHE_ERR_INVALID, "%s", msg.c_str());
+        else build_ms_consts(hp, t_plain, pe->ms[l]);
+    }
+    if (rc == DPFHE_OK && lo <= Lq) rc = ensure_hyb(ctx);
+    cudaStream_t st = pick(ctx, nullptr);
+    if (rc == DPFHE_OK && lo <= Lq) {
+        pe->lev_lo = lo;
+        pe->lev.resize(Lq - lo + 1);
+        for (unsigned l = lo; l <= Lq && rc == DPFHE_OK; ++l) rc = pe_level(pe, pe->lev[l - lo], l, h_relin_key, st);
+    }
+    ctx->object_bytes += pe->fixed_bytes;
+    if (rc == DPFHE_OK) {
+        const cudaError_t e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) rc = fail(DPFHE_ERR_CUDA, "polynomial evaluator keys: %s", cudaGetErrorString(e));
+    }
+    if (rc != DPFHE_OK) {
+        pe_free(pe);
+        return rc;
+    }
+    *out = pe;
+    return DPFHE_OK;
+}
+
+unsigned dpfhe_polyeval_result_limbs(const dpfhe_polyeval *pe) { return pe ? pe->Lf : 0; }
+
+void dpfhe_polyeval_destroy(dpfhe_polyeval *pe) {
+    if (!pe) return;
+    if (pe->ctx) {
+        cudaSetDevice(pe->ctx->lc.device);
+        dpfhe_synchronize(pe->ctx);
+    }
+    pe_free(pe);
+}
+
+// launches per application: one per product, two per modulus switch, one for the combination (DESIGN.md §2.15)
+int dpfhe_polyeval_apply(dpfhe_polyeval *pe, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
+    if (!pe) return fail(DPFHE_ERR_INVALID, "null evaluator");
+    int rc = enter(pe->ctx);
+    if (rc) return rc;
+    CHECK_PTR(d_ct); CHECK_PTR(d_out);
+    if (batch == 0) return DPFHE_OK;
+    const size_t N = pe->ctx->N();
+    if (overlaps(d_out, batch * 2 * pe->Lf * N * 8, d_ct, batch * 2 * pe->Lq * N * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    rc = pe_reserve(pe, batch);
+    if (rc) return rc;
+    return pe_apply_on(pe, d_ct, d_out, batch, stream);
+}
+
+int dpfhe_polyeval_apply_host(dpfhe_polyeval *pe, const uint64_t *h_ct, uint64_t *h_out, size_t batch) {
+    if (!pe) return fail(DPFHE_ERR_INVALID, "null evaluator");
+    dpfhe_ctx *ctx = pe->ctx;
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (batch == 0) return DPFHE_OK;
+    if (!h_ct || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    // chunks of about a fifth of the batch in whole rounds of the persistent key-switch grid, as dpfhe_linear_apply_host
+    const size_t groups = std::max<size_t>(1, (size_t)ctx->lc.num_sms * 3 / ctx->hp.L);
+    size_t rounds = (batch / 5 + groups / 2) / groups;
+    if (rounds < 1) rounds = 1;
+    size_t chunk = rounds * groups;
+    if (chunk > 512) chunk = std::max<size_t>(groups, 512 / groups * groups);
+    if (const char *e = getenv("DPFHE_POLYEVAL_CHUNK")) chunk = std::max<size_t>(1, (size_t)atol(e));   // tests: several chunks at a small batch
+    if (chunk > batch) chunk = batch;
+    rc = pe_reserve(pe, chunk);
+    if (rc) return rc;
+    const size_t N = ctx->N();
+    return run_pipeline(ctx, h_ct, nullptr, h_out, batch, 2 * pe->Lq * N, 2 * pe->Lf * N, chunk,
+                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int { return pe_apply_on(pe, din, dout, cnt, st); });
 }
 
 int dpfhe_describe(const dpfhe_ctx *ctx, char *buf, size_t buf_len) {

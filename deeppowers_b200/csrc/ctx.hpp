@@ -18,6 +18,7 @@ struct dpfhe_ctx {
     dpfhe::LimbParams *d_lp = nullptr;
     dpfhe::Twiddle *d_tw = nullptr, *d_itw = nullptr;
     size_t device_bytes = 0;
+    size_t object_bytes = 0;                // device memory of the polynomial evaluators built on the context (keys, tables, scratch)
     uint64_t launches = 0;
     // Ordering between calls: every entry point may run on a different stream (the caller's, or the context's own when NULL
     // is passed), but they all share the context's scratch.  Each call makes its stream wait for the previous call's work

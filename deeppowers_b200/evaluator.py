@@ -460,6 +460,23 @@ class Context:
         pq = 2 * (self.L - n_special) * self.N
         self._chk(self._l.dpfhe_rotate_grouped_host(self._h, int(n_special), _hptr(ct), int(galois_elt), _hptr(gk), _hptr(out, True), ct.size // pq,
                                                     int(t_plain)))
+    # scalar linear combinations (DESIGN.md section 2.15) over all L limbs of this context: out = sum_i coeffs[i] cts[i] + constant
+    # (on the c0 rows), int64 coefficients reduced by floor-mod; cts: 1 .. 64 device tensors [batch][2][L][N], out may be one of them
+    def ct_lincomb(self, cts, coeffs, constant, out, batch, stream=None):
+        n = len(cts)
+        if len(coeffs) != n:
+            raise ValueError("need one coefficient per ciphertext")
+        ptrs = (C.c_void_p * max(n, 1))(*[_ptr(c) for c in cts])
+        cs = (C.c_int64 * max(n, 1))(*[int(c) for c in coeffs])
+        self._chk(self._l.dpfhe_ct_lincomb(self._h, n, ptrs, cs, int(constant), _ptr(out), batch, _stream(stream)))
+
+    def ct_add_plain(self, ct, pt, out, batch, stream=None):
+        """out = (c0 + pt, c1); pt [L][N] shared by the batch"""
+        self._chk(self._l.dpfhe_ct_add_plain(self._h, _ptr(ct), _ptr(pt), _ptr(out), batch, _stream(stream)))
+
+    def ct_add_plain_host(self, ct, pt, out):
+        self._chk(self._l.dpfhe_ct_add_plain_host(self._h, _hptr(ct), _hptr(pt), _hptr(out, True), ct.size // (2 * self.P)))
+
     def mod_switch_down_host(self, polys, out, t_plain=0):
         self._chk(self._l.dpfhe_mod_switch_down_host(self._h, _hptr(polys), _hptr(out, True), polys.size // self.P, int(t_plain)))
 
@@ -572,6 +589,41 @@ class LinearLayer:
 
     def apply_host(self, ct, out):
         self.ctx._chk(self._l.dpfhe_linear_apply_host(self._h, _hptr(ct), _hptr(out, True), ct.size // (2 * self.Lq * self.ctx.N)))
+
+
+class PolyEval:
+    """BGV polynomial evaluation on encrypted slots down the modulus chain (dpfhe_polyeval_*, DESIGN.md section 2.15): slot-wise
+    p(x) = sum_k coeffs[k] x^k mod t_plain.  ctx's last n_special limbs are special primes; relin_key is the grouped relinearisation
+    key [dnum][2][L][N] of the top level (C-contiguous numpy uint64).  apply / apply_host take ciphertexts [batch][2][Lq][N] and
+    write [batch][2][result_limbs][N], which decrypt under the first result_limbs limbs of the secret."""
+
+    def __init__(self, ctx, n_special, t_plain, coeffs, relin_key):
+        self._l, self.ctx = ctx._l, ctx
+        self._h = C.c_void_p()
+        self.n_special = int(n_special)
+        self.Lq = ctx.L - self.n_special
+        cs = np.ascontiguousarray([int(c) for c in coeffs], dtype=np.int64)
+        rc = self._l.dpfhe_polyeval_create_grouped(ctx._h, self.n_special, int(t_plain), C.c_void_p(cs.ctypes.data), len(cs) - 1, _hptr(relin_key),
+                                                   C.byref(self._h))
+        if rc != 0:
+            self._h = C.c_void_p()
+            raise DpfheError(self._l.dpfhe_last_error().decode())
+        self.result_limbs = int(self._l.dpfhe_polyeval_result_limbs(self._h))
+
+    def close(self):
+        """Close the evaluator before its context (as LinearLayer.close)."""
+        if getattr(self, "_h", None) and self._h.value:
+            if self.ctx._h.value:
+                self._l.dpfhe_polyeval_destroy(self._h)
+            self._h = C.c_void_p()
+
+    __del__ = close
+
+    def apply(self, ct, out, batch, stream=None):
+        self.ctx._chk(self._l.dpfhe_polyeval_apply(self._h, _ptr(ct), _ptr(out), batch, _stream(stream)))
+
+    def apply_host(self, ct, out):
+        self.ctx._chk(self._l.dpfhe_polyeval_apply_host(self._h, _hptr(ct), _hptr(out, True), ct.size // (2 * self.Lq * self.ctx.N)))
 
 
 class MultiContext:

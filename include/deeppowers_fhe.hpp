@@ -259,6 +259,20 @@ public:
     void add_device(const std::uint64_t *a, const std::uint64_t *b, std::uint64_t *out, std::size_t count, void *stream = nullptr) {
         check(dpfhe_poly_add(ctx_, a, b, out, 2 * count, stream));   // a ciphertext is two polynomials
     }
+    // out = (c0 + plain_eval, c1) over all limbs, plain_eval [L][N] shared by the batch: host buffers (pipelined) and device buffers
+    void add_plain(ConstCiphertextBatch ct, const std::uint64_t *plain_eval, CiphertextBatch out) {
+        if (ct.count != out.count) throw std::runtime_error("ciphertext batches must have the same count");
+        check(dpfhe_ct_add_plain_host(ctx_, ct.data, plain_eval, out.data, ct.count));
+    }
+    void add_plain_device(const std::uint64_t *ct, const std::uint64_t *plain_eval, std::uint64_t *out, std::size_t count, void *stream = nullptr) {
+        check(dpfhe_ct_add_plain(ctx_, ct, plain_eval, out, count, stream));
+    }
+    // out = sum_i coeffs[i] cts[i] + constant (on c0), 1 .. 64 device batches of `count` ciphertexts; out may be one of them
+    void lincomb_device(const std::vector<const std::uint64_t *> &cts, const std::vector<std::int64_t> &coeffs, std::int64_t constant,
+                        std::uint64_t *out, std::size_t count, void *stream = nullptr) {
+        if (cts.size() != coeffs.size()) throw std::runtime_error("one coefficient per ciphertext batch");
+        check(dpfhe_ct_lincomb(ctx_, cts.size(), cts.data(), coeffs.data(), constant, out, count, stream));
+    }
     void multiply_plain_accumulate_device(const std::uint64_t *ct, const std::uint64_t *plain_eval, std::uint64_t *acc, std::size_t count,
                                           void *stream = nullptr) {
         check(dpfhe_ct_mul_plain_acc(ctx_, ct, plain_eval, acc, count, stream));
@@ -301,6 +315,7 @@ public:
 
 private:
     friend class LinearLayer;
+    friend class PolyEval;
     static void check(int status) {
         if (status != DPFHE_OK) throw std::runtime_error(dpfhe_last_error());
     }
@@ -364,6 +379,31 @@ public:
 
 private:
     dpfhe_linear *h_ = nullptr;
+};
+
+// BGV polynomial evaluation on encrypted slots down the modulus chain (dpfhe_polyeval_*): p(x) = sum_k coeffs[k] x^k mod
+// plain_modulus, slot by slot.  The evaluator's last `special` limbs are special primes; relin_key is the grouped relinearisation key
+// [dnum][2][limbs()][N] of the top level (host memory).  Inputs carry limbs()-special limbs, results result_limbs().
+class PolyEval {
+public:
+    PolyEval(Evaluator &ev, unsigned special, std::uint64_t plain_modulus, const std::vector<std::int64_t> &coeffs, const std::uint64_t *relin_key) {
+        if (coeffs.size() < 2) throw std::runtime_error("a polynomial of degree at least 1");
+        Evaluator::check(dpfhe_polyeval_create_grouped(ev.native_handle(), special, plain_modulus, coeffs.data(), coeffs.size() - 1, relin_key, &h_));
+    }
+    ~PolyEval() { dpfhe_polyeval_destroy(h_); }
+    PolyEval(const PolyEval &) = delete;
+    PolyEval &operator=(const PolyEval &) = delete;
+    unsigned result_limbs() const { return dpfhe_polyeval_result_limbs(h_); }
+    void apply(ConstCiphertextBatch in, CiphertextBatch out) {   // host buffers, pipelined
+        if (in.count != out.count) throw std::runtime_error("ciphertext batches must have the same count");
+        Evaluator::check(dpfhe_polyeval_apply_host(h_, in.data, out.data, in.count));
+    }
+    void apply_device(const std::uint64_t *in, std::uint64_t *out, std::size_t count, void *stream = nullptr) {
+        Evaluator::check(dpfhe_polyeval_apply(h_, in, out, count, stream));
+    }
+
+private:
+    dpfhe_polyeval *h_ = nullptr;
 };
 
 // Several GPUs behind one object (dpfhe_multi_*): contiguous shards of every batch, one context and host thread per device, no

@@ -169,6 +169,31 @@ void dpfhe_linear_destroy(dpfhe_linear *layer);
 int dpfhe_linear_apply(dpfhe_linear *layer, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream);
 int dpfhe_linear_apply_host(dpfhe_linear *layer, const uint64_t *h_ct, uint64_t *h_out, size_t batch);
 
+/* ---- scalar linear combinations (DESIGN.md §2.15): d_out = sum_i (coeffs[i] mod q_l) d_cts[i], plus (constant mod q_l) at every
+ *      position of every c0 row; coefficients reduced by floor-mod, results canonical.  d_cts: a HOST array of n_terms (1 .. 64)
+ *      device pointers, each [batch][2][L][N] over all L limbs of the context; d_out may be any of them.  One launch.
+ *      dpfhe_ct_add_plain: d_out = (c0 + d_pt, c1), d_pt [L][N] shared by the batch (it must not overlap d_out). ---- */
+int dpfhe_ct_lincomb(dpfhe_ctx *ctx, size_t n_terms, const uint64_t *const *d_cts, const int64_t *coeffs, int64_t constant, uint64_t *d_out,
+                     size_t batch, void *stream);
+int dpfhe_ct_add_plain(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch, void *stream);
+/*      host-buffer form: h_pt uploaded once, the batch pipelined in chunks (synchronous) */
+int dpfhe_ct_add_plain_host(dpfhe_ctx *ctx, const uint64_t *h_ct, const uint64_t *h_pt, uint64_t *h_out, size_t batch);
+
+/* ---- BGV polynomial evaluation down the modulus chain (DESIGN.md §2.15): slot-wise p(x) = sum_k coeffs[k] x^k mod t_plain,
+ *      degree d = 1 .. 64, 2 <= t_plain < 2^31.  The context's last n_special limbs are special primes, ciphertexts come at the
+ *      top level Lq = L - n_special; h_relin_key is the grouped relinearisation key [dnum][2][L][N] of the top level (the keys of
+ *      the lower levels are restricted from it at creation).  D = ceil(log2 d) must satisfy D <= Lq - 1 and D <= Lq - K + 1.
+ *      apply: d_ct [batch][2][Lq][N] -> d_out [batch][2][Lf][N], Lf = Lq - D (dpfhe_polyeval_result_limbs), decrypting under the
+ *      first Lf limbs of the secret to p(slots) mod t exactly; asynchronous, d_out must not overlap d_ct.  apply_host: host
+ *      buffers, pipelined in chunks (synchronous).  Scratch grows with the batch and counts in dpfhe_context_device_bytes. ---- */
+typedef struct dpfhe_polyeval dpfhe_polyeval;
+int dpfhe_polyeval_create_grouped(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const int64_t *coeffs, size_t degree,
+                                  const uint64_t *h_relin_key, dpfhe_polyeval **out);
+unsigned dpfhe_polyeval_result_limbs(const dpfhe_polyeval *pe);
+int dpfhe_polyeval_apply(dpfhe_polyeval *pe, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream);
+int dpfhe_polyeval_apply_host(dpfhe_polyeval *pe, const uint64_t *h_ct, uint64_t *h_out, size_t batch);
+void dpfhe_polyeval_destroy(dpfhe_polyeval *pe);
+
 /* ---- modulus switching / rescale (DESIGN.md §2.9): drop the last limb of every polynomial.
  *      in [n_polys][L][N] -> out [n_polys][L-1][N] (a ciphertext is two polynomials), evaluation form.
  *      t_plain > 0: BGV modulus switch (the plaintext is scaled by q_last^-1 mod t); t_plain == 0: plain rounding.
