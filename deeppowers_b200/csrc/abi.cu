@@ -81,35 +81,23 @@ void note_launch(dpfhe_ctx *ctx, uint64_t n) {
     }
 }
 
-int ensure_staging(dpfhe_ctx *ctx, size_t in_bytes, size_t out_bytes, size_t key_bytes) {
-    // a size is only recorded once every buffer of its group exists: a failed cudaMalloc leaves the group marked empty
-    if (in_bytes > ctx->stage_in_bytes) {
-        ctx->stage_in_bytes = 0;
-        for (int k = 0; k < PIPE_DEPTH; ++k) {
-            if (ctx->stage_in[k]) cudaFree(ctx->stage_in[k]);
-            ctx->stage_in[k] = nullptr;
-            CU_TRY(cudaMalloc(&ctx->stage_in[k], in_bytes));
-        }
-        ctx->stage_in_bytes = in_bytes;
+}  // namespace
+
+int DeviceScratch::reserve(dpfhe_ctx *ctx, size_t bytes) {
+    if (bytes <= bytes_) return DPFHE_OK;
+    if (p_) {
+        const int rc = dpfhe_synchronize(ctx);
+        if (rc) return rc;
+        release();
     }
-    if (out_bytes > ctx->stage_out_bytes) {
-        ctx->stage_out_bytes = 0;
-        for (int k = 0; k < PIPE_DEPTH; ++k) {
-            if (ctx->stage_out[k]) cudaFree(ctx->stage_out[k]);
-            ctx->stage_out[k] = nullptr;
-            CU_TRY(cudaMalloc(&ctx->stage_out[k], out_bytes));
-        }
-        ctx->stage_out_bytes = out_bytes;
-    }
-    if (key_bytes > ctx->stage_key_bytes) {
-        ctx->stage_key_bytes = 0;
-        if (ctx->stage_key) cudaFree(ctx->stage_key);
-        ctx->stage_key = nullptr;
-        CU_TRY(cudaMalloc(&ctx->stage_key, key_bytes));
-        ctx->stage_key_bytes = key_bytes;
-    }
+    void *p = nullptr;
+    CU_TRY(cudaMalloc(&p, bytes));
+    p_ = p;
+    bytes_ = bytes;
     return DPFHE_OK;
 }
+
+namespace {
 
 // Generic three-stage pipeline over `n_items` items split into chunks:
 //   upload(chunk -> stage_in[slot]) on s_h2d, compute on ctx->stream, download(stage_out[slot]) on s_d2h.
@@ -118,13 +106,15 @@ template <class Compute>
 int run_pipeline_body(dpfhe_ctx *ctx, const u64 *h_in0, const u64 *h_in1, u64 *h_out, size_t n_items, size_t in_item_words,
                       size_t out_item_words, size_t chunk_items, Compute compute) {
     const size_t n_in = h_in1 ? 2 : 1;
-    int rc = ensure_staging(ctx, n_in * chunk_items * in_item_words * 8, chunk_items * out_item_words * 8, 0);
+    int rc = DPFHE_OK;
+    for (int k = 0; k < PIPE_DEPTH && !rc; ++k) rc = ctx->stage_in[k].reserve(ctx, n_in * chunk_items * in_item_words * 8);
+    for (int k = 0; k < PIPE_DEPTH && !rc; ++k) rc = ctx->stage_out[k].reserve(ctx, chunk_items * out_item_words * 8);
     if (rc) return rc;
     size_t k = 0;
     for (size_t first = 0; first < n_items; first += chunk_items, ++k) {
         const size_t cnt = n_items - first < chunk_items ? n_items - first : chunk_items;
         const int slot = (int)(k % PIPE_DEPTH);
-        u64 *din0 = ctx->stage_in[slot], *din1 = din0 + chunk_items * in_item_words, *dout = ctx->stage_out[slot];
+        u64 *din0 = ctx->stage_in[slot].get(), *din1 = din0 + chunk_items * in_item_words, *dout = ctx->stage_out[slot].get();
         if (k >= PIPE_DEPTH) CU_TRY(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_comp[slot], 0));   // stage_in[slot] free again
         CU_TRY(cudaMemcpyAsync(din0, h_in0 + first * in_item_words, cnt * in_item_words * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
         if (h_in1)
@@ -170,6 +160,103 @@ size_t pick_chunk(const dpfhe_ctx *ctx, size_t item_bytes, size_t n_items) {
     if (c < wave && n_items >= wave) c = wave;
     if (c > n_items) c = n_items;
     return c;
+}
+
+int upload_key(dpfhe_ctx *ctx, const uint64_t *h_key, size_t words) {
+    int rc = ctx->stage_key.reserve(ctx, words * 8);
+    if (rc) return rc;
+    CU_TRY(cudaMemcpyAsync(ctx->stage_key.get(), h_key, words * 8, cudaMemcpyHostToDevice, pick(ctx, nullptr)));
+    return DPFHE_OK;
+}
+
+int no_check() { return DPFHE_OK; }
+
+// The host-buffer form of an entry point: the host pointers `ptrs` must not be null, then `check()` runs the call's remaining
+// argument checks.  The operand every item shares (a key, a plaintext or a secret of `shared_words` words; none when
+// shared_words is 0) is uploaded once into the key staging buffer, and the items are pipelined through `compute` in chunks.
+template <class Compute, class Check = int (*)()>
+int host_call(dpfhe_ctx *ctx, std::initializer_list<const void *> ptrs, const uint64_t *h_shared, size_t shared_words, const u64 *h_in0,
+              const u64 *h_in1, u64 *h_out, size_t n_items, size_t in_item_words, size_t out_item_words, Compute compute, Check check = no_check) {
+    for (const void *p : ptrs)
+        if (!p) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    int rc = check();
+    if (rc) return rc;
+    if (shared_words) {
+        rc = upload_key(ctx, h_shared, shared_words);
+        if (rc) return rc;
+    }
+    const size_t chunk = pick_chunk(ctx, std::max(in_item_words, out_item_words) * 8, n_items);
+    return run_pipeline(ctx, h_in0, h_in1, h_out, n_items, in_item_words, out_item_words, chunk, compute);
+}
+
+int check_galois(const dpfhe_ctx *ctx, uint64_t galois) {
+    if (!(galois & 1) || galois >= ((uint64_t)2 << ctx->hp.log_n)) return fail(DPFHE_ERR_INVALID, "galois element must be odd and < 2N");
+    return DPFHE_OK;
+}
+
+// the elements and keys of n_rot hoisted rotations
+int check_rotations(const dpfhe_ctx *ctx, size_t n_rot, const uint64_t *galois_elts, const uint64_t *const *d_gks) {
+    for (size_t r = 0; r < n_rot; ++r) {
+        const int rc = check_galois(ctx, galois_elts[r]);
+        if (rc) return rc;
+        if (!d_gks[r] || !aligned16(d_gks[r])) return fail(DPFHE_ERR_INVALID, "null or misaligned Galois key");
+    }
+    return DPFHE_OK;
+}
+
+// the plaintext modulus of a division by the last K limbs (`what` names them in the message)
+int check_t_below_special(const dpfhe_ctx *ctx, unsigned K, uint64_t t_plain, const char *what = "the special prime") {
+    for (unsigned k = 0; k < K; ++k)
+        if (t_plain >= ctx->hp.limbs[ctx->hp.L - 1 - k].lp.q) return fail(DPFHE_ERR_INVALID, "plaintext modulus must be below %s", what);
+    return DPFHE_OK;
+}
+
+// Ciphertexts per chunk of the hoisted rotations' scratch (`per_ct` bytes each): at most ~4 GiB at a time, or
+// DPFHE_HOIST_CAP_MB (diagnostics / tests: smaller scratch, more chunks).
+size_t hoist_chunk(size_t per_ct, size_t batch) {
+    size_t cap = (size_t)4 << 30;
+    if (const char *e = getenv("DPFHE_HOIST_CAP_MB")) {
+        const long mb = atol(e);
+        if (mb > 0) cap = (size_t)mb << 20;
+    }
+    return std::max<size_t>(1, std::min(cap / per_ct, batch));
+}
+
+// Chunks of the host forms of the linear layer and the polynomial evaluator: about a fifth of the batch, rounded to whole rounds
+// of the persistent key-switch grid (3 CTAs per SM, L CTAs per ciphertext: with grouped keys L = Lq + K, every limb of the
+// context).  A chunk that leaves the grid's last round mostly empty costs more than the transfers it hides; the first upload and
+// the last download are the only transfers not overlapped with a neighbouring chunk's compute.  `rounds_env` names a variable
+// that sets the rounds instead (tuning).  Not capped by the batch.
+size_t grid_round_chunk(const dpfhe_ctx *ctx, size_t batch, const char *rounds_env) {
+    const size_t groups = std::max<size_t>(1, (size_t)ctx->lc.num_sms * 3 / ctx->hp.L);
+    size_t rounds = (batch / 5 + groups / 2) / groups;
+    if (const char *e = rounds_env ? getenv(rounds_env) : nullptr) rounds = (size_t)atol(e);
+    if (rounds < 1) rounds = 1;
+    const size_t chunk = rounds * groups;
+    return chunk > 512 ? std::max<size_t>(groups, 512 / groups * groups) : chunk;
+}
+
+// The device tables of a modulus basis: limb constants d_lp [L] (also copied into lt, for the kernels' parameter blocks) and the
+// forward and inverse twiddles [L][N]; adds their size to `bytes`.  lift_reduce: the key-switch kernels reduce the lifted
+// digits unless every modulus is below twice the smallest (or always, with DPFHE_LIFT_REDUCE set).
+int upload_basis(const HostParams &hp, LimbParams *&d_lp, Twiddle *&d_tw, Twiddle *&d_itw, LimbTable &lt, bool &lift_reduce, size_t &bytes) {
+    const size_t L = hp.L, N = (size_t)1 << hp.log_n;
+    CU_TRY(cudaMalloc(&d_lp, L * sizeof(LimbParams)));
+    CU_TRY(cudaMalloc(&d_tw, L * N * sizeof(Twiddle)));
+    CU_TRY(cudaMalloc(&d_itw, L * N * sizeof(Twiddle)));
+    bytes += L * sizeof(LimbParams) + 2 * L * N * sizeof(Twiddle);
+    memset(&lt, 0, sizeof(lt));
+    uint64_t qmin = ~0ull, qmax = 0;
+    for (size_t l = 0; l < L; ++l) {
+        lt.lp[l] = hp.limbs[l].lp;
+        qmin = std::min(qmin, lt.lp[l].q);
+        qmax = std::max(qmax, lt.lp[l].q);
+        CU_TRY(cudaMemcpy(d_tw + l * N, hp.limbs[l].tw.data(), N * sizeof(Twiddle), cudaMemcpyHostToDevice));
+        CU_TRY(cudaMemcpy(d_itw + l * N, hp.limbs[l].itw.data(), N * sizeof(Twiddle), cudaMemcpyHostToDevice));
+    }
+    CU_TRY(cudaMemcpy(d_lp, lt.lp, L * sizeof(LimbParams), cudaMemcpyHostToDevice));
+    lift_reduce = !(qmax < 2 * qmin) || getenv("DPFHE_LIFT_REDUCE") != nullptr;
+    return DPFHE_OK;
 }
 
 }  // namespace
@@ -232,35 +319,19 @@ int dpfhe_context_create(const dpfhe_params *p, int device_id, dpfhe_ctx **out) 
     }
     CTX_TRY(cudaEventCreateWithFlags(&ctx->ev_last, cudaEventDisableTiming));
     const size_t N = ctx->N(), L = ctx->hp.L;
-    CTX_TRY(cudaMalloc(&ctx->d_lp, L * sizeof(LimbParams)));
-    CTX_TRY(cudaMalloc(&ctx->d_tw, L * N * sizeof(Twiddle)));
-    CTX_TRY(cudaMalloc(&ctx->d_itw, L * N * sizeof(Twiddle)));
-    ctx->device_bytes += L * sizeof(LimbParams) + 2 * L * N * sizeof(Twiddle);
-    std::vector<LimbParams> lps(L);
-    for (size_t l = 0; l < L; ++l) {
-        lps[l] = ctx->hp.limbs[l].lp;
-        CTX_TRY(cudaMemcpy(ctx->d_tw + l * N, ctx->hp.limbs[l].tw.data(), N * sizeof(Twiddle), cudaMemcpyHostToDevice));
-        CTX_TRY(cudaMemcpy(ctx->d_itw + l * N, ctx->hp.limbs[l].itw.data(), N * sizeof(Twiddle), cudaMemcpyHostToDevice));
-    }
-    CTX_TRY(cudaMemcpy(ctx->d_lp, lps.data(), L * sizeof(LimbParams), cudaMemcpyHostToDevice));
     LaunchCtx &lc = ctx->lc;
+    const int rc = upload_basis(ctx->hp, ctx->d_lp, ctx->d_tw, ctx->d_itw, lc.lt, lc.lift_reduce, ctx->device_bytes);
+    if (rc) {
+        dpfhe_context_destroy(ctx);
+        return rc;
+    }
     lc.num_sms = prop.multiProcessorCount;
     lc.log_n = ctx->hp.log_n;
     lc.L = ctx->hp.L;
     lc.fast = true;
-    for (size_t l = 0; l < L; ++l) lc.fast = lc.fast && lps[l].nqh != 0;
+    for (size_t l = 0; l < L; ++l) lc.fast = lc.fast && lc.lt.lp[l].nqh != 0;
     if (getenv("DPFHE_FORCE_GENERIC")) lc.fast = false;   // diagnostics: run fast-class moduli through the generic kernels
-    {
-        uint64_t qmin = ~0ull, qmax = 0;
-        for (size_t l = 0; l < L; ++l) {
-            qmin = lps[l].q < qmin ? lps[l].q : qmin;
-            qmax = lps[l].q > qmax ? lps[l].q : qmax;
-        }
-        lc.lift_reduce = !(qmax < 2 * qmin) || getenv("DPFHE_LIFT_REDUCE") != nullptr;
-    }
     lc.lp = ctx->d_lp;
-    memset(&lc.lt, 0, sizeof(lc.lt));
-    for (size_t l = 0; l < L; ++l) lc.lt.lp[l] = lps[l];
     if (const char *env = getenv("DPFHE_NTT_CFG")) lc.ntt_cfg = atoi(env);
     if (const char *env = getenv("DPFHE_NTT_TMA")) lc.ntt_tma = atoi(env);
     if (const char *env = getenv("DPFHE_EPOCH_LIMIT")) lc.ks_epoch_limit = strtoull(env, nullptr, 10);
@@ -299,6 +370,7 @@ int dpfhe_context_create(const dpfhe_params *p, int device_id, dpfhe_ctx **out) 
     ctx->device_bytes += ks_parts * lc.ks_slots * 2 * N * 8 + lc.ks_slots * (2 * sizeof(u32) + sizeof(u64)) + 64;
     if (getenv("DPFHE_KS_PROF")) {   // diagnostics: per-phase cycle counters of the fused kernel
         CTX_TRY(cudaMalloc(&lc.ks_prof, lc.ks_slots * 16 * sizeof(unsigned long long)));
+        ctx->device_bytes += lc.ks_slots * 16 * sizeof(unsigned long long);
         CTX_TRY(cudaMemset(lc.ks_prof, 0, lc.ks_slots * 16 * sizeof(unsigned long long)));
     }
     CTX_TRY(cudaDeviceSynchronize());
@@ -322,21 +394,8 @@ void dpfhe_context_destroy(dpfhe_ctx *ctx) {
     cudaFree(ctx->lc.ks_ticket);
     cudaFree(ctx->lc.ks_mail);
     cudaFree(ctx->lc.ks_prof);
-    cudaFree(ctx->stage_key);
-    cudaFree(ctx->ms_tau);
-    cudaFree(ctx->hoist_U);
-    cudaFree(ctx->hoist_M);
-    cudaFree(ctx->hoist_kprime);
-    cudaFree(ctx->hoist_delta);
-    cudaFree(ctx->hoist_zero);
-    cudaFree(ctx->hoistg_buf);
-    cudaFree(ctx->ckks_tab);
-    cudaFree(ctx->bgv_tab);
-    cudaFree(ctx->enc_work);
     cudaFree(ctx->lc.ks_hyb);
     for (int k = 0; k < PIPE_DEPTH; ++k) {
-        cudaFree(ctx->stage_in[k]);
-        cudaFree(ctx->stage_out[k]);
         if (ctx->ev_h2d[k]) cudaEventDestroy(ctx->ev_h2d[k]);
         if (ctx->ev_comp[k]) cudaEventDestroy(ctx->ev_comp[k]);
         if (ctx->ev_d2h[k]) cudaEventDestroy(ctx->ev_d2h[k]);
@@ -345,7 +404,7 @@ void dpfhe_context_destroy(dpfhe_ctx *ctx) {
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
     if (ctx->s_h2d) cudaStreamDestroy(ctx->s_h2d);
     if (ctx->s_d2h) cudaStreamDestroy(ctx->s_d2h);
-    delete ctx;
+    delete ctx;   // frees the scratch
 }
 
 int dpfhe_get_modulus(const dpfhe_ctx *ctx, uint32_t limb, uint64_t *q) {
@@ -366,40 +425,24 @@ int dpfhe_get_root_powers(const dpfhe_ctx *ctx, uint32_t limb, int inverse, uint
 }
 size_t dpfhe_context_device_bytes(const dpfhe_ctx *ctx) {
     if (!ctx) return 0;
-    const size_t P8 = ctx->P() * 8, L = ctx->hp.L;
-    size_t n = ctx->device_bytes;                                                    // tables, key companions, digit slots, accumulators, flags (+ hybrid rows)
-    n += PIPE_DEPTH * (ctx->stage_in_bytes + ctx->stage_out_bytes) + ctx->stage_key_bytes;   // host-entry staging
-    n += ctx->ms_tau_bytes;                                                          // modulus-switch scratch
-    n += ctx->hoist_chunk * (L * P8 + sizeof(u32));                                  // hoisted rotations: shared transforms + zero flags
-    if (ctx->hoist_M) n += 3 * P8 + L * L * 8;                                       //   per-rotation constants
-    n += ctx->hoistg_bytes;                                                          //   grouped hybrid keys: lifted digits + accumulators
-    n += ctx->ckks_tab_bytes + ctx->bgv_tab_bytes + ctx->enc_work_bytes;             // CKKS and BGV encoding tables, their scratch
-    if (ctx->lc.ks_prof) n += ctx->lc.ks_slots * 16 * sizeof(unsigned long long);
-    n += ctx->object_bytes;                                                          // polynomial evaluators: level tables, keys, scratch
+    size_t n = ctx->device_bytes;   // tables, key companions, digit slots, accumulators, flags (+ hybrid rows)
+    dpfhe_ctx::each_trimmed(*ctx, [&](const DeviceScratch &s) { n += s.bytes(); });
+    n += ctx->hoist_M.bytes() + ctx->hoist_kprime.bytes() + ctx->hoist_delta.bytes();
+    n += ctx->object_bytes;         // polynomial evaluators: level tables, keys, scratch
     return n;
 }
 
-// frees the scratch that grows with use (hoisted-rotation transforms, modulus-switch rows, host staging); it comes back on demand
+// frees the scratch that grows with use (hoisted-rotation transforms, modulus-switch rows, encoding tables, host staging); it comes
+// back on demand
 int dpfhe_context_trim(dpfhe_ctx *ctx) {
     int rc = enter(ctx);
     if (rc) return rc;
     rc = dpfhe_synchronize(ctx);
     if (rc) return rc;
-    cudaFree(ctx->hoist_U); cudaFree(ctx->hoist_zero); cudaFree(ctx->ms_tau); cudaFree(ctx->stage_key);
-    ctx->hoist_U = nullptr; ctx->hoist_zero = nullptr; ctx->hoist_chunk = 0;
-    cudaFree(ctx->hoistg_buf);
-    ctx->hoistg_buf = nullptr; ctx->hoistg_bytes = 0;
-    cudaFree(ctx->ckks_tab); cudaFree(ctx->bgv_tab); cudaFree(ctx->enc_work);
-    ctx->ckks_tab = nullptr; ctx->ckks_tab_bytes = 0; ctx->ckks = CkksTables();
-    ctx->bgv_tab = nullptr; ctx->bgv_tab_bytes = 0; ctx->bgv_t = 0; ctx->bgv = BgvTables();
-    ctx->enc_work = nullptr; ctx->enc_work_bytes = 0;
-    ctx->ms_tau = nullptr; ctx->ms_tau_bytes = 0;
-    ctx->stage_key = nullptr; ctx->stage_key_bytes = 0;
-    for (int k = 0; k < PIPE_DEPTH; ++k) {
-        cudaFree(ctx->stage_in[k]); cudaFree(ctx->stage_out[k]);
-        ctx->stage_in[k] = ctx->stage_out[k] = nullptr;
-    }
-    ctx->stage_in_bytes = ctx->stage_out_bytes = 0;
+    dpfhe_ctx::each_trimmed(*ctx, [](DeviceScratch &s) { s.release(); });
+    ctx->ckks = CkksTables();
+    ctx->bgv_t = 0;
+    ctx->bgv = BgvTables();
     return DPFHE_OK;
 }
 uint64_t dpfhe_launch_count(const dpfhe_ctx *ctx) { return ctx ? ctx->launches : 0; }
@@ -466,10 +509,8 @@ static int ks_common(dpfhe_ctx *ctx, int mode, const uint64_t *a, const uint64_t
     if (batch == 0) return DPFHE_OK;
     CHECK_PTR(a); CHECK_PTR(key); CHECK_PTR(out);
     if (mode == KS_MUL_RELIN) CHECK_PTR(b);
-    if (mode == KS_ROTATE) {
-        const uint64_t two_n = (uint64_t)2 << ctx->hp.log_n;
-        if (!(galois & 1) || galois >= two_n) return fail(DPFHE_ERR_INVALID, "galois element must be odd and < 2N");
-    }
+    rc = mode == KS_ROTATE ? check_galois(ctx, galois) : DPFHE_OK;
+    if (rc) return rc;
     {   // the output rows are written while other work items still read their inputs: no overlap at all, not only out == in
         const size_t ct_bytes = 2 * ctx->P() * 8, in_bytes = batch * (mode == KS_PLAIN ? ct_bytes / 2 : ct_bytes);
         if (overlaps(out, batch * ct_bytes, a, in_bytes) || overlaps(out, batch * ct_bytes, b, in_bytes))
@@ -502,6 +543,12 @@ static int check_special(const dpfhe_ctx *ctx, unsigned n_special) {
     return DPFHE_OK;
 }
 
+// digits of a key: groups of n_special limbs of the L - n_special ciphertext moduli; n_special = 0: per-limb digits, L of them
+static size_t key_digits(const dpfhe_ctx *ctx, unsigned n_special) {
+    const unsigned L = ctx->hp.L;
+    return n_special ? (L - n_special + n_special - 1) / n_special : L;
+}
+
 // the special-prime accumulator and tau' rows of the hybrid / grouped key-switch kernels, allocated at the first call that needs them
 static int ensure_hyb(dpfhe_ctx *ctx) {
     if (ctx->lc.ks_hyb) return DPFHE_OK;
@@ -514,8 +561,8 @@ static int ensure_hyb(dpfhe_ctx *ctx) {
     return DPFHE_OK;
 }
 
-static int ks_hybrid_common(dpfhe_ctx *ctx, int mode, const uint64_t *a, const uint64_t *b, const uint64_t *key, uint64_t *out,
-                            size_t batch, uint64_t galois, uint64_t t_plain, void *stream, unsigned n_special = 1) {
+static int ks_hybrid_common(dpfhe_ctx *ctx, unsigned n_special, int mode, const uint64_t *a, const uint64_t *b, const uint64_t *key,
+                            uint64_t *out, size_t batch, uint64_t galois, uint64_t t_plain, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
@@ -524,12 +571,10 @@ static int ks_hybrid_common(dpfhe_ctx *ctx, int mode, const uint64_t *a, const u
     const unsigned L = ctx->hp.L;
     rc = check_special(ctx, n_special);
     if (rc) return rc;
-    for (unsigned k = 0; k < n_special; ++k)
-        if (t_plain >= ctx->hp.limbs[L - 1 - k].lp.q) return fail(DPFHE_ERR_INVALID, "plaintext modulus must be below the special prime");
-    if (mode == KS_ROTATE) {
-        const uint64_t two_n = (uint64_t)2 << ctx->hp.log_n;
-        if (!(galois & 1) || galois >= two_n) return fail(DPFHE_ERR_INVALID, "galois element must be odd and < 2N");
-    }
+    rc = check_t_below_special(ctx, n_special, t_plain);
+    if (rc) return rc;
+    rc = mode == KS_ROTATE ? check_galois(ctx, galois) : DPFHE_OK;
+    if (rc) return rc;
     {
         const size_t ct_bytes = 2 * (size_t)(L - n_special) * ctx->N() * 8, in_bytes = batch * (mode == KS_PLAIN ? ct_bytes / 2 : ct_bytes);
         if (overlaps(out, batch * ct_bytes, a, in_bytes) || overlaps(out, batch * ct_bytes, b, in_bytes))
@@ -551,34 +596,34 @@ static int ks_hybrid_common(dpfhe_ctx *ctx, int mode, const uint64_t *a, const u
 }
 int dpfhe_keyswitch_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_d, const uint64_t *d_key, uint64_t *d_out, size_t batch,
                             uint64_t t_plain, void *stream) {
-    return ks_hybrid_common(ctx, KS_PLAIN, d_d, nullptr, d_key, d_out, batch, 0, t_plain, stream, n_special);
+    return ks_hybrid_common(ctx, n_special, KS_PLAIN, d_d, nullptr, d_key, d_out, batch, 0, t_plain, stream);
 }
 int dpfhe_ct_mul_relin_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_a, const uint64_t *d_b, const uint64_t *d_evk,
                                uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
-    return ks_hybrid_common(ctx, KS_MUL_RELIN, d_a, d_b, d_evk, d_out, batch, 0, t_plain, stream, n_special);
+    return ks_hybrid_common(ctx, n_special, KS_MUL_RELIN, d_a, d_b, d_evk, d_out, batch, 0, t_plain, stream);
 }
 int dpfhe_rotate_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_ct, uint64_t galois_elt, const uint64_t *d_gk, uint64_t *d_out,
                          size_t batch, uint64_t t_plain, void *stream) {
-    return ks_hybrid_common(ctx, KS_ROTATE, d_ct, nullptr, d_gk, d_out, batch, galois_elt, t_plain, stream, n_special);
+    return ks_hybrid_common(ctx, n_special, KS_ROTATE, d_ct, nullptr, d_gk, d_out, batch, galois_elt, t_plain, stream);
 }
 int dpfhe_grouped_digits(const dpfhe_ctx *ctx, unsigned n_special, unsigned *digits) {
     if (!ctx || !digits) return fail(DPFHE_ERR_INVALID, "null argument");
     int rc = check_special(ctx, n_special);
     if (rc) return rc;
-    *digits = (ctx->hp.L - n_special + n_special - 1) / n_special;
+    *digits = (unsigned)key_digits(ctx, n_special);
     return DPFHE_OK;
 }
 int dpfhe_keyswitch_hybrid(dpfhe_ctx *ctx, const uint64_t *d_d, const uint64_t *d_key, uint64_t *d_out, size_t batch, uint64_t t_plain,
                            void *stream) {
-    return ks_hybrid_common(ctx, KS_PLAIN, d_d, nullptr, d_key, d_out, batch, 0, t_plain, stream);
+    return dpfhe_keyswitch_grouped(ctx, 1, d_d, d_key, d_out, batch, t_plain, stream);
 }
 int dpfhe_ct_mul_relin_hybrid(dpfhe_ctx *ctx, const uint64_t *d_a, const uint64_t *d_b, const uint64_t *d_evk, uint64_t *d_out,
                               size_t batch, uint64_t t_plain, void *stream) {
-    return ks_hybrid_common(ctx, KS_MUL_RELIN, d_a, d_b, d_evk, d_out, batch, 0, t_plain, stream);
+    return dpfhe_ct_mul_relin_grouped(ctx, 1, d_a, d_b, d_evk, d_out, batch, t_plain, stream);
 }
 int dpfhe_rotate_hybrid(dpfhe_ctx *ctx, const uint64_t *d_ct, uint64_t galois_elt, const uint64_t *d_gk, uint64_t *d_out, size_t batch,
                         uint64_t t_plain, void *stream) {
-    return ks_hybrid_common(ctx, KS_ROTATE, d_ct, nullptr, d_gk, d_out, batch, galois_elt, t_plain, stream);
+    return dpfhe_rotate_grouped(ctx, 1, d_ct, galois_elt, d_gk, d_out, batch, t_plain, stream);
 }
 
 // Hoisted rotations: n_rot rotations of the SAME ciphertexts.  Bit-identical to n_rot calls of dpfhe_rotate; the digit
@@ -589,14 +634,15 @@ int dpfhe_rotate_hybrid(dpfhe_ctx *ctx, const uint64_t *d_ct, uint64_t galois_el
 // for rotation r, prepared[2r] = the key's Shoup companions [L][2][L][N], prepared[2r+1] = kprime [2][L][N].
 static int ensure_hoist_consts(dpfhe_ctx *ctx) {
     const size_t L = ctx->hp.L, P = ctx->P();
-    if (ctx->hoist_M) return DPFHE_OK;
-    CU_TRY(cudaMalloc(&ctx->hoist_M, P * sizeof(u64)));
-    CU_TRY(cudaMalloc(&ctx->hoist_kprime, 2 * P * sizeof(u64)));
-    CU_TRY(cudaMalloc(&ctx->hoist_delta, L * L * sizeof(u64)));
+    if (ctx->hoist_delta.bytes()) return DPFHE_OK;   // allocated last
+    int rc = ctx->hoist_M.reserve(ctx, P * sizeof(u64));
+    if (!rc) rc = ctx->hoist_kprime.reserve(ctx, 2 * P * sizeof(u64));
+    if (!rc) rc = ctx->hoist_delta.reserve(ctx, L * L * sizeof(u64));
+    if (rc) return rc;
     std::vector<u64> delta(L * L);
     for (size_t j = 0; j < L; ++j)
         for (size_t i = 0; i < L; ++i) delta[j * L + i] = ctx->hp.limbs[j].lp.q % ctx->hp.limbs[i].lp.q;
-    CU_TRY(cudaMemcpy(ctx->hoist_delta, delta.data(), delta.size() * sizeof(u64), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemcpy(ctx->hoist_delta.get(), delta.data(), delta.size() * sizeof(u64), cudaMemcpyHostToDevice));
     return DPFHE_OK;
 }
 
@@ -607,56 +653,38 @@ static int rotate_hoisted_impl(dpfhe_ctx *ctx, const uint64_t *d_ct, size_t n_ro
     if (batch == 0 || n_rot == 0) return DPFHE_OK;
     CHECK_PTR(d_ct); CHECK_PTR(d_out);
     if (!galois_elts || !d_gks) return fail(DPFHE_ERR_INVALID, "null argument");
-    const uint64_t two_n = (uint64_t)2 << ctx->hp.log_n;
     const size_t N = ctx->N(), L = ctx->hp.L, P = ctx->P();
-    for (size_t r = 0; r < n_rot; ++r) {
-        if (!(galois_elts[r] & 1) || galois_elts[r] >= two_n) return fail(DPFHE_ERR_INVALID, "galois element must be odd and < 2N");
-        if (!d_gks[r] || !aligned16(d_gks[r])) return fail(DPFHE_ERR_INVALID, "null or misaligned Galois key");
-    }
+    rc = check_rotations(ctx, n_rot, galois_elts, d_gks);
+    if (rc) return rc;
     if (overlaps(d_out, n_rot * batch * 2 * P * 8, d_ct, batch * 2 * P * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
     cudaStream_t st = pick(ctx, stream);
-    // scratch: at most ~4 GiB of shared transforms at a time (the batch is processed in chunks of that many ciphertexts)
-    const size_t per_ct = L * L * N * sizeof(u64);
-    size_t cap = (size_t)4 << 30;
-    if (const char *e = getenv("DPFHE_HOIST_CAP_MB")) {   // diagnostics / tests: smaller scratch, more chunks
-        const long mb = atol(e);
-        if (mb > 0) cap = (size_t)mb << 20;
-    }
-    size_t chunk = cap / per_ct;
-    if (chunk < 1) chunk = 1;
-    if (chunk > batch) chunk = batch;
-    if (chunk > ctx->hoist_chunk) {
-        CU_TRY(cudaStreamSynchronize(st));
-        cudaFree(ctx->hoist_U);
-        cudaFree(ctx->hoist_zero);
-        ctx->hoist_U = nullptr;
-        ctx->hoist_zero = nullptr;
-        ctx->hoist_chunk = 0;
-        CU_TRY(cudaMalloc(&ctx->hoist_U, chunk * per_ct));
-        CU_TRY(cudaMalloc(&ctx->hoist_zero, chunk * sizeof(u32)));
-        ctx->hoist_chunk = chunk;
-    }
-    rc = ensure_hoist_consts(ctx);
+    // scratch: the shared transforms and zero flags of a chunk of the batch
+    const size_t per_ct = L * L * N * sizeof(u64), chunk = hoist_chunk(per_ct, batch);
+    rc = ctx->hoist_U.reserve(ctx, chunk * per_ct);
+    if (!rc) rc = ctx->hoist_zero.reserve(ctx, chunk * sizeof(u32));
+    if (!rc) rc = ensure_hoist_consts(ctx);
     if (rc) return rc;
+    u64 *U = ctx->hoist_U.get(), *M = ctx->hoist_M.get(), *kp = ctx->hoist_kprime.get(), *delta = ctx->hoist_delta.get();
+    u32 *zero = ctx->hoist_zero.get<u32>();
     for (size_t first = 0; first < batch; first += chunk) {
         const size_t cnt = batch - first < chunk ? batch - first : chunk;
         const u64 *in = d_ct + first * 2 * P;
-        CU_TRY(cudaMemsetAsync(ctx->hoist_zero, 0, cnt * sizeof(u32), st));
+        CU_TRY(cudaMemsetAsync(zero, 0, cnt * sizeof(u32), st));
         if (L > 1) {
-            CU_TRY(VCALL(launch_hoist, ctx->lc, in, ctx->hoist_U, ctx->hoist_zero, cnt, st));
+            CU_TRY(VCALL(launch_hoist, ctx->lc, in, U, zero, cnt, st));
             note_launch(ctx, 1);
         }
         for (size_t r = 0; r < n_rot; ++r) {
             u64 *out = d_out + (r * batch + first) * 2 * P;
-            const u64 *key_s = prepared ? prepared[2 * r] : nullptr, *kprime = prepared ? prepared[2 * r + 1] : ctx->hoist_kprime;
+            const u64 *key_s = prepared ? prepared[2 * r] : nullptr, *kprime = prepared ? prepared[2 * r + 1] : kp;
             if (!prepared) {
-                CU_TRY(VCALL(launch_rot_prepare, ctx->lc, d_gks[r], (u32)galois_elts[r], ctx->hoist_delta, ctx->hoist_M, ctx->hoist_kprime, st));
+                CU_TRY(VCALL(launch_rot_prepare, ctx->lc, d_gks[r], (u32)galois_elts[r], delta, M, kp, st));
                 note_launch(ctx, 4);   // key_prepare, negmask, ntt, kprime
             }
-            CU_TRY(VCALL(launch_rot_apply, ctx->lc, in, L > 1 ? ctx->hoist_U : nullptr, d_gks[r], kprime, (u32)galois_elts[r], out, cnt, st, key_s));
+            CU_TRY(VCALL(launch_rot_apply, ctx->lc, in, L > 1 ? U : nullptr, d_gks[r], kprime, (u32)galois_elts[r], out, cnt, st, key_s));
             note_launch(ctx, 1);
             if (L > 1) {
-                CU_TRY(VCALL(launch_ks, ctx->lc, KS_ROTATE, in, nullptr, d_gks[r], out, cnt, (u32)galois_elts[r], st, ctx->hoist_zero, true, key_s));
+                CU_TRY(VCALL(launch_ks, ctx->lc, KS_ROTATE, in, nullptr, d_gks[r], out, cnt, (u32)galois_elts[r], st, zero, true, key_s));
                 note_launch(ctx, 1);
             }
         }
@@ -684,36 +712,19 @@ static int rotate_hoisted_grouped_impl(dpfhe_ctx *ctx, unsigned n_special, const
     if (!galois_elts || !d_gks) return fail(DPFHE_ERR_INVALID, "null argument");
     rc = check_special(ctx, n_special);
     if (rc) return rc;
-    const uint64_t two_n = (uint64_t)2 << ctx->hp.log_n;
     const size_t N = ctx->N(), L = ctx->hp.L, Lq = L - n_special, Pq = Lq * N, dnum = (Lq + n_special - 1) / n_special;
-    for (unsigned k = 0; k < n_special; ++k)
-        if (t_plain >= ctx->hp.limbs[L - 1 - k].lp.q) return fail(DPFHE_ERR_INVALID, "plaintext modulus must be below the special prime");
-    for (size_t r = 0; r < n_rot; ++r) {
-        if (!(galois_elts[r] & 1) || galois_elts[r] >= two_n) return fail(DPFHE_ERR_INVALID, "galois element must be odd and < 2N");
-        if (!d_gks[r] || !aligned16(d_gks[r])) return fail(DPFHE_ERR_INVALID, "null or misaligned Galois key");
-    }
+    rc = check_t_below_special(ctx, n_special, t_plain);
+    if (rc) return rc;
+    rc = check_rotations(ctx, n_rot, galois_elts, d_gks);
+    if (rc) return rc;
     if (overlaps(d_out, n_rot * batch * 2 * Pq * 8, d_ct, batch * 2 * Pq * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
     cudaStream_t st = pick(ctx, stream);
-    // scratch per ciphertext: lifted digits [dnum][L][N], accumulators [2][L][N], tau' rows [2][K][N]; at most ~4 GiB at a time
+    // scratch per ciphertext of a chunk: lifted digits [dnum][L][N], accumulators [2][L][N], tau' rows [2][K][N]
     const size_t u_words = dnum * L * N, acc_words = 2 * L * N, tau_words = 2 * (size_t)n_special * N;
-    const size_t per_ct = (u_words + acc_words + tau_words) * sizeof(u64);
-    size_t cap = (size_t)4 << 30;
-    if (const char *e = getenv("DPFHE_HOIST_CAP_MB")) {
-        const long mb = atol(e);
-        if (mb > 0) cap = (size_t)mb << 20;
-    }
-    size_t chunk = cap / per_ct;
-    if (chunk < 1) chunk = 1;
-    if (chunk > batch) chunk = batch;
-    if (chunk * per_ct > ctx->hoistg_bytes) {
-        CU_TRY(cudaStreamSynchronize(st));
-        cudaFree(ctx->hoistg_buf);
-        ctx->hoistg_buf = nullptr;
-        ctx->hoistg_bytes = 0;
-        CU_TRY(cudaMalloc(&ctx->hoistg_buf, chunk * per_ct));
-        ctx->hoistg_bytes = chunk * per_ct;
-    }
-    u64 *U = ctx->hoistg_buf, *acc = U + chunk * u_words, *tau = acc + chunk * acc_words;
+    const size_t per_ct = (u_words + acc_words + tau_words) * sizeof(u64), chunk = hoist_chunk(per_ct, batch);
+    rc = ctx->hoistg.reserve(ctx, chunk * per_ct);
+    if (rc) return rc;
+    u64 *U = ctx->hoistg.get(), *acc = U + chunk * u_words, *tau = acc + chunk * acc_words;
     MsConsts K;
     GroupConsts G;
     build_group_consts(ctx->hp, n_special, t_plain, G, K);
@@ -784,18 +795,11 @@ int dpfhe_mod_switch_down(dpfhe_ctx *ctx, const uint64_t *d_in, uint64_t *d_out,
         return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
     const uint64_t ql = ctx->hp.limbs[L - 1].lp.q;
     if (t_plain >= ql || (t_plain && t_plain % ql == 0)) return fail(DPFHE_ERR_INVALID, "plaintext modulus must be below the dropped modulus");
-    const size_t need = n_polys * ctx->N() * 8;
-    if (need > ctx->ms_tau_bytes) {
-        CU_TRY(cudaStreamSynchronize(pick(ctx, stream)));   // the old scratch may still be in use on this stream
-        if (ctx->ms_tau) cudaFree(ctx->ms_tau);
-        ctx->ms_tau = nullptr;
-        ctx->ms_tau_bytes = 0;
-        CU_TRY(cudaMalloc(&ctx->ms_tau, need));
-        ctx->ms_tau_bytes = need;
-    }
+    rc = ctx->ms_tau.reserve(ctx, n_polys * ctx->N() * 8);
+    if (rc) return rc;
     MsConsts K;
     build_ms_consts(ctx->hp, t_plain, K);
-    CU_TRY(VCALL(launch_mod_switch, ctx->lc, d_in, ctx->ms_tau, d_out, K, n_polys, pick(ctx, stream)));
+    CU_TRY(VCALL(launch_mod_switch, ctx->lc, d_in, ctx->ms_tau.get(), d_out, K, n_polys, pick(ctx, stream)));
     note_launch(ctx, 2);
     return DPFHE_OK;
 }
@@ -812,21 +816,14 @@ int dpfhe_mod_down_special(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d
         return fail(DPFHE_ERR_INVALID, "n_special must be between 1 and %d and below the context's %u limbs", KS_MAX_SPECIAL, L);
     if (overlaps(d_out, n_polys * (size_t)(L - n_special) * ctx->N() * 8, d_in, n_polys * ctx->P() * 8))
         return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
-    for (unsigned k = 0; k < n_special; ++k)
-        if (t_plain >= ctx->hp.limbs[L - 1 - k].lp.q) return fail(DPFHE_ERR_INVALID, "plaintext modulus must be below the dropped moduli");
-    const size_t need = n_polys * n_special * ctx->N() * 8;
-    if (need > ctx->ms_tau_bytes) {
-        CU_TRY(cudaStreamSynchronize(pick(ctx, stream)));   // the old scratch may still be in use on this stream
-        if (ctx->ms_tau) cudaFree(ctx->ms_tau);
-        ctx->ms_tau = nullptr;
-        ctx->ms_tau_bytes = 0;
-        CU_TRY(cudaMalloc(&ctx->ms_tau, need));
-        ctx->ms_tau_bytes = need;
-    }
+    rc = check_t_below_special(ctx, n_special, t_plain, "the dropped moduli");
+    if (rc) return rc;
+    rc = ctx->ms_tau.reserve(ctx, n_polys * n_special * ctx->N() * 8);
+    if (rc) return rc;
     MsConsts K;
     GroupConsts G;
     build_group_consts(ctx->hp, n_special, t_plain, G, K);
-    CU_TRY(VCALL(launch_mod_down_special, ctx->lc, d_in, ctx->ms_tau, d_out, K, G, n_polys, pick(ctx, stream)));
+    CU_TRY(VCALL(launch_mod_down_special, ctx->lc, d_in, ctx->ms_tau.get(), d_out, K, G, n_polys, pick(ctx, stream)));
     note_launch(ctx, 2);
     return DPFHE_OK;
 }
@@ -849,87 +846,37 @@ static int ntt_host(dpfhe_ctx *ctx, uint64_t *h_data, size_t n_polys, bool inver
     if (n_polys == 0) return DPFHE_OK;
     if (!h_data) return fail(DPFHE_ERR_INVALID, "null pointer: h_data");
     const size_t P = ctx->P();
-    const size_t chunk = pick_chunk(ctx, P * 8, n_polys);
-    return run_pipeline(ctx, h_data, nullptr, h_data, n_polys, P, P, chunk,
-                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            CU_TRY(VCALL(launch_ntt, ctx->lc, din, cnt, inverse, st));
-                            note_launch(ctx, 1);
-                            CU_TRY(cudaMemcpyAsync(dout, din, cnt * P * 8, cudaMemcpyDeviceToDevice, st));
-                            return DPFHE_OK;
-                        });
+    return host_call(ctx, {}, nullptr, 0, h_data, nullptr, h_data, n_polys, P, P,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                         CU_TRY(VCALL(launch_ntt, ctx->lc, din, cnt, inverse, st));
+                         note_launch(ctx, 1);
+                         CU_TRY(cudaMemcpyAsync(dout, din, cnt * P * 8, cudaMemcpyDeviceToDevice, st));
+                         return DPFHE_OK;
+                     });
 }
 int dpfhe_ntt_fwd_host(dpfhe_ctx *ctx, uint64_t *h_data, size_t n_polys) { return ntt_host(ctx, h_data, n_polys, false); }
 int dpfhe_ntt_inv_host(dpfhe_ctx *ctx, uint64_t *h_data, size_t n_polys) { return ntt_host(ctx, h_data, n_polys, true); }
-
-static int upload_key(dpfhe_ctx *ctx, const uint64_t *h_key, size_t words) {
-    int rc = ensure_staging(ctx, 0, 0, words * 8);
-    if (rc) return rc;
-    CU_TRY(cudaMemcpyAsync(ctx->stage_key, h_key, words * 8, cudaMemcpyHostToDevice, pick(ctx, nullptr)));
-    return DPFHE_OK;
-}
 
 int dpfhe_ct_mul_relin_host(dpfhe_ctx *ctx, const uint64_t *h_a, const uint64_t *h_b, const uint64_t *h_evk, uint64_t *h_out, size_t batch) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
-    if (!h_a || !h_b || !h_evk || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
     const size_t P = ctx->P();
-    rc = upload_key(ctx, h_evk, 2 * ctx->hp.L * P);
-    if (rc) return rc;
-    const size_t chunk = pick_chunk(ctx, 2 * P * 8, batch);
-    return run_pipeline(ctx, h_a, h_b, h_out, batch, 2 * P, 2 * P, chunk,
-                        [&](u64 *da, u64 *db, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return ks_common(ctx, KS_MUL_RELIN, da, db, ctx->stage_key, dout, cnt, 0, st);
-                        });
+    return host_call(ctx, {h_a, h_b, h_evk, h_out}, h_evk, 2 * ctx->hp.L * P, h_a, h_b, h_out, batch, 2 * P, 2 * P,
+                     [&](u64 *da, u64 *db, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return ks_common(ctx, KS_MUL_RELIN, da, db, ctx->stage_key.get(), dout, cnt, 0, st);
+                     });
 }
 
 int dpfhe_rotate_host(dpfhe_ctx *ctx, const uint64_t *h_ct, uint64_t galois_elt, const uint64_t *h_gk, uint64_t *h_out, size_t batch) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
-    if (!h_ct || !h_gk || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
     const size_t P = ctx->P();
-    rc = upload_key(ctx, h_gk, 2 * ctx->hp.L * P);
-    if (rc) return rc;
-    const size_t chunk = pick_chunk(ctx, 2 * P * 8, batch);
-    return run_pipeline(ctx, h_ct, nullptr, h_out, batch, 2 * P, 2 * P, chunk,
-                        [&](u64 *dc, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return ks_common(ctx, KS_ROTATE, dc, nullptr, ctx->stage_key, dout, cnt, galois_elt, st);
-                        });
-}
-
-int dpfhe_ct_mul_relin_hybrid_host(dpfhe_ctx *ctx, const uint64_t *h_a, const uint64_t *h_b, const uint64_t *h_evk, uint64_t *h_out,
-                                   size_t batch, uint64_t t_plain) {
-    int rc = enter(ctx);
-    if (rc) return rc;
-    if (batch == 0) return DPFHE_OK;
-    if (!h_a || !h_b || !h_evk || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    if (ctx->hp.L < 2) return fail(DPFHE_ERR_INVALID, "hybrid key switching needs a special prime: create the context with at least two limbs");
-    const size_t Pq = (ctx->hp.L - 1) * ctx->N();   // words of a ciphertext polynomial (L-1 limbs)
-    rc = upload_key(ctx, h_evk, 2 * (ctx->hp.L - 1) * ctx->P());
-    if (rc) return rc;
-    const size_t chunk = pick_chunk(ctx, 2 * Pq * 8, batch);
-    return run_pipeline(ctx, h_a, h_b, h_out, batch, 2 * Pq, 2 * Pq, chunk,
-                        [&](u64 *da, u64 *db, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return ks_hybrid_common(ctx, KS_MUL_RELIN, da, db, ctx->stage_key, dout, cnt, 0, t_plain, st);
-                        });
-}
-
-int dpfhe_rotate_hybrid_host(dpfhe_ctx *ctx, const uint64_t *h_ct, uint64_t galois_elt, const uint64_t *h_gk, uint64_t *h_out,
-                             size_t batch, uint64_t t_plain) {
-    int rc = enter(ctx);
-    if (rc) return rc;
-    if (batch == 0) return DPFHE_OK;
-    if (!h_ct || !h_gk || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    if (ctx->hp.L < 2) return fail(DPFHE_ERR_INVALID, "hybrid key switching needs a special prime: create the context with at least two limbs");
-    const size_t Pq = (ctx->hp.L - 1) * ctx->N();
-    rc = upload_key(ctx, h_gk, 2 * (ctx->hp.L - 1) * ctx->P());
-    if (rc) return rc;
-    const size_t chunk = pick_chunk(ctx, 2 * Pq * 8, batch);
-    return run_pipeline(ctx, h_ct, nullptr, h_out, batch, 2 * Pq, 2 * Pq, chunk,
-                        [&](u64 *dc, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return ks_hybrid_common(ctx, KS_ROTATE, dc, nullptr, ctx->stage_key, dout, cnt, galois_elt, t_plain, st);
-                        });
+    return host_call(ctx, {h_ct, h_gk, h_out}, h_gk, 2 * ctx->hp.L * P, h_ct, nullptr, h_out, batch, 2 * P, 2 * P,
+                     [&](u64 *dc, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return ks_common(ctx, KS_ROTATE, dc, nullptr, ctx->stage_key.get(), dout, cnt, galois_elt, st);
+                     });
 }
 
 int dpfhe_ct_mul_relin_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_a, const uint64_t *h_b, const uint64_t *h_evk,
@@ -937,17 +884,12 @@ int dpfhe_ct_mul_relin_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const ui
     int rc = enter(ctx);
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
-    if (!h_a || !h_b || !h_evk || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    rc = check_special(ctx, n_special);
-    if (rc) return rc;
-    const size_t Lq = ctx->hp.L - n_special, Pq = Lq * ctx->N(), dnum = (Lq + n_special - 1) / n_special;
-    rc = upload_key(ctx, h_evk, 2 * dnum * ctx->P());
-    if (rc) return rc;
-    const size_t chunk = pick_chunk(ctx, 2 * Pq * 8, batch);
-    return run_pipeline(ctx, h_a, h_b, h_out, batch, 2 * Pq, 2 * Pq, chunk,
-                        [&](u64 *da, u64 *db, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return ks_hybrid_common(ctx, KS_MUL_RELIN, da, db, ctx->stage_key, dout, cnt, 0, t_plain, st, n_special);
-                        });
+    const size_t Pq = (ctx->hp.L - n_special) * ctx->N();   // words of a ciphertext polynomial (L - K limbs)
+    return host_call(ctx, {h_a, h_b, h_evk, h_out}, h_evk, 2 * key_digits(ctx, n_special) * ctx->P(), h_a, h_b, h_out, batch, 2 * Pq, 2 * Pq,
+                     [&](u64 *da, u64 *db, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return ks_hybrid_common(ctx, n_special, KS_MUL_RELIN, da, db, ctx->stage_key.get(), dout, cnt, 0, t_plain, st);
+                     },
+                     [&] { return check_special(ctx, n_special); });
 }
 
 int dpfhe_rotate_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_ct, uint64_t galois_elt, const uint64_t *h_gk,
@@ -955,103 +897,88 @@ int dpfhe_rotate_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t
     int rc = enter(ctx);
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
-    if (!h_ct || !h_gk || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    rc = check_special(ctx, n_special);
-    if (rc) return rc;
-    const size_t Lq = ctx->hp.L - n_special, Pq = Lq * ctx->N(), dnum = (Lq + n_special - 1) / n_special;
-    rc = upload_key(ctx, h_gk, 2 * dnum * ctx->P());
-    if (rc) return rc;
-    const size_t chunk = pick_chunk(ctx, 2 * Pq * 8, batch);
-    return run_pipeline(ctx, h_ct, nullptr, h_out, batch, 2 * Pq, 2 * Pq, chunk,
-                        [&](u64 *dc, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return ks_hybrid_common(ctx, KS_ROTATE, dc, nullptr, ctx->stage_key, dout, cnt, galois_elt, t_plain, st, n_special);
-                        });
+    const size_t Pq = (ctx->hp.L - n_special) * ctx->N();
+    return host_call(ctx, {h_ct, h_gk, h_out}, h_gk, 2 * key_digits(ctx, n_special) * ctx->P(), h_ct, nullptr, h_out, batch, 2 * Pq, 2 * Pq,
+                     [&](u64 *dc, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return ks_hybrid_common(ctx, n_special, KS_ROTATE, dc, nullptr, ctx->stage_key.get(), dout, cnt, galois_elt, t_plain, st);
+                     },
+                     [&] { return check_special(ctx, n_special); });
+}
+
+int dpfhe_ct_mul_relin_hybrid_host(dpfhe_ctx *ctx, const uint64_t *h_a, const uint64_t *h_b, const uint64_t *h_evk, uint64_t *h_out,
+                                   size_t batch, uint64_t t_plain) {
+    return dpfhe_ct_mul_relin_grouped_host(ctx, 1, h_a, h_b, h_evk, h_out, batch, t_plain);
+}
+
+int dpfhe_rotate_hybrid_host(dpfhe_ctx *ctx, const uint64_t *h_ct, uint64_t galois_elt, const uint64_t *h_gk, uint64_t *h_out,
+                             size_t batch, uint64_t t_plain) {
+    return dpfhe_rotate_grouped_host(ctx, 1, h_ct, galois_elt, h_gk, h_out, batch, t_plain);
 }
 
 int dpfhe_mod_switch_down_host(dpfhe_ctx *ctx, const uint64_t *h_in, uint64_t *h_out, size_t n_polys, uint64_t t_plain) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (n_polys == 0) return DPFHE_OK;
-    if (!h_in || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    if (ctx->hp.L < 2) return fail(DPFHE_ERR_INVALID, "mod_switch_down needs at least two limbs");
     const size_t P = ctx->P(), Pq = (ctx->hp.L - 1) * ctx->N();
-    const size_t chunk = pick_chunk(ctx, P * 8, n_polys);
-    return run_pipeline(ctx, h_in, nullptr, h_out, n_polys, P, Pq, chunk,
-                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return dpfhe_mod_switch_down(ctx, din, dout, cnt, t_plain, st);
-                        });
+    return host_call(ctx, {h_in, h_out}, nullptr, 0, h_in, nullptr, h_out, n_polys, P, Pq,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return dpfhe_mod_switch_down(ctx, din, dout, cnt, t_plain, st);
+                     },
+                     [&] { return ctx->hp.L < 2 ? fail(DPFHE_ERR_INVALID, "mod_switch_down needs at least two limbs") : DPFHE_OK; });
 }
 
 int dpfhe_mod_down_special_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_in, uint64_t *h_out, size_t n_polys, uint64_t t_plain) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (n_polys == 0) return DPFHE_OK;
-    if (!h_in || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    if (n_special < 1 || n_special >= ctx->hp.L) return fail(DPFHE_ERR_INVALID, "n_special must be at least 1 and below the context's limbs");
     const size_t P = ctx->P(), Pq = (ctx->hp.L - n_special) * ctx->N();
-    const size_t chunk = pick_chunk(ctx, P * 8, n_polys);
-    return run_pipeline(ctx, h_in, nullptr, h_out, n_polys, P, Pq, chunk,
-                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return dpfhe_mod_down_special(ctx, n_special, din, dout, cnt, t_plain, st);
-                        });
+    return host_call(ctx, {h_in, h_out}, nullptr, 0, h_in, nullptr, h_out, n_polys, P, Pq,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return dpfhe_mod_down_special(ctx, n_special, din, dout, cnt, t_plain, st);
+                     },
+                     [&] {
+                         return n_special < 1 || n_special >= ctx->hp.L
+                                    ? fail(DPFHE_ERR_INVALID, "n_special must be at least 1 and below the context's limbs") : DPFHE_OK;
+                     });
 }
 
 int dpfhe_ct_mul_plain_host(dpfhe_ctx *ctx, const uint64_t *h_ct, const uint64_t *h_pt, uint64_t *h_out, size_t batch) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
-    if (!h_ct || !h_pt || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
     const size_t P = ctx->P();
-    rc = upload_key(ctx, h_pt, P);
-    if (rc) return rc;
-    const size_t chunk = pick_chunk(ctx, 2 * P * 8, batch);
-    return run_pipeline(ctx, h_ct, nullptr, h_out, batch, 2 * P, 2 * P, chunk,
-                        [&](u64 *dc, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            CU_TRY(VCALL(launch_ct_mul_plain, ctx->lc, dc, ctx->stage_key, dout, cnt, st));
-                            note_launch(ctx, 1);
-                            return DPFHE_OK;
-                        });
+    return host_call(ctx, {h_ct, h_pt, h_out}, h_pt, P, h_ct, nullptr, h_out, batch, 2 * P, 2 * P,
+                     [&](u64 *dc, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                         CU_TRY(VCALL(launch_ct_mul_plain, ctx->lc, dc, ctx->stage_key.get(), dout, cnt, st));
+                         note_launch(ctx, 1);
+                         return DPFHE_OK;
+                     });
 }
 
 // ---------------------------------------------------------------- CKKS slot encoding (DESIGN.md §2.12)
 
-// `need` bytes of the slot encoders' scratch
-static int enc_work_prepare(dpfhe_ctx *ctx, size_t need, cudaStream_t st) {
-    if (need > ctx->enc_work_bytes) {
-        CU_TRY(cudaStreamSynchronize(st));   // the old scratch may still be in use on this stream
-        if (ctx->enc_work) cudaFree(ctx->enc_work);
-        ctx->enc_work = nullptr;
-        ctx->enc_work_bytes = 0;
-        CU_TRY(cudaMalloc(&ctx->enc_work, need));
-        ctx->enc_work_bytes = need;
-    }
-    return DPFHE_OK;
-}
-
-// the context's encoding tables (built and uploaded once) and `need` bytes of scratch
-static int ckks_prepare(dpfhe_ctx *ctx, size_t need, cudaStream_t st) {
-    if (!ctx->ckks_tab) {
+// the context's encoding tables (built and uploaded once) and `need` bytes of the slot encoders' scratch
+static int ckks_prepare(dpfhe_ctx *ctx, size_t need) {
+    if (!ctx->ckks_tab.bytes()) {
         std::vector<Cplx> tw;
         std::vector<uint32_t> tj;
         std::vector<uint64_t> pow2;
         build_ckks_tables(ctx->hp, tw, tj, pow2);
         const size_t b_tw = tw.size() * sizeof(Cplx), b_tj = tj.size() * 4, b_p2 = pow2.size() * 8;
-        void *p = nullptr;
-        CU_TRY(cudaMalloc(&p, b_tw + b_tj + b_p2));
-        unsigned char *base = (unsigned char *)p;
+        const int rc = ctx->ckks_tab.reserve(ctx, b_tw + b_tj + b_p2);
+        if (rc) return rc;
+        unsigned char *base = ctx->ckks_tab.get<unsigned char>();
         if (cudaMemcpy(base, tw.data(), b_tw, cudaMemcpyHostToDevice) != cudaSuccess ||
             cudaMemcpy(base + b_tw, pow2.data(), b_p2, cudaMemcpyHostToDevice) != cudaSuccess ||
             cudaMemcpy(base + b_tw + b_p2, tj.data(), b_tj, cudaMemcpyHostToDevice) != cudaSuccess) {
-            cudaFree(p);
+            ctx->ckks_tab.release();
             return fail(DPFHE_ERR_CUDA, "CUDA error at %s:%d: uploading the CKKS tables failed", __FILE__, __LINE__);
         }
-        ctx->ckks_tab = p;
-        ctx->ckks_tab_bytes = b_tw + b_tj + b_p2;
         ctx->ckks.tw = (const Cplx *)base;
         ctx->ckks.pow2 = (const u64 *)(base + b_tw);
         ctx->ckks.tj = (const u32 *)(base + b_tw + b_p2);
     }
-    return enc_work_prepare(ctx, need, st);
+    return ctx->enc_work.reserve(ctx, need);
 }
 
 static bool valid_scale(double scale) { return scale > 0.0 && scale <= 1.7976931348623157e308; }   // finite and positive (NaN fails both)
@@ -1063,10 +990,10 @@ int dpfhe_ckks_encode(dpfhe_ctx *ctx, const double *d_slots, uint64_t *d_pt, siz
     if (n_vec == 0) return DPFHE_OK;
     CHECK_PTR(d_slots); CHECK_PTR(d_pt);
     cudaStream_t st = pick(ctx, stream);
-    rc = ckks_prepare(ctx, n_vec * ctx->N() * sizeof(double), st);
+    rc = ckks_prepare(ctx, n_vec * ctx->N() * sizeof(double));
     if (rc) return rc;
     const double sc = scale * (2.0 / (double)ctx->N());
-    CU_TRY(VCALL(launch_ckks_encode, ctx->lc, (const Cplx *)d_slots, (double *)ctx->enc_work, d_pt, ctx->ckks, sc, n_vec, st));
+    CU_TRY(VCALL(launch_ckks_encode, ctx->lc, (const Cplx *)d_slots, ctx->enc_work.get<double>(), d_pt, ctx->ckks, sc, n_vec, st));
     note_launch(ctx, 2);   // ckks_enc_fft_kernel + ckks_enc_ntt(_pair)_kernel
     return DPFHE_OK;
 }
@@ -1079,9 +1006,9 @@ int dpfhe_ckks_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, double *d_slots, siz
     CHECK_PTR(d_pt); CHECK_PTR(d_slots);
     cudaStream_t st = pick(ctx, stream);
     const size_t bytes = n_vec * ctx->P() * 8;
-    rc = ckks_prepare(ctx, bytes, st);
+    rc = ckks_prepare(ctx, bytes);
     if (rc) return rc;
-    u64 *work = (u64 *)ctx->enc_work;
+    u64 *work = ctx->enc_work.get();
     CU_TRY(cudaMemcpyAsync(work, d_pt, bytes, cudaMemcpyDeviceToDevice, st));   // the caller's plaintexts stay unchanged
     CU_TRY(VCALL(launch_ntt, ctx->lc, work, n_vec, true, st));
     CkksConsts K;
@@ -1096,13 +1023,11 @@ int dpfhe_ckks_encode_host(dpfhe_ctx *ctx, const double *h_slots, uint64_t *h_pt
     if (rc) return rc;
     if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
     if (n_vec == 0) return DPFHE_OK;
-    if (!h_slots || !h_pt) return fail(DPFHE_ERR_INVALID, "null host pointer");
     const size_t P = ctx->P(), S = ctx->N();   // words of a plaintext, and of a slot vector (N/2 complex doubles)
-    const size_t chunk = pick_chunk(ctx, P * 8, n_vec);
-    return run_pipeline(ctx, (const u64 *)h_slots, nullptr, h_pt, n_vec, S, P, chunk,
-                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return dpfhe_ckks_encode(ctx, (const double *)din, dout, cnt, scale, st);
-                        });
+    return host_call(ctx, {h_slots, h_pt}, nullptr, 0, (const u64 *)h_slots, nullptr, h_pt, n_vec, S, P,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return dpfhe_ckks_encode(ctx, (const double *)din, dout, cnt, scale, st);
+                     });
 }
 
 int dpfhe_ckks_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, double *h_slots, size_t n_vec, double scale) {
@@ -1110,13 +1035,11 @@ int dpfhe_ckks_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, double *h_slots
     if (rc) return rc;
     if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
     if (n_vec == 0) return DPFHE_OK;
-    if (!h_slots || !h_pt) return fail(DPFHE_ERR_INVALID, "null host pointer");
     const size_t P = ctx->P(), S = ctx->N();
-    const size_t chunk = pick_chunk(ctx, P * 8, n_vec);
-    return run_pipeline(ctx, h_pt, nullptr, (u64 *)h_slots, n_vec, P, S, chunk,
-                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return dpfhe_ckks_decode(ctx, din, (double *)dout, cnt, scale, st);
-                        });
+    return host_call(ctx, {h_slots, h_pt}, nullptr, 0, h_pt, nullptr, (u64 *)h_slots, n_vec, P, S,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return dpfhe_ckks_decode(ctx, din, (double *)dout, cnt, scale, st);
+                     });
 }
 
 // ---------------------------------------------------------------- BGV slot encoding (DESIGN.md §2.13)
@@ -1130,36 +1053,28 @@ int dpfhe_ckks_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, double *h_slots
 
 // the tables of plaintext modulus t (kept for the last t used: built and uploaded on first use and whenever t changes) and
 // `need` bytes of scratch
-static int bgv_prepare(dpfhe_ctx *ctx, uint64_t t, size_t need, cudaStream_t st) {
+static int bgv_prepare(dpfhe_ctx *ctx, uint64_t t, size_t need) {
     if (ctx->bgv_t != t) {
         std::vector<uint32_t> tab;
         BgvTables T;
         if (!build_bgv_tables(ctx->hp, t, tab, T)) return fail(DPFHE_ERR_INVALID, "invalid plaintext modulus");
-        if (ctx->bgv_tab) {
-            // earlier calls may still read the old tables; st already waits for the last of them, whatever its stream (§4.7)
-            CU_TRY(cudaStreamSynchronize(st));
-            cudaFree(ctx->bgv_tab);
-            ctx->bgv_tab = nullptr;
-            ctx->bgv_tab_bytes = 0;
-            ctx->bgv_t = 0;
-            ctx->bgv = BgvTables();
-        }
+        int rc = ctx->bgv_tab.bytes() ? dpfhe_synchronize(ctx) : DPFHE_OK;   // earlier calls may still read the old tables
+        if (rc) return rc;
+        ctx->bgv_t = 0;
+        ctx->bgv = BgvTables();
         const size_t bytes = tab.size() * sizeof(uint32_t);
-        void *p = nullptr;
-        CU_TRY(cudaMalloc(&p, bytes));
-        if (cudaMemcpy(p, tab.data(), bytes, cudaMemcpyHostToDevice) != cudaSuccess) {
-            cudaFree(p);
+        rc = ctx->bgv_tab.reserve(ctx, bytes);
+        if (rc) return rc;
+        if (cudaMemcpy(ctx->bgv_tab.get<void>(), tab.data(), bytes, cudaMemcpyHostToDevice) != cudaSuccess) {
+            ctx->bgv_tab.release();
             return fail(DPFHE_ERR_CUDA, "CUDA error at %s:%d: uploading the BGV tables failed", __FILE__, __LINE__);
         }
-        const size_t N = ctx->N();
-        T.tw = (const u32 *)p;
-        T.pos = (const u32 *)p + 4 * N;
-        ctx->bgv_tab = p;
-        ctx->bgv_tab_bytes = bytes;
+        T.tw = ctx->bgv_tab.get<const u32>();
+        T.pos = T.tw + 4 * ctx->N();
         ctx->bgv = T;
         ctx->bgv_t = t;
     }
-    return enc_work_prepare(ctx, need, st);
+    return ctx->enc_work.reserve(ctx, need);
 }
 
 int dpfhe_bgv_encode(dpfhe_ctx *ctx, const int64_t *d_slots, uint64_t *d_pt, size_t n_vec, uint64_t t_plain, void *stream) {
@@ -1169,9 +1084,9 @@ int dpfhe_bgv_encode(dpfhe_ctx *ctx, const int64_t *d_slots, uint64_t *d_pt, siz
     if (n_vec == 0) return DPFHE_OK;
     CHECK_PTR(d_slots); CHECK_PTR(d_pt);
     cudaStream_t st = pick(ctx, stream);
-    rc = bgv_prepare(ctx, t_plain, n_vec * ctx->N() * sizeof(u32), st);
+    rc = bgv_prepare(ctx, t_plain, n_vec * ctx->N() * sizeof(u32));
     if (rc) return rc;
-    CU_TRY(VCALL(launch_bgv_encode, ctx->lc, d_slots, (u32 *)ctx->enc_work, d_pt, ctx->bgv, n_vec, st));
+    CU_TRY(VCALL(launch_bgv_encode, ctx->lc, d_slots, ctx->enc_work.get<u32>(), d_pt, ctx->bgv, n_vec, st));
     note_launch(ctx, 2);   // bgv_enc_kernel + bgv_enc_ntt(_pair)_kernel
     return DPFHE_OK;
 }
@@ -1184,9 +1099,9 @@ int dpfhe_bgv_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, uint64_t *d_slots, si
     CHECK_PTR(d_pt); CHECK_PTR(d_slots);
     cudaStream_t st = pick(ctx, stream);
     const size_t bytes = n_vec * ctx->P() * 8;
-    rc = bgv_prepare(ctx, t_plain, bytes, st);
+    rc = bgv_prepare(ctx, t_plain, bytes);
     if (rc) return rc;
-    u64 *work = (u64 *)ctx->enc_work;
+    u64 *work = ctx->enc_work.get();
     CU_TRY(cudaMemcpyAsync(work, d_pt, bytes, cudaMemcpyDeviceToDevice, st));   // the caller's plaintexts stay unchanged
     CU_TRY(VCALL(launch_ntt, ctx->lc, work, n_vec, true, st));
     BgvConsts K;
@@ -1201,13 +1116,11 @@ int dpfhe_bgv_encode_host(dpfhe_ctx *ctx, const int64_t *h_slots, uint64_t *h_pt
     if (rc) return rc;
     CHECK_T(t_plain);
     if (n_vec == 0) return DPFHE_OK;
-    if (!h_slots || !h_pt) return fail(DPFHE_ERR_INVALID, "null host pointer");
     const size_t P = ctx->P(), S = ctx->N();   // words of a plaintext, and of a slot vector
-    const size_t chunk = pick_chunk(ctx, P * 8, n_vec);
-    return run_pipeline(ctx, (const u64 *)h_slots, nullptr, h_pt, n_vec, S, P, chunk,
-                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return dpfhe_bgv_encode(ctx, (const int64_t *)din, dout, cnt, t_plain, st);
-                        });
+    return host_call(ctx, {h_slots, h_pt}, nullptr, 0, (const u64 *)h_slots, nullptr, h_pt, n_vec, S, P,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return dpfhe_bgv_encode(ctx, (const int64_t *)din, dout, cnt, t_plain, st);
+                     });
 }
 
 int dpfhe_bgv_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, uint64_t *h_slots, size_t n_vec, uint64_t t_plain) {
@@ -1215,13 +1128,11 @@ int dpfhe_bgv_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, uint64_t *h_slot
     if (rc) return rc;
     CHECK_T(t_plain);
     if (n_vec == 0) return DPFHE_OK;
-    if (!h_slots || !h_pt) return fail(DPFHE_ERR_INVALID, "null host pointer");
     const size_t P = ctx->P(), S = ctx->N();
-    const size_t chunk = pick_chunk(ctx, P * 8, n_vec);
-    return run_pipeline(ctx, h_pt, nullptr, h_slots, n_vec, P, S, chunk,
-                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return dpfhe_bgv_decode(ctx, din, dout, cnt, t_plain, st);
-                        });
+    return host_call(ctx, {h_slots, h_pt}, nullptr, 0, h_pt, nullptr, h_slots, n_vec, P, S,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return dpfhe_bgv_decode(ctx, din, dout, cnt, t_plain, st);
+                     });
 }
 #undef CHECK_T
 
@@ -1284,9 +1195,10 @@ int dpfhe_galois_keygen(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, co
     if (rc) return rc;
     if (n_elts == 0) return DPFHE_OK;
     if (!galois_elts) return fail(DPFHE_ERR_INVALID, "null galois_elts");
-    const uint64_t two_n = (uint64_t)2 << ctx->hp.log_n;
-    for (size_t e = 0; e < n_elts; ++e)
-        if (!(galois_elts[e] & 1) || galois_elts[e] >= two_n) return fail(DPFHE_ERR_INVALID, "galois element must be odd and < 2N");
+    for (size_t e = 0; e < n_elts; ++e) {
+        rc = check_galois(ctx, galois_elts[e]);
+        if (rc) return rc;
+    }
     CHECK_PTR(d_sk); CHECK_PTR(d_keys);
     KeyArgs A = build_key_args(ctx->hp, seed, n_special, t_plain);
     A.s = d_sk;
@@ -1380,9 +1292,8 @@ int dpfhe_relin_keygen_host(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain
     rc = check_key_special(ctx, n_special);
     if (rc) return rc;
     if (!h_sk) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    const unsigned L = ctx->hp.L, ndig = n_special ? (L - n_special + n_special - 1) / n_special : L;
     const KeygenHostArgs args{n_special, t_plain, seed, 0, nullptr};
-    return keygen_host(ctx, h_sk, (size_t)ndig * 2 * ctx->P(), h_key,
+    return keygen_host(ctx, h_sk, key_digits(ctx, n_special) * 2 * ctx->P(), h_key,
                        [](dpfhe_ctx *c, const uint64_t *sk, uint64_t *out, const void *a) {
                            const KeygenHostArgs &k = *(const KeygenHostArgs *)a;
                            return dpfhe_relin_keygen(c, k.n_special, k.t_plain, sk, k.seed, out, nullptr);
@@ -1398,9 +1309,8 @@ int dpfhe_galois_keygen_host(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plai
     if (rc) return rc;
     if (n_elts == 0) return DPFHE_OK;
     if (!h_sk) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    const unsigned L = ctx->hp.L, ndig = n_special ? (L - n_special + n_special - 1) / n_special : L;
     const KeygenHostArgs args{n_special, t_plain, seed, n_elts, galois_elts};
-    return keygen_host(ctx, h_sk, n_elts * ndig * 2 * ctx->P(), h_keys,
+    return keygen_host(ctx, h_sk, n_elts * key_digits(ctx, n_special) * 2 * ctx->P(), h_keys,
                        [](dpfhe_ctx *c, const uint64_t *sk, uint64_t *out, const void *a) {
                            const KeygenHostArgs &k = *(const KeygenHostArgs *)a;
                            return dpfhe_galois_keygen(c, k.n_special, k.t_plain, sk, k.n_elts, k.galois_elts, k.seed, out, nullptr);
@@ -1413,18 +1323,14 @@ int dpfhe_encrypt_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_sk, c
     if (rc) return rc;
     CHECK_SEED(seed);
     if (n == 0) return DPFHE_OK;
-    if (!h_sk || !h_pt || !h_ct) return fail(DPFHE_ERR_INVALID, "null host pointer");
     const size_t P = ctx->P();
-    rc = upload_key(ctx, h_sk, P);
-    if (rc) return rc;
-    const size_t chunk = pick_chunk(ctx, 2 * P * 8, n);
     uint64_t next = first_index;   // the chunks run in order: ciphertext k keeps item number first_index + k
-    return run_pipeline(ctx, h_pt, nullptr, h_ct, n, P, 2 * P, chunk,
-                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            const int r = dpfhe_encrypt(ctx, t_plain, ctx->stage_key, seed, next, din, dout, cnt, st);
-                            next += cnt;
-                            return r;
-                        });
+    return host_call(ctx, {h_sk, h_pt, h_ct}, h_sk, P, h_pt, nullptr, h_ct, n, P, 2 * P,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         const int r = dpfhe_encrypt(ctx, t_plain, ctx->stage_key.get(), seed, next, din, dout, cnt, st);
+                         next += cnt;
+                         return r;
+                     });
 }
 
 int dpfhe_decrypt_host(dpfhe_ctx *ctx, const uint64_t *h_sk, const uint64_t *h_ct, unsigned n_comp, uint64_t *h_pt, size_t n) {
@@ -1432,15 +1338,11 @@ int dpfhe_decrypt_host(dpfhe_ctx *ctx, const uint64_t *h_sk, const uint64_t *h_c
     if (rc) return rc;
     if (n_comp != 2 && n_comp != 3) return fail(DPFHE_ERR_INVALID, "n_comp must be 2 or 3");
     if (n == 0) return DPFHE_OK;
-    if (!h_sk || !h_ct || !h_pt) return fail(DPFHE_ERR_INVALID, "null host pointer");
     const size_t P = ctx->P();
-    rc = upload_key(ctx, h_sk, P);
-    if (rc) return rc;
-    const size_t chunk = pick_chunk(ctx, n_comp * P * 8, n);
-    return run_pipeline(ctx, h_ct, nullptr, h_pt, n, n_comp * P, P, chunk,
-                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            return dpfhe_decrypt(ctx, ctx->stage_key, din, n_comp, dout, cnt, st);
-                        });
+    return host_call(ctx, {h_sk, h_ct, h_pt}, h_sk, P, h_ct, nullptr, h_pt, n, n_comp * P, P,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return dpfhe_decrypt(ctx, ctx->stage_key.get(), din, n_comp, dout, cnt, st);
+                     });
 }
 #undef CHECK_SEED
 
@@ -1579,21 +1481,12 @@ struct dpfhe_linear {
     uint64_t t_plain = 0;                   // grouped: plaintext modulus of the divisions by P (0: plain rounding)
     MsConsts K;                             // grouped: constants of the division by P
     GroupConsts G;
-    u64 *scratch = nullptr;                 // [baby + giant + 1][cap][2][Lq][N]
-    size_t cap = 0;                         // ciphertexts the scratch holds
+    DeviceScratch scratch;                  // [baby + giant + 1][batch][2][Lq][N] for the largest batch applied so far
 };
 
+// the scratch of an application to `batch` ciphertexts
 static int linear_reserve(dpfhe_linear *lin, size_t batch) {
-    if (batch <= lin->cap) return DPFHE_OK;
-    dpfhe_ctx *ctx = lin->ctx;
-    int rc = dpfhe_synchronize(ctx);
-    if (rc) return rc;
-    cudaFree(lin->scratch);
-    lin->scratch = nullptr;
-    lin->cap = 0;
-    CU_TRY(cudaMalloc(&lin->scratch, (lin->baby + lin->giant + 1) * batch * 2 * lin->Lq * ctx->N() * 8));
-    lin->cap = batch;
-    return DPFHE_OK;
+    return lin->scratch.reserve(lin->ctx, (lin->baby + lin->giant + 1) * batch * 2 * lin->Lq * lin->ctx->N() * 8);
 }
 
 static int linear_check_shape(size_t n_diags, size_t baby, const uint64_t *h_gk_baby, const uint64_t *h_gk_giant) {
@@ -1604,81 +1497,18 @@ static int linear_check_shape(size_t n_diags, size_t baby, const uint64_t *h_gk_
     return DPFHE_OK;
 }
 
-int dpfhe_linear_create(dpfhe_ctx *ctx, const uint64_t *h_diags, size_t n_diags, size_t baby, const uint64_t *h_gk_baby, const uint64_t *h_gk_giant,
-                        dpfhe_linear **out) {
-    int rc = enter(ctx);
-    if (rc) return rc;
-    if (!out || !h_diags) return fail(DPFHE_ERR_INVALID, "null argument");
-    *out = nullptr;
-    rc = linear_check_shape(n_diags, baby, h_gk_baby, h_gk_giant);
-    if (rc) return rc;
-    const size_t giant = n_diags / baby;
+// The start of both constructors: a layer with its diagonals and keys on the device (grouped keys: and room for the companions of
+// every key), and the Galois elements of its rotations.
+static int linear_new(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *h_diags, size_t n_diags, size_t baby,
+                      const uint64_t *h_gk_baby, const uint64_t *h_gk_giant, dpfhe_linear **out) {
     dpfhe_linear *lin = new (std::nothrow) dpfhe_linear();
     if (!lin) return fail(DPFHE_ERR_NOMEM, "out of host memory");
-    lin->ctx = ctx; lin->n = n_diags; lin->baby = baby; lin->giant = giant; lin->Lq = ctx->hp.L;
-    const size_t P8 = ctx->P() * 8, key_bytes = 2 * ctx->hp.L * P8;
-    cudaError_t e = cudaMalloc(&lin->d_diags, n_diags * P8);
-    if (e == cudaSuccess) e = cudaMalloc(&lin->d_keys, baby * key_bytes);
-    if (e == cudaSuccess) e = cudaMemcpy(lin->d_diags, h_diags, n_diags * P8, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess && baby > 1) e = cudaMemcpy(lin->d_keys, h_gk_baby, (baby - 1) * key_bytes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess && giant > 1) e = cudaMemcpy(lin->d_keys + (baby - 1) * key_bytes / 8, h_gk_giant, key_bytes, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-        dpfhe_linear_destroy(lin);
-        return fail(DPFHE_ERR_CUDA, "linear layer upload: %s", cudaGetErrorString(e));
-    }
-    for (size_t b = 1; b < baby; ++b) {
-        uint64_t g = 0;
-        dpfhe_galois_element(ctx, (int)b, &g);
-        lin->g_baby.push_back(g);
-        lin->k_baby.push_back(lin->d_keys + (b - 1) * key_bytes / 8);
-    }
-    dpfhe_galois_element(ctx, (int)baby, &lin->g_giant);
-    // the constants of the baby-step rotations do not depend on the data: prepare them once (four small launches per rotation
-    // that every hoisted call would otherwise repeat — a tenth of a 31-rotation call at batch 512, more for smaller chunks)
-    if (baby > 1) {
-        const size_t ks_words = 2 * ctx->hp.L * ctx->P(), kp_words = 2 * ctx->P();
-        int rc2 = ensure_hoist_consts(ctx);
-        e = rc2 == DPFHE_OK ? cudaMalloc(&lin->d_prep, (baby - 1) * (ks_words + kp_words) * 8) : cudaErrorMemoryAllocation;
-        cudaStream_t st = pick(ctx, nullptr);
-        for (size_t b = 1; b < baby && e == cudaSuccess; ++b) {
-            u64 *ks = lin->d_prep + (b - 1) * (ks_words + kp_words), *kp = ks + ks_words;
-            e = VCALL(launch_rot_prepare, ctx->lc, lin->k_baby[b - 1], (u32)lin->g_baby[b - 1], ctx->hoist_delta, ctx->hoist_M, kp, st, ks);
-            note_launch(ctx, 4);
-            lin->prep.push_back(ks);
-            lin->prep.push_back(kp);
-        }
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) {
-            dpfhe_linear_destroy(lin);
-            return fail(DPFHE_ERR_CUDA, "linear layer constants: %s", cudaGetErrorString(e));
-        }
-    }
-    *out = lin;
-    return DPFHE_OK;
-}
-
-int dpfhe_linear_create_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_diags, size_t n_diags, size_t baby,
-                                const uint64_t *h_gk_baby, const uint64_t *h_gk_giant, uint64_t t_plain, dpfhe_linear **out) {
-    int rc = enter(ctx);
-    if (rc) return rc;
-    if (!out || !h_diags) return fail(DPFHE_ERR_INVALID, "null argument");
-    *out = nullptr;
-    rc = check_special(ctx, n_special);
-    if (rc) return rc;
-    const unsigned L = ctx->hp.L;
-    for (unsigned k = 0; k < n_special; ++k)
-        if (t_plain >= ctx->hp.limbs[L - 1 - k].lp.q) return fail(DPFHE_ERR_INVALID, "plaintext modulus must be below the special prime");
-    rc = linear_check_shape(n_diags, baby, h_gk_baby, h_gk_giant);
-    if (rc) return rc;
-    dpfhe_linear *lin = new (std::nothrow) dpfhe_linear();
-    if (!lin) return fail(DPFHE_ERR_NOMEM, "out of host memory");
-    const size_t N = ctx->N(), Lq = L - n_special, dnum = (Lq + n_special - 1) / n_special, key_bytes = dnum * 2 * L * N * 8;
+    const size_t Lq = ctx->hp.L - n_special, diag_bytes = n_diags * Lq * ctx->N() * 8, key_bytes = key_digits(ctx, n_special) * 2 * ctx->P() * 8;
     lin->ctx = ctx; lin->n = n_diags; lin->baby = baby; lin->giant = n_diags / baby; lin->n_special = n_special; lin->Lq = Lq; lin->t_plain = t_plain;
-    build_group_consts(ctx->hp, n_special, t_plain, lin->G, lin->K);
-    cudaError_t e = cudaMalloc(&lin->d_diags, n_diags * Lq * N * 8);
+    cudaError_t e = cudaMalloc(&lin->d_diags, diag_bytes);
     if (e == cudaSuccess) e = cudaMalloc(&lin->d_keys, baby * key_bytes);
-    if (e == cudaSuccess) e = cudaMalloc(&lin->d_prep, baby * key_bytes);
-    if (e == cudaSuccess) e = cudaMemcpy(lin->d_diags, h_diags, n_diags * Lq * N * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && n_special) e = cudaMalloc(&lin->d_prep, baby * key_bytes);
+    if (e == cudaSuccess) e = cudaMemcpy(lin->d_diags, h_diags, diag_bytes, cudaMemcpyHostToDevice);
     if (e == cudaSuccess && baby > 1) e = cudaMemcpy(lin->d_keys, h_gk_baby, (baby - 1) * key_bytes, cudaMemcpyHostToDevice);
     if (e == cudaSuccess && lin->giant > 1) e = cudaMemcpy(lin->d_keys + (baby - 1) * key_bytes / 8, h_gk_giant, key_bytes, cudaMemcpyHostToDevice);
     if (e != cudaSuccess) {
@@ -1690,23 +1520,15 @@ int dpfhe_linear_create_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64
         dpfhe_galois_element(ctx, (int)b, &g);
         lin->g_baby.push_back(g);
         lin->k_baby.push_back(lin->d_keys + (b - 1) * key_bytes / 8);
-        lin->prep.push_back(lin->d_prep + (b - 1) * key_bytes / 8);
     }
     dpfhe_galois_element(ctx, (int)baby, &lin->g_giant);
-    lin->prep_giant = lin->d_prep + (baby - 1) * key_bytes / 8;
-    // the Shoup companions of every key, once: each application would otherwise rebuild them for every rotation
-    rc = lin->giant > 1 ? ensure_hyb(ctx) : DPFHE_OK;   // the special-prime rows of the giant steps' kernel
-    if (rc) {
-        dpfhe_linear_destroy(lin);
-        return rc;
-    }
-    cudaStream_t st = pick(ctx, nullptr);
-    for (size_t b = 0; b < baby && e == cudaSuccess; ++b) {
-        if (b + 1 < baby || lin->giant > 1) {
-            e = VCALL(launch_key_prepare_grouped, ctx->lc, lin->d_keys + b * key_bytes / 8, lin->d_prep + b * key_bytes / 8, (u32)dnum, st);
-            note_launch(ctx, 1);
-        }
-    }
+    *out = lin;
+    return DPFHE_OK;
+}
+
+// The end of both constructors: waits for the launches on `st` that prepared the layer's constants (e: the first error of
+// issuing them) and hands out the layer, or destroys it.
+static int linear_finish(dpfhe_linear *lin, cudaError_t e, cudaStream_t st, dpfhe_linear **out) {
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) {
         dpfhe_linear_destroy(lin);
@@ -1714,6 +1536,71 @@ int dpfhe_linear_create_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64
     }
     *out = lin;
     return DPFHE_OK;
+}
+
+int dpfhe_linear_create(dpfhe_ctx *ctx, const uint64_t *h_diags, size_t n_diags, size_t baby, const uint64_t *h_gk_baby, const uint64_t *h_gk_giant,
+                        dpfhe_linear **out) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!out || !h_diags) return fail(DPFHE_ERR_INVALID, "null argument");
+    *out = nullptr;
+    rc = linear_check_shape(n_diags, baby, h_gk_baby, h_gk_giant);
+    if (rc) return rc;
+    dpfhe_linear *lin = nullptr;
+    rc = linear_new(ctx, 0, 0, h_diags, n_diags, baby, h_gk_baby, h_gk_giant, &lin);
+    if (rc) return rc;
+    // the constants of the baby-step rotations do not depend on the data: prepare them once (four small launches per rotation
+    // that every hoisted call would otherwise repeat — a tenth of a 31-rotation call at batch 512, more for smaller chunks)
+    cudaError_t e = cudaSuccess;
+    cudaStream_t st = pick(ctx, nullptr);
+    if (baby > 1) {
+        const size_t ks_words = 2 * ctx->hp.L * ctx->P(), kp_words = 2 * ctx->P();
+        e = ensure_hoist_consts(ctx) == DPFHE_OK ? cudaMalloc(&lin->d_prep, (baby - 1) * (ks_words + kp_words) * 8) : cudaErrorMemoryAllocation;
+        for (size_t b = 1; b < baby && e == cudaSuccess; ++b) {
+            u64 *ks = lin->d_prep + (b - 1) * (ks_words + kp_words), *kp = ks + ks_words;
+            e = VCALL(launch_rot_prepare, ctx->lc, lin->k_baby[b - 1], (u32)lin->g_baby[b - 1], ctx->hoist_delta.get(), ctx->hoist_M.get(), kp, st, ks);
+            note_launch(ctx, 4);
+            lin->prep.push_back(ks);
+            lin->prep.push_back(kp);
+        }
+    }
+    return linear_finish(lin, e, st, out);
+}
+
+int dpfhe_linear_create_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_diags, size_t n_diags, size_t baby,
+                                const uint64_t *h_gk_baby, const uint64_t *h_gk_giant, uint64_t t_plain, dpfhe_linear **out) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!out || !h_diags) return fail(DPFHE_ERR_INVALID, "null argument");
+    *out = nullptr;
+    rc = check_special(ctx, n_special);
+    if (rc) return rc;
+    rc = check_t_below_special(ctx, n_special, t_plain);
+    if (rc) return rc;
+    rc = linear_check_shape(n_diags, baby, h_gk_baby, h_gk_giant);
+    if (rc) return rc;
+    dpfhe_linear *lin = nullptr;
+    rc = linear_new(ctx, n_special, t_plain, h_diags, n_diags, baby, h_gk_baby, h_gk_giant, &lin);
+    if (rc) return rc;
+    build_group_consts(ctx->hp, n_special, t_plain, lin->G, lin->K);
+    const size_t dnum = key_digits(ctx, n_special), key_words = dnum * 2 * ctx->P();
+    for (size_t b = 1; b < baby; ++b) lin->prep.push_back(lin->d_prep + (b - 1) * key_words);
+    lin->prep_giant = lin->d_prep + (baby - 1) * key_words;
+    // the Shoup companions of every key, once: each application would otherwise rebuild them for every rotation
+    rc = lin->giant > 1 ? ensure_hyb(ctx) : DPFHE_OK;   // the special-prime rows of the giant steps' kernel
+    if (rc) {
+        dpfhe_linear_destroy(lin);
+        return rc;
+    }
+    cudaError_t e = cudaSuccess;
+    cudaStream_t st = pick(ctx, nullptr);
+    for (size_t b = 0; b < baby && e == cudaSuccess; ++b) {
+        if (b + 1 < baby || lin->giant > 1) {
+            e = VCALL(launch_key_prepare_grouped, ctx->lc, lin->d_keys + b * key_words, lin->d_prep + b * key_words, (u32)dnum, st);
+            note_launch(ctx, 1);
+        }
+    }
+    return linear_finish(lin, e, st, out);
 }
 
 void dpfhe_linear_destroy(dpfhe_linear *lin) {
@@ -1725,8 +1612,7 @@ void dpfhe_linear_destroy(dpfhe_linear *lin) {
     cudaFree(lin->d_diags);
     cudaFree(lin->d_keys);
     cudaFree(lin->d_prep);
-    cudaFree(lin->scratch);
-    delete lin;
+    delete lin;   // frees the scratch
 }
 
 // grouped keys: hoisted baby steps, the inner sums on the ciphertext moduli, giant - 1 fused Horner steps.  Launches per application
@@ -1735,7 +1621,7 @@ void dpfhe_linear_destroy(dpfhe_linear *lin) {
 static int linear_apply_grouped_on(dpfhe_linear *lin, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
     dpfhe_ctx *ctx = lin->ctx;
     const size_t ctb = batch * 2 * lin->Lq * ctx->N();          // words of one ciphertext batch
-    u64 *steps = lin->scratch, *inner = steps + lin->baby * ctb, *tmp = inner + lin->giant * ctb;
+    u64 *steps = lin->scratch.get(), *inner = steps + lin->baby * ctb, *tmp = inner + lin->giant * ctb;
     cudaStream_t st = pick(ctx, stream);
     CU_TRY(cudaMemcpyAsync(steps, d_ct, ctb * 8, cudaMemcpyDeviceToDevice, st));
     int rc = DPFHE_OK;
@@ -1773,7 +1659,7 @@ static int linear_apply_on(dpfhe_linear *lin, const uint64_t *d_ct, uint64_t *d_
     if (lin->n_special) return linear_apply_grouped_on(lin, d_ct, d_out, batch, stream);
     dpfhe_ctx *ctx = lin->ctx;
     const size_t ctb = batch * 2 * ctx->P();                 // words of one ciphertext batch
-    u64 *steps = lin->scratch, *inner = steps + lin->baby * ctb, *tmp = inner + lin->giant * ctb;
+    u64 *steps = lin->scratch.get(), *inner = steps + lin->baby * ctb, *tmp = inner + lin->giant * ctb;
     cudaStream_t st = pick(ctx, stream);
     CU_TRY(cudaMemcpyAsync(steps, d_ct, ctb * 8, cudaMemcpyDeviceToDevice, st));
     int rc = DPFHE_OK;
@@ -1814,17 +1700,7 @@ int dpfhe_linear_apply_host(dpfhe_linear *lin, const uint64_t *h_ct, uint64_t *h
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
     if (!h_ct || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    // Chunks of about a fifth of the batch, rounded to whole rounds of the persistent key-switch grid (3 CTAs per SM, L CTAs
-    // per ciphertext: with grouped keys L = Lq + K, every limb of the context): a chunk that leaves the grid's last round mostly
-    // empty costs more than the transfers it hides.  The
-    // first upload and the last download are the only transfers not overlapped with a neighbouring chunk's compute.
-    const size_t groups = std::max<size_t>(1, (size_t)ctx->lc.num_sms * 3 / ctx->hp.L);
-    size_t rounds = (batch / 5 + groups / 2) / groups;
-    if (const char *e = getenv("DPFHE_LINEAR_CHUNK_ROUNDS")) rounds = (size_t)atol(e);   // tuning
-    if (rounds < 1) rounds = 1;
-    size_t chunk = rounds * groups;
-    if (chunk > 512) chunk = std::max<size_t>(groups, 512 / groups * groups);
-    if (chunk > batch) chunk = batch;
+    const size_t chunk = std::min(grid_round_chunk(ctx, batch, "DPFHE_LINEAR_CHUNK_ROUNDS"), batch);
     rc = linear_reserve(lin, chunk);
     if (rc) return rc;
     const size_t ct_words = 2 * lin->Lq * ctx->N();
@@ -1871,19 +1747,15 @@ int dpfhe_ct_add_plain_host(dpfhe_ctx *ctx, const uint64_t *h_ct, const uint64_t
     int rc = enter(ctx);
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
-    if (!h_ct || !h_pt || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
     const size_t P = ctx->P();
-    rc = upload_key(ctx, h_pt, P);
-    if (rc) return rc;
-    const size_t chunk = pick_chunk(ctx, 2 * P * 8, batch);
     const int64_t one = 1;
-    return run_pipeline(ctx, h_ct, nullptr, h_out, batch, 2 * P, 2 * P, chunk,
-                        [&](u64 *dc, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
-                            const u64 *in = dc;
-                            CU_TRY(VCALL(launch_lincomb, ctx->lc, &in, &one, 1u, (int64_t)0, ctx->stage_key, dout, cnt, st));
-                            note_launch(ctx, 1);
-                            return DPFHE_OK;
-                        });
+    return host_call(ctx, {h_ct, h_pt, h_out}, h_pt, P, h_ct, nullptr, h_out, batch, 2 * P, 2 * P,
+                     [&](u64 *dc, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                         const u64 *in = dc;
+                         CU_TRY(VCALL(launch_lincomb, ctx->lc, &in, &one, 1u, (int64_t)0, ctx->stage_key.get(), dout, cnt, st));
+                         note_launch(ctx, 1);
+                         return DPFHE_OK;
+                     });
 }
 
 namespace {
@@ -1943,8 +1815,7 @@ struct dpfhe_polyeval {
     std::vector<PeOp> ops;
     std::vector<unsigned> bufs;          // level of every scratch buffer
     size_t fixed_bytes = 0;              // level tables and keys
-    u64 *scratch = nullptr;              // the buffers back to back, then the switch's tau rows [2 cap][N]
-    size_t cap = 0, scratch_bytes = 0;
+    DeviceScratch scratch;               // the buffers back to back, then the switch's tau rows [2 batch][N], for the largest batch so far
 };
 
 namespace {
@@ -1965,27 +1836,16 @@ void pe_free(dpfhe_polyeval *pe) {
         cudaFree(v.key);
         cudaFree(v.key_s);
     }
-    cudaFree(pe->scratch);
-    if (pe->ctx) pe->ctx->object_bytes -= pe->fixed_bytes + pe->scratch_bytes;
+    if (pe->ctx) pe->ctx->object_bytes -= pe->fixed_bytes + pe->scratch.bytes();
     delete pe;
 }
 
+// the scratch of an application to `batch` ciphertexts, counted in the context's device bytes
 int pe_reserve(dpfhe_polyeval *pe, size_t batch) {
-    if (batch <= pe->cap || pe->bufs.empty()) return DPFHE_OK;
-    dpfhe_ctx *ctx = pe->ctx;
-    int rc = dpfhe_synchronize(ctx);
-    if (rc) return rc;
-    cudaFree(pe->scratch);
-    pe->scratch = nullptr;
-    ctx->object_bytes -= pe->scratch_bytes;
-    pe->scratch_bytes = 0;
-    pe->cap = 0;
-    const size_t bytes = pe_scratch_words(pe, batch) * 8;
-    CU_TRY(cudaMalloc(&pe->scratch, bytes));
-    pe->scratch_bytes = bytes;
-    ctx->object_bytes += bytes;
-    pe->cap = batch;
-    return DPFHE_OK;
+    pe->ctx->object_bytes -= pe->scratch.bytes();
+    const int rc = pe->scratch.reserve(pe->ctx, pe_scratch_words(pe, batch) * 8);
+    pe->ctx->object_bytes += pe->scratch.bytes();
+    return rc;
 }
 
 // the schedule of DESIGN.md §2.15: powers in increasing order, each operand brought to the product's level by single-limb switches
@@ -2109,28 +1969,15 @@ int pe_level(dpfhe_polyeval *pe, PeLevel &v, unsigned l, const uint64_t *h_key, 
     std::string msg = build_host_params(ctx->hp.log_n, Ll, mod.data(), v.hp);
     if (!msg.empty()) return fail(DPFHE_ERR_INVALID, "%s", msg.c_str());
     build_group_consts(v.hp, K, pe->t, v.G, v.K);
-    memset(&v.lt, 0, sizeof(v.lt));
-    uint64_t qmin = ~0ull, qmax = 0;
-    for (unsigned i = 0; i < Ll; ++i) {
-        v.lt.lp[i] = v.hp.limbs[i].lp;
-        qmin = std::min(qmin, mod[i]);
-        qmax = std::max(qmax, mod[i]);
-    }
-    v.lift_reduce = !(qmax < 2 * qmin) || getenv("DPFHE_LIFT_REDUCE") != nullptr;   // as dpfhe_context_create
-    if (l == Lq) {
+    if (l == Lq) {   // the context's own basis
         v.d_lp = ctx->d_lp;
         v.d_tw = ctx->d_tw;
         v.d_itw = ctx->d_itw;
+        v.lt = ctx->lc.lt;
+        v.lift_reduce = ctx->lc.lift_reduce;
     } else {
-        CU_TRY(cudaMalloc(&v.d_lp, Ll * sizeof(LimbParams)));
-        CU_TRY(cudaMalloc(&v.d_tw, Ll * N * sizeof(Twiddle)));
-        CU_TRY(cudaMalloc(&v.d_itw, Ll * N * sizeof(Twiddle)));
-        pe->fixed_bytes += Ll * sizeof(LimbParams) + 2 * Ll * N * sizeof(Twiddle);
-        for (unsigned i = 0; i < Ll; ++i) {
-            CU_TRY(cudaMemcpy(v.d_tw + i * N, v.hp.limbs[i].tw.data(), N * sizeof(Twiddle), cudaMemcpyHostToDevice));
-            CU_TRY(cudaMemcpy(v.d_itw + i * N, v.hp.limbs[i].itw.data(), N * sizeof(Twiddle), cudaMemcpyHostToDevice));
-        }
-        CU_TRY(cudaMemcpy(v.d_lp, v.lt.lp, Ll * sizeof(LimbParams), cudaMemcpyHostToDevice));
+        const int rc = upload_basis(v.hp, v.d_lp, v.d_tw, v.d_itw, v.lt, v.lift_reduce, pe->fixed_bytes);
+        if (rc) return rc;
     }
     // the key of level l: digits g < ceil(l / K), limb rows 0 .. l-1 and the special rows Lq .. Lq+K-1 of the top-level key
     const size_t key_words = dl * 2 * Ll * N;
@@ -2154,7 +2001,7 @@ int pe_apply_on(dpfhe_polyeval *pe, const u64 *d_ct, u64 *d_out, size_t batch, v
     dpfhe_ctx *ctx = pe->ctx;
     const size_t N = ctx->N();
     std::vector<u64 *> ptr(pe->bufs.size());
-    u64 *p = pe->scratch;
+    u64 *p = pe->scratch.get();
     for (size_t i = 0; i < pe->bufs.size(); ++i) {
         ptr[i] = p;
         p += batch * 2 * pe->bufs[i] * N;
@@ -2276,14 +2123,9 @@ int dpfhe_polyeval_apply_host(dpfhe_polyeval *pe, const uint64_t *h_ct, uint64_t
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
     if (!h_ct || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    // chunks of about a fifth of the batch in whole rounds of the persistent key-switch grid, as dpfhe_linear_apply_host
-    const size_t groups = std::max<size_t>(1, (size_t)ctx->lc.num_sms * 3 / ctx->hp.L);
-    size_t rounds = (batch / 5 + groups / 2) / groups;
-    if (rounds < 1) rounds = 1;
-    size_t chunk = rounds * groups;
-    if (chunk > 512) chunk = std::max<size_t>(groups, 512 / groups * groups);
+    size_t chunk = grid_round_chunk(ctx, batch, nullptr);
     if (const char *e = getenv("DPFHE_POLYEVAL_CHUNK")) chunk = std::max<size_t>(1, (size_t)atol(e));   // tests: several chunks at a small batch
-    if (chunk > batch) chunk = batch;
+    chunk = std::min(chunk, batch);
     rc = pe_reserve(pe, chunk);
     if (rc) return rc;
     const size_t N = ctx->N();

@@ -4,11 +4,38 @@
 
 #include <cstddef>
 #include <cstdint>
+#include <initializer_list>
 
 #include "host_params.hpp"
 #include "launch.hpp"
 
 constexpr int DPFHE_PIPE_DEPTH = 3;
+
+struct dpfhe_ctx;
+
+// A device buffer that grows on demand and is owned by one context (or by an object built on it).  reserve() replaces it by a
+// larger one only after all of the context's earlier work has finished, since any earlier call may still use it; a failed
+// allocation leaves it empty, so the next call retries.
+class DeviceScratch {
+public:
+    DeviceScratch() = default;
+    DeviceScratch(const DeviceScratch &) = delete;
+    DeviceScratch &operator=(const DeviceScratch &) = delete;
+    ~DeviceScratch() { release(); }
+    int reserve(dpfhe_ctx *ctx, size_t bytes);   // abi.cu
+    void release() {
+        cudaFree(p_);
+        p_ = nullptr;
+        bytes_ = 0;
+    }
+    size_t bytes() const { return bytes_; }
+    template <class T = dpfhe::u64>
+    T *get() const { return static_cast<T *>(p_); }
+
+private:
+    void *p_ = nullptr;
+    size_t bytes_ = 0;
+};
 
 struct dpfhe_ctx {
     dpfhe::HostParams hp;
@@ -26,33 +53,28 @@ struct dpfhe_ctx {
     cudaStream_t cur = nullptr, last_stream = nullptr;
     cudaEvent_t ev_last = nullptr;
     bool have_last = false;
-    // staging for the host-buffer entry points (allocated on first use)
-    dpfhe::u64 *ms_tau = nullptr;                   // scratch of dpfhe_mod_switch_down: [n_polys][N]
-    size_t ms_tau_bytes = 0;
-    // hoisted rotations (allocated on first use): shared transforms U [chunk][L][L][N], zero flags [chunk],
-    // per-rotation constants M [L][N] and kprime [2][L][N], and the table delta[j][i] = q_j mod q_i
-    dpfhe::u64 *hoist_U = nullptr, *hoist_M = nullptr, *hoist_kprime = nullptr, *hoist_delta = nullptr;
-    dpfhe::u32 *hoist_zero = nullptr;
-    size_t hoist_chunk = 0;                  // ciphertexts the current U / zero buffers hold
-    dpfhe::u64 *hoistg_buf = nullptr;        // hoisted rotations with grouped hybrid keys: lifted digits, accumulators and tau' rows of a chunk
-    size_t hoistg_bytes = 0;
-    // CKKS slot encoding (allocated on first use): twiddles, slot permutation and 2^e mod q tables in one allocation
-    void *ckks_tab = nullptr;
-    size_t ckks_tab_bytes = 0;
+    // scratch and tables allocated on first use, released by dpfhe_context_trim (see each_trimmed())
+    DeviceScratch ms_tau;                   // dpfhe_mod_switch_down / dpfhe_mod_down_special: [n_polys][K][N]
+    DeviceScratch hoist_U, hoist_zero;      // hoisted rotations: shared transforms U [chunk][L][L][N], zero flags [chunk] (u32)
+    DeviceScratch hoistg;                   // hoisted rotations with grouped hybrid keys: lifted digits, accumulators and tau' rows of a chunk
+    DeviceScratch ckks_tab;                 // CKKS slot encoding: twiddles, 2^e mod q and slot permutation in one allocation
     dpfhe::CkksTables ckks;
-    // BGV slot encoding: the twiddles mod t and slot positions of the plaintext modulus bgv_t last used (0: none), in one
-    // allocation, replaced when t changes
-    void *bgv_tab = nullptr;
-    size_t bgv_tab_bytes = 0;
-    uint64_t bgv_t = 0;
+    DeviceScratch bgv_tab;                  // BGV slot encoding: the twiddles mod t and slot positions of the plaintext modulus bgv_t
+    uint64_t bgv_t = 0;                     //   last used (0: none), rewritten when t changes
     dpfhe::BgvTables bgv;
-    // scratch rows of both slot encoders (encode: [n_vec][N] coefficients; decode: [n_vec][L][N] inverse transforms)
-    void *enc_work = nullptr;
-    size_t enc_work_bytes = 0;
-    dpfhe::u64 *stage_in[DPFHE_PIPE_DEPTH] = {}, *stage_out[DPFHE_PIPE_DEPTH] = {}, *stage_key = nullptr;
-    size_t stage_in_bytes = 0, stage_out_bytes = 0, stage_key_bytes = 0;
+    DeviceScratch enc_work;                 // both slot encoders (encode: [n_vec][N] coefficients; decode: [n_vec][L][N] inverse transforms)
+    DeviceScratch stage_in[DPFHE_PIPE_DEPTH], stage_out[DPFHE_PIPE_DEPTH], stage_key;   // staging of the host-buffer entry points
+    // allocated on first use and kept: per-rotation constants of the hoisted rotations, M [L][N] and kprime [2][L][N], and the
+    // table delta[j][i] = q_j mod q_i
+    DeviceScratch hoist_M, hoist_kprime, hoist_delta;
     cudaEvent_t ev_h2d[DPFHE_PIPE_DEPTH] = {}, ev_comp[DPFHE_PIPE_DEPTH] = {}, ev_d2h[DPFHE_PIPE_DEPTH] = {};
     size_t N() const { return (size_t)1 << hp.log_n; }
     size_t P() const { return N() * hp.L; }
+    // calls f on each buffer that dpfhe_context_trim releases (Self: dpfhe_ctx or const dpfhe_ctx)
+    template <class Self, class F>
+    static void each_trimmed(Self &c, F f) {
+        for (auto *s : {&c.ms_tau, &c.hoist_U, &c.hoist_zero, &c.hoistg, &c.ckks_tab, &c.bgv_tab, &c.enc_work, &c.stage_key}) f(*s);
+        for (auto &s : c.stage_in) f(s);
+        for (auto &s : c.stage_out) f(s);
+    }
 };
-
