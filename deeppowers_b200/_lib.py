@@ -68,6 +68,10 @@ SYMBOLS = {
     "dpfhe_galois_keygen_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint64, C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_void_p]),
     "dpfhe_encrypt_host": (C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t]),
     "dpfhe_decrypt_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint, C.c_void_p, C.c_size_t]),
+    "dpfhe_public_keygen": (C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p]),
+    "dpfhe_encrypt_public": (C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_public_keygen_host": (C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_void_p]),
+    "dpfhe_encrypt_public_host": (C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_char_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t]),
     "dpfhe_fill_uniform": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_size_t, C.c_void_p]),
     "dpfhe_ntt_fwd_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "dpfhe_ntt_inv_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),

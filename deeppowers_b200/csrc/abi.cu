@@ -1236,6 +1236,40 @@ int dpfhe_encrypt(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_sk, const 
     return DPFHE_OK;
 }
 
+// the public key (b, a) = (-a s + t NTT(e), a): the encryption of zero with its own nonce domains and item 0
+int dpfhe_public_keygen(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32], uint64_t *d_pk, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    CHECK_PTR(d_sk); CHECK_PTR(d_pk);
+    if (overlaps(d_pk, 2 * ctx->P() * 8, d_sk, ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the secret");
+    KeyArgs A = build_key_args(ctx->hp, seed, 0, t_plain);
+    A.s = d_sk;
+    A.out = d_pk;
+    CU_TRY(VCALL(launch_keys, ctx->lc, KM_PUBLIC_KEY, A, 1, pick(ctx, stream)));
+    note_launch(ctx, 1);
+    return DPFHE_OK;
+}
+
+int dpfhe_encrypt_public(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_pk, const uint8_t seed[32], uint64_t first_index,
+                         const uint64_t *d_pt, uint64_t *d_ct, size_t n, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    if (n == 0) return DPFHE_OK;
+    CHECK_PTR(d_pk); CHECK_PTR(d_pt); CHECK_PTR(d_ct);
+    if (overlaps(d_ct, n * 2 * ctx->P() * 8, d_pt, n * ctx->P() * 8) || overlaps(d_ct, n * 2 * ctx->P() * 8, d_pk, 2 * ctx->P() * 8))
+        return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+    KeyArgs A = build_key_args(ctx->hp, seed, 0, t_plain);
+    A.s = d_pk;   // b at s, a at s + L N
+    A.pt = d_pt;
+    A.out = d_ct;
+    A.item0 = first_index;
+    CU_TRY(VCALL(launch_keys, ctx->lc, KM_ENC_PUBLIC, A, n, pick(ctx, stream)));
+    note_launch(ctx, 1);
+    return DPFHE_OK;
+}
+
 int dpfhe_decrypt(dpfhe_ctx *ctx, const uint64_t *d_sk, const uint64_t *d_ct, unsigned n_comp, uint64_t *d_pt, size_t n, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
@@ -1328,6 +1362,36 @@ int dpfhe_encrypt_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_sk, c
     return host_call(ctx, {h_sk, h_pt, h_ct}, h_sk, P, h_pt, nullptr, h_ct, n, P, 2 * P,
                      [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
                          const int r = dpfhe_encrypt(ctx, t_plain, ctx->stage_key.get(), seed, next, din, dout, cnt, st);
+                         next += cnt;
+                         return r;
+                     });
+}
+
+int dpfhe_public_keygen_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t *h_pk) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    if (!h_sk) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const KeygenHostArgs args{0, t_plain, seed, 0, nullptr};
+    return keygen_host(ctx, h_sk, 2 * ctx->P(), h_pk,
+                       [](dpfhe_ctx *c, const uint64_t *sk, uint64_t *out, const void *a) {
+                           const KeygenHostArgs &k = *(const KeygenHostArgs *)a;
+                           return dpfhe_public_keygen(c, k.t_plain, sk, k.seed, out, nullptr);
+                       }, &args);
+}
+
+// the public key (2P words) is the staged shared operand; item numbers continue across chunks as in dpfhe_encrypt_host
+int dpfhe_encrypt_public_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_pk, const uint8_t seed[32], uint64_t first_index,
+                              const uint64_t *h_pt, uint64_t *h_ct, size_t n) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    if (n == 0) return DPFHE_OK;
+    const size_t P = ctx->P();
+    uint64_t next = first_index;
+    return host_call(ctx, {h_pk, h_pt, h_ct}, h_pk, 2 * P, h_pt, nullptr, h_ct, n, P, 2 * P,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         const int r = dpfhe_encrypt_public(ctx, t_plain, ctx->stage_key.get(), seed, next, din, dout, cnt, st);
                          next += cnt;
                          return r;
                      });

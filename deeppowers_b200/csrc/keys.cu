@@ -43,7 +43,8 @@ __global__ void __launch_bounds__(NT, MINB) keys_ntt_kernel(const __grid_constan
     KeyCta<NT> cta;
     const size_t w = blockIdx.x;
     const u32 l = (u32)(w % L);
-    keys_limb_body<LOGN, NT, MODE>(cta, buf, small, A, tw + (size_t)l * N, lt.lp[l], l, L, w / L);
+    if constexpr (MODE == KM_ENC_PUBLIC) pub_enc_body<LOGN, NT>(cta, buf, small, A, tw + (size_t)l * N, lt.lp[l], l, L, w / L, 0);
+    else keys_limb_body<LOGN, NT, MODE>(cta, buf, small, A, tw + (size_t)l * N, lt.lp[l], l, L, w / L);
 }
 
 // N = 16384: two CTAs per (item, limb), each keeping half of the outer radix-4 step
@@ -58,7 +59,8 @@ __global__ void __launch_bounds__(NT, MINB) keys_ntt_pair_kernel(const __grid_co
     const size_t w = blockIdx.x / 2;
     const int h = (int)(blockIdx.x & 1);
     const u32 l = (u32)(w % L);
-    keys_half_body<NT, MODE>(cta, buf, small, A, tw + (size_t)l * N, lt.lp[l], l, L, w / L, h);
+    if constexpr (MODE == KM_ENC_PUBLIC) pub_enc_body<NTT_PAIR_LOGN, NT>(cta, buf, small, A, tw + (size_t)l * N, lt.lp[l], l, L, w / L, h);
+    else keys_half_body<NT, MODE>(cta, buf, small, A, tw + (size_t)l * N, lt.lp[l], l, L, w / L, h);
 }
 
 // pt [n][L][N] = c0 + c1 s (+ c2 s^2), ct [n][n_comp][L][N], s [L][N]
@@ -117,13 +119,15 @@ cudaError_t launch_keys_n(const LaunchCtx &lc, int mode, const KeyArgs &A, size_
         case KM_ENC: return launch_keys_mode<LOGN, KM_ENC>(lc, A, n_items, st);
         case KM_RELIN: return launch_keys_mode<LOGN, KM_RELIN>(lc, A, n_items, st);
         case KM_GALOIS: return launch_keys_mode<LOGN, KM_GALOIS>(lc, A, n_items, st);
+        case KM_PUBLIC_KEY: return launch_keys_mode<LOGN, KM_PUBLIC_KEY>(lc, A, n_items, st);
+        case KM_ENC_PUBLIC: return launch_keys_mode<LOGN, KM_ENC_PUBLIC>(lc, A, n_items, st);
     }
     return cudaErrorInvalidValue;
 }
 
 }  // namespace
 
-// n_items: 1 (secret), ciphertexts (encryption), n_elts * ndig (keys); one launch
+// n_items: 1 (secret, public key), ciphertexts (encryption, public-key encryption), n_elts * ndig (switch keys); one launch
 cudaError_t launch_keys(const LaunchCtx &lc, int mode, const KeyArgs &A, size_t n_items, cudaStream_t st) {
     if (n_items == 0) return cudaSuccess;
     if (n_items * lc.L * 2 > 0x7fffffffull) return cudaErrorInvalidValue;

@@ -8,7 +8,11 @@
 namespace dpfhe {
 
 // nonce word n0 = domain | K << 8 | digit << 16 | limb << 24 (DESIGN.md §2.14)
-enum KeyDomain : u32 { KD_SECRET = 1, KD_KEY_A = 2, KD_KEY_E = 3, KD_ENC_A = 4, KD_ENC_E = 5 };
+enum KeyDomain : u32 {
+    KD_SECRET = 1, KD_KEY_A = 2, KD_KEY_E = 3, KD_ENC_A = 4, KD_ENC_E = 5,
+    KD_PK_A = 6, KD_PK_E = 7,                          // public key (the key owner's seed)
+    KD_PENC_U = 8, KD_PENC_E0 = 9, KD_PENC_E1 = 10     // public-key encryption (the encryptor's seed)
+};
 DPFHE_HD u32 key_nonce0(u32 domain, u32 K, u32 digit, u32 limb) { return domain | K << 8 | digit << 16 | limb << 24; }
 
 namespace DPFHE_VNS {
@@ -86,10 +90,11 @@ DPFHE_HD void sample_small(signed char *small, const u32 seed[8], bool ternary, 
 // Output rows of one (item, limb) from the forward transform `buf` of t * small: the store stage.  Coefficient pair chunks
 // [c_lo, c_hi) of the limb, two chunks (one ChaCha20 block of uniform values) per step; buf chunk = chunk - c_lo.
 //   SECRET: out row = the transform.
-//   ENC / KEY: a from its stream, c0 / b = transform - a s + (plaintext | gadget term), c1 / a = a.
+//   ENC / KEY / PUBLIC_KEY: a from its stream, c0 / b = transform - a s + (plaintext | gadget term | nothing), c1 / a = a.
 
 template <int LOGN, int NT, int MODE>
 DPFHE_HD void keys_store(const u64 *buf, const KeyArgs &A, const LimbParams &p, u32 l, u32 L, size_t item, int c_lo, int c_hi, int tid) {
+    constexpr bool SWITCH_KEY = MODE == KM_RELIN || MODE == KM_GALOIS;
     constexpr size_t N = (size_t)1 << LOGN;
     const U64x2 *sb = reinterpret_cast<const U64x2 *>(buf);
     if (MODE == KM_SECRET) {
@@ -102,20 +107,22 @@ DPFHE_HD void keys_store(const u64 *buf, const KeyArgs &A, const LimbParams &p, 
         }
         return;
     }
-    // item numbering: encryption: ciphertext item; keys: item = e * ndig + digit
+    // item numbering: encryption: ciphertext item; public key: 0; switch keys: item = e * ndig + digit
     u32 digit = 0;
     u64 item_no;
     u32 g = 0;
     if (MODE == KM_ENC) {
         item_no = A.item0 + item;
+    } else if (MODE == KM_PUBLIC_KEY) {
+        item_no = 0;
     } else {
         digit = (u32)(item % A.ndig);
         const size_t e = item / A.ndig;
         item_no = MODE == KM_GALOIS ? A.galois[e] : 0;
         g = (u32)item_no;
     }
-    const u32 n0 = key_nonce0(MODE == KM_ENC ? KD_ENC_A : KD_KEY_A, A.K, digit, l);
-    const bool in_digit = MODE != KM_ENC && (A.K == 0 ? l == digit : (l < A.Lq && l / A.K == digit));
+    const u32 n0 = key_nonce0(MODE == KM_ENC ? KD_ENC_A : MODE == KM_PUBLIC_KEY ? KD_PK_A : KD_KEY_A, A.K, digit, l);
+    const bool in_digit = SWITCH_KEY && (A.K == 0 ? l == digit : (l < A.Lq && l / A.K == digit));
     const u64 r64 = A.r64[l], r64_s = A.r64_s[l], fac = A.fac[l];
     const u64 *srow = A.s + (size_t)l * N;
     U64x2 *ob = reinterpret_cast<U64x2 *>(A.out + (item * 2 + 0) * L * N + (size_t)l * N);
@@ -174,6 +181,9 @@ DPFHE_HD void keys_small_nonce(const KeyArgs &A, size_t item, u32 &n0, u64 &item
     } else if (MODE == KM_ENC) {
         n0 = key_nonce0(KD_ENC_E, 0, 0, 0);
         item_no = A.item0 + item;
+    } else if (MODE == KM_PUBLIC_KEY) {
+        n0 = key_nonce0(KD_PK_E, 0, 0, 0);
+        item_no = 0;
     } else {
         const u32 digit = (u32)(item % A.ndig);
         n0 = key_nonce0(KD_KEY_E, A.K, digit, 0);
@@ -220,6 +230,77 @@ DPFHE_HD void keys_half_body(CTA &cta, u64 *buf, signed char *small, const KeyAr
     ntt_fwd_half_load_src<NT>(cta, buf, src, tw, p, h);
     fwd_passes_blk<LOGN, NT, 1, 2>(cta, buf, tw, p, 2 * h);
     cta.par([&](int tid) { keys_store<LOGN, NT, MODE>(buf, A, p, l, L, item, h * HC, (h + 1) * HC, tid); });
+}
+
+// Public-key encryption (KM_ENC_PUBLIC): ct = (b U + t E0 + pt, a U + t E1) with U = NTT(u), E0 = NTT(e0), E1 = NTT(e1) and the
+// public key (b, a) at A.s / A.s + L N.  One limb buffer: pass 0 (buf = U) writes c0 = b U + pt and c1 = a U, pass 1 (buf = t E0)
+// adds into c0, pass 2 (buf = t E1) into c1.  A thread owns the same chunks in every pass, so it reads back only its own stores
+// (through L2: .cg); the rows it finishes in a pass are written with st_stream.
+template <int LOGN, int NT, int PASS>
+DPFHE_HD void pub_enc_store(const u64 *buf, const KeyArgs &A, const LimbParams &p, u32 l, u32 L, size_t item, int c_lo, int c_hi, int tid) {
+    constexpr size_t N = (size_t)1 << LOGN;
+    const U64x2 *sb = reinterpret_cast<const U64x2 *>(buf);
+    U64x2 *o0 = reinterpret_cast<U64x2 *>(A.out + (item * 2 + 0) * L * N + (size_t)l * N);
+    U64x2 *o1 = reinterpret_cast<U64x2 *>(A.out + (item * 2 + 1) * L * N + (size_t)l * N);
+    const U64x2 *pkb = reinterpret_cast<const U64x2 *>(A.s + (size_t)l * N);
+    const U64x2 *pka = reinterpret_cast<const U64x2 *>(A.s + ((size_t)L + l) * N);
+    const U64x2 *pt = reinterpret_cast<const U64x2 *>(A.pt + (item * L + l) * N);
+    for (int c = c_lo + tid; c < c_hi; c += NT) {
+        const U64x2 v = sb[swz_chunk(c - c_lo)];
+        const u64 ev[2] = {canon_store(v.x, p), canon_store(v.y, p)};
+        if (PASS == 0) {
+            const U64x2 b = ld_keep(pkb + c), a = ld_keep(pka + c), m = ld_stream(pt + c);
+            U64x2 r0, r1;
+            r0.x = csub(mulmod(ev[0], b.x, p) + m.x, p.q);
+            r0.y = csub(mulmod(ev[1], b.y, p) + m.y, p.q);
+            r1.x = mulmod(ev[0], a.x, p);
+            r1.y = mulmod(ev[1], a.y, p);
+            st_cg(o0 + c, r0);
+            st_cg(o1 + c, r1);
+        } else {
+            U64x2 *o = PASS == 1 ? o0 : o1;
+            U64x2 r = ld_cg(o + c);
+            r.x = csub(r.x + ev[0], p.q);
+            r.y = csub(r.y + ev[1], p.q);
+            st_stream(o + c, r);
+        }
+    }
+}
+
+// one pass of public-key encryption: sample u (ternary; PASS 0), e0 or e1 (noise), the forward transform with the lift (u by 1,
+// the noise by t) in the load stage, then the pass's store stage.  N <= 8192: the whole limb (h unused); N = 16384: CTA h of the
+// pair keeps output blocks {2h, 2h+1} and regenerates the whole small row, as keys_half_body
+template <int LOGN, int NT, int PASS, class CTA>
+DPFHE_HD void pub_enc_pass(CTA &cta, u64 *buf, signed char *small, const KeyArgs &A, const Twiddle *tw, const LimbParams &p, u32 l, u32 L,
+                           size_t item, int h) {
+    const u32 n0 = key_nonce0(KD_PENC_U + PASS, 0, 0, 0);
+    cta.par([&](int tid) { sample_small<LOGN, NT>(small, A.seed, PASS == 0, n0, A.item0 + item, tid); });
+    const u64 tq = PASS == 0 ? 1 : A.tq[l];
+    auto src = [&](int c) {
+        U64x2 r;
+        r.x = small_lift(small[2 * c], tq, p);
+        r.y = small_lift(small[2 * c + 1], tq, p);
+        return r;
+    };
+    if constexpr (LOGN == NTT_PAIR_LOGN) {
+        constexpr int HC = 1 << (LOGN - 2);
+        ntt_fwd_half_load_src<NT>(cta, buf, src, tw, p, h);
+        fwd_passes_blk<LOGN, NT, 1, 2>(cta, buf, tw, p, 2 * h);
+        cta.par([&](int tid) { pub_enc_store<LOGN, NT, PASS>(buf, A, p, l, L, item, h * HC, (h + 1) * HC, tid); });
+    } else {
+        cta.par([&](int tid) { fwd_load_stage<LOGN, NT, false>(buf, tw, p, tid, src); });
+        fwd_passes<LOGN, NT, 1>(cta, buf, tw, p);
+        cta.par([&](int tid) { pub_enc_store<LOGN, NT, PASS>(buf, A, p, l, L, item, 0, 1 << (LOGN - 1), tid); });
+    }
+}
+
+// one (item, limb) of public-key encryption (h: the CTA of the pair at N = 16384, else 0)
+template <int LOGN, int NT, class CTA>
+DPFHE_HD void pub_enc_body(CTA &cta, u64 *buf, signed char *small, const KeyArgs &A, const Twiddle *tw, const LimbParams &p, u32 l, u32 L,
+                           size_t item, int h) {
+    pub_enc_pass<LOGN, NT, 0>(cta, buf, small, A, tw, p, l, L, item, h);
+    pub_enc_pass<LOGN, NT, 1>(cta, buf, small, A, tw, p, l, L, item, h);
+    pub_enc_pass<LOGN, NT, 2>(cta, buf, small, A, tw, p, l, L, item, h);
 }
 
 // decryption, one 16-byte chunk c of [n][L][N]: c0 + c1 s (+ c2 s^2)

@@ -156,7 +156,7 @@ struct BgvConsts {
 
 // Key generation and encryption (DESIGN.md §2.14): what one launch of the key / encryption kernels (keys.cu) produces, built in
 // abi.cu and passed by value in the kernel parameter block
-enum KeyMode { KM_SECRET = 0, KM_ENC = 1, KM_RELIN = 2, KM_GALOIS = 3 };
+enum KeyMode { KM_SECRET = 0, KM_ENC = 1, KM_RELIN = 2, KM_GALOIS = 3, KM_PUBLIC_KEY = 4, KM_ENC_PUBLIC = 5 };
 constexpr int KEYS_MAX_ELTS = 64;   // Galois elements per launch (abi.cu splits longer lists)
 struct KeyArgs {
     u32 seed[8];                  // the 32-byte seed as little-endian words (the ChaCha20 key)
@@ -167,9 +167,9 @@ struct KeyArgs {
     u64 r64[16], r64_s[16];       // 2^64 mod q_l and its Shoup companion (exact uniform reduction)
     u64 tq[16];                   // t mod q_l (1 for t = 0, and for the secret): the factor of the small row
     u64 fac[16];                  // gadget factor on the limbs of a digit: 1 (K = 0) or P mod q_l
-    const u64 *s;                 // secret [L][N], evaluation form
+    const u64 *s;                 // secret [L][N], evaluation form (public-key encryption: the public key [2][L][N])
     const u64 *pt;                // encryption: plaintexts [n][L][N]
-    u64 *out;                     // secret [L][N], keys [n_elts][ndig][2][L][N], ciphertexts [n][2][L][N]
+    u64 *out;                     // secret [L][N], keys [n_elts][ndig][2][L][N], public key [2][L][N], ciphertexts [n][2][L][N]
 };
 
 enum KsMode { KS_MUL_RELIN = 0, KS_PLAIN = 1, KS_ROTATE = 2 };

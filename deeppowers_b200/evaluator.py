@@ -390,6 +390,21 @@ class Context:
     def decrypt_host(self, sk, ct, n_comp, pt):
         self._chk(self._l.dpfhe_decrypt_host(self._h, _hptr(sk), _hptr(ct), int(n_comp), _hptr(pt, True), pt.size // self.P))
 
+    # public keys [2][L][N] (the key owner's secret and seed) and public-key encryption (the encryptor's own seed; no secret)
+    def public_keygen(self, t_plain, sk, seed, pk, stream=None):
+        self._chk(self._l.dpfhe_public_keygen(self._h, int(t_plain), _ptr(sk), _seed(seed), _ptr(pk), _stream(stream)))
+
+    def encrypt_public(self, t_plain, pk, seed, first_index, pt, ct, n, stream=None):
+        self._chk(self._l.dpfhe_encrypt_public(self._h, int(t_plain), _ptr(pk), _seed(seed), int(first_index), _ptr(pt), _ptr(ct), n,
+                                               _stream(stream)))
+
+    def public_keygen_host(self, t_plain, sk, seed, pk):
+        self._chk(self._l.dpfhe_public_keygen_host(self._h, int(t_plain), _hptr(sk), _seed(seed), _hptr(pk, True)))
+
+    def encrypt_public_host(self, t_plain, pk, seed, first_index, pt, ct):
+        self._chk(self._l.dpfhe_encrypt_public_host(self._h, int(t_plain), _hptr(pk), _seed(seed), int(first_index), _hptr(pt),
+                                                    _hptr(ct, True), pt.size // self.P))
+
     def fill_uniform(self, seed, data, n_polys, first_poly=0, stream=None):
         self._chk(self._l.dpfhe_fill_uniform(self._h, int(seed), int(first_poly), _ptr(data), n_polys, _stream(stream)))
 

@@ -6,13 +6,14 @@ import numpy as np
 MAGIC = b"DPFHEv1\x00"
 CIPHERTEXTS, SWITCH_KEY, PLAINTEXTS, HYBRID_SWITCH_KEY, GROUPED_SWITCH_KEY = 1, 2, 3, 4, 5   # hybrid / grouped: n_limbs includes the special primes;
 # a grouped key's `count` is the number of special primes K, its payload [ceil((n_limbs-K)/K)][2][n_limbs][N]
+PUBLIC_KEY = 6   # (b, a): payload [2][n_limbs][N], count = 1
 _HDR = struct.Struct("<8sIIIIQ16Q")
 
 
 def payload_words(log_n, n_limbs, kind, count):
     if not (1 <= log_n <= 17 and 1 <= n_limbs <= 16):
         raise ValueError("bad parameters")
-    if kind not in (CIPHERTEXTS, SWITCH_KEY, PLAINTEXTS, HYBRID_SWITCH_KEY, GROUPED_SWITCH_KEY):
+    if kind not in (CIPHERTEXTS, SWITCH_KEY, PLAINTEXTS, HYBRID_SWITCH_KEY, GROUPED_SWITCH_KEY, PUBLIC_KEY):
         raise ValueError("unknown kind")
     poly = (1 << log_n) * n_limbs
     if kind == GROUPED_SWITCH_KEY:
@@ -20,7 +21,7 @@ def payload_words(log_n, n_limbs, kind, count):
             raise ValueError("bad number of special primes")
         return 2 * (-(-(n_limbs - count) // count)) * poly
     return {CIPHERTEXTS: count * 2 * poly, SWITCH_KEY: 2 * n_limbs * poly, PLAINTEXTS: count * poly,
-            HYBRID_SWITCH_KEY: 2 * (n_limbs - 1) * poly}[kind]
+            HYBRID_SWITCH_KEY: 2 * (n_limbs - 1) * poly, PUBLIC_KEY: 2 * poly}[kind]
 
 
 def write(path, log_n, n_limbs, kind, count, moduli, payload, form=1):

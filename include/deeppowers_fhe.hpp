@@ -156,6 +156,24 @@ public:
                         void *stream = nullptr) {
         check(dpfhe_decrypt(ctx_, secret, ct.data, n_comp, plain_eval, ct.count, stream));
     }
+    // ---- public keys: public_key [2 * poly_words()] made by the key owner (secret and seed); anyone holding it encrypts with a
+    //      seed of their own, which must stay as secret as the plaintexts.  Use a public key with the plain_modulus it was made with.
+    std::size_t public_key_words() const { return 2 * poly_words(); }
+    void generate_public_key(std::uint64_t plain_modulus, const std::uint64_t *secret, const Seed &seed, std::uint64_t *public_key) {
+        check(dpfhe_public_keygen_host(ctx_, plain_modulus, secret, seed.data(), public_key));
+    }
+    void generate_public_key_device(std::uint64_t plain_modulus, const std::uint64_t *secret, const Seed &seed, std::uint64_t *public_key,
+                                    void *stream = nullptr) {
+        check(dpfhe_public_keygen(ctx_, plain_modulus, secret, seed.data(), public_key, stream));
+    }
+    void encrypt_public(std::uint64_t plain_modulus, const std::uint64_t *public_key, const Seed &seed, std::uint64_t first_index,
+                        const std::uint64_t *plain_eval, CiphertextBatch out) {
+        check(dpfhe_encrypt_public_host(ctx_, plain_modulus, public_key, seed.data(), first_index, plain_eval, out.data, out.count));
+    }
+    void encrypt_public_device(std::uint64_t plain_modulus, const std::uint64_t *public_key, const Seed &seed, std::uint64_t first_index,
+                               const std::uint64_t *plain_eval, CiphertextBatch out, void *stream = nullptr) {
+        check(dpfhe_encrypt_public(ctx_, plain_modulus, public_key, seed.data(), first_index, plain_eval, out.data, out.count, stream));
+    }
     std::vector<std::uint64_t> galois_elements(const std::vector<long> &steps) const {
         std::vector<std::uint64_t> elts;
         for (long k : steps) elts.push_back(galois_element(k));
@@ -346,6 +364,30 @@ private:
     Evaluator &ev_;
     Memory where_;
     const std::uint64_t *secret_;
+    Evaluator::Seed seed_;
+    std::uint64_t t_, next_;
+};
+
+// Encrypts under a public key with the encrypting party's own seed, numbering the ciphertexts itself as Encryptor does.  It takes
+// no secret: whoever holds the public key can encrypt, and only the key owner can decrypt.  The seed must be kept as secret as the
+// plaintexts (Evaluator::random_seed() draws one).  The public key is in host memory (Memory::host) or device memory (Memory::device).
+class PublicEncryptor {
+public:
+    using Memory = Encryptor::Memory;
+    PublicEncryptor(Evaluator &ev, Memory where, const std::uint64_t *public_key, const Evaluator::Seed &seed, std::uint64_t plain_modulus,
+                    std::uint64_t first_index = 0)
+        : ev_(ev), where_(where), pk_(public_key), seed_(seed), t_(plain_modulus), next_(first_index) {}
+    void encrypt(const std::uint64_t *plain_eval, CiphertextBatch out, void *stream = nullptr) {
+        if (where_ == Memory::host) ev_.encrypt_public(t_, pk_, seed_, next_, plain_eval, out);
+        else ev_.encrypt_public_device(t_, pk_, seed_, next_, plain_eval, out, stream);
+        next_ += out.count;
+    }
+    std::uint64_t next_index() const { return next_; }
+
+private:
+    Evaluator &ev_;
+    Memory where_;
+    const std::uint64_t *pk_;
     Evaluator::Seed seed_;
     std::uint64_t t_, next_;
 };

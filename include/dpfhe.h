@@ -299,9 +299,16 @@ int dpfhe_bgv_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, uint64_t *h_slot
  *        k is drawn with index first_index + k.  Under a context with special primes, encrypt and decrypt with the context over
  *        the ciphertext moduli and the first rows of the secret.
  *      decrypt: d_ct [n][n_comp][L][N], n_comp 2 or 3 -> d_pt [n][L][N] = c0 + c1 o s (+ c2 o s^2), ready for the decoders.
+ *      public_keygen: d_pk [2][L][N] = (b, a) = (-a o s + t NTT(e), a), the encryption of zero under the key owner's seed with
+ *        nonce domains of its own.  Its first l rows of both components are the public key of the context over the first l
+ *        moduli; under a context with special primes, generate it with the context over the ciphertext moduli.
+ *      encrypt_public: encryption by anyone who holds d_pk, with the ENCRYPTOR's own seed (not the key owner's): ciphertext k
+ *        = (b o NTT(u) + t NTT(e0) + pt_k, a o NTT(u) + t NTT(e1)), drawn with index first_index + k; decrypt as usual with the
+ *        secret.  The encryptor's seed must be kept as secret as the plaintexts: (seed, index) and the public key give pt back.
+ *        Use a public key with the t_plain it was made with.
  *      The *_host forms take host buffers (encrypt / decrypt pipelined in chunks; synchronous).
  *      dpfhe_random_seed fills 32 bytes from the operating system (getrandom; DPFHE_ERR_OS if that fails).
- *      Outputs must not overlap the secret, the plaintexts or each other's inputs. ---- */
+ *      Outputs must not overlap the secret, the public key, the plaintexts or each other's inputs. ---- */
 int dpfhe_random_seed(uint8_t seed[32]);
 int dpfhe_secret_keygen(dpfhe_ctx *ctx, const uint8_t seed[32], uint64_t *d_sk, void *stream);
 int dpfhe_relin_keygen(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32],
@@ -320,6 +327,12 @@ int dpfhe_galois_keygen_host(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plai
 int dpfhe_encrypt_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t first_index,
                        const uint64_t *h_pt, uint64_t *h_ct, size_t n);
 int dpfhe_decrypt_host(dpfhe_ctx *ctx, const uint64_t *h_sk, const uint64_t *h_ct, unsigned n_comp, uint64_t *h_pt, size_t n);
+int dpfhe_public_keygen(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32], uint64_t *d_pk, void *stream);
+int dpfhe_encrypt_public(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_pk, const uint8_t seed[32], uint64_t first_index,
+                         const uint64_t *d_pt, uint64_t *d_ct, size_t n, void *stream);
+int dpfhe_public_keygen_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t *h_pk);
+int dpfhe_encrypt_public_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_pk, const uint8_t seed[32], uint64_t first_index,
+                              const uint64_t *h_pt, uint64_t *h_ct, size_t n);
 
 /* ---- synthetic data (DESIGN.md §5): x[k] = mulhi64(splitmix64(seed + k), q_limb),
  *      k = (first_poly + p)*L*N + l*N + n.  Fills [n_polys][L][N]. ---- */

@@ -13,6 +13,7 @@
 //                       3 = plaintext [count][L][N]
 //                       4 = hybrid switch key [L-1][2][L][N] (the last modulus is the special prime; count = 1),
 //                       5 = grouped hybrid switch key [ceil((L-K)/K)][2][L][N] with count = K special primes (1 <= K <= 4, 2K <= L)
+//                       6 = public key [2][L][N] (b, a) (count = 1)
 //   20      4     form: 1 = evaluation (NTT, bit-reversed order), 0 = coefficient
 //   24      8     count
 //   32      128   moduli[16] (unused entries 0)
@@ -32,7 +33,7 @@ namespace fhe {
 
 // HybridSwitchKey: n_limbs counts the special prime (the last modulus); payload [n_limbs-1][2][n_limbs][N]
 // GroupedSwitchKey: n_limbs counts the K = count special primes at the end of the basis; payload [ceil((n_limbs-K)/K)][2][n_limbs][N]
-enum class WireKind : std::uint32_t { Ciphertexts = 1, SwitchKey = 2, Plaintexts = 3, HybridSwitchKey = 4, GroupedSwitchKey = 5 };
+enum class WireKind : std::uint32_t { Ciphertexts = 1, SwitchKey = 2, Plaintexts = 3, HybridSwitchKey = 4, GroupedSwitchKey = 5, PublicKey = 6 };
 
 struct WireHeader {
     char magic[8];
@@ -57,6 +58,7 @@ inline std::size_t wire_payload_words(const WireHeader &h) {
         case WireKind::SwitchKey: return std::size_t(2) * h.n_limbs * poly;
         case WireKind::Plaintexts: return checked(h.count, poly);
         case WireKind::HybridSwitchKey: return std::size_t(2) * (h.n_limbs - 1) * poly;
+        case WireKind::PublicKey: return std::size_t(2) * poly;
         case WireKind::GroupedSwitchKey: {
             if (h.count < 1 || h.count > 4 || 2 * h.count > h.n_limbs) throw std::runtime_error("dpfhe wire: bad number of special primes");
             const std::size_t k = static_cast<std::size_t>(h.count), digits = (h.n_limbs - k + k - 1) / k;
