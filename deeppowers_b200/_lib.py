@@ -115,6 +115,8 @@ SYMBOLS = {
     "dpfhe_polyeval_apply": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "dpfhe_polyeval_apply_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "dpfhe_polyeval_destroy": (None, [C.c_void_p]),
+    "dpfhe_polyeval_create_ckks": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_size_t, C.c_double, C.c_double, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "dpfhe_polyeval_result_scale": (C.c_double, [C.c_void_p]),
     "dpfhe_host_alloc": (C.c_int, [C.POINTER(C.c_void_p), C.c_size_t]),
     "dpfhe_host_free": (C.c_int, [C.c_void_p]),
     "dpfhe_launch_count": (C.c_uint64, [C.c_void_p]),

@@ -1856,15 +1856,19 @@ struct PeLevel {
 };
 
 // one step of an application.  Buffers: >= 0 an entry of bufs, IN the input, OUT the output
-enum PeOpKind { PE_MUL = 0, PE_SWITCH = 1, PE_LINCOMB = 2 };
+enum PeOpKind { PE_MUL = 0, PE_SWITCH = 1, PE_LINCOMB = 2, PE_CUT = 3, PE_CKKS_COMB = 4 };
 constexpr int PE_IN = -1, PE_OUT = -2;
 struct PeOp {
     int kind;
-    unsigned level;           // PE_MUL: level of the product; PE_SWITCH: level of the input (drops q_{level-1}); PE_LINCOMB: its level
-    int a, b, out;
-    std::vector<int> terms;   // PE_LINCOMB
+    unsigned level;           // PE_MUL: level of the product; PE_SWITCH: level of the input (drops q_{level-1}); PE_LINCOMB: its level;
+                              // PE_CUT: level of the copy (the first `level` rows of each polynomial of a); PE_CKKS_COMB: Lc
+    int a, b, out;            // PE_CUT: b is the level of a
+    std::vector<int> terms;   // PE_LINCOMB, PE_CKKS_COMB
     std::vector<int64_t> coeffs;
     int64_t constant = 0;
+    std::vector<unsigned> levels;   // PE_CKKS_COMB: the level of every term (>= Lc; rows below Lc are read)
+    std::vector<double> dcoeffs;    // PE_CKKS_COMB: the integer-valued doubles c_k and c_0
+    double dconstant = 0;
 };
 
 }  // namespace
@@ -1875,7 +1879,9 @@ struct dpfhe_polyeval {
     uint64_t t = 0;
     std::vector<PeLevel> lev;            // by level: lev[l - lev_lo]
     unsigned lev_lo = 0;
-    std::vector<MsConsts> ms;            // BGV modulus switch dropping q_{l-1}: ms[l]
+    std::vector<MsConsts> ms;            // modulus switch dropping q_{l-1} (BGV; CKKS: t = 0): ms[l]
+    bool ckks = false;                   // DESIGN.md §2.16: Lf is then the result's level Lc - 1
+    double scale_out = 0;                // CKKS: the scale S of the result
     std::vector<PeOp> ops;
     std::vector<unsigned> bufs;          // level of every scratch buffer
     size_t fixed_bytes = 0;              // level tables and keys
@@ -1887,7 +1893,7 @@ namespace {
 size_t pe_scratch_words(const dpfhe_polyeval *pe, size_t batch) {
     size_t w = 0;
     for (unsigned l : pe->bufs) w += batch * 2 * l * pe->ctx->N();
-    return w + (pe->bufs.empty() ? 0 : 2 * batch * pe->ctx->N());
+    return w + (pe->bufs.empty() && !pe->ckks ? 0 : 2 * batch * pe->ctx->N());
 }
 
 void pe_free(dpfhe_polyeval *pe) {
@@ -2009,6 +2015,73 @@ int pe_plan(dpfhe_polyeval *pe, const int64_t *coeffs, size_t d) {
     return DPFHE_OK;
 }
 
+// the schedule of DESIGN.md §2.16: the powers of §2.15, each product rescaled right away (x^k at level Lq - ceil(log2 k)), an operand
+// above a product's level cut to its first rows (each cut made once per power and level), the scales tracked in doubles, and the
+// combination over the prefixes at Lc = Lq - D fused into the final rescale
+int pe_plan_ckks(dpfhe_polyeval *pe, const double *a, size_t d, double scale_in) {
+    const unsigned Lq = pe->Lq, D = ceil_log2(d), Lc = Lq - D;
+    const HostParams &hp = pe->ctx->hp;
+    std::vector<char> need(d + 1, 0);
+    bool any = false;
+    for (size_t k = 1; k <= d; ++k) any |= (need[k] = a[k] != 0.0);
+    if (!any) need[1] = 1;
+    auto split = [](size_t k, size_t &u, size_t &v) {
+        size_t p = 1;
+        while (2 * p < k) p *= 2;
+        u = p;
+        v = k - p;
+    };
+    for (size_t k = d; k >= 2; --k)
+        if (need[k]) {
+            size_t u, v;
+            split(k, u, v);
+            need[u] = need[v] = 1;
+        }
+    std::vector<std::vector<int>> at(d + 1, std::vector<int>(Lq + 1, -3));
+    std::vector<unsigned> home(d + 1, 0);
+    std::vector<double> s(d + 1, 0.0);
+    at[1][Lq] = PE_IN;
+    home[1] = Lq;
+    s[1] = scale_in;
+    auto new_buf = [&](unsigned l) {
+        pe->bufs.push_back(l);
+        return (int)pe->bufs.size() - 1;
+    };
+    auto get = [&](size_t k, unsigned l) {
+        if (at[k][l] != -3) return;
+        const int b = new_buf(l);
+        pe->ops.push_back(PeOp{PE_CUT, l, at[k][home[k]], (int)home[k], b});
+        at[k][l] = b;
+    };
+    int tmp = -3;   // the product before its rescale: one buffer at the top level, reused
+    for (size_t k = 2; k <= d; ++k) {
+        if (!need[k]) continue;
+        size_t u, v;
+        split(k, u, v);
+        const unsigned l = Lq - ceil_log2(k) + 1;
+        get(u, l);
+        get(v, l);
+        if (tmp == -3) tmp = new_buf(Lq);
+        pe->ops.push_back(PeOp{PE_MUL, l, at[u][l], at[v][l], tmp});
+        const int b = new_buf(l - 1);
+        pe->ops.push_back(PeOp{PE_SWITCH, l, tmp, 0, b});
+        at[k][l - 1] = b;
+        home[k] = l - 1;
+        s[k] = (s[u] * s[v]) / (double)hp.limbs[l - 1].lp.q;
+    }
+    const double m = pe->scale_out * (double)hp.limbs[Lc - 1].lp.q;
+    PeOp c{PE_CKKS_COMB, Lc, 0, 0, PE_OUT};
+    for (size_t k = 1; k <= d; ++k) {
+        if (any ? a[k] == 0.0 : k != 1) continue;
+        c.terms.push_back(at[k][home[k]]);
+        c.levels.push_back(home[k]);
+        c.dcoeffs.push_back(ckks_comb_coeff(a[k], m, s[k]));
+    }
+    c.dconstant = ckks_comb_coeff(a[0], m, 1.0);
+    pe->ops.push_back(c);
+    return DPFHE_OK;
+}
+
 // the launch state of key switching at level l: the context's, with the level's limb tables (DESIGN.md §4.11)
 LaunchCtx pe_view(const dpfhe_polyeval *pe, const PeLevel &v) {
     LaunchCtx lc = pe->ctx->lc;
@@ -2090,17 +2163,30 @@ int pe_apply_on(dpfhe_polyeval *pe, const u64 *d_ct, u64 *d_out, size_t batch, v
             lc.L = op.level;
             CU_TRY(VCALL(launch_mod_switch, lc, buf(op.a), tau, buf(op.out), pe->ms[op.level], 2 * batch, st));
             note_launch(ctx, 2);
-        } else {
+        } else if (op.kind == PE_LINCOMB) {
             LaunchCtx lc = ctx->lc;
             lc.L = op.level;
             std::vector<const u64 *> in;
             for (int b : op.terms) in.push_back(buf(b));
             CU_TRY(VCALL(launch_lincomb, lc, in.data(), op.coeffs.data(), (u32)in.size(), op.constant, nullptr, buf(op.out), batch, st));
             note_launch(ctx, 1);
+        } else if (op.kind == PE_CUT) {   // a strided device copy, not a kernel
+            const size_t row = (size_t)op.level * N * 8;
+            CU_TRY(cudaMemcpy2DAsync(buf(op.out), row, buf(op.a), (size_t)op.b * N * 8, row, 2 * batch, cudaMemcpyDeviceToDevice, st));
+        } else {   // PE_CKKS_COMB
+            LaunchCtx lc = ctx->lc;
+            lc.L = op.level;
+            std::vector<const u64 *> in;
+            for (int b : op.terms) in.push_back(buf(b));
+            CU_TRY(VCALL(launch_ckks_comb, lc, in.data(), op.levels.data(), op.dcoeffs.data(), (u32)in.size(), op.dconstant, pe->ms[op.level], tau,
+                         buf(op.out), batch, st));
+            note_launch(ctx, 2);
         }
     }
     return DPFHE_OK;
 }
+
+int pe_create_finish(dpfhe_polyeval *pe, int rc, unsigned ms_lo, const uint64_t *h_relin_key, dpfhe_polyeval **out);
 
 }  // namespace
 
@@ -2122,18 +2208,28 @@ int dpfhe_polyeval_create_grouped(dpfhe_ctx *ctx, unsigned n_special, uint64_t t
     if (!pe) return fail(DPFHE_ERR_NOMEM, "out of host memory");
     pe->ctx = ctx; pe->K = K; pe->Lq = Lq; pe->Lf = Lq - D; pe->t = t_plain;
     rc = pe_plan(pe, coeffs, degree);
-    // the levels of the products, and the BGV switch constants of every level a switch starts from
+    return pe_create_finish(pe, rc, D > 0 ? pe->Lf + 1 : Lq + 1, h_relin_key, out);
+}
+
+namespace {
+
+// the rest of an evaluator's creation after its plan (rc: the planner's result): the switch constants of every level from ms_lo to
+// Lq, the level views, keys and companions of the products' levels; frees the evaluator on failure
+int pe_create_finish(dpfhe_polyeval *pe, int rc, unsigned ms_lo, const uint64_t *h_relin_key, dpfhe_polyeval **out) {
+    dpfhe_ctx *ctx = pe->ctx;
+    const unsigned Lq = pe->Lq;
+    // the levels of the products, and the switch constants of every level a switch starts from
     unsigned lo = Lq + 1;
     for (const PeOp &op : pe->ops)
         if (op.kind == PE_MUL) lo = std::min(lo, op.level);
     pe->ms.resize(Lq + 1);
-    for (unsigned l = pe->Lf + 1; l <= Lq && rc == DPFHE_OK && D > 0; ++l) {
+    for (unsigned l = ms_lo; l <= Lq && rc == DPFHE_OK; ++l) {
         HostParams hp;
         std::vector<uint64_t> mod(l);
         for (unsigned i = 0; i < l; ++i) mod[i] = ctx->hp.limbs[i].lp.q;
         std::string msg = build_host_params(ctx->hp.log_n, l, mod.data(), hp);
         if (!msg.empty()) rc = fail(DPFHE_ERR_INVALID, "%s", msg.c_str());
-        else build_ms_consts(hp, t_plain, pe->ms[l]);
+        else build_ms_consts(hp, pe->t, pe->ms[l]);
     }
     if (rc == DPFHE_OK && lo <= Lq) rc = ensure_hyb(ctx);
     cudaStream_t st = pick(ctx, nullptr);
@@ -2155,7 +2251,36 @@ int dpfhe_polyeval_create_grouped(dpfhe_ctx *ctx, unsigned n_special, uint64_t t
     return DPFHE_OK;
 }
 
+}  // namespace
+
+int dpfhe_polyeval_create_ckks(dpfhe_ctx *ctx, unsigned n_special, const double *coeffs, size_t degree, double scale_in, double scale_out,
+                               const uint64_t *h_relin_key, dpfhe_polyeval **out) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!out || !coeffs || !h_relin_key) return fail(DPFHE_ERR_INVALID, "null argument");
+    *out = nullptr;
+    rc = check_special(ctx, n_special);
+    if (rc) return rc;
+    if (degree < 1 || degree > 64) return fail(DPFHE_ERR_INVALID, "the degree must be in [1, 64]");
+    for (size_t k = 0; k <= degree; ++k)
+        if (!std::isfinite(coeffs[k])) return fail(DPFHE_ERR_INVALID, "coefficient %zu is not finite", k);
+    if (!(std::isfinite(scale_in) && scale_in > 0) || !(std::isfinite(scale_out) && scale_out > 0))
+        return fail(DPFHE_ERR_INVALID, "the scales must be finite and positive");
+    const unsigned L = ctx->hp.L, K = n_special, Lq = L - K, D = ceil_log2(degree);
+    if (D + 2 > Lq || D > Lq - K + 1)
+        return fail(DPFHE_ERR_INVALID, "degree %zu needs %u levels: at most min(Lq - 2, Lq - K + 1) with Lq = %u, K = %u", degree, D, Lq, K);
+    dpfhe_polyeval *pe = new (std::nothrow) dpfhe_polyeval();
+    if (!pe) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    pe->ctx = ctx; pe->K = K; pe->Lq = Lq; pe->Lf = Lq - D - 1; pe->t = 0;
+    pe->ckks = true;
+    pe->scale_out = scale_out;
+    rc = pe_plan_ckks(pe, coeffs, degree, scale_in);
+    return pe_create_finish(pe, rc, Lq - D, h_relin_key, out);
+}
+
 unsigned dpfhe_polyeval_result_limbs(const dpfhe_polyeval *pe) { return pe ? pe->Lf : 0; }
+
+double dpfhe_polyeval_result_scale(const dpfhe_polyeval *pe) { return pe && pe->ckks ? pe->scale_out : 0.0; }
 
 void dpfhe_polyeval_destroy(dpfhe_polyeval *pe) {
     if (!pe) return;

@@ -607,8 +607,8 @@ class LinearLayer:
 
 
 class PolyEval:
-    """BGV polynomial evaluation on encrypted slots down the modulus chain (dpfhe_polyeval_*, DESIGN.md section 2.15): slot-wise
-    p(x) = sum_k coeffs[k] x^k mod t_plain.  ctx's last n_special limbs are special primes; relin_key is the grouped relinearisation
+    """BGV polynomial evaluation on encrypted slots down the modulus chain (dpfhe_polyeval_*, DESIGN.md section 2.15; PolyEval.ckks for
+    CKKS, section 2.16): slot-wise p(x) = sum_k coeffs[k] x^k mod t_plain.  ctx's last n_special limbs are special primes; relin_key is the grouped relinearisation
     key [dnum][2][L][N] of the top level (C-contiguous numpy uint64).  apply / apply_host take ciphertexts [batch][2][Lq][N] and
     write [batch][2][result_limbs][N], which decrypt under the first result_limbs limbs of the secret."""
 
@@ -620,10 +620,32 @@ class PolyEval:
         cs = np.ascontiguousarray([int(c) for c in coeffs], dtype=np.int64)
         rc = self._l.dpfhe_polyeval_create_grouped(ctx._h, self.n_special, int(t_plain), C.c_void_p(cs.ctypes.data), len(cs) - 1, _hptr(relin_key),
                                                    C.byref(self._h))
+        self._finish(rc)
+
+    @classmethod
+    def ckks(cls, ctx, n_special, coeffs, scale_in, relin_key, scale_out=None):
+        """CKKS polynomial evaluation down the rescaling chain (dpfhe_polyeval_create_ckks, DESIGN.md section 2.16): slot-wise
+        p(z) = sum_k coeffs[k] z^k with real coefficients, inputs at scale scale_in, the result at scale_out (default scale_in),
+        which result_scale reports.  relin_key: the grouped key of the top level generated with t_plain = 0.  The result has
+        result_limbs = Lq - ceil(log2 d) - 1 limbs and decodes with ckks_decode at result_scale."""
+        self = cls.__new__(cls)
+        self._l, self.ctx = ctx._l, ctx
+        self._h = C.c_void_p()
+        self.n_special = int(n_special)
+        self.Lq = ctx.L - self.n_special
+        cs = np.ascontiguousarray([float(c) for c in coeffs], dtype=np.float64)
+        so = float(scale_in if scale_out is None else scale_out)
+        rc = self._l.dpfhe_polyeval_create_ckks(ctx._h, self.n_special, C.c_void_p(cs.ctypes.data), len(cs) - 1, float(scale_in), so,
+                                                _hptr(relin_key), C.byref(self._h))
+        self._finish(rc)
+        return self
+
+    def _finish(self, rc):
         if rc != 0:
             self._h = C.c_void_p()
             raise DpfheError(self._l.dpfhe_last_error().decode())
         self.result_limbs = int(self._l.dpfhe_polyeval_result_limbs(self._h))
+        self.result_scale = float(self._l.dpfhe_polyeval_result_scale(self._h))
 
     def close(self):
         """Close the evaluator before its context (as LinearLayer.close)."""

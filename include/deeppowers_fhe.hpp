@@ -334,6 +334,7 @@ public:
 private:
     friend class LinearLayer;
     friend class PolyEval;
+    friend class CkksPolyEval;
     static void check(int status) {
         if (status != DPFHE_OK) throw std::runtime_error(dpfhe_last_error());
     }
@@ -436,6 +437,35 @@ public:
     PolyEval(const PolyEval &) = delete;
     PolyEval &operator=(const PolyEval &) = delete;
     unsigned result_limbs() const { return dpfhe_polyeval_result_limbs(h_); }
+    void apply(ConstCiphertextBatch in, CiphertextBatch out) {   // host buffers, pipelined
+        if (in.count != out.count) throw std::runtime_error("ciphertext batches must have the same count");
+        Evaluator::check(dpfhe_polyeval_apply_host(h_, in.data, out.data, in.count));
+    }
+    void apply_device(const std::uint64_t *in, std::uint64_t *out, std::size_t count, void *stream = nullptr) {
+        Evaluator::check(dpfhe_polyeval_apply(h_, in, out, count, stream));
+    }
+
+private:
+    dpfhe_polyeval *h_ = nullptr;
+};
+
+// CKKS polynomial evaluation on encrypted slots down the rescaling chain (dpfhe_polyeval_create_ckks, DESIGN.md §2.16): p(z) = sum_k
+// coeffs[k] z^k with real coefficients, slot by slot.  Inputs at scale scale_in carry limbs()-special limbs; results carry
+// result_limbs() limbs at result_scale() (scale_out, or scale_in when scale_out is 0).  relin_key: the grouped relinearisation key
+// of the top level generated with plain modulus 0 (host memory).
+class CkksPolyEval {
+public:
+    CkksPolyEval(Evaluator &ev, unsigned special, const std::vector<double> &coeffs, double scale_in, const std::uint64_t *relin_key,
+                 double scale_out = 0) {
+        if (coeffs.size() < 2) throw std::runtime_error("a polynomial of degree at least 1");
+        Evaluator::check(dpfhe_polyeval_create_ckks(ev.native_handle(), special, coeffs.data(), coeffs.size() - 1, scale_in,
+                                                    scale_out == 0 ? scale_in : scale_out, relin_key, &h_));
+    }
+    ~CkksPolyEval() { dpfhe_polyeval_destroy(h_); }
+    CkksPolyEval(const CkksPolyEval &) = delete;
+    CkksPolyEval &operator=(const CkksPolyEval &) = delete;
+    unsigned result_limbs() const { return dpfhe_polyeval_result_limbs(h_); }
+    double result_scale() const { return dpfhe_polyeval_result_scale(h_); }
     void apply(ConstCiphertextBatch in, CiphertextBatch out) {   // host buffers, pipelined
         if (in.count != out.count) throw std::runtime_error("ciphertext batches must have the same count");
         Evaluator::check(dpfhe_polyeval_apply_host(h_, in.data, out.data, in.count));

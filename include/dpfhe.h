@@ -193,6 +193,14 @@ unsigned dpfhe_polyeval_result_limbs(const dpfhe_polyeval *pe);
 int dpfhe_polyeval_apply(dpfhe_polyeval *pe, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream);
 int dpfhe_polyeval_apply_host(dpfhe_polyeval *pe, const uint64_t *h_ct, uint64_t *h_out, size_t batch);
 void dpfhe_polyeval_destroy(dpfhe_polyeval *pe);
+/*      CKKS (DESIGN.md §2.16): slot-wise p(z) = sum_k coeffs[k] z^k with real coefficients (finite doubles), inputs at scale
+ *      scale_in, the result at scale scale_out (both finite and > 0).  h_relin_key generated with t_plain = 0.  D = ceil(log2 d)
+ *      must satisfy D <= Lq - 2 and D <= Lq - K + 1; the result has Lq - D - 1 limbs (dpfhe_polyeval_result_limbs) and decodes
+ *      with dpfhe_ckks_decode at dpfhe_polyeval_result_scale (scale_out; 0 for a BGV evaluator).  _apply, _apply_host and
+ *      _destroy serve both kinds. */
+int dpfhe_polyeval_create_ckks(dpfhe_ctx *ctx, unsigned n_special, const double *coeffs, size_t degree, double scale_in, double scale_out,
+                               const uint64_t *h_relin_key, dpfhe_polyeval **out);
+double dpfhe_polyeval_result_scale(const dpfhe_polyeval *pe);
 
 /* ---- modulus switching / rescale (DESIGN.md §2.9): drop the last limb of every polynomial.
  *      in [n_polys][L][N] -> out [n_polys][L-1][N] (a ciphertext is two polynomials), evaluation form.
