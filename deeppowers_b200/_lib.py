@@ -117,6 +117,15 @@ SYMBOLS = {
     "dpfhe_polyeval_destroy": (None, [C.c_void_p]),
     "dpfhe_polyeval_create_ckks": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_size_t, C.c_double, C.c_double, C.c_void_p, C.POINTER(C.c_void_p)]),
     "dpfhe_polyeval_result_scale": (C.c_double, [C.c_void_p]),
+    "dpfhe_rotate_sum_grouped": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64,
+                                           C.c_void_p]),
+    "dpfhe_rotate_sum_grouped_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                C.c_uint64]),
+    "dpfhe_slotsum_steps": (C.c_int, [C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_size_t)]),
+    "dpfhe_slotsum_create_grouped": (C.c_int, [C.c_void_p, C.c_uint, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint64, C.POINTER(C.c_void_p)]),
+    "dpfhe_slotsum_apply": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_slotsum_apply_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "dpfhe_slotsum_destroy": (None, [C.c_void_p]),
     "dpfhe_host_alloc": (C.c_int, [C.POINTER(C.c_void_p), C.c_size_t]),
     "dpfhe_host_free": (C.c_int, [C.c_void_p]),
     "dpfhe_launch_count": (C.c_uint64, [C.c_void_p]),

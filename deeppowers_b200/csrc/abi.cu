@@ -748,6 +748,121 @@ int dpfhe_rotate_hoisted_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint6
     return rotate_hoisted_grouped_impl(ctx, n_special, d_ct, n_rot, galois_elts, d_gks, nullptr, d_out, batch, t_plain, stream);
 }
 
+// Summed rotations (DESIGN.md §2.17).  Scratch in ctx->hoistg: `head` words first (the key companions of a dpfhe_rotate_sum_grouped
+// call; 0 for a slot-sum object, which keeps its own), then per ciphertext of a chunk the lifted digits [dnum][L][N], the summed
+// accumulators [2][L][N] and the tau' rows [2][K][N].
+static size_t rotate_sum_per_ct(const dpfhe_ctx *ctx, unsigned K) {
+    const size_t N = ctx->N(), L = ctx->hp.L;
+    return (key_digits(ctx, K) * L * N + 2 * L * N + 2 * (size_t)K * N) * sizeof(u64);
+}
+
+static int rotate_sum_reserve(dpfhe_ctx *ctx, unsigned K, size_t head, size_t batch) {
+    const size_t per_ct = rotate_sum_per_ct(ctx, K);
+    return ctx->hoistg.reserve(ctx, head * sizeof(u64) + hoist_chunk(per_ct, batch) * per_ct);
+}
+
+// one stage: per chunk of the batch the mod-up of c1 (ks_hoistg_kernel), the summed multiply-accumulate of every rotation
+// (rot_sum_grouped_kernel) and the division by P (md_tau, md_limb); 4 launches.  The scratch is reserved by the caller.
+static int rotate_sum_stage(dpfhe_ctx *ctx, unsigned K, size_t head, const u64 *d_ct, u32 n_rot, const u32 *galois, const u64 *const *keys,
+                            const u64 *const *key_s, u64 *d_out, size_t batch, const MsConsts &Kc, const GroupConsts &G, cudaStream_t st) {
+    const size_t N = ctx->N(), L = ctx->hp.L, Pq = (L - K) * N;
+    const size_t u_words = key_digits(ctx, K) * L * N, acc_words = 2 * L * N, per_ct = rotate_sum_per_ct(ctx, K), chunk = hoist_chunk(per_ct, batch);
+    if (ctx->hoistg.bytes() < head * sizeof(u64) + chunk * per_ct) return fail(DPFHE_ERR_INVALID, "summed rotations: scratch not reserved");
+    u64 *U = ctx->hoistg.get() + head, *acc = U + chunk * u_words, *tau = acc + chunk * acc_words;
+    for (size_t first = 0; first < batch; first += chunk) {
+        const size_t cnt = batch - first < chunk ? batch - first : chunk;
+        const u64 *in = d_ct + first * 2 * Pq;
+        CU_TRY(VCALL(launch_hoist_grouped, ctx->lc, in, U, G, cnt, st));
+        CU_TRY(VCALL(launch_rot_sum_grouped, ctx->lc, in, U, n_rot, keys, key_s, galois, acc, Kc, G, cnt, st));
+        CU_TRY(VCALL(launch_mod_down_special, ctx->lc, acc, tau, d_out + first * 2 * Pq, Kc, G, 2 * cnt, st));
+        note_launch(ctx, 4);   // ks_hoistg, rot_sum_grouped, md_tau, md_limb
+    }
+    return DPFHE_OK;
+}
+
+// the checks of dpfhe_rotate_hoisted_grouped, and 1 <= n_rot <= 15
+static int check_rotate_sum(dpfhe_ctx *ctx, unsigned n_special, size_t n_rot, const uint64_t *galois_elts, uint64_t t_plain) {
+    if (!galois_elts) return fail(DPFHE_ERR_INVALID, "null argument");
+    int rc = check_special(ctx, n_special);
+    if (!rc) rc = check_t_below_special(ctx, n_special, t_plain);
+    if (rc) return rc;
+    if (n_rot < 1 || n_rot > (size_t)ROT_SUM_MAX) return fail(DPFHE_ERR_INVALID, "summed rotations take 1 to %d rotations", ROT_SUM_MAX);
+    for (size_t r = 0; r < n_rot; ++r) {
+        rc = check_galois(ctx, galois_elts[r]);
+        if (rc) return rc;
+    }
+    return DPFHE_OK;
+}
+
+// what a dpfhe_rotate_sum_grouped call shares between its chunks: the Shoup companions of its n_rot keys (at the head of
+// ctx->hoistg, built once per call), the Galois elements and the constants of the division by P
+struct RotSumPrep {
+    const u64 *key_s[ROT_SUM_MAX];
+    u32 galois[ROT_SUM_MAX];
+    size_t head = 0;
+    MsConsts K;
+    GroupConsts G;
+};
+
+// reserves the scratch of chunks of up to `batch` ciphertexts and builds the companions (n_rot launches)
+static int rotate_sum_prepare(dpfhe_ctx *ctx, unsigned n_special, size_t n_rot, const uint64_t *galois_elts, const uint64_t *const *d_gks,
+                              uint64_t t_plain, size_t batch, cudaStream_t st, RotSumPrep &pr) {
+    const size_t dnum = key_digits(ctx, n_special), key_words = dnum * 2 * ctx->P();
+    pr.head = n_rot * key_words;
+    int rc = rotate_sum_reserve(ctx, n_special, pr.head, batch);
+    if (rc) return rc;
+    u64 *key_s = ctx->hoistg.get();
+    for (size_t r = 0; r < n_rot; ++r) {
+        CU_TRY(VCALL(launch_key_prepare_grouped, ctx->lc, d_gks[r], key_s + r * key_words, (u32)dnum, st));
+        note_launch(ctx, 1);
+        pr.key_s[r] = key_s + r * key_words;
+        pr.galois[r] = (u32)galois_elts[r];
+    }
+    build_group_consts(ctx->hp, n_special, t_plain, pr.G, pr.K);
+    return DPFHE_OK;
+}
+
+int dpfhe_rotate_sum_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_ct, size_t n_rot, const uint64_t *galois_elts,
+                             const uint64_t *const *d_gks, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (batch == 0) return DPFHE_OK;
+    CHECK_PTR(d_ct); CHECK_PTR(d_out);
+    if (!d_gks) return fail(DPFHE_ERR_INVALID, "null argument");
+    rc = check_rotate_sum(ctx, n_special, n_rot, galois_elts, t_plain);
+    if (!rc) rc = check_rotations(ctx, n_rot, galois_elts, d_gks);
+    if (rc) return rc;
+    const size_t ct_bytes = batch * 2 * (ctx->hp.L - n_special) * ctx->N() * 8;
+    if (overlaps(d_out, ct_bytes, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    cudaStream_t st = pick(ctx, stream);
+    RotSumPrep pr;
+    rc = rotate_sum_prepare(ctx, n_special, n_rot, galois_elts, d_gks, t_plain, batch, st, pr);
+    if (rc) return rc;
+    return rotate_sum_stage(ctx, n_special, pr.head, d_ct, (u32)n_rot, pr.galois, d_gks, pr.key_s, d_out, batch, pr.K, pr.G, st);
+}
+
+int dpfhe_rotate_sum_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_ct, size_t n_rot, const uint64_t *galois_elts,
+                                  const uint64_t *h_gks, uint64_t *h_out, size_t batch, uint64_t t_plain) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (batch == 0) return DPFHE_OK;
+    if (!h_ct || !h_gks || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    rc = check_rotate_sum(ctx, n_special, n_rot, galois_elts, t_plain);
+    if (rc) return rc;
+    const size_t key_words = key_digits(ctx, n_special) * 2 * ctx->P(), Pq = (ctx->hp.L - n_special) * ctx->N();
+    rc = upload_key(ctx, h_gks, n_rot * key_words);
+    if (rc) return rc;
+    const u64 *keys[ROT_SUM_MAX];
+    for (size_t r = 0; r < n_rot; ++r) keys[r] = ctx->stage_key.get() + r * key_words;
+    const size_t chunk = pick_chunk(ctx, 2 * Pq * 8, batch);
+    RotSumPrep pr;   // the companions once, for every chunk
+    rc = rotate_sum_prepare(ctx, n_special, n_rot, galois_elts, keys, t_plain, chunk, pick(ctx, nullptr), pr);
+    if (rc) return rc;
+    return run_pipeline(ctx, h_ct, nullptr, h_out, batch, 2 * Pq, 2 * Pq, chunk, [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+        return rotate_sum_stage(ctx, n_special, pr.head, din, (u32)n_rot, pr.galois, keys, pr.key_s, dout, cnt, pr.K, pr.G, pick(ctx, st));
+    });
+}
+
 int dpfhe_ct_mul_plain(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
@@ -2320,6 +2435,175 @@ int dpfhe_polyeval_apply_host(dpfhe_polyeval *pe, const uint64_t *h_ct, uint64_t
     const size_t N = ctx->N();
     return run_pipeline(ctx, h_ct, nullptr, h_out, batch, 2 * pe->Lq * N, 2 * pe->Lf * N, chunk,
                         [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int { return pe_apply_on(pe, din, dout, cnt, st); });
+}
+
+// ---------------------------------------------------------------- slot sums (DESIGN.md §2.17)
+int dpfhe_slotsum_steps(size_t stride, const unsigned *radices, size_t n_stages, int *steps, size_t *n_steps) {
+    if (!radices || !n_steps) return fail(DPFHE_ERR_INVALID, "null argument");
+    if (stride < 1) return fail(DPFHE_ERR_INVALID, "the stride must be at least 1");
+    if (n_stages < 1 || n_stages > 16) return fail(DPFHE_ERR_INVALID, "a slot sum has 1 to 16 stages");
+    constexpr size_t max_half = (size_t)1 << 13;   // N/2 at the largest ring, N = 16384
+    size_t count = 1, n = 0;
+    for (size_t t = 0; t < n_stages; ++t) {
+        if (radices[t] < 2 || radices[t] > 16) return fail(DPFHE_ERR_INVALID, "radix %u of stage %zu is outside [2, 16]", radices[t], t);
+        count *= radices[t];
+        if (stride > max_half / count) return fail(DPFHE_ERR_INVALID, "stride * prod(radices) must be at most N/2 <= %zu", max_half);
+        n += radices[t] - 1;
+    }
+    if (steps) {
+        size_t k = 0, span = stride;
+        for (size_t t = 0; t < n_stages; ++t) {
+            for (unsigned m = 1; m < radices[t]; ++m) steps[k++] = (int)(m * span);
+            span *= radices[t];
+        }
+    }
+    *n_steps = n;
+    return DPFHE_OK;
+}
+
+struct dpfhe_slotsum {
+    dpfhe_ctx *ctx = nullptr;
+    unsigned K = 0;
+    size_t Lq = 0;
+    std::vector<u32> n_rot;              // rotations of each stage
+    std::vector<u32> galois;             // Galois elements of every step, stage by stage
+    std::vector<const u64 *> keys, key_s;
+    u64 *d_keys = nullptr;               // [n_steps][dnum][2][L][N]
+    u64 *d_key_s = nullptr;              // their Shoup companions, same layout
+    MsConsts Kc;
+    GroupConsts G;
+    size_t fixed_bytes = 0;              // keys and companions
+    DeviceScratch scratch;               // one intermediate batch [batch][2][Lq][N] (two or more stages), for the largest batch so far
+};
+
+namespace {
+
+void ss_free(dpfhe_slotsum *ss) {
+    cudaFree(ss->d_keys);
+    cudaFree(ss->d_key_s);
+    if (ss->ctx) ss->ctx->object_bytes -= ss->fixed_bytes + ss->scratch.bytes();
+    delete ss;
+}
+
+// the scratch of an application to `batch` ciphertexts: the object's intermediate batch (counted in the context's device bytes) and
+// the context's hoisted-rotation scratch
+int ss_reserve(dpfhe_slotsum *ss, size_t batch) {
+    dpfhe_ctx *ctx = ss->ctx;
+    int rc = DPFHE_OK;
+    if (ss->n_rot.size() > 1) {
+        ctx->object_bytes -= ss->scratch.bytes();
+        rc = ss->scratch.reserve(ctx, batch * 2 * ss->Lq * ctx->N() * 8);
+        ctx->object_bytes += ss->scratch.bytes();
+    }
+    return rc ? rc : rotate_sum_reserve(ctx, ss->K, 0, batch);
+}
+
+// S stages, alternating between the scratch batch and d_out so that the last one writes d_out; 4 launches per stage and chunk
+int ss_apply_on(dpfhe_slotsum *ss, const u64 *d_ct, u64 *d_out, size_t batch, void *stream) {
+    dpfhe_ctx *ctx = ss->ctx;
+    cudaStream_t st = pick(ctx, stream);
+    const size_t S = ss->n_rot.size();
+    const u64 *in = d_ct;
+    size_t first = 0;
+    for (size_t t = 0; t < S; ++t) {
+        u64 *dst = (S - 1 - t) % 2 == 0 ? d_out : ss->scratch.get();
+        const int rc = rotate_sum_stage(ctx, ss->K, 0, in, ss->n_rot[t], ss->galois.data() + first, ss->keys.data() + first, ss->key_s.data() + first,
+                                        dst, batch, ss->Kc, ss->G, st);
+        if (rc) return rc;
+        first += ss->n_rot[t];
+        in = dst;
+    }
+    return DPFHE_OK;
+}
+
+}  // namespace
+
+int dpfhe_slotsum_create_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t stride, const unsigned *radices, size_t n_stages,
+                                 const uint64_t *h_gks, uint64_t t_plain, dpfhe_slotsum **out) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!out || !h_gks) return fail(DPFHE_ERR_INVALID, "null argument");
+    *out = nullptr;
+    rc = check_special(ctx, n_special);
+    if (!rc) rc = check_t_below_special(ctx, n_special, t_plain);
+    if (rc) return rc;
+    size_t n_steps = 0;
+    rc = dpfhe_slotsum_steps(stride, radices, n_stages, nullptr, &n_steps);
+    if (rc) return rc;
+    size_t count = 1;
+    for (size_t t = 0; t < n_stages; ++t) count *= radices[t];
+    if (stride * count > ctx->N() / 2) return fail(DPFHE_ERR_INVALID, "stride * prod(radices) = %zu exceeds N/2 = %zu", stride * count, ctx->N() / 2);
+    std::vector<int> steps(n_steps);
+    dpfhe_slotsum_steps(stride, radices, n_stages, steps.data(), &n_steps);
+    dpfhe_slotsum *ss = new (std::nothrow) dpfhe_slotsum();
+    if (!ss) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    ss->ctx = ctx; ss->K = n_special; ss->Lq = ctx->hp.L - n_special;
+    for (size_t t = 0; t < n_stages; ++t) ss->n_rot.push_back(radices[t] - 1);
+    build_group_consts(ctx->hp, n_special, t_plain, ss->G, ss->Kc);
+    const size_t dnum = key_digits(ctx, n_special), key_words = dnum * 2 * ctx->P();
+    cudaStream_t st = pick(ctx, nullptr);
+    cudaError_t e = cudaMalloc(&ss->d_keys, n_steps * key_words * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&ss->d_key_s, n_steps * key_words * 8);
+    if (e == cudaSuccess) {
+        ss->fixed_bytes = 2 * n_steps * key_words * 8;
+        ctx->object_bytes += ss->fixed_bytes;
+        e = cudaMemcpyAsync(ss->d_keys, h_gks, n_steps * key_words * 8, cudaMemcpyHostToDevice, st);
+    }
+    for (size_t k = 0; k < n_steps && e == cudaSuccess; ++k) {
+        uint64_t g = 0;
+        dpfhe_galois_element(ctx, steps[k], &g);
+        ss->galois.push_back((u32)g);
+        ss->keys.push_back(ss->d_keys + k * key_words);
+        ss->key_s.push_back(ss->d_key_s + k * key_words);
+        e = VCALL(launch_key_prepare_grouped, ctx->lc, ss->keys[k], ss->d_key_s + k * key_words, (u32)dnum, st);
+        note_launch(ctx, 1);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) {
+        ss_free(ss);
+        return fail(DPFHE_ERR_CUDA, "slot sum keys: %s", cudaGetErrorString(e));
+    }
+    *out = ss;
+    return DPFHE_OK;
+}
+
+void dpfhe_slotsum_destroy(dpfhe_slotsum *ss) {
+    if (!ss) return;
+    if (ss->ctx) {
+        cudaSetDevice(ss->ctx->lc.device);
+        dpfhe_synchronize(ss->ctx);
+    }
+    ss_free(ss);
+}
+
+int dpfhe_slotsum_apply(dpfhe_slotsum *ss, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
+    if (!ss) return fail(DPFHE_ERR_INVALID, "null slot sum");
+    int rc = enter(ss->ctx);
+    if (rc) return rc;
+    if (batch == 0) return DPFHE_OK;
+    CHECK_PTR(d_ct); CHECK_PTR(d_out);
+    const size_t ct_bytes = batch * 2 * ss->Lq * ss->ctx->N() * 8;
+    if (overlaps(d_out, ct_bytes, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    rc = ss_reserve(ss, batch);
+    if (rc) return rc;
+    return ss_apply_on(ss, d_ct, d_out, batch, stream);
+}
+
+int dpfhe_slotsum_apply_host(dpfhe_slotsum *ss, const uint64_t *h_ct, uint64_t *h_out, size_t batch) {
+    if (!ss) return fail(DPFHE_ERR_INVALID, "null slot sum");
+    dpfhe_ctx *ctx = ss->ctx;
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (batch == 0) return DPFHE_OK;
+    if (!h_ct || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    size_t chunk = grid_round_chunk(ctx, batch, nullptr);
+    if (const char *e = getenv("DPFHE_SLOTSUM_CHUNK")) chunk = std::max<size_t>(1, (size_t)atol(e));   // tests: several chunks at a small batch
+    chunk = std::min(chunk, batch);
+    rc = ss_reserve(ss, chunk);
+    if (rc) return rc;
+    const size_t ct_words = 2 * ss->Lq * ctx->N();
+    return run_pipeline(ctx, h_ct, nullptr, h_out, batch, ct_words, ct_words, chunk,
+                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int { return ss_apply_on(ss, din, dout, cnt, st); });
 }
 
 int dpfhe_describe(const dpfhe_ctx *ctx, char *buf, size_t buf_len) {

@@ -1184,6 +1184,139 @@ DPFHE_HD void rot_apply_grouped_rows(CTA &cta, const RotApplyGArgs &A, const Gro
     });
 }
 
+// ---- summed rotations with grouped hybrid keys (DESIGN.md §2.17) --------------------------------------
+// The key-switch accumulators of n_rot rotations of the same ciphertexts, summed before ONE division by P:
+//   acc[ct][0][i] = [i < Lq] P * (c0[i] + sum_m perm_m(c0[i])) + sum_m sum_g perm_m(U[ct][g][i]) o key_m[g][0][i]
+//   acc[ct][1][i] = [i < Lq] P * c1[i]                         + sum_m sum_g perm_m(U[ct][g][i]) o key_m[g][1][i]
+// for all L limbs, canonical; md_tau / md_limb then yield (c0 + sum_m perm_m(c0) + ks0, c1 + ks1).  The carried terms are
+// multiples of P, so they pass the division exactly (their special residues are 0).
+struct RotSumGArgs {
+    const u64 *ct;                     // [batch][2][Lq][N]
+    const u64 *U;                      // [batch][dnum][L][N]
+    const u64 *key[ROT_SUM_MAX];       // [dnum][2][L][N] Galois key of rotation m
+    const u64 *key_s[ROT_SUM_MAX];     // its Shoup companions
+    u64 *acc;                          // [batch][2][L][N]
+    u32 galois[ROT_SUM_MAX];
+    u32 n_rot;
+};
+
+// The trim schedule of a lazy accumulator row that starts below SB*q and gains one Shoup product (< SB*q) per add(): the running
+// bound b (multiples of q) never passes 16; add() returns whether the row takes csub(8q) right after the addition, which it does
+// whenever the next addition could pass 16q (the rule of acc_trim_after, kept incrementally).
+struct LazyBound {
+    int b = SB;
+    DPFHE_HD bool add() {
+        b += SB;
+        const bool t = b + SB > 16;
+        if (t) b = 8;
+        return t;
+    }
+};
+
+// The rotation loop runs inside the per-chunk loop on the same register accumulators and the operands of rot_apply_grouped_rows
+// (RotOperands): the registers do not grow with n_rot.  On a ciphertext limb every rotation has one more "digit" after its dnum
+// digits: its gathered c0 times the constant P mod q_i (key row 1: zero), which carries P * perm_m(c0) into r0.
+// Lazy bound: both rows start below SB*q (P * c0 and P * c1, ciphertext limbs) and gain one Shoup product (< SB*q) per pair,
+// n_rot * (dnum + 1) <= 15 (dnum + 1) of them; a row takes csub(8q) after a pair whenever the next addition could pass 16q (the
+// rule of acc_trim_after, kept as a running bound), so every value stays below 16q, what canon accepts.
+template <int LOGN, int NT, int CB, class CTA>
+DPFHE_HD void rot_sum_grouped_rows(CTA &cta, const RotSumGArgs &A, const GroupConsts &G, const MsConsts &K, const LimbParams &p, size_t ct0,
+                                   u32 n_ct, u32 i, int c_lo = 0, int c_hi = 1 << (LOGN - 1)) {
+    constexpr int N = 1 << LOGN;
+    const u32 L = G.Lq + G.K, D = G.dnum;
+    const size_t P = (size_t)L * N, Pq = (size_t)G.Lq * N;
+    const bool limb = i < G.Lq;
+    const u32 DM = D + (limb ? 1u : 0u), T = A.n_rot * DM;   // pairs per rotation; T (rotation, digit) pairs, rotation-major
+    // P mod q_i and its companion are read from the parameter block where they are used (K.qlm[i], K.qlm_s[i]; ciphertext limbs
+    // only) rather than held in registers across the loop: the generic variant's body fits its 80 registers that way
+    cta.par([&](int tid) {
+#pragma unroll 1
+        for (int c = c_lo + tid; c < c_hi; c += NT) {
+            auto ct_of = [&](int b) { return ct0 + ((u32)b < n_ct ? (u32)b : n_ct - 1); };   // rows past the end repeat the last one, not stored
+            // the operands of pair k + 1 (key chunks and gathered rows) are requested before the arithmetic of pair k, as in
+            // rot_apply_grouped_rows; the gather positions of a pair are those of its rotation
+            auto fetch = [&](u32 k, RotOperands<CB> &o) {
+                const u32 m = k / DM, d = k - m * DM;
+                const int pi0 = galois_index<LOGN>(2 * c, A.galois[m]);
+                const int pc = pi0 >> 1;
+                const bool swap = (pi0 & 1) != 0;
+                auto gather = [&](const u64 *row) {
+                    const U64x2 v = ld_stream(reinterpret_cast<const U64x2 *>(row) + pc);
+                    U64x2 r;
+                    r.x = swap ? v.y : v.x;
+                    r.y = swap ? v.x : v.y;
+                    return r;
+                };
+                if (d < D) {
+                    const size_t kb = ((size_t)d * 2 + 0) * P + (size_t)i * N, ka = ((size_t)d * 2 + 1) * P + (size_t)i * N;
+                    o.vb = ld_keep(reinterpret_cast<const U64x2 *>(A.key[m] + kb) + c);
+                    o.vbs = ld_keep(reinterpret_cast<const U64x2 *>(A.key_s[m] + kb) + c);
+                    o.va = ld_keep(reinterpret_cast<const U64x2 *>(A.key[m] + ka) + c);
+                    o.vas = ld_keep(reinterpret_cast<const U64x2 *>(A.key_s[m] + ka) + c);
+#pragma unroll
+                    for (int b = 0; b < CB; ++b) o.u[b] = gather(A.U + ((ct_of(b) * D + d) * L + i) * N);
+                } else {   // the carried term perm_m(c0) * P
+                    o.vb.x = o.vb.y = K.qlm[i];
+                    o.vbs.x = o.vbs.y = K.qlm_s[i];
+                    o.va.x = o.va.y = o.vas.x = o.vas.y = 0;
+#pragma unroll
+                    for (int b = 0; b < CB; ++b) o.u[b] = gather(A.ct + ct_of(b) * 2 * Pq + (size_t)i * N);
+                }
+            };
+            U64x2 r0[CB], r1[CB];
+            LazyBound bnd;   // running bound of both rows
+            auto mac = [&](const RotOperands<CB> &o) {
+                const bool trim = bnd.add();
+#pragma unroll
+                for (int b = 0; b < CB; ++b) {
+                    r0[b].x += shoup_lazy(o.u[b].x, o.vb.x, o.vbs.x, p);
+                    r0[b].y += shoup_lazy(o.u[b].y, o.vb.y, o.vbs.y, p);
+                    r1[b].x += shoup_lazy(o.u[b].x, o.va.x, o.vas.x, p);
+                    r1[b].y += shoup_lazy(o.u[b].y, o.va.y, o.vas.y, p);
+                    if (trim) {
+                        r0[b].x = csub(r0[b].x, p.q8); r0[b].y = csub(r0[b].y, p.q8);
+                        r1[b].x = csub(r1[b].x, p.q8); r1[b].y = csub(r1[b].y, p.q8);
+                    }
+                }
+            };
+            RotOperands<CB> oa, ob;
+            fetch(0, oa);
+#pragma unroll
+            for (int b = 0; b < CB; ++b) {
+                r0[b].x = r0[b].y = r1[b].x = r1[b].y = 0;
+                if (limb) {   // the unrotated ciphertext, times P
+                    const size_t row = ct_of(b) * 2 * Pq + (size_t)i * N;
+                    const U64x2 v0 = ld_stream(reinterpret_cast<const U64x2 *>(A.ct + row) + c);
+                    const U64x2 v1 = ld_stream(reinterpret_cast<const U64x2 *>(A.ct + row + Pq) + c);
+                    const u64 pm = K.qlm[i], pm_s = K.qlm_s[i];
+                    r0[b].x = shoup_lazy(v0.x, pm, pm_s, p);   // < SB*q
+                    r0[b].y = shoup_lazy(v0.y, pm, pm_s, p);
+                    r1[b].x = shoup_lazy(v1.x, pm, pm_s, p);
+                    r1[b].y = shoup_lazy(v1.y, pm, pm_s, p);
+                }
+            }
+            for (u32 k = 0; k < T; k += 2) {
+                if (k + 1 < T) fetch(k + 1, ob);
+                mac(oa);
+                if (k + 1 < T) {
+                    if (k + 2 < T) fetch(k + 2, oa);
+                    mac(ob);
+                }
+            }
+#pragma unroll
+            for (int b = 0; b < CB; ++b) {
+                if ((u32)b < n_ct) {
+                    U64x2 o0, o1;
+                    o0.x = canon(r0[b].x, p); o0.y = canon(r0[b].y, p);
+                    o1.x = canon(r1[b].x, p); o1.y = canon(r1[b].y, p);
+                    st_stream(reinterpret_cast<U64x2 *>(A.acc + (ct0 + b) * 2 * P + (size_t)i * N) + c, o0);
+                    st_stream(reinterpret_cast<U64x2 *>(A.acc + (ct0 + b) * 2 * P + P + (size_t)i * N) + c, o1);
+                }
+            }
+        }
+    });
+}
+
 // one (ciphertext, limb i) row pair of one rotation: out = (perm(c0) + ks0, ks1) with the switched pair assembled from the
 // shared transforms.  pi(2c + 1) = pi(2c) ^ 1 (flipping the lowest index bit flips the highest exponent bit, and g is odd),
 // so the two coefficients of an output chunk come from one 16-byte chunk of the source row.

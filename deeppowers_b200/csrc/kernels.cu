@@ -962,6 +962,25 @@ __global__ void __launch_bounds__(NT, MINB) rot_apply_grouped_kernel(RotApplyGAr
     }
 }
 
+// summed rotations (DESIGN.md §2.17): the accumulators of every rotation of a stage, summed, for blocks of ROT_CB ciphertexts x one
+// limb x one segment of the row; the work split of rot_apply_grouped_kernel
+template <int LOGN, int NT, int MINB, int ROT_CB>
+__global__ void __launch_bounds__(NT, MINB) rot_sum_grouped_kernel(const __grid_constant__ RotSumGArgs A, const __grid_constant__ LimbTable lt,
+                                                                   const __grid_constant__ MsConsts K, const __grid_constant__ GroupConsts G,
+                                                                   size_t batch, u32 nseg) {
+    DevCta<NT> cta;
+    constexpr int NC = 1 << (LOGN - 1);
+    const u32 L = G.Lq + G.K;
+    const size_t n_blocks = (batch + ROT_CB - 1) / ROT_CB, n_items = n_blocks * L * nseg;
+    const int seg_chunks = NC / (int)nseg;
+    for (size_t w = blockIdx.x; w < n_items; w += gridDim.x) {
+        const u32 seg = (u32)(w % nseg), i = (u32)((w / nseg) % L);
+        const size_t ct0 = (w / nseg / L) * ROT_CB;
+        const u32 n_ct = (u32)(batch - ct0 < (size_t)ROT_CB ? batch - ct0 : (size_t)ROT_CB);
+        rot_sum_grouped_rows<LOGN, NT, ROT_CB>(cta, A, G, K, lt.lp[i], ct0, n_ct, i, (int)seg * seg_chunks, ((int)seg + 1) * seg_chunks);
+    }
+}
+
 #endif
 #if DPFHE_PART_MAIN
 // ------------------------------------------------------------------ plaintext inner products (BSGS inner loop)
@@ -1894,6 +1913,35 @@ cudaError_t launch_rot_apply_grouped(LaunchCtx &lc, const u64 *ct, const u64 *U,
         case 12: rot_apply_grouped_kernel<12, 256, 3, 2><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
         case 13: rot_apply_grouped_kernel<13, 256, 3, 2><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
         case 14: rot_apply_grouped_kernel<14, 256, 3, 2><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
+        default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
+}
+
+// summed rotations: acc [batch][2][L][N] of n_rot (1 .. ROT_SUM_MAX) rotations with their keys' Shoup companions key_s[m]
+cudaError_t launch_rot_sum_grouped(const LaunchCtx &lc, const u64 *ct, const u64 *U, u32 n_rot, const u64 *const *keys, const u64 *const *key_s,
+                                   const u32 *galois, u64 *acc, const MsConsts &K, const GroupConsts &G, size_t batch, cudaStream_t st) {
+    if (batch == 0) return cudaSuccess;
+    if (n_rot < 1 || n_rot > (u32)ROT_SUM_MAX || G.Lq + G.K != lc.L) return cudaErrorInvalidValue;
+    RotSumGArgs A;
+    memset(&A, 0, sizeof(A));
+    A.ct = ct; A.U = U; A.acc = acc; A.n_rot = n_rot;
+    for (u32 m = 0; m < n_rot; ++m) {
+        A.key[m] = keys[m];
+        A.key_s[m] = key_s[m];
+        A.galois[m] = galois[m];
+    }
+    // one ciphertext per work item: with two (the rot_apply_grouped split) the 80 registers of three CTAs per SM spill
+    const size_t rows = batch * lc.L, want = (size_t)lc.num_sms * 12;
+    u32 nseg = 1;
+    const u32 max_seg = (1u << (lc.log_n - 1)) / 256;
+    while (nseg < max_seg && rows * nseg < want) nseg *= 2;
+    const size_t n_items = rows * nseg, cap = (size_t)lc.num_sms * 8;
+    const unsigned grid = (unsigned)(n_items < cap ? n_items : cap);
+    switch (lc.log_n) {
+        case 12: rot_sum_grouped_kernel<12, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
+        case 13: rot_sum_grouped_kernel<13, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
+        case 14: rot_sum_grouped_kernel<14, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
         default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();

@@ -64,6 +64,9 @@ struct LaunchCtx {
     cudaError_t launch_key_prepare_grouped(const LaunchCtx &lc, const u64 *key, u64 *key_s, u32 dnum, cudaStream_t st); \
     cudaError_t launch_rot_apply_grouped(LaunchCtx &lc, const u64 *ct, const u64 *U, const u64 *key, const u64 *key_s, u32 galois, u64 *acc, \
                                          const MsConsts &K, const GroupConsts &G, size_t batch, cudaStream_t st); \
+    cudaError_t launch_rot_sum_grouped(const LaunchCtx &lc, const u64 *ct, const u64 *U, u32 n_rot, const u64 *const *keys, \
+                                       const u64 *const *key_s, const u32 *galois, u64 *acc, const MsConsts &K, const GroupConsts &G, \
+                                       size_t batch, cudaStream_t st); \
     cudaError_t launch_pt_inner(const LaunchCtx &lc, const u64 *steps, u32 nb, const u64 *pts, u32 ng, u64 *out, size_t batch, cudaStream_t st, \
                                 unsigned *launches); \
     cudaError_t launch_pointwise_mul(const LaunchCtx &lc, const u64 *a, const u64 *b, u64 *out, size_t n_polys, cudaStream_t st); \
@@ -101,5 +104,6 @@ DPFHE_DECLARE_LAUNCHERS
 // (or, with key_s == nullptr, in lc.ks_key_s).  launch_rot_prepare / launch_rot_apply: key_s(_out) == nullptr means lc.ks_key_s.
 // launch_ks_grouped: key_s == nullptr builds the companions into lc.ks_key_s (two launches), otherwise one launch; addend (KS_ROTATE
 // only) is added to the result in the kernel's final store.
+// launch_rot_sum_grouped: keys[m] / key_s[m] / galois[m] of n_rot (1 .. ROT_SUM_MAX) rotations; the companions are required.
 
 }  // namespace dpfhe

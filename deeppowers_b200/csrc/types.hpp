@@ -88,6 +88,7 @@ struct MsConsts {
 // host (host_params.cpp:build_group_consts) and passed by value in the kernel parameter block, so that every use is a
 // constant-bank operand with a CTA-uniform index.  The MsConsts of such a call describe the division by P (inv = P^-1 ...).
 constexpr int KS_MAX_SPECIAL = 4;
+constexpr int ROT_SUM_MAX = 15;   // rotations of one summed-rotation call (DESIGN.md §2.17)
 struct GroupConsts {
     u32 Lq, K, dnum, pad_;
     // limb parameters whose N^-1 (ninv, wninv) carries the factor that the basis conversion wants on the inverse transform's

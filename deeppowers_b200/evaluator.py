@@ -460,6 +460,24 @@ class Context:
         kp = (C.c_void_p * n)(*[_ptr(k) for k in gks])
         self._chk(self._l.dpfhe_rotate_hoisted_grouped(self._h, int(n_special), _ptr(ct), n, ge, kp, _ptr(out), batch, int(t_plain), _stream(stream)))
 
+    def rotate_sum_grouped(self, n_special, ct, galois_elts, gks, out, batch, t_plain=0, stream=None):
+        """out = ct + sum_r rot_r(ct) with one division by P for all rotations (DESIGN.md section 2.17); 1 .. 15 rotations, gks: list
+        of device tensors [dnum][2][L][N]; ct, out: [batch][2][L-n_special][N], out must not overlap ct"""
+        n = len(galois_elts)
+        if len(gks) != n:
+            raise ValueError("need one key per Galois element")
+        ge = (C.c_uint64 * max(n, 1))(*[int(g) for g in galois_elts])
+        kp = (C.c_void_p * max(n, 1))(*[_ptr(k) for k in gks])
+        self._chk(self._l.dpfhe_rotate_sum_grouped(self._h, int(n_special), _ptr(ct), n, ge, kp, _ptr(out), batch, int(t_plain), _stream(stream)))
+
+    def rotate_sum_grouped_host(self, n_special, ct, galois_elts, gks, out, t_plain=0):
+        """host form of rotate_sum_grouped: gks [n_rot][dnum][2][L][N] (C-contiguous numpy uint64)"""
+        n = len(galois_elts)
+        ge = (C.c_uint64 * max(n, 1))(*[int(g) for g in galois_elts])
+        pq = 2 * (self.L - n_special) * self.N
+        self._chk(self._l.dpfhe_rotate_sum_grouped_host(self._h, int(n_special), _hptr(ct), n, ge, _hptr(gks), _hptr(out, True), ct.size // pq,
+                                                        int(t_plain)))
+
     def mod_down_special(self, n_special, polys, out, n_polys, t_plain=0, stream=None):
         self._chk(self._l.dpfhe_mod_down_special(self._h, int(n_special), _ptr(polys), _ptr(out), n_polys, int(t_plain), _stream(stream)))
 
@@ -661,6 +679,60 @@ class PolyEval:
 
     def apply_host(self, ct, out):
         self.ctx._chk(self._l.dpfhe_polyeval_apply_host(self._h, _hptr(ct), _hptr(out, True), ct.size // (2 * self.Lq * self.ctx.N)))
+
+
+def slotsum_steps(stride, radices):
+    """The rotation steps of a slot sum (dpfhe_slotsum_steps, DESIGN.md section 2.17), stage by stage and ascending within a stage:
+    the order of the Galois keys SlotSum.grouped takes."""
+    lib = _lib.load()
+    rs = (C.c_uint * max(len(radices), 1))(*[int(r) for r in radices])
+    n = C.c_size_t(0)
+    if lib.dpfhe_slotsum_steps(int(stride), rs, len(radices), None, C.byref(n)) != 0:
+        raise DpfheError(lib.dpfhe_last_error().decode())
+    out = (C.c_int * max(n.value, 1))()
+    if lib.dpfhe_slotsum_steps(int(stride), rs, len(radices), out, C.byref(n)) != 0:
+        raise DpfheError(lib.dpfhe_last_error().decode())
+    return [int(out[k]) for k in range(n.value)]
+
+
+class SlotSum:
+    """Encrypted slot sums as a library object (dpfhe_slotsum_*, DESIGN.md section 2.17): slot i of the result is
+    sum_{j < count} x[(i + j * stride) mod N/2] in every row, count = prod(radices), one summed-rotation call per radix.  Build it
+    with SlotSum.grouped; apply / apply_host take ciphertexts [batch][2][Lq][N]."""
+
+    def __init__(self, ctx, n_special, stride, radices, gks, t_plain=0):
+        self._l, self.ctx = ctx._l, ctx
+        self._h = C.c_void_p()
+        self.n_special = int(n_special)
+        self.Lq = ctx.L - self.n_special
+        self.stride, self.radices = int(stride), [int(r) for r in radices]
+        rs = (C.c_uint * max(len(self.radices), 1))(*self.radices)
+        rc = self._l.dpfhe_slotsum_create_grouped(ctx._h, self.n_special, self.stride, rs, len(self.radices), _hptr(gks), int(t_plain),
+                                                  C.byref(self._h))
+        if rc != 0:
+            self._h = C.c_void_p()
+            raise DpfheError(self._l.dpfhe_last_error().decode())
+
+    @classmethod
+    def grouped(cls, ctx, n_special, stride, radices, gks, t_plain=0):
+        """ctx's last n_special limbs are special primes; gks [n_steps][dnum][2][L][N] (C-contiguous numpy uint64): the grouped Galois
+        keys of the rotations by slotsum_steps(stride, radices), in that order; t_plain as rotate_hoisted_grouped (0: CKKS)"""
+        return cls(ctx, n_special, stride, radices, gks, t_plain)
+
+    def close(self):
+        """Close the object before its context (as LinearLayer.close)."""
+        if getattr(self, "_h", None) and self._h.value:
+            if self.ctx._h.value:
+                self._l.dpfhe_slotsum_destroy(self._h)
+            self._h = C.c_void_p()
+
+    __del__ = close
+
+    def apply(self, ct, out, batch, stream=None):
+        self.ctx._chk(self._l.dpfhe_slotsum_apply(self._h, _ptr(ct), _ptr(out), batch, _stream(stream)))
+
+    def apply_host(self, ct, out):
+        self.ctx._chk(self._l.dpfhe_slotsum_apply_host(self._h, _hptr(ct), _hptr(out, True), ct.size // (2 * self.Lq * self.ctx.N)))
 
 
 class MultiContext:

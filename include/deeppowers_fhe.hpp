@@ -239,6 +239,16 @@ public:
         for (std::size_t r = 0; r < steps.size(); ++r) elts[r] = galois_element(steps[r]);
         check(dpfhe_rotate_hoisted_grouped(ctx_, special, ct, steps.size(), elts.data(), galois_keys.data(), out, count, plain_modulus, stream));
     }
+    // out = ct + the sum of ct rotated by every steps[r] (1 .. 15 rotations), with one division by P for all of them (DESIGN.md §2.17);
+    // out must not overlap ct
+    void rotate_sum_grouped_device(unsigned special, const std::uint64_t *ct, const std::vector<long> &steps,
+                                   const std::vector<const std::uint64_t *> &galois_keys, std::uint64_t *out, std::size_t count,
+                                   std::uint64_t plain_modulus = 0, void *stream = nullptr) {
+        if (steps.size() != galois_keys.size()) throw std::invalid_argument("one Galois key per rotation");
+        std::vector<std::uint64_t> elts(steps.size());
+        for (std::size_t r = 0; r < steps.size(); ++r) elts[r] = galois_element(steps[r]);
+        check(dpfhe_rotate_sum_grouped(ctx_, special, ct, steps.size(), elts.data(), galois_keys.data(), out, count, plain_modulus, stream));
+    }
     // divide by the product of the last `special` limbs: in holds limbs() limbs per polynomial, out limbs()-special
     void mod_down_special_device(unsigned special, const std::uint64_t *ct, std::uint64_t *out, std::size_t count, std::uint64_t plain_modulus = 0,
                                  void *stream = nullptr) {
@@ -334,6 +344,7 @@ public:
 private:
     friend class LinearLayer;
     friend class PolyEval;
+    friend class SlotSum;
     friend class CkksPolyEval;
     static void check(int status) {
         if (status != DPFHE_OK) throw std::runtime_error(dpfhe_last_error());
@@ -447,6 +458,39 @@ public:
 
 private:
     dpfhe_polyeval *h_ = nullptr;
+};
+
+// Slot sums (dpfhe_slotsum_*, DESIGN.md §2.17): slot i of the result is sum_{j < prod(radices)} x[(i + j * stride) mod N/2] in every
+// row.  galois_keys: the grouped Galois keys of the rotations by SlotSum::steps(stride, radices), in that order, back to back in host
+// memory (what Evaluator::generate_galois_keys writes); plain_modulus 0 for CKKS.
+class SlotSum {
+public:
+    SlotSum(Evaluator &ev, unsigned special, std::size_t stride, const std::vector<unsigned> &radices, const std::uint64_t *galois_keys,
+            std::uint64_t plain_modulus = 0) {
+        Evaluator::check(dpfhe_slotsum_create_grouped(ev.native_handle(), special, stride, radices.data(), radices.size(), galois_keys, plain_modulus,
+                                                      &h_));
+    }
+    ~SlotSum() { dpfhe_slotsum_destroy(h_); }
+    SlotSum(const SlotSum &) = delete;
+    SlotSum &operator=(const SlotSum &) = delete;
+    // the rotation steps, stage by stage and ascending within a stage: the order of the keys
+    static std::vector<long> steps(std::size_t stride, const std::vector<unsigned> &radices) {
+        std::size_t n = 0;
+        Evaluator::check(dpfhe_slotsum_steps(stride, radices.data(), radices.size(), nullptr, &n));
+        std::vector<int> s(n);
+        Evaluator::check(dpfhe_slotsum_steps(stride, radices.data(), radices.size(), s.data(), &n));
+        return std::vector<long>(s.begin(), s.end());
+    }
+    void apply(ConstCiphertextBatch in, CiphertextBatch out) {   // host buffers, pipelined
+        if (in.count != out.count) throw std::runtime_error("ciphertext batches must have the same count");
+        Evaluator::check(dpfhe_slotsum_apply_host(h_, in.data, out.data, in.count));
+    }
+    void apply_device(const std::uint64_t *in, std::uint64_t *out, std::size_t count, void *stream = nullptr) {
+        Evaluator::check(dpfhe_slotsum_apply(h_, in, out, count, stream));
+    }
+
+private:
+    dpfhe_slotsum *h_ = nullptr;
 };
 
 // CKKS polynomial evaluation on encrypted slots down the rescaling chain (dpfhe_polyeval_create_ckks, DESIGN.md §2.16): p(z) = sum_k

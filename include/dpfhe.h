@@ -253,6 +253,35 @@ int dpfhe_rotate_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_c
  * keys) as well. */
 int dpfhe_rotate_hoisted_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_ct, size_t n_rot, const uint64_t *galois_elts,
                                  const uint64_t *const *d_gks, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream);
+/* Summed rotations (DESIGN.md §2.17): d_out = ct + sum_r rot_r(ct) for n_rot = 1 .. 15 rotations of the same ciphertexts,
+ * [batch][2][L-K][N].  The key-switch accumulators of all rotations are summed over the L limbs and divided by P ONCE: one
+ * mod-up, one summed multiply-accumulate and one division per ciphertext (24 transforms at Lq = 4, K = 2, whatever n_rot is).
+ * n_rot = 1 is dpfhe_rotate_hoisted_grouped + dpfhe_poly_add with ct, bit for bit; n_rot >= 2 decrypts to the same plaintext as
+ * that composition summed, not the same bits (one rounding instead of n_rot).  Argument checks of dpfhe_rotate_hoisted_grouped;
+ * d_out must not overlap d_ct.  The keys' Shoup companions are built per call (n_rot launches), then 4 launches per chunk. */
+int dpfhe_rotate_sum_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_ct, size_t n_rot, const uint64_t *galois_elts,
+                             const uint64_t *const *d_gks, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream);
+/* host-buffer form: h_gks [n_rot][dnum][2][L][N] back to back, uploaded once; the batch pipelined in chunks (synchronous) */
+int dpfhe_rotate_sum_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_ct, size_t n_rot, const uint64_t *galois_elts,
+                                  const uint64_t *h_gks, uint64_t *h_out, size_t batch, uint64_t t_plain);
+/* ---- slot sums (DESIGN.md §2.17): slot i of the result is sum_{j < count} x[(i + j * stride) mod N/2] in every row, count =
+ *      prod radices[t], computed in n_stages (1 .. 16) summed-rotation stages; stage t rotates by m * stride * prod_{u<t} radices[u],
+ *      m = 1 .. radices[t] - 1 (2 <= radices[t] <= 16), and stride * count must be at most N/2.
+ *      dpfhe_slotsum_steps: the rotation steps, stage by stage and m ascending, which is the order of the keys (stateless, so
+ *      that the keys can be generated first); steps may be NULL (then only *n_steps is written), otherwise it holds
+ *      sum (radices[t] - 1) entries.  Without a context it checks stride * count <= 8192 (N/2 at N = 16384); creation checks N/2.
+ *      dpfhe_slotsum_create_grouped: h_gks [n_steps][dnum][2][L][N], the grouped Galois keys of 5^step in that order (what
+ *      dpfhe_galois_keygen writes), uploaded with their Shoup companions once.  apply: d_ct, d_out [batch][2][L-K][N], d_out must
+ *      not overlap d_ct; 4 launches per stage (per chunk of the hoisted-rotation scratch); the intermediate stage results are
+ *      scratch that grows with the batch and counts in dpfhe_context_device_bytes.  apply_host: host buffers, pipelined in
+ *      chunks (synchronous). ---- */
+typedef struct dpfhe_slotsum dpfhe_slotsum;
+int dpfhe_slotsum_steps(size_t stride, const unsigned *radices, size_t n_stages, int *steps, size_t *n_steps);
+int dpfhe_slotsum_create_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t stride, const unsigned *radices, size_t n_stages,
+                                 const uint64_t *h_gks, uint64_t t_plain, dpfhe_slotsum **out);
+int dpfhe_slotsum_apply(dpfhe_slotsum *ss, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream);
+int dpfhe_slotsum_apply_host(dpfhe_slotsum *ss, const uint64_t *h_ct, uint64_t *h_out, size_t batch);
+void dpfhe_slotsum_destroy(dpfhe_slotsum *ss);
 /* division by the product of the last n_special limbs alone (the mod-down half of the calls above; n_special = 1 is
  * dpfhe_mod_switch_down): in [n_polys][L][N] -> out [n_polys][L - n_special][N], 1 <= n_special <= 4, n_special < L */
 int dpfhe_mod_down_special(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_in, uint64_t *d_out, size_t n_polys,
