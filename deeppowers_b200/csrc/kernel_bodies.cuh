@@ -633,10 +633,10 @@ DPFHE_HD void ks_blk_p1_terms(const KsP1Operands &o, const LimbParams &p, U64x2 
         s0 = o.a0;
         s1.x = s1.y = 0;
     }
-    r0.x = s0.x + shoup_lazy(d.x, o.kb.x, o.kbs.x, p);
-    r0.y = s0.y + shoup_lazy(d.y, o.kb.y, o.kbs.y, p);
-    r1.x = s1.x + shoup_lazy(d.x, o.ka.x, o.kas.x, p);
-    r1.y = s1.y + shoup_lazy(d.y, o.ka.y, o.kas.y, p);
+    r0.x = s0.x + shoup_lazy_cc(d.x, o.kb.x, o.kbs.x, p);
+    r0.y = s0.y + shoup_lazy_cc(d.y, o.kb.y, o.kbs.y, p);
+    r1.x = s1.x + shoup_lazy_cc(d.x, o.ka.x, o.kas.x, p);
+    r1.y = s1.y + shoup_lazy_cc(d.y, o.ka.y, o.kas.y, p);
 }
 
 template <int LOGN, int NT, int MODE, class CTA>

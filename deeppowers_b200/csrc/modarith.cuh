@@ -63,6 +63,32 @@ DPFHE_HD u64 mulhi_approx(u64 x, u64 y) {
 #endif
 }
 
+// mulhi_approx, the same value, with the middle sum pinned as a 32-bit add with carry that is the addend of the xh*yh
+// multiply-add (IADD3, one carry instruction, IMAD.WIDE).  Where a product feeds several sums while its operand stays live (the
+// forward butterfly: x + t and x + SB*q - t; the Barrett quotient of the tensor), ptxas folds the plain sums the other way,
+// xh*yh + hi(a) through a zero-extended register pair and then + hi(b), which costs two IMAD.MOV on the multiplier pipe per
+// product.  The inverse butterfly keeps mulhi_approx: there the plain sums compile to fewer instructions than this block.
+DPFHE_HD u64 mulhi_approx_cc(u64 x, u64 y) {
+#if DPFHE_SHOUP_APPROX == 0 || !defined(__CUDA_ARCH__)
+    return mulhi_approx(x, y);
+#else
+    const u32 xl = (u32)x, xh = (u32)(x >> 32), yl = (u32)y, yh = (u32)(y >> 32);
+    const u64 a = mul_wide(xh, yl), b = mul_wide(xl, yh);
+    u64 r;
+    asm("{\n\t"
+        ".reg .u32 ml, mh;\n\t"
+        ".reg .u64 m;\n\t"
+        "add.cc.u32 ml, %1, %2;\n\t"
+        "addc.u32 mh, 0, 0;\n\t"
+        "mov.b64 m, {ml, mh};\n\t"
+        "mad.wide.u32 %0, %3, %4, m;\n\t"
+        "}"
+        : "=l"(r)
+        : "r"((u32)(a >> 32)), "r"((u32)(b >> 32)), "r"(xh), "r"(yh));
+    return r;
+#endif
+}
+
 // x >= m ? x - m : x, branch-free.  Correct for every 64-bit x when m <= 2^63.
 // Device: subtract with borrow and select on the borrow (IADD3, IADD3.X, 2x SEL).
 DPFHE_HD u64 csub(u64 x, u64 m) {
@@ -173,6 +199,8 @@ DPFHE_HD u64 shoup_tail(u64 x, u64 w, u64 h, const LimbParams &p) {
 //   shoup_lazy:  e <= 2 (mulhi_approx, 3 IMAD.WIDE), r in [0, SB*q)
 DPFHE_HD u64 shoup_exact(u64 x, u64 w, u64 ws, const LimbParams &p) { return shoup_tail(x, w, umulhi64(x, ws), p); }
 DPFHE_HD u64 shoup_lazy(u64 x, u64 w, u64 ws, const LimbParams &p) { return shoup_tail(x, w, mulhi_approx(x, ws), p); }
+// shoup_lazy with mulhi_approx_cc: the same value
+DPFHE_HD u64 shoup_lazy_cc(u64 x, u64 w, u64 ws, const LimbParams &p) { return shoup_tail(x, w, mulhi_approx_cc(x, ws), p); }
 
 // 128-bit product (hi:lo) of two 64-bit words.  Device: four IMAD.WIDE partial products combined once
 // (nvcc's separate a*b and __umul64hi(a,b) would recompute the low partial product: 5 IMAD.WIDE + 2 IMAD).
@@ -231,7 +259,7 @@ DPFHE_HD u64 barrett_lazy(u64 hi, u64 lo, const LimbParams &p) {
 #else
     const u64 zt = (hi << (64 - s)) | (lo >> s);     // floor(z / 2^s) < 2^64
 #endif
-    return sub_mul_q(lo, mulhi_approx(zt, p.bar_mu), p);   // lo - qhat*q
+    return sub_mul_q(lo, mulhi_approx_cc(zt, p.bar_mu), p);   // lo - qhat*q
 }
 
 // Barrett reduction of a longer sum z = hi:lo < 2^(2b+4), b = bit length of q (e.g. 16 products of canonical factors):

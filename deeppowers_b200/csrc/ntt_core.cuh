@@ -30,7 +30,7 @@ DPFHE_HD int swz_chunk(int cg) { return cg ^ ((cg >> 3) & 7); }
 // ---- butterflies -----------------------------------------------------------------------
 // forward, fully lazy: x' = x + w*y, y' = x - w*y + SB*q; bound grows by SB per stage (SB*q: bound of shoup_lazy).
 DPFHE_HD void ct_bfly(u64 &x, u64 &y, const Twiddle &w, const LimbParams &p) {
-    u64 t = shoup_lazy(y, w.x, w.y, p);
+    u64 t = shoup_lazy_cc(y, w.x, w.y, p);
     u64 a = x;
     x = a + t;
     y = a + p.qsb - t;
@@ -57,21 +57,35 @@ DPFHE_HD constexpr int fwd_bound_after(int bin, int stages) {
     for (int s = 0; s < stages; ++s) b = (b + SB > 16 ? 8 : b) + SB;
     return b;
 }
+// fwd_needs_csub(bin, u) for u < 4 as bit u.  Kernels take the schedule from a constexpr mask: called per butterfly inside an
+// unrolled pass, fwd_needs_csub is left as a runtime loop (one per butterfly of stages 2 and 3) that selects the subtraction
+// at run time and cuts the pass into basic blocks the scheduler cannot interleave.
+DPFHE_HD constexpr unsigned fwd_csub_mask16(int bin) {
+    unsigned m = 0;
+    for (int u = 0; u < 4; ++u) m |= fwd_needs_csub(bin, u) ? 1u << u : 0u;
+    return m;
+}
 
 // 16-point register kernels.  `x[k]` holds element k of a radix-16 group; stage u pairs
 // k with k + (8 >> u).  tw(u, j) returns the twiddle of sub-group j at local stage u.
 template <int BIN, class TW>
 DPFHE_HD void fwd16(u64 (&x)[16], const LimbParams &p, TW tw) {
+    // constant trip counts, as in inv16 below
+    constexpr unsigned CSUB = fwd_csub_mask16(BIN);
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
         const int half = 8 >> u;
 #pragma unroll
-        for (int j = 0; j < (1 << u); ++j) {
-            const Twiddle w = tw(u, j);
+        for (int j = 0; j < 8; ++j) {
+            if (j < (1 << u)) {
+                const Twiddle w = tw(u, j);
 #pragma unroll
-            for (int i = 0; i < half; ++i) {
-                if (fwd_needs_csub(BIN, u)) x[j * 2 * half + i] = csub(x[j * 2 * half + i], p.q8);
-                ct_bfly(x[j * 2 * half + i], x[j * 2 * half + half + i], w, p);
+                for (int i = 0; i < 8; ++i) {
+                    if (i < half) {
+                        if ((CSUB >> u) & 1u) x[j * 2 * half + i] = csub(x[j * 2 * half + i], p.q8);
+                        ct_bfly(x[j * 2 * half + i], x[j * 2 * half + half + i], w, p);
+                    }
+                }
             }
         }
     }
@@ -368,7 +382,7 @@ DPFHE_HD void fwd_load_stage_blk(u64 *buf, const Twiddle *__restrict__ tw, const
             for (int e = 0; e < 2; ++e) {
                 const u64 x = IN_REDUCE ? word_reduce(e ? vx.y : vx.x, p) : (e ? vx.y : vx.x);
                 const u64 y = IN_REDUCE ? word_reduce(e ? vy.y : vy.x, p) : (e ? vy.y : vy.x);
-                const u64 t = shoup_lazy(y, w.x, w.y, p);
+                const u64 t = shoup_lazy_cc(y, w.x, w.y, p);
                 (e ? o.y : o.x) = h == 0 ? x + t : x + p.qsb - t;
             }
             reinterpret_cast<U64x2 *>(buf)[swz_chunk(c)] = o;

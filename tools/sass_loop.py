@@ -2,8 +2,8 @@
 usage: sass_loop.py <cubin-or-so> <kernel-name-regex> [per]   (per = divide counts by this number)"""
 import collections, re, subprocess, sys
 
-def kernels(path):
-    out = subprocess.run(["cuobjdump", "-sass", path], capture_output=True, text=True).stdout
+def kernels(path, cuobjdump="cuobjdump"):
+    out = subprocess.run([cuobjdump, "-sass", path], capture_output=True, text=True).stdout
     cur, res = None, {}
     for line in out.splitlines():
         m = re.search(r"Function : (\S+)", line)
