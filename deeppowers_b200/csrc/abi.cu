@@ -51,6 +51,12 @@ namespace {
 
 bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+#define CHECK_PTR(p)                                                                          \
+    do {                                                                                      \
+        if (!(p)) return fail(DPFHE_ERR_INVALID, "null pointer: %s", #p);                     \
+        if (!aligned16(p)) return fail(DPFHE_ERR_INVALID, "%s must be 16-byte aligned", #p);  \
+    } while (0)
+
 // byte ranges [a, a + na) and [b, b + nb) intersect (unified addressing: valid across devices too)
 bool overlaps(const void *a, size_t na, const void *b, size_t nb) {
     if (!a || !b || !na || !nb) return false;
@@ -234,6 +240,114 @@ size_t grid_round_chunk(const dpfhe_ctx *ctx, size_t batch, const char *rounds_e
     if (rounds < 1) rounds = 1;
     const size_t chunk = rounds * groups;
     return chunk > 512 ? std::max<size_t>(groups, 512 / groups * groups) : chunk;
+}
+
+// the same, unless the variable `items_env` gives the chunk in ciphertexts (tests: several chunks at a small batch)
+size_t item_chunk(const dpfhe_ctx *ctx, size_t batch, const char *items_env) {
+    if (const char *e = getenv(items_env)) return std::max<size_t>(1, (size_t)atol(e));
+    return grid_round_chunk(ctx, batch, nullptr);
+}
+
+// The context's launch state restricted to its first l limbs.  That prefix is a basis of its own: the limb constants and twiddles
+// are rows indexed by limb with the ciphertext moduli first, and nothing else in the launch state depends on L.  So a view costs
+// no device memory, and driven on the stream of the call it keeps the calls' order.
+LaunchCtx level_view(const dpfhe_ctx *ctx, unsigned l) {
+    LaunchCtx lc = ctx->lc;
+    lc.L = l;
+    return lc;
+}
+
+// n grouped keys [n][dnum][2][L][N] on the device, back to back, and their Shoup companions in a second allocation of the same
+// layout; keys[k] / key_s[k] point at key k.  Copyable: whoever holds it calls release().
+struct PreparedKeys {
+    u64 *d_keys = nullptr, *d_key_s = nullptr;
+    std::vector<const u64 *> keys, key_s;
+    size_t bytes = 0;   // of both allocations
+    void release() {
+        cudaFree(d_keys);
+        cudaFree(d_key_s);
+        *this = PreparedKeys();
+    }
+};
+
+// Allocates both arrays, has `upload(d_keys)` copy the keys up (all of them, or the rows a level keeps) and issues the companions'
+// launches on `st` with the launch state `lc`, one per key; the caller waits for them.  On failure nothing stays allocated.
+template <class Upload>
+int prepare_keys(dpfhe_ctx *ctx, const LaunchCtx &lc, size_t n, size_t dnum, cudaStream_t st, const char *what, Upload upload, PreparedKeys &pk) {
+    const size_t key_words = dnum * 2 * lc.L * ((size_t)1 << lc.log_n);
+    cudaError_t e = cudaMalloc(&pk.d_keys, n * key_words * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&pk.d_key_s, n * key_words * 8);
+    if (e == cudaSuccess) e = upload(pk.d_keys);
+    for (size_t k = 0; k < n && e == cudaSuccess; ++k) {
+        pk.keys.push_back(pk.d_keys + k * key_words);
+        pk.key_s.push_back(pk.d_key_s + k * key_words);
+        e = VCALL(launch_key_prepare_grouped, lc, pk.keys[k], pk.d_key_s + k * key_words, (u32)dnum, st);
+        note_launch(ctx, 1);
+    }
+    if (e != cudaSuccess) {
+        pk.release();
+        return fail(DPFHE_ERR_CUDA, "%s: %s", what, cudaGetErrorString(e));
+    }
+    pk.bytes = 2 * n * key_words * 8;
+    return DPFHE_OK;
+}
+
+// ---- The lifecycle of a library object built on a context (DESIGN.md §4.14).  Obj provides: ctx; `what`, the message for a null
+// handle; in_words() / out_words(), the words of a ciphertext in and out; reserve(batch), the scratch of an application;
+// apply_on(d_ct, d_out, batch, stream), the launches; host_chunk(batch), the ciphertexts per chunk of the host form (capped by the
+// batch here); and a destructor that frees its device memory.
+
+template <class Obj>
+int object_apply(Obj *obj, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
+    if (!obj) return fail(DPFHE_ERR_INVALID, "%s", Obj::what);
+    int rc = enter(obj->ctx);
+    if (rc) return rc;
+    if (batch == 0) return DPFHE_OK;
+    CHECK_PTR(d_ct); CHECK_PTR(d_out);
+    if (overlaps(d_out, batch * obj->out_words() * 8, d_ct, batch * obj->in_words() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    rc = obj->reserve(batch);
+    if (rc) return rc;
+    return obj->apply_on(d_ct, d_out, batch, stream);
+}
+
+// host buffers: chunks of the batch pipelined through apply_on (upload / compute / download overlapped)
+template <class Obj>
+int object_apply_host(Obj *obj, const uint64_t *h_ct, uint64_t *h_out, size_t batch) {
+    if (!obj) return fail(DPFHE_ERR_INVALID, "%s", Obj::what);
+    int rc = enter(obj->ctx);
+    if (rc) return rc;
+    if (batch == 0) return DPFHE_OK;
+    if (!h_ct || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const size_t chunk = std::min(obj->host_chunk(batch), batch);
+    rc = obj->reserve(chunk);
+    if (rc) return rc;
+    return run_pipeline(obj->ctx, h_ct, nullptr, h_out, batch, obj->in_words(), obj->out_words(), chunk,
+                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int { return obj->apply_on(din, dout, cnt, st); });
+}
+
+// waits for the context's work, which may still use the object's buffers
+template <class Obj>
+void object_destroy(Obj *obj) {
+    if (!obj) return;
+    cudaSetDevice(obj->ctx->lc.device);
+    dpfhe_synchronize(obj->ctx);
+    delete obj;
+}
+
+// The end of a constructor (rc: the result of everything before): waits for the launches on `st` that prepared the object's
+// constants and hands the object out, or deletes it and reports the failure.
+template <class Obj>
+int object_finish(Obj *obj, int rc, cudaStream_t st, const char *what, Obj **out) {
+    if (rc == DPFHE_OK) {
+        const cudaError_t e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) rc = fail(DPFHE_ERR_CUDA, "%s: %s", what, cudaGetErrorString(e));
+    }
+    if (rc != DPFHE_OK) {
+        delete obj;   // cudaFree waits for the device
+        return rc;
+    }
+    *out = obj;
+    return DPFHE_OK;
 }
 
 // The device tables of a modulus basis: limb constants d_lp [L] (also copied into lt, for the kernels' parameter blocks) and the
@@ -428,7 +542,7 @@ size_t dpfhe_context_device_bytes(const dpfhe_ctx *ctx) {
     size_t n = ctx->device_bytes;   // tables, key companions, digit slots, accumulators, flags (+ hybrid rows)
     dpfhe_ctx::each_trimmed(*ctx, [&](const DeviceScratch &s) { n += s.bytes(); });
     n += ctx->hoist_M.bytes() + ctx->hoist_kprime.bytes() + ctx->hoist_delta.bytes();
-    n += ctx->object_bytes;         // polynomial evaluators: level tables, keys, scratch
+    n += ctx->object_bytes;         // polynomial evaluators and slot sums: level tables, keys, scratch (CountedScratch)
     return n;
 }
 
@@ -446,12 +560,6 @@ int dpfhe_context_trim(dpfhe_ctx *ctx) {
     return DPFHE_OK;
 }
 uint64_t dpfhe_launch_count(const dpfhe_ctx *ctx) { return ctx ? ctx->launches : 0; }
-
-#define CHECK_PTR(p)                                                                          \
-    do {                                                                                      \
-        if (!(p)) return fail(DPFHE_ERR_INVALID, "null pointer: %s", #p);                     \
-        if (!aligned16(p)) return fail(DPFHE_ERR_INVALID, "%s must be 16-byte aligned", #p);  \
-    } while (0)
 
 int dpfhe_ntt_fwd(dpfhe_ctx *ctx, uint64_t *d_data, size_t n_polys, void *stream) {
     int rc = enter(ctx);
@@ -543,6 +651,12 @@ static int check_special(const dpfhe_ctx *ctx, unsigned n_special) {
     return DPFHE_OK;
 }
 
+// a call with grouped special-prime keys that ends in a division by the special primes with plaintext modulus t_plain
+static int check_grouped(const dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain) {
+    const int rc = check_special(ctx, n_special);
+    return rc ? rc : check_t_below_special(ctx, n_special, t_plain);
+}
+
 // digits of a key: groups of n_special limbs of the L - n_special ciphertext moduli; n_special = 0: per-limb digits, L of them
 static size_t key_digits(const dpfhe_ctx *ctx, unsigned n_special) {
     const unsigned L = ctx->hp.L;
@@ -569,9 +683,7 @@ static int ks_hybrid_common(dpfhe_ctx *ctx, unsigned n_special, int mode, const 
     CHECK_PTR(a); CHECK_PTR(key); CHECK_PTR(out);
     if (mode == KS_MUL_RELIN) CHECK_PTR(b);
     const unsigned L = ctx->hp.L;
-    rc = check_special(ctx, n_special);
-    if (rc) return rc;
-    rc = check_t_below_special(ctx, n_special, t_plain);
+    rc = check_grouped(ctx, n_special, t_plain);
     if (rc) return rc;
     rc = mode == KS_ROTATE ? check_galois(ctx, galois) : DPFHE_OK;
     if (rc) return rc;
@@ -710,11 +822,9 @@ static int rotate_hoisted_grouped_impl(dpfhe_ctx *ctx, unsigned n_special, const
     if (batch == 0 || n_rot == 0) return DPFHE_OK;
     CHECK_PTR(d_ct); CHECK_PTR(d_out);
     if (!galois_elts || !d_gks) return fail(DPFHE_ERR_INVALID, "null argument");
-    rc = check_special(ctx, n_special);
+    rc = check_grouped(ctx, n_special, t_plain);
     if (rc) return rc;
     const size_t N = ctx->N(), L = ctx->hp.L, Lq = L - n_special, Pq = Lq * N, dnum = (Lq + n_special - 1) / n_special;
-    rc = check_t_below_special(ctx, n_special, t_plain);
-    if (rc) return rc;
     rc = check_rotations(ctx, n_rot, galois_elts, d_gks);
     if (rc) return rc;
     if (overlaps(d_out, n_rot * batch * 2 * Pq * 8, d_ct, batch * 2 * Pq * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
@@ -783,8 +893,7 @@ static int rotate_sum_stage(dpfhe_ctx *ctx, unsigned K, size_t head, const u64 *
 // the checks of dpfhe_rotate_hoisted_grouped, and 1 <= n_rot <= 15
 static int check_rotate_sum(dpfhe_ctx *ctx, unsigned n_special, size_t n_rot, const uint64_t *galois_elts, uint64_t t_plain) {
     if (!galois_elts) return fail(DPFHE_ERR_INVALID, "null argument");
-    int rc = check_special(ctx, n_special);
-    if (!rc) rc = check_t_below_special(ctx, n_special, t_plain);
+    int rc = check_grouped(ctx, n_special, t_plain);
     if (rc) return rc;
     if (n_rot < 1 || n_rot > (size_t)ROT_SUM_MAX) return fail(DPFHE_ERR_INVALID, "summed rotations take 1 to %d rotations", ROT_SUM_MAX);
     for (size_t r = 0; r < n_rot; ++r) {
@@ -1643,30 +1752,41 @@ int dpfhe_debug_phase_cycles(dpfhe_ctx *ctx, uint64_t *out16) {
 // grouped rotations with companions prepared at creation, the inner sums run on an Lq-limb view of the context, and every
 // Horner step is ONE launch: the grouped rotation adds inner[g] in its final store (ks_grouped_kernel<..., ADD>).
 struct dpfhe_linear {
-    dpfhe_ctx *ctx = nullptr;
-    size_t n = 0, baby = 0, giant = 0;
+    static constexpr const char *what = "null layer";
+    dpfhe_ctx *const ctx;
+    size_t baby = 0, giant = 0;
     unsigned n_special = 0;                 // 0: per-limb-digit keys; K > 0: grouped keys with K special primes
     size_t Lq = 0;                          // limbs of a ciphertext polynomial: L, or L - K with grouped keys
     u64 *d_diags = nullptr;                 // [n][Lq][N]
-    u64 *d_keys = nullptr;                  // [baby-1 + 1][key]: baby-step keys, then the giant-step key; key [L][2][L][N] or grouped [dnum][2][L][N]
     std::vector<uint64_t> g_baby;           // Galois elements 5^b, b = 1 .. baby-1
-    std::vector<const uint64_t *> k_baby;   // device pointers of the baby-step keys
-    u64 *d_prep = nullptr;                  // per baby step: Shoup companions of its key [L][2][L][N] + kprime [2][L][N], built once;
-                                            //   grouped: the companions of every key [baby-1 + 1][dnum][2][L][N]
-    std::vector<const uint64_t *> prep;     // {companions, kprime} pointers per baby step (rotate_hoisted_impl); grouped: companions per
-                                            //   baby step (rotate_hoisted_grouped_impl)
-    const u64 *prep_giant = nullptr;        // grouped: companions of the giant-step key
     uint64_t g_giant = 0;
-    uint64_t t_plain = 0;                   // grouped: plaintext modulus of the divisions by P (0: plain rounding)
-    MsConsts K;                             // grouped: constants of the division by P
+    // per-limb-digit keys
+    u64 *d_keys = nullptr;                  // [baby-1 + 1][L][2][L][N]: baby-step keys, then the giant-step key
+    std::vector<const uint64_t *> k_baby;   // device pointers of the baby-step keys
+    u64 *d_prep = nullptr;                  // per baby step: Shoup companions of its key [L][2][L][N] + kprime [2][L][N], built once
+    std::vector<const uint64_t *> prep;     // {companions, kprime} pointers per baby step (rotate_hoisted_impl)
+    // grouped keys
+    PreparedKeys gk;                        // baby-step keys, then the giant-step key when there are giant steps to rotate (giant > 1)
+    uint64_t t_plain = 0;                   // plaintext modulus of the divisions by P (0: plain rounding)
+    MsConsts K;                             // constants of the division by P
     GroupConsts G;
-    DeviceScratch scratch;                  // [baby + giant + 1][batch][2][Lq][N] for the largest batch applied so far
-};
+    DeviceScratch scratch;                  // [baby + giant + 1][batch][2][Lq][N] for the largest batch applied so far; like the rest of
+                                            //   the layer, not counted in the context's device bytes
 
-// the scratch of an application to `batch` ciphertexts
-static int linear_reserve(dpfhe_linear *lin, size_t batch) {
-    return lin->scratch.reserve(lin->ctx, (lin->baby + lin->giant + 1) * batch * 2 * lin->Lq * lin->ctx->N() * 8);
-}
+    explicit dpfhe_linear(dpfhe_ctx *c) : ctx(c) {}
+    ~dpfhe_linear() {
+        cudaFree(d_diags);
+        cudaFree(d_keys);
+        cudaFree(d_prep);
+        gk.release();
+    }
+    size_t in_words() const { return 2 * Lq * ctx->N(); }
+    size_t out_words() const { return in_words(); }
+    int reserve(size_t batch) { return scratch.reserve(ctx, (baby + giant + 1) * batch * in_words() * 8); }
+    size_t host_chunk(size_t batch) const { return grid_round_chunk(ctx, batch, "DPFHE_LINEAR_CHUNK_ROUNDS"); }
+    int apply_on(const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream);
+    int apply_grouped_on(const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream);
+};
 
 static int linear_check_shape(size_t n_diags, size_t baby, const uint64_t *h_gk_baby, const uint64_t *h_gk_giant) {
     if (baby == 0 || baby > 128 || n_diags == 0 || n_diags % baby) return fail(DPFHE_ERR_INVALID, "need 1 <= baby <= 128 and a multiple of baby diagonals");
@@ -1676,45 +1796,34 @@ static int linear_check_shape(size_t n_diags, size_t baby, const uint64_t *h_gk_
     return DPFHE_OK;
 }
 
-// The start of both constructors: a layer with its diagonals and keys on the device (grouped keys: and room for the companions of
-// every key), and the Galois elements of its rotations.
-static int linear_new(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *h_diags, size_t n_diags, size_t baby,
-                      const uint64_t *h_gk_baby, const uint64_t *h_gk_giant, dpfhe_linear **out) {
-    dpfhe_linear *lin = new (std::nothrow) dpfhe_linear();
+// The start of both constructors: a layer with its diagonals on the device, and the Galois elements of its rotations.
+static int linear_new(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *h_diags, size_t n_diags, size_t baby, dpfhe_linear **out) {
+    dpfhe_linear *lin = new (std::nothrow) dpfhe_linear(ctx);
     if (!lin) return fail(DPFHE_ERR_NOMEM, "out of host memory");
-    const size_t Lq = ctx->hp.L - n_special, diag_bytes = n_diags * Lq * ctx->N() * 8, key_bytes = key_digits(ctx, n_special) * 2 * ctx->P() * 8;
-    lin->ctx = ctx; lin->n = n_diags; lin->baby = baby; lin->giant = n_diags / baby; lin->n_special = n_special; lin->Lq = Lq; lin->t_plain = t_plain;
+    lin->baby = baby; lin->giant = n_diags / baby; lin->n_special = n_special; lin->Lq = ctx->hp.L - n_special; lin->t_plain = t_plain;
+    const size_t diag_bytes = n_diags * lin->Lq * ctx->N() * 8;
     cudaError_t e = cudaMalloc(&lin->d_diags, diag_bytes);
-    if (e == cudaSuccess) e = cudaMalloc(&lin->d_keys, baby * key_bytes);
-    if (e == cudaSuccess && n_special) e = cudaMalloc(&lin->d_prep, baby * key_bytes);
     if (e == cudaSuccess) e = cudaMemcpy(lin->d_diags, h_diags, diag_bytes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess && baby > 1) e = cudaMemcpy(lin->d_keys, h_gk_baby, (baby - 1) * key_bytes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess && lin->giant > 1) e = cudaMemcpy(lin->d_keys + (baby - 1) * key_bytes / 8, h_gk_giant, key_bytes, cudaMemcpyHostToDevice);
     if (e != cudaSuccess) {
-        dpfhe_linear_destroy(lin);
+        delete lin;
         return fail(DPFHE_ERR_CUDA, "linear layer upload: %s", cudaGetErrorString(e));
     }
     for (size_t b = 1; b < baby; ++b) {
         uint64_t g = 0;
         dpfhe_galois_element(ctx, (int)b, &g);
         lin->g_baby.push_back(g);
-        lin->k_baby.push_back(lin->d_keys + (b - 1) * key_bytes / 8);
     }
     dpfhe_galois_element(ctx, (int)baby, &lin->g_giant);
     *out = lin;
     return DPFHE_OK;
 }
 
-// The end of both constructors: waits for the launches on `st` that prepared the layer's constants (e: the first error of
-// issuing them) and hands out the layer, or destroys it.
-static int linear_finish(dpfhe_linear *lin, cudaError_t e, cudaStream_t st, dpfhe_linear **out) {
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) {
-        dpfhe_linear_destroy(lin);
-        return fail(DPFHE_ERR_CUDA, "linear layer constants: %s", cudaGetErrorString(e));
-    }
-    *out = lin;
-    return DPFHE_OK;
+// copies a layer's keys of key_words words each to d_keys: the baby-step keys, then the giant-step key if the layer rotates by it
+static cudaError_t linear_upload_keys(const dpfhe_linear *lin, u64 *d_keys, size_t key_words, const uint64_t *h_gk_baby, const uint64_t *h_gk_giant) {
+    cudaError_t e = cudaSuccess;
+    if (lin->baby > 1) e = cudaMemcpy(d_keys, h_gk_baby, (lin->baby - 1) * key_words * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && lin->giant > 1) e = cudaMemcpy(d_keys + (lin->baby - 1) * key_words, h_gk_giant, key_words * 8, cudaMemcpyHostToDevice);
+    return e;
 }
 
 int dpfhe_linear_create(dpfhe_ctx *ctx, const uint64_t *h_diags, size_t n_diags, size_t baby, const uint64_t *h_gk_baby, const uint64_t *h_gk_giant,
@@ -1726,24 +1835,28 @@ int dpfhe_linear_create(dpfhe_ctx *ctx, const uint64_t *h_diags, size_t n_diags,
     rc = linear_check_shape(n_diags, baby, h_gk_baby, h_gk_giant);
     if (rc) return rc;
     dpfhe_linear *lin = nullptr;
-    rc = linear_new(ctx, 0, 0, h_diags, n_diags, baby, h_gk_baby, h_gk_giant, &lin);
+    rc = linear_new(ctx, 0, 0, h_diags, n_diags, baby, &lin);
     if (rc) return rc;
+    cudaStream_t st = pick(ctx, nullptr);
+    const size_t key_words = 2 * ctx->hp.L * ctx->P(), kp_words = 2 * ctx->P();
+    cudaError_t e = cudaMalloc(&lin->d_keys, baby * key_words * 8);
+    if (e == cudaSuccess) e = linear_upload_keys(lin, lin->d_keys, key_words, h_gk_baby, h_gk_giant);
+    if (e != cudaSuccess) return object_finish(lin, fail(DPFHE_ERR_CUDA, "linear layer upload: %s", cudaGetErrorString(e)), st, nullptr, out);
     // the constants of the baby-step rotations do not depend on the data: prepare them once (four small launches per rotation
     // that every hoisted call would otherwise repeat — a tenth of a 31-rotation call at batch 512, more for smaller chunks)
-    cudaError_t e = cudaSuccess;
-    cudaStream_t st = pick(ctx, nullptr);
     if (baby > 1) {
-        const size_t ks_words = 2 * ctx->hp.L * ctx->P(), kp_words = 2 * ctx->P();
-        e = ensure_hoist_consts(ctx) == DPFHE_OK ? cudaMalloc(&lin->d_prep, (baby - 1) * (ks_words + kp_words) * 8) : cudaErrorMemoryAllocation;
+        e = ensure_hoist_consts(ctx) == DPFHE_OK ? cudaMalloc(&lin->d_prep, (baby - 1) * (key_words + kp_words) * 8) : cudaErrorMemoryAllocation;
         for (size_t b = 1; b < baby && e == cudaSuccess; ++b) {
-            u64 *ks = lin->d_prep + (b - 1) * (ks_words + kp_words), *kp = ks + ks_words;
+            u64 *ks = lin->d_prep + (b - 1) * (key_words + kp_words), *kp = ks + key_words;
+            lin->k_baby.push_back(lin->d_keys + (b - 1) * key_words);
             e = VCALL(launch_rot_prepare, ctx->lc, lin->k_baby[b - 1], (u32)lin->g_baby[b - 1], ctx->hoist_delta.get(), ctx->hoist_M.get(), kp, st, ks);
             note_launch(ctx, 4);
             lin->prep.push_back(ks);
             lin->prep.push_back(kp);
         }
     }
-    return linear_finish(lin, e, st, out);
+    rc = e == cudaSuccess ? DPFHE_OK : fail(DPFHE_ERR_CUDA, "linear layer constants: %s", cudaGetErrorString(e));
+    return object_finish(lin, rc, st, "linear layer constants", out);
 }
 
 int dpfhe_linear_create_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_diags, size_t n_diags, size_t baby,
@@ -1752,106 +1865,78 @@ int dpfhe_linear_create_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64
     if (rc) return rc;
     if (!out || !h_diags) return fail(DPFHE_ERR_INVALID, "null argument");
     *out = nullptr;
-    rc = check_special(ctx, n_special);
-    if (rc) return rc;
-    rc = check_t_below_special(ctx, n_special, t_plain);
+    rc = check_grouped(ctx, n_special, t_plain);
     if (rc) return rc;
     rc = linear_check_shape(n_diags, baby, h_gk_baby, h_gk_giant);
     if (rc) return rc;
     dpfhe_linear *lin = nullptr;
-    rc = linear_new(ctx, n_special, t_plain, h_diags, n_diags, baby, h_gk_baby, h_gk_giant, &lin);
+    rc = linear_new(ctx, n_special, t_plain, h_diags, n_diags, baby, &lin);
     if (rc) return rc;
     build_group_consts(ctx->hp, n_special, t_plain, lin->G, lin->K);
-    const size_t dnum = key_digits(ctx, n_special), key_words = dnum * 2 * ctx->P();
-    for (size_t b = 1; b < baby; ++b) lin->prep.push_back(lin->d_prep + (b - 1) * key_words);
-    lin->prep_giant = lin->d_prep + (baby - 1) * key_words;
-    // the Shoup companions of every key, once: each application would otherwise rebuild them for every rotation
     rc = lin->giant > 1 ? ensure_hyb(ctx) : DPFHE_OK;   // the special-prime rows of the giant steps' kernel
-    if (rc) {
-        dpfhe_linear_destroy(lin);
-        return rc;
-    }
-    cudaError_t e = cudaSuccess;
     cudaStream_t st = pick(ctx, nullptr);
-    for (size_t b = 0; b < baby && e == cudaSuccess; ++b) {
-        if (b + 1 < baby || lin->giant > 1) {
-            e = VCALL(launch_key_prepare_grouped, ctx->lc, lin->d_keys + b * key_words, lin->d_prep + b * key_words, (u32)dnum, st);
-            note_launch(ctx, 1);
-        }
-    }
-    return linear_finish(lin, e, st, out);
+    // the Shoup companions of every key, once: each application would otherwise rebuild them for every rotation
+    const size_t dnum = key_digits(ctx, n_special);
+    if (rc == DPFHE_OK)
+        rc = prepare_keys(ctx, ctx->lc, baby - 1 + (lin->giant > 1), dnum, st, "linear layer keys",
+                          [&](u64 *d_keys) { return linear_upload_keys(lin, d_keys, dnum * 2 * ctx->P(), h_gk_baby, h_gk_giant); }, lin->gk);
+    return object_finish(lin, rc, st, "linear layer constants", out);
 }
 
-void dpfhe_linear_destroy(dpfhe_linear *lin) {
-    if (!lin) return;
-    if (lin->ctx) {
-        cudaSetDevice(lin->ctx->lc.device);
-        dpfhe_synchronize(lin->ctx);
-    }
-    cudaFree(lin->d_diags);
-    cudaFree(lin->d_keys);
-    cudaFree(lin->d_prep);
-    delete lin;   // frees the scratch
-}
+void dpfhe_linear_destroy(dpfhe_linear *lin) { object_destroy(lin); }
 
 // grouped keys: hoisted baby steps, the inner sums on the ciphertext moduli, giant - 1 fused Horner steps.  Launches per application
 // (a batch within one chunk of the hoisted-rotation scratch): [baby > 1] * (1 + 3 (baby-1)) + ceil(giant / gmax(baby)) + (giant - 1),
 // gmax = the giant steps one inner-product launch holds.
-static int linear_apply_grouped_on(dpfhe_linear *lin, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
-    dpfhe_ctx *ctx = lin->ctx;
-    const size_t ctb = batch * 2 * lin->Lq * ctx->N();          // words of one ciphertext batch
-    u64 *steps = lin->scratch.get(), *inner = steps + lin->baby * ctb, *tmp = inner + lin->giant * ctb;
+int dpfhe_linear::apply_grouped_on(const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
+    const size_t ctb = batch * in_words();                      // words of one ciphertext batch
+    u64 *steps = scratch.get(), *inner = steps + baby * ctb, *tmp = inner + giant * ctb;
     cudaStream_t st = pick(ctx, stream);
     CU_TRY(cudaMemcpyAsync(steps, d_ct, ctb * 8, cudaMemcpyDeviceToDevice, st));
     int rc = DPFHE_OK;
-    if (lin->baby > 1)
-        rc = rotate_hoisted_grouped_impl(ctx, lin->n_special, steps, lin->baby - 1, lin->g_baby.data(), lin->k_baby.data(), lin->prep.data(),
-                                         steps + ctb, batch, lin->t_plain, stream);
+    if (baby > 1)
+        rc = rotate_hoisted_grouped_impl(ctx, n_special, steps, baby - 1, g_baby.data(), gk.keys.data(), gk.key_s.data(), steps + ctb, batch, t_plain,
+                                         stream);
     if (rc) return rc;
-    // every inner sum in one pass, on the first Lq limbs: a view of the context's launch state (its tables of those limbs come
-    // first), driven on the stream of this call, so it costs no device memory and keeps the calls' order
+    // every inner sum in one pass, on the ciphertext moduli
     st = pick(ctx, stream);
-    LaunchCtx lcq = ctx->lc;
-    lcq.L = (u32)lin->Lq;
+    const LaunchCtx lcq = level_view(ctx, (unsigned)Lq);
     unsigned launches = 0;
-    CU_TRY(VCALL(launch_pt_inner, lcq, steps, (u32)lin->baby, lin->d_diags, (u32)lin->giant, inner, batch, st, &launches));
+    CU_TRY(VCALL(launch_pt_inner, lcq, steps, (u32)baby, d_diags, (u32)giant, inner, batch, st, &launches));
     note_launch(ctx, launches);
-    if (lin->giant == 1) {
+    if (giant == 1) {
         CU_TRY(cudaMemcpyAsync(d_out, inner, ctb * 8, cudaMemcpyDeviceToDevice, st));
         return DPFHE_OK;
     }
     // Horner: acc = rot_baby(acc) + inner[g], one launch per step.  The output may not alias the rotated input or the addend: the
     // steps alternate between tmp and d_out so that the last one (g = 0) writes d_out.
-    const u64 *gk_giant = lin->d_keys + (lin->prep_giant - lin->d_prep);   // same position in the key array as its companions
-    const u64 *acc = inner + (lin->giant - 1) * ctb;
-    for (size_t g = lin->giant - 1; g-- > 0;) {
+    const u64 *acc = inner + (giant - 1) * ctb;
+    for (size_t g = giant - 1; g-- > 0;) {
         u64 *dst = g % 2 == 0 ? d_out : tmp;
-        CU_TRY(VCALL(launch_ks_grouped, ctx->lc, KS_ROTATE, acc, nullptr, gk_giant, dst, batch, (u32)lin->g_giant, lin->K, lin->G, st, inner + g * ctb,
-                     lin->prep_giant));
+        CU_TRY(VCALL(launch_ks_grouped, ctx->lc, KS_ROTATE, acc, nullptr, gk.keys[baby - 1], dst, batch, (u32)g_giant, K, G, st, inner + g * ctb,
+                     gk.key_s[baby - 1]));
         note_launch(ctx, 1);
         acc = dst;
     }
     return DPFHE_OK;
 }
 
-static int linear_apply_on(dpfhe_linear *lin, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
-    if (lin->n_special) return linear_apply_grouped_on(lin, d_ct, d_out, batch, stream);
-    dpfhe_ctx *ctx = lin->ctx;
-    const size_t ctb = batch * 2 * ctx->P();                 // words of one ciphertext batch
-    u64 *steps = lin->scratch.get(), *inner = steps + lin->baby * ctb, *tmp = inner + lin->giant * ctb;
+int dpfhe_linear::apply_on(const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
+    if (n_special) return apply_grouped_on(d_ct, d_out, batch, stream);
+    const size_t ctb = batch * in_words();                      // words of one ciphertext batch
+    u64 *steps = scratch.get(), *inner = steps + baby * ctb, *tmp = inner + giant * ctb;
     cudaStream_t st = pick(ctx, stream);
     CU_TRY(cudaMemcpyAsync(steps, d_ct, ctb * 8, cudaMemcpyDeviceToDevice, st));
     int rc = DPFHE_OK;
-    if (lin->baby > 1)
-        rc = rotate_hoisted_impl(ctx, steps, lin->baby - 1, lin->g_baby.data(), lin->k_baby.data(), lin->prep.data(), steps + ctb, batch, stream);
+    if (baby > 1) rc = rotate_hoisted_impl(ctx, steps, baby - 1, g_baby.data(), k_baby.data(), prep.data(), steps + ctb, batch, stream);
     if (rc) return rc;
-    rc = dpfhe_ct_mul_plain_inner(ctx, steps, lin->baby, lin->d_diags, lin->giant, inner, batch, stream);
+    rc = dpfhe_ct_mul_plain_inner(ctx, steps, baby, d_diags, giant, inner, batch, stream);
     if (rc) return rc;
     st = pick(ctx, stream);
-    CU_TRY(cudaMemcpyAsync(d_out, inner + (lin->giant - 1) * ctb, ctb * 8, cudaMemcpyDeviceToDevice, st));
-    const u64 *gk_giant = lin->d_keys + (lin->baby - 1) * 2 * ctx->hp.L * ctx->P();
-    for (size_t g = lin->giant - 1; g-- > 0;) {
-        rc = dpfhe_rotate(ctx, d_out, lin->g_giant, gk_giant, tmp, batch, stream);           // Horner step: acc = rot_baby(acc) + inner[g]
+    CU_TRY(cudaMemcpyAsync(d_out, inner + (giant - 1) * ctb, ctb * 8, cudaMemcpyDeviceToDevice, st));
+    const u64 *gk_giant = d_keys + (baby - 1) * 2 * ctx->hp.L * ctx->P();
+    for (size_t g = giant - 1; g-- > 0;) {
+        rc = dpfhe_rotate(ctx, d_out, g_giant, gk_giant, tmp, batch, stream);           // Horner step: acc = rot_baby(acc) + inner[g]
         if (rc) return rc;
         rc = dpfhe_poly_add(ctx, tmp, inner + g * ctb, d_out, 2 * batch, stream);
         if (rc) return rc;
@@ -1860,32 +1945,10 @@ static int linear_apply_on(dpfhe_linear *lin, const uint64_t *d_ct, uint64_t *d_
 }
 
 int dpfhe_linear_apply(dpfhe_linear *lin, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
-    if (!lin) return fail(DPFHE_ERR_INVALID, "null layer");
-    int rc = enter(lin->ctx);
-    if (rc) return rc;
-    if (batch == 0) return DPFHE_OK;
-    CHECK_PTR(d_ct); CHECK_PTR(d_out);
-    const size_t ct_bytes = batch * 2 * lin->Lq * lin->ctx->N() * 8;   // Lq = L - K limbs with grouped keys
-    if (overlaps(d_out, ct_bytes, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
-    rc = linear_reserve(lin, batch);
-    if (rc) return rc;
-    return linear_apply_on(lin, d_ct, d_out, batch, stream);
+    return object_apply(lin, d_ct, d_out, batch, stream);
 }
 
-int dpfhe_linear_apply_host(dpfhe_linear *lin, const uint64_t *h_ct, uint64_t *h_out, size_t batch) {
-    if (!lin) return fail(DPFHE_ERR_INVALID, "null layer");
-    dpfhe_ctx *ctx = lin->ctx;
-    int rc = enter(ctx);
-    if (rc) return rc;
-    if (batch == 0) return DPFHE_OK;
-    if (!h_ct || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    const size_t chunk = std::min(grid_round_chunk(ctx, batch, "DPFHE_LINEAR_CHUNK_ROUNDS"), batch);
-    rc = linear_reserve(lin, chunk);
-    if (rc) return rc;
-    const size_t ct_words = 2 * lin->Lq * ctx->N();
-    return run_pipeline(ctx, h_ct, nullptr, h_out, batch, ct_words, ct_words, chunk,
-                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int { return linear_apply_on(lin, din, dout, cnt, st); });
-}
+int dpfhe_linear_apply_host(dpfhe_linear *lin, const uint64_t *h_ct, uint64_t *h_out, size_t batch) { return object_apply_host(lin, h_ct, h_out, batch); }
 
 // ---------------------------------------------------------------- scalar linear combinations, BGV polynomial evaluation (DESIGN.md §2.15)
 int dpfhe_ct_lincomb(dpfhe_ctx *ctx, size_t n_terms, const uint64_t *const *d_cts, const int64_t *coeffs, int64_t constant, uint64_t *d_out,
@@ -1967,7 +2030,7 @@ struct PeLevel {
     bool lift_reduce = true;
     MsConsts K;
     GroupConsts G;
-    u64 *key = nullptr, *key_s = nullptr;
+    PreparedKeys key;   // one key: key.keys[0], key.key_s[0]
 };
 
 // one step of an application.  Buffers: >= 0 an entry of bufs, IN the input, OUT the output
@@ -1989,7 +2052,8 @@ struct PeOp {
 }  // namespace
 
 struct dpfhe_polyeval {
-    dpfhe_ctx *ctx = nullptr;
+    static constexpr const char *what = "null evaluator";
+    dpfhe_ctx *const ctx;
     unsigned K = 0, Lq = 0, Lf = 0;
     uint64_t t = 0;
     std::vector<PeLevel> lev;            // by level: lev[l - lev_lo]
@@ -1999,39 +2063,32 @@ struct dpfhe_polyeval {
     double scale_out = 0;                // CKKS: the scale S of the result
     std::vector<PeOp> ops;
     std::vector<unsigned> bufs;          // level of every scratch buffer
-    size_t fixed_bytes = 0;              // level tables and keys
-    DeviceScratch scratch;               // the buffers back to back, then the switch's tau rows [2 batch][N], for the largest batch so far
+    CountedScratch mem;                  // counts the level tables and keys; its scratch: the buffers back to back, then the switch's
+                                         //   tau rows [2 batch][N], for the largest batch so far
+
+    explicit dpfhe_polyeval(dpfhe_ctx *c) : ctx(c), mem(c) {}
+    ~dpfhe_polyeval() {
+        for (auto &v : lev) {
+            if (v.l != Lq) {   // the top level's tables are the context's
+                cudaFree(v.d_lp);
+                cudaFree(v.d_tw);
+                cudaFree(v.d_itw);
+            }
+            v.key.release();
+        }
+    }
+    size_t in_words() const { return 2 * Lq * ctx->N(); }
+    size_t out_words() const { return 2 * Lf * ctx->N(); }
+    int reserve(size_t batch) {
+        size_t w = bufs.empty() && !ckks ? 0 : 2 * batch * ctx->N();
+        for (unsigned l : bufs) w += batch * 2 * l * ctx->N();
+        return mem.reserve(w * 8);
+    }
+    size_t host_chunk(size_t batch) const { return item_chunk(ctx, batch, "DPFHE_POLYEVAL_CHUNK"); }
+    int apply_on(const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream);
 };
 
 namespace {
-
-size_t pe_scratch_words(const dpfhe_polyeval *pe, size_t batch) {
-    size_t w = 0;
-    for (unsigned l : pe->bufs) w += batch * 2 * l * pe->ctx->N();
-    return w + (pe->bufs.empty() && !pe->ckks ? 0 : 2 * batch * pe->ctx->N());
-}
-
-void pe_free(dpfhe_polyeval *pe) {
-    for (auto &v : pe->lev) {
-        if (v.l != pe->Lq) {
-            cudaFree(v.d_lp);
-            cudaFree(v.d_tw);
-            cudaFree(v.d_itw);
-        }
-        cudaFree(v.key);
-        cudaFree(v.key_s);
-    }
-    if (pe->ctx) pe->ctx->object_bytes -= pe->fixed_bytes + pe->scratch.bytes();
-    delete pe;
-}
-
-// the scratch of an application to `batch` ciphertexts, counted in the context's device bytes
-int pe_reserve(dpfhe_polyeval *pe, size_t batch) {
-    pe->ctx->object_bytes -= pe->scratch.bytes();
-    const int rc = pe->scratch.reserve(pe->ctx, pe_scratch_words(pe, batch) * 8);
-    pe->ctx->object_bytes += pe->scratch.bytes();
-    return rc;
-}
 
 // the schedule of DESIGN.md §2.15: powers in increasing order, each operand brought to the product's level by single-limb switches
 // (each copy made once, from the copy one level above), the combination one level above the last switch
@@ -2197,7 +2254,8 @@ int pe_plan_ckks(dpfhe_polyeval *pe, const double *a, size_t d, double scale_in)
     return DPFHE_OK;
 }
 
-// the launch state of key switching at level l: the context's, with the level's limb tables (DESIGN.md §4.11)
+// the launch state of key switching at level l: unlike level_view, not a prefix of the context's basis but the l + K limbs
+// {q_0 .. q_{l-1}, p_0 .. p_{K-1}} with the level's own tables (DESIGN.md §4.11)
 LaunchCtx pe_view(const dpfhe_polyeval *pe, const PeLevel &v) {
     LaunchCtx lc = pe->ctx->lc;
     lc.L = v.l + pe->K;
@@ -2228,109 +2286,29 @@ int pe_level(dpfhe_polyeval *pe, PeLevel &v, unsigned l, const uint64_t *h_key, 
         v.lt = ctx->lc.lt;
         v.lift_reduce = ctx->lc.lift_reduce;
     } else {
-        const int rc = upload_basis(v.hp, v.d_lp, v.d_tw, v.d_itw, v.lt, v.lift_reduce, pe->fixed_bytes);
+        size_t bytes = 0;
+        const int rc = upload_basis(v.hp, v.d_lp, v.d_tw, v.d_itw, v.lt, v.lift_reduce, bytes);
         if (rc) return rc;
+        pe->mem.count_fixed(bytes);
     }
     // the key of level l: digits g < ceil(l / K), limb rows 0 .. l-1 and the special rows Lq .. Lq+K-1 of the top-level key
-    const size_t key_words = dl * 2 * Ll * N;
-    CU_TRY(cudaMalloc(&v.key, key_words * 8));
-    CU_TRY(cudaMalloc(&v.key_s, key_words * 8));
-    pe->fixed_bytes += 2 * key_words * 8;
-    for (size_t g = 0; g < dl; ++g)
-        for (size_t c = 0; c < 2; ++c) {
-            const uint64_t *src = h_key + (g * 2 + c) * L * N;
-            u64 *dst = v.key + (g * 2 + c) * Ll * N;
-            CU_TRY(cudaMemcpy(dst, src, l * N * 8, cudaMemcpyHostToDevice));
-            CU_TRY(cudaMemcpy(dst + l * N, src + Lq * N, K * N * 8, cudaMemcpyHostToDevice));
+    const int rc = prepare_keys(ctx, pe_view(pe, v), 1, dl, st, "polynomial evaluator keys", [&](u64 *d_key) {
+        cudaError_t e = cudaSuccess;
+        for (size_t gc = 0; gc < 2 * dl && e == cudaSuccess; ++gc) {   // (digit, component) rows
+            const uint64_t *src = h_key + gc * L * N;
+            u64 *dst = d_key + gc * Ll * N;
+            e = cudaMemcpy(dst, src, l * N * 8, cudaMemcpyHostToDevice);
+            if (e == cudaSuccess) e = cudaMemcpy(dst + l * N, src + Lq * N, K * N * 8, cudaMemcpyHostToDevice);
         }
-    const LaunchCtx lc = pe_view(pe, v);
-    CU_TRY(VCALL(launch_key_prepare_grouped, lc, v.key, v.key_s, (u32)dl, st));
-    note_launch(ctx, 1);
-    return DPFHE_OK;
+        return e;
+    }, v.key);
+    if (rc == DPFHE_OK) pe->mem.count_fixed(v.key.bytes);
+    return rc;
 }
 
-int pe_apply_on(dpfhe_polyeval *pe, const u64 *d_ct, u64 *d_out, size_t batch, void *stream) {
-    dpfhe_ctx *ctx = pe->ctx;
-    const size_t N = ctx->N();
-    std::vector<u64 *> ptr(pe->bufs.size());
-    u64 *p = pe->scratch.get();
-    for (size_t i = 0; i < pe->bufs.size(); ++i) {
-        ptr[i] = p;
-        p += batch * 2 * pe->bufs[i] * N;
-    }
-    u64 *tau = p;
-    auto buf = [&](int b) -> u64 * { return b == PE_IN ? const_cast<u64 *>(d_ct) : b == PE_OUT ? d_out : ptr[b]; };
-    cudaStream_t st = pick(ctx, stream);
-    for (const PeOp &op : pe->ops) {
-        if (op.kind == PE_MUL) {
-            const PeLevel &v = pe->lev[op.level - pe->lev_lo];
-            LaunchCtx lc = pe_view(pe, v);
-            lc.ks_epoch = ctx->lc.ks_epoch;
-            const cudaError_t e = VCALL(launch_ks_grouped, lc, KS_MUL_RELIN, buf(op.a), buf(op.b), v.key, buf(op.out), batch, 0u, v.K, v.G, st, nullptr,
-                                        v.key_s);
-            // the round numbering is the context's: the next key switch on any view must continue from here
-            ctx->lc.ks_epoch = lc.ks_epoch;
-            ctx->lc.ks_epoch_restarts = lc.ks_epoch_restarts;
-            CU_TRY(e);
-            note_launch(ctx, 1);
-        } else if (op.kind == PE_SWITCH) {
-            LaunchCtx lc = ctx->lc;   // the ciphertext moduli q_0 .. q_{l-1} are the first l limbs of the context
-            lc.L = op.level;
-            CU_TRY(VCALL(launch_mod_switch, lc, buf(op.a), tau, buf(op.out), pe->ms[op.level], 2 * batch, st));
-            note_launch(ctx, 2);
-        } else if (op.kind == PE_LINCOMB) {
-            LaunchCtx lc = ctx->lc;
-            lc.L = op.level;
-            std::vector<const u64 *> in;
-            for (int b : op.terms) in.push_back(buf(b));
-            CU_TRY(VCALL(launch_lincomb, lc, in.data(), op.coeffs.data(), (u32)in.size(), op.constant, nullptr, buf(op.out), batch, st));
-            note_launch(ctx, 1);
-        } else if (op.kind == PE_CUT) {   // a strided device copy, not a kernel
-            const size_t row = (size_t)op.level * N * 8;
-            CU_TRY(cudaMemcpy2DAsync(buf(op.out), row, buf(op.a), (size_t)op.b * N * 8, row, 2 * batch, cudaMemcpyDeviceToDevice, st));
-        } else {   // PE_CKKS_COMB
-            LaunchCtx lc = ctx->lc;
-            lc.L = op.level;
-            std::vector<const u64 *> in;
-            for (int b : op.terms) in.push_back(buf(b));
-            CU_TRY(VCALL(launch_ckks_comb, lc, in.data(), op.levels.data(), op.dcoeffs.data(), (u32)in.size(), op.dconstant, pe->ms[op.level], tau,
-                         buf(op.out), batch, st));
-            note_launch(ctx, 2);
-        }
-    }
-    return DPFHE_OK;
-}
-
-int pe_create_finish(dpfhe_polyeval *pe, int rc, unsigned ms_lo, const uint64_t *h_relin_key, dpfhe_polyeval **out);
-
-}  // namespace
-
-int dpfhe_polyeval_create_grouped(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const int64_t *coeffs, size_t degree,
-                                  const uint64_t *h_relin_key, dpfhe_polyeval **out) {
-    int rc = enter(ctx);
-    if (rc) return rc;
-    if (!out || !coeffs || !h_relin_key) return fail(DPFHE_ERR_INVALID, "null argument");
-    *out = nullptr;
-    rc = check_special(ctx, n_special);
-    if (rc) return rc;
-    if (t_plain < 2 || t_plain >= ((uint64_t)1 << 31)) return fail(DPFHE_ERR_INVALID, "the plaintext modulus must be in [2, 2^31)");
-    if (degree < 1 || degree > 64) return fail(DPFHE_ERR_INVALID, "the degree must be in [1, 64]");
-    const unsigned L = ctx->hp.L, K = n_special, Lq = L - K, D = ceil_log2(degree);
-    if (D > Lq - 1 || D > Lq - K + 1)
-        return fail(DPFHE_ERR_INVALID, "degree %zu needs %u levels: at most min(Lq - 1, Lq - K + 1) = %u with Lq = %u, K = %u", degree, D,
-                    std::min(Lq - 1, Lq - K + 1), Lq, K);
-    dpfhe_polyeval *pe = new (std::nothrow) dpfhe_polyeval();
-    if (!pe) return fail(DPFHE_ERR_NOMEM, "out of host memory");
-    pe->ctx = ctx; pe->K = K; pe->Lq = Lq; pe->Lf = Lq - D; pe->t = t_plain;
-    rc = pe_plan(pe, coeffs, degree);
-    return pe_create_finish(pe, rc, D > 0 ? pe->Lf + 1 : Lq + 1, h_relin_key, out);
-}
-
-namespace {
-
-// the rest of an evaluator's creation after its plan (rc: the planner's result): the switch constants of every level from ms_lo to
-// Lq, the level views, keys and companions of the products' levels; frees the evaluator on failure
-int pe_create_finish(dpfhe_polyeval *pe, int rc, unsigned ms_lo, const uint64_t *h_relin_key, dpfhe_polyeval **out) {
+// The rest of an evaluator's creation after its plan (rc: the planner's result): the switch constants of every level from ms_lo to
+// Lq, the level views, keys and companions of the products' levels.
+int pe_finish(dpfhe_polyeval *pe, int rc, unsigned ms_lo, const uint64_t *h_relin_key, dpfhe_polyeval **out) {
     dpfhe_ctx *ctx = pe->ctx;
     const unsigned Lq = pe->Lq;
     // the levels of the products, and the switch constants of every level a switch starts from
@@ -2353,20 +2331,80 @@ int pe_create_finish(dpfhe_polyeval *pe, int rc, unsigned ms_lo, const uint64_t 
         pe->lev.resize(Lq - lo + 1);
         for (unsigned l = lo; l <= Lq && rc == DPFHE_OK; ++l) rc = pe_level(pe, pe->lev[l - lo], l, h_relin_key, st);
     }
-    ctx->object_bytes += pe->fixed_bytes;
-    if (rc == DPFHE_OK) {
-        const cudaError_t e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) rc = fail(DPFHE_ERR_CUDA, "polynomial evaluator keys: %s", cudaGetErrorString(e));
-    }
-    if (rc != DPFHE_OK) {
-        pe_free(pe);
-        return rc;
-    }
-    *out = pe;
-    return DPFHE_OK;
+    return object_finish(pe, rc, st, "polynomial evaluator keys", out);
 }
 
 }  // namespace
+
+// launches per application: one per product, two per modulus switch, one for the combination (DESIGN.md §2.15)
+int dpfhe_polyeval::apply_on(const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
+    const size_t N = ctx->N();
+    std::vector<u64 *> ptr(bufs.size());
+    u64 *p = mem.get();
+    for (size_t i = 0; i < bufs.size(); ++i) {
+        ptr[i] = p;
+        p += batch * 2 * bufs[i] * N;
+    }
+    u64 *tau = p;
+    auto buf = [&](int b) -> u64 * { return b == PE_IN ? const_cast<u64 *>(d_ct) : b == PE_OUT ? d_out : ptr[b]; };
+    cudaStream_t st = pick(ctx, stream);
+    for (const PeOp &op : ops) {
+        if (op.kind == PE_MUL) {
+            const PeLevel &v = lev[op.level - lev_lo];
+            LaunchCtx lc = pe_view(this, v);
+            lc.ks_epoch = ctx->lc.ks_epoch;
+            const cudaError_t e = VCALL(launch_ks_grouped, lc, KS_MUL_RELIN, buf(op.a), buf(op.b), v.key.keys[0], buf(op.out), batch, 0u, v.K, v.G, st,
+                                        nullptr, v.key.key_s[0]);
+            // the round numbering is the context's: the next key switch on any view must continue from here
+            ctx->lc.ks_epoch = lc.ks_epoch;
+            ctx->lc.ks_epoch_restarts = lc.ks_epoch_restarts;
+            CU_TRY(e);
+            note_launch(ctx, 1);
+        } else if (op.kind == PE_SWITCH) {
+            const LaunchCtx lc = level_view(ctx, op.level);
+            CU_TRY(VCALL(launch_mod_switch, lc, buf(op.a), tau, buf(op.out), ms[op.level], 2 * batch, st));
+            note_launch(ctx, 2);
+        } else if (op.kind == PE_LINCOMB) {
+            const LaunchCtx lc = level_view(ctx, op.level);
+            std::vector<const u64 *> in;
+            for (int b : op.terms) in.push_back(buf(b));
+            CU_TRY(VCALL(launch_lincomb, lc, in.data(), op.coeffs.data(), (u32)in.size(), op.constant, nullptr, buf(op.out), batch, st));
+            note_launch(ctx, 1);
+        } else if (op.kind == PE_CUT) {   // a strided device copy, not a kernel
+            const size_t row = (size_t)op.level * N * 8;
+            CU_TRY(cudaMemcpy2DAsync(buf(op.out), row, buf(op.a), (size_t)op.b * N * 8, row, 2 * batch, cudaMemcpyDeviceToDevice, st));
+        } else {   // PE_CKKS_COMB
+            const LaunchCtx lc = level_view(ctx, op.level);
+            std::vector<const u64 *> in;
+            for (int b : op.terms) in.push_back(buf(b));
+            CU_TRY(VCALL(launch_ckks_comb, lc, in.data(), op.levels.data(), op.dcoeffs.data(), (u32)in.size(), op.dconstant, ms[op.level], tau,
+                         buf(op.out), batch, st));
+            note_launch(ctx, 2);
+        }
+    }
+    return DPFHE_OK;
+}
+
+int dpfhe_polyeval_create_grouped(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const int64_t *coeffs, size_t degree,
+                                  const uint64_t *h_relin_key, dpfhe_polyeval **out) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!out || !coeffs || !h_relin_key) return fail(DPFHE_ERR_INVALID, "null argument");
+    *out = nullptr;
+    rc = check_special(ctx, n_special);
+    if (rc) return rc;
+    if (t_plain < 2 || t_plain >= ((uint64_t)1 << 31)) return fail(DPFHE_ERR_INVALID, "the plaintext modulus must be in [2, 2^31)");
+    if (degree < 1 || degree > 64) return fail(DPFHE_ERR_INVALID, "the degree must be in [1, 64]");
+    const unsigned L = ctx->hp.L, K = n_special, Lq = L - K, D = ceil_log2(degree);
+    if (D > Lq - 1 || D > Lq - K + 1)
+        return fail(DPFHE_ERR_INVALID, "degree %zu needs %u levels: at most min(Lq - 1, Lq - K + 1) = %u with Lq = %u, K = %u", degree, D,
+                    std::min(Lq - 1, Lq - K + 1), Lq, K);
+    dpfhe_polyeval *pe = new (std::nothrow) dpfhe_polyeval(ctx);
+    if (!pe) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    pe->K = K; pe->Lq = Lq; pe->Lf = Lq - D; pe->t = t_plain;
+    rc = pe_plan(pe, coeffs, degree);
+    return pe_finish(pe, rc, D > 0 ? pe->Lf + 1 : Lq + 1, h_relin_key, out);
+}
 
 int dpfhe_polyeval_create_ckks(dpfhe_ctx *ctx, unsigned n_special, const double *coeffs, size_t degree, double scale_in, double scale_out,
                                const uint64_t *h_relin_key, dpfhe_polyeval **out) {
@@ -2384,58 +2422,26 @@ int dpfhe_polyeval_create_ckks(dpfhe_ctx *ctx, unsigned n_special, const double 
     const unsigned L = ctx->hp.L, K = n_special, Lq = L - K, D = ceil_log2(degree);
     if (D + 2 > Lq || D > Lq - K + 1)
         return fail(DPFHE_ERR_INVALID, "degree %zu needs %u levels: at most min(Lq - 2, Lq - K + 1) with Lq = %u, K = %u", degree, D, Lq, K);
-    dpfhe_polyeval *pe = new (std::nothrow) dpfhe_polyeval();
+    dpfhe_polyeval *pe = new (std::nothrow) dpfhe_polyeval(ctx);
     if (!pe) return fail(DPFHE_ERR_NOMEM, "out of host memory");
-    pe->ctx = ctx; pe->K = K; pe->Lq = Lq; pe->Lf = Lq - D - 1; pe->t = 0;
+    pe->K = K; pe->Lq = Lq; pe->Lf = Lq - D - 1; pe->t = 0;
     pe->ckks = true;
     pe->scale_out = scale_out;
     rc = pe_plan_ckks(pe, coeffs, degree, scale_in);
-    return pe_create_finish(pe, rc, Lq - D, h_relin_key, out);
+    return pe_finish(pe, rc, Lq - D, h_relin_key, out);
 }
 
 unsigned dpfhe_polyeval_result_limbs(const dpfhe_polyeval *pe) { return pe ? pe->Lf : 0; }
 
 double dpfhe_polyeval_result_scale(const dpfhe_polyeval *pe) { return pe && pe->ckks ? pe->scale_out : 0.0; }
 
-void dpfhe_polyeval_destroy(dpfhe_polyeval *pe) {
-    if (!pe) return;
-    if (pe->ctx) {
-        cudaSetDevice(pe->ctx->lc.device);
-        dpfhe_synchronize(pe->ctx);
-    }
-    pe_free(pe);
-}
+void dpfhe_polyeval_destroy(dpfhe_polyeval *pe) { object_destroy(pe); }
 
-// launches per application: one per product, two per modulus switch, one for the combination (DESIGN.md §2.15)
 int dpfhe_polyeval_apply(dpfhe_polyeval *pe, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
-    if (!pe) return fail(DPFHE_ERR_INVALID, "null evaluator");
-    int rc = enter(pe->ctx);
-    if (rc) return rc;
-    CHECK_PTR(d_ct); CHECK_PTR(d_out);
-    if (batch == 0) return DPFHE_OK;
-    const size_t N = pe->ctx->N();
-    if (overlaps(d_out, batch * 2 * pe->Lf * N * 8, d_ct, batch * 2 * pe->Lq * N * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
-    rc = pe_reserve(pe, batch);
-    if (rc) return rc;
-    return pe_apply_on(pe, d_ct, d_out, batch, stream);
+    return object_apply(pe, d_ct, d_out, batch, stream);
 }
 
-int dpfhe_polyeval_apply_host(dpfhe_polyeval *pe, const uint64_t *h_ct, uint64_t *h_out, size_t batch) {
-    if (!pe) return fail(DPFHE_ERR_INVALID, "null evaluator");
-    dpfhe_ctx *ctx = pe->ctx;
-    int rc = enter(ctx);
-    if (rc) return rc;
-    if (batch == 0) return DPFHE_OK;
-    if (!h_ct || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    size_t chunk = grid_round_chunk(ctx, batch, nullptr);
-    if (const char *e = getenv("DPFHE_POLYEVAL_CHUNK")) chunk = std::max<size_t>(1, (size_t)atol(e));   // tests: several chunks at a small batch
-    chunk = std::min(chunk, batch);
-    rc = pe_reserve(pe, chunk);
-    if (rc) return rc;
-    const size_t N = ctx->N();
-    return run_pipeline(ctx, h_ct, nullptr, h_out, batch, 2 * pe->Lq * N, 2 * pe->Lf * N, chunk,
-                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int { return pe_apply_on(pe, din, dout, cnt, st); });
-}
+int dpfhe_polyeval_apply_host(dpfhe_polyeval *pe, const uint64_t *h_ct, uint64_t *h_out, size_t batch) { return object_apply_host(pe, h_ct, h_out, batch); }
 
 // ---------------------------------------------------------------- slot sums (DESIGN.md §2.17)
 int dpfhe_slotsum_steps(size_t stride, const unsigned *radices, size_t n_stages, int *steps, size_t *n_steps) {
@@ -2462,61 +2468,46 @@ int dpfhe_slotsum_steps(size_t stride, const unsigned *radices, size_t n_stages,
 }
 
 struct dpfhe_slotsum {
-    dpfhe_ctx *ctx = nullptr;
+    static constexpr const char *what = "null slot sum";
+    dpfhe_ctx *const ctx;
     unsigned K = 0;
     size_t Lq = 0;
     std::vector<u32> n_rot;              // rotations of each stage
     std::vector<u32> galois;             // Galois elements of every step, stage by stage
-    std::vector<const u64 *> keys, key_s;
-    u64 *d_keys = nullptr;               // [n_steps][dnum][2][L][N]
-    u64 *d_key_s = nullptr;              // their Shoup companions, same layout
+    PreparedKeys gk;                     // the keys of every step, in the same order
     MsConsts Kc;
     GroupConsts G;
-    size_t fixed_bytes = 0;              // keys and companions
-    DeviceScratch scratch;               // one intermediate batch [batch][2][Lq][N] (two or more stages), for the largest batch so far
+    CountedScratch mem;                  // counts the keys; its scratch: one intermediate batch [batch][2][Lq][N] (two or more stages), for
+                                         //   the largest batch so far
+
+    explicit dpfhe_slotsum(dpfhe_ctx *c) : ctx(c), mem(c) {}
+    ~dpfhe_slotsum() { gk.release(); }
+    size_t in_words() const { return 2 * Lq * ctx->N(); }
+    size_t out_words() const { return in_words(); }
+    // the object's intermediate batch and the context's hoisted-rotation scratch
+    int reserve(size_t batch) {
+        const int rc = n_rot.size() > 1 ? mem.reserve(batch * in_words() * 8) : DPFHE_OK;
+        return rc ? rc : rotate_sum_reserve(ctx, K, 0, batch);
+    }
+    size_t host_chunk(size_t batch) const { return item_chunk(ctx, batch, "DPFHE_SLOTSUM_CHUNK"); }
+    int apply_on(const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream);
 };
 
-namespace {
-
-void ss_free(dpfhe_slotsum *ss) {
-    cudaFree(ss->d_keys);
-    cudaFree(ss->d_key_s);
-    if (ss->ctx) ss->ctx->object_bytes -= ss->fixed_bytes + ss->scratch.bytes();
-    delete ss;
-}
-
-// the scratch of an application to `batch` ciphertexts: the object's intermediate batch (counted in the context's device bytes) and
-// the context's hoisted-rotation scratch
-int ss_reserve(dpfhe_slotsum *ss, size_t batch) {
-    dpfhe_ctx *ctx = ss->ctx;
-    int rc = DPFHE_OK;
-    if (ss->n_rot.size() > 1) {
-        ctx->object_bytes -= ss->scratch.bytes();
-        rc = ss->scratch.reserve(ctx, batch * 2 * ss->Lq * ctx->N() * 8);
-        ctx->object_bytes += ss->scratch.bytes();
-    }
-    return rc ? rc : rotate_sum_reserve(ctx, ss->K, 0, batch);
-}
-
 // S stages, alternating between the scratch batch and d_out so that the last one writes d_out; 4 launches per stage and chunk
-int ss_apply_on(dpfhe_slotsum *ss, const u64 *d_ct, u64 *d_out, size_t batch, void *stream) {
-    dpfhe_ctx *ctx = ss->ctx;
+int dpfhe_slotsum::apply_on(const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
     cudaStream_t st = pick(ctx, stream);
-    const size_t S = ss->n_rot.size();
+    const size_t S = n_rot.size();
     const u64 *in = d_ct;
     size_t first = 0;
     for (size_t t = 0; t < S; ++t) {
-        u64 *dst = (S - 1 - t) % 2 == 0 ? d_out : ss->scratch.get();
-        const int rc = rotate_sum_stage(ctx, ss->K, 0, in, ss->n_rot[t], ss->galois.data() + first, ss->keys.data() + first, ss->key_s.data() + first,
-                                        dst, batch, ss->Kc, ss->G, st);
+        u64 *dst = (S - 1 - t) % 2 == 0 ? d_out : mem.get();
+        const int rc = rotate_sum_stage(ctx, K, 0, in, n_rot[t], galois.data() + first, gk.keys.data() + first, gk.key_s.data() + first, dst, batch, Kc, G, st);
         if (rc) return rc;
-        first += ss->n_rot[t];
+        first += n_rot[t];
         in = dst;
     }
     return DPFHE_OK;
 }
-
-}  // namespace
 
 int dpfhe_slotsum_create_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t stride, const unsigned *radices, size_t n_stages,
                                  const uint64_t *h_gks, uint64_t t_plain, dpfhe_slotsum **out) {
@@ -2524,87 +2515,41 @@ int dpfhe_slotsum_create_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t stri
     if (rc) return rc;
     if (!out || !h_gks) return fail(DPFHE_ERR_INVALID, "null argument");
     *out = nullptr;
-    rc = check_special(ctx, n_special);
-    if (!rc) rc = check_t_below_special(ctx, n_special, t_plain);
+    rc = check_grouped(ctx, n_special, t_plain);
     if (rc) return rc;
+    int steps[16 * 15];   // the most dpfhe_slotsum_steps accepts: 16 stages of radix 16
     size_t n_steps = 0;
-    rc = dpfhe_slotsum_steps(stride, radices, n_stages, nullptr, &n_steps);
+    rc = dpfhe_slotsum_steps(stride, radices, n_stages, steps, &n_steps);
     if (rc) return rc;
-    size_t count = 1;
-    for (size_t t = 0; t < n_stages; ++t) count *= radices[t];
-    if (stride * count > ctx->N() / 2) return fail(DPFHE_ERR_INVALID, "stride * prod(radices) = %zu exceeds N/2 = %zu", stride * count, ctx->N() / 2);
-    std::vector<int> steps(n_steps);
-    dpfhe_slotsum_steps(stride, radices, n_stages, steps.data(), &n_steps);
-    dpfhe_slotsum *ss = new (std::nothrow) dpfhe_slotsum();
+    // stride * prod(radices) is the last stage's span, its first step, times its radix
+    const unsigned r_last = radices[n_stages - 1];
+    const size_t total = (size_t)steps[n_steps - (r_last - 1)] * r_last;
+    if (total > ctx->N() / 2) return fail(DPFHE_ERR_INVALID, "stride * prod(radices) = %zu exceeds N/2 = %zu", total, ctx->N() / 2);
+    dpfhe_slotsum *ss = new (std::nothrow) dpfhe_slotsum(ctx);
     if (!ss) return fail(DPFHE_ERR_NOMEM, "out of host memory");
-    ss->ctx = ctx; ss->K = n_special; ss->Lq = ctx->hp.L - n_special;
+    ss->K = n_special; ss->Lq = ctx->hp.L - n_special;
     for (size_t t = 0; t < n_stages; ++t) ss->n_rot.push_back(radices[t] - 1);
-    build_group_consts(ctx->hp, n_special, t_plain, ss->G, ss->Kc);
-    const size_t dnum = key_digits(ctx, n_special), key_words = dnum * 2 * ctx->P();
-    cudaStream_t st = pick(ctx, nullptr);
-    cudaError_t e = cudaMalloc(&ss->d_keys, n_steps * key_words * 8);
-    if (e == cudaSuccess) e = cudaMalloc(&ss->d_key_s, n_steps * key_words * 8);
-    if (e == cudaSuccess) {
-        ss->fixed_bytes = 2 * n_steps * key_words * 8;
-        ctx->object_bytes += ss->fixed_bytes;
-        e = cudaMemcpyAsync(ss->d_keys, h_gks, n_steps * key_words * 8, cudaMemcpyHostToDevice, st);
-    }
-    for (size_t k = 0; k < n_steps && e == cudaSuccess; ++k) {
+    for (size_t k = 0; k < n_steps; ++k) {
         uint64_t g = 0;
         dpfhe_galois_element(ctx, steps[k], &g);
         ss->galois.push_back((u32)g);
-        ss->keys.push_back(ss->d_keys + k * key_words);
-        ss->key_s.push_back(ss->d_key_s + k * key_words);
-        e = VCALL(launch_key_prepare_grouped, ctx->lc, ss->keys[k], ss->d_key_s + k * key_words, (u32)dnum, st);
-        note_launch(ctx, 1);
     }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) {
-        ss_free(ss);
-        return fail(DPFHE_ERR_CUDA, "slot sum keys: %s", cudaGetErrorString(e));
-    }
-    *out = ss;
-    return DPFHE_OK;
+    build_group_consts(ctx->hp, n_special, t_plain, ss->G, ss->Kc);
+    const size_t dnum = key_digits(ctx, n_special);
+    cudaStream_t st = pick(ctx, nullptr);
+    rc = prepare_keys(ctx, ctx->lc, n_steps, dnum, st, "slot sum keys",
+                      [&](u64 *d_keys) { return cudaMemcpyAsync(d_keys, h_gks, n_steps * dnum * 2 * ctx->P() * 8, cudaMemcpyHostToDevice, st); }, ss->gk);
+    if (rc == DPFHE_OK) ss->mem.count_fixed(ss->gk.bytes);
+    return object_finish(ss, rc, st, "slot sum keys", out);
 }
 
-void dpfhe_slotsum_destroy(dpfhe_slotsum *ss) {
-    if (!ss) return;
-    if (ss->ctx) {
-        cudaSetDevice(ss->ctx->lc.device);
-        dpfhe_synchronize(ss->ctx);
-    }
-    ss_free(ss);
-}
+void dpfhe_slotsum_destroy(dpfhe_slotsum *ss) { object_destroy(ss); }
 
 int dpfhe_slotsum_apply(dpfhe_slotsum *ss, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
-    if (!ss) return fail(DPFHE_ERR_INVALID, "null slot sum");
-    int rc = enter(ss->ctx);
-    if (rc) return rc;
-    if (batch == 0) return DPFHE_OK;
-    CHECK_PTR(d_ct); CHECK_PTR(d_out);
-    const size_t ct_bytes = batch * 2 * ss->Lq * ss->ctx->N() * 8;
-    if (overlaps(d_out, ct_bytes, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
-    rc = ss_reserve(ss, batch);
-    if (rc) return rc;
-    return ss_apply_on(ss, d_ct, d_out, batch, stream);
+    return object_apply(ss, d_ct, d_out, batch, stream);
 }
 
-int dpfhe_slotsum_apply_host(dpfhe_slotsum *ss, const uint64_t *h_ct, uint64_t *h_out, size_t batch) {
-    if (!ss) return fail(DPFHE_ERR_INVALID, "null slot sum");
-    dpfhe_ctx *ctx = ss->ctx;
-    int rc = enter(ctx);
-    if (rc) return rc;
-    if (batch == 0) return DPFHE_OK;
-    if (!h_ct || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    size_t chunk = grid_round_chunk(ctx, batch, nullptr);
-    if (const char *e = getenv("DPFHE_SLOTSUM_CHUNK")) chunk = std::max<size_t>(1, (size_t)atol(e));   // tests: several chunks at a small batch
-    chunk = std::min(chunk, batch);
-    rc = ss_reserve(ss, chunk);
-    if (rc) return rc;
-    const size_t ct_words = 2 * ss->Lq * ctx->N();
-    return run_pipeline(ctx, h_ct, nullptr, h_out, batch, ct_words, ct_words, chunk,
-                        [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int { return ss_apply_on(ss, din, dout, cnt, st); });
-}
+int dpfhe_slotsum_apply_host(dpfhe_slotsum *ss, const uint64_t *h_ct, uint64_t *h_out, size_t batch) { return object_apply_host(ss, h_ct, h_out, batch); }
 
 int dpfhe_describe(const dpfhe_ctx *ctx, char *buf, size_t buf_len) {
     if (!ctx || !buf || !buf_len) return fail(DPFHE_ERR_INVALID, "bad argument");

@@ -45,7 +45,8 @@ struct dpfhe_ctx {
     dpfhe::LimbParams *d_lp = nullptr;
     dpfhe::Twiddle *d_tw = nullptr, *d_itw = nullptr;
     size_t device_bytes = 0;
-    size_t object_bytes = 0;                // device memory of the polynomial evaluators built on the context (keys, tables, scratch)
+    size_t object_bytes = 0;                // device memory of the counted objects built on the context (polynomial evaluators, slot sums):
+                                            //   level tables, keys, scratch; CountedScratch is its one writer
     uint64_t launches = 0;
     // Ordering between calls: every entry point may run on a different stream (the caller's, or the context's own when NULL
     // is passed), but they all share the context's scratch.  Each call makes its stream wait for the previous call's work
@@ -77,4 +78,30 @@ struct dpfhe_ctx {
         for (auto &s : c.stage_in) f(s);
         for (auto &s : c.stage_out) f(s);
     }
+};
+
+// The device memory of an object built on a context that dpfhe_context_device_bytes reports: a scratch that grows with the batch,
+// and the object's fixed allocations (keys, tables), which it makes itself and declares with count_fixed().  Every change of
+// ctx->object_bytes happens here, and the destructor takes back all that was counted, so an object can neither reserve without
+// counting nor go away without uncounting.
+class CountedScratch {
+public:
+    explicit CountedScratch(dpfhe_ctx *ctx) : ctx_(ctx) {}
+    ~CountedScratch() { ctx_->object_bytes -= fixed_ + s_.bytes(); }
+    void count_fixed(size_t bytes) {
+        fixed_ += bytes;
+        ctx_->object_bytes += bytes;
+    }
+    int reserve(size_t bytes) {
+        ctx_->object_bytes -= s_.bytes();
+        const int rc = s_.reserve(ctx_, bytes);   // a failed allocation leaves it empty
+        ctx_->object_bytes += s_.bytes();
+        return rc;
+    }
+    dpfhe::u64 *get() const { return s_.get(); }
+
+private:
+    dpfhe_ctx *ctx_;
+    size_t fixed_ = 0;
+    DeviceScratch s_;
 };

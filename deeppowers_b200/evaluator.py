@@ -575,17 +575,55 @@ def linear_bsgs_grouped(ctx, ctx_q, n_special, ct, diags, gk_baby, gk_giant, bab
     return out
 
 
-class LinearLayer:
+class _ContextObject:
+    """What the library objects built on a context share: the handle, close(), apply() and apply_host() over the C functions
+    <_prefix>_destroy / _apply / _apply_host."""
+
+    _prefix = None
+
+    def __init__(self, ctx, n_special):
+        self._l, self.ctx = ctx._l, ctx
+        self._h = C.c_void_p()
+        self.n_special = int(n_special)
+        self.Lq = ctx.L - self.n_special                     # limbs of a ciphertext polynomial
+
+    def _adopt(self, rc):
+        """The end of a constructor: rc is the status of the C constructor that filled self._h."""
+        if rc != 0:
+            self._h = C.c_void_p()
+            raise DpfheError(self._l.dpfhe_last_error().decode())
+
+    def _fn(self, name):
+        return getattr(self._l, self._prefix + name)
+
+    def close(self):
+        """Close the object before its context.  Its destroy function reads the context, so once the context is closed (for example
+        when the garbage collector finalizes both in the wrong order) the object is dropped without it and its device buffers go
+        with the process."""
+        if getattr(self, "_h", None) and self._h.value:
+            if self.ctx._h.value:
+                self._fn("_destroy")(self._h)
+            self._h = C.c_void_p()
+
+    __del__ = close
+
+    def apply(self, ct, out, batch, stream=None):
+        self.ctx._chk(self._fn("_apply")(self._h, _ptr(ct), _ptr(out), batch, _stream(stream)))
+
+    def apply_host(self, ct, out):
+        self.ctx._chk(self._fn("_apply_host")(self._h, _hptr(ct), _hptr(out, True), ct.size // (2 * self.Lq * self.ctx.N)))
+
+
+class LinearLayer(_ContextObject):
     """Encrypted linear layer as a library object (dpfhe_linear_*): diagonal plaintexts and Galois keys live on the device; apply()
     takes device buffers, apply_host() host buffers (pipelined in chunks).  diags [n][L][N], gk_baby [baby-1][L][2][L][N] (keys of the
     rotations by 1 .. baby-1), gk_giant [L][2][L][N] (rotation by `baby`): C-contiguous numpy uint64 arrays.
     LinearLayer.grouped(...) builds the same layer with grouped special-prime keys."""
 
+    _prefix = "dpfhe_linear"
+
     def __init__(self, ctx, diags, baby, gk_baby, gk_giant, _n_special=0, _t_plain=0):
-        self._l, self.ctx = ctx._l, ctx
-        self._h = C.c_void_p()
-        self.n_special = int(_n_special)
-        self.Lq = ctx.L - self.n_special                     # limbs of a ciphertext polynomial
+        super().__init__(ctx, _n_special)
         n = diags.shape[0]
         kb = _hptr(gk_baby) if gk_baby is not None else None
         kg = _hptr(gk_giant) if gk_giant is not None else None
@@ -593,9 +631,7 @@ class LinearLayer:
             rc = self._l.dpfhe_linear_create_grouped(ctx._h, self.n_special, _hptr(diags), n, int(baby), kb, kg, int(_t_plain), C.byref(self._h))
         else:
             rc = self._l.dpfhe_linear_create(ctx._h, _hptr(diags), n, int(baby), kb, kg, C.byref(self._h))
-        if rc != 0:
-            self._h = C.c_void_p()
-            raise DpfheError(self._l.dpfhe_last_error().decode())
+        self._adopt(rc)
 
     @classmethod
     def grouped(cls, ctx, n_special, diags, baby, gk_baby, gk_giant, t_plain=0):
@@ -606,39 +642,20 @@ class LinearLayer:
             raise ValueError("n_special must be at least 1")
         return cls(ctx, diags, baby, gk_baby, gk_giant, _n_special=n_special, _t_plain=t_plain)
 
-    def close(self):
-        """Close the layer before its context.  dpfhe_linear_destroy reads the context, so once the context is closed (for example
-        when the garbage collector finalizes both in the wrong order) the layer is dropped without it and its device buffers go
-        with the process."""
-        if getattr(self, "_h", None) and self._h.value:
-            if self.ctx._h.value:
-                self._l.dpfhe_linear_destroy(self._h)
-            self._h = C.c_void_p()
 
-    __del__ = close
-
-    def apply(self, ct, out, batch, stream=None):
-        self.ctx._chk(self._l.dpfhe_linear_apply(self._h, _ptr(ct), _ptr(out), batch, _stream(stream)))
-
-    def apply_host(self, ct, out):
-        self.ctx._chk(self._l.dpfhe_linear_apply_host(self._h, _hptr(ct), _hptr(out, True), ct.size // (2 * self.Lq * self.ctx.N)))
-
-
-class PolyEval:
+class PolyEval(_ContextObject):
     """BGV polynomial evaluation on encrypted slots down the modulus chain (dpfhe_polyeval_*, DESIGN.md section 2.15; PolyEval.ckks for
     CKKS, section 2.16): slot-wise p(x) = sum_k coeffs[k] x^k mod t_plain.  ctx's last n_special limbs are special primes; relin_key is the grouped relinearisation
     key [dnum][2][L][N] of the top level (C-contiguous numpy uint64).  apply / apply_host take ciphertexts [batch][2][Lq][N] and
     write [batch][2][result_limbs][N], which decrypt under the first result_limbs limbs of the secret."""
 
+    _prefix = "dpfhe_polyeval"
+
     def __init__(self, ctx, n_special, t_plain, coeffs, relin_key):
-        self._l, self.ctx = ctx._l, ctx
-        self._h = C.c_void_p()
-        self.n_special = int(n_special)
-        self.Lq = ctx.L - self.n_special
+        super().__init__(ctx, n_special)
         cs = np.ascontiguousarray([int(c) for c in coeffs], dtype=np.int64)
-        rc = self._l.dpfhe_polyeval_create_grouped(ctx._h, self.n_special, int(t_plain), C.c_void_p(cs.ctypes.data), len(cs) - 1, _hptr(relin_key),
-                                                   C.byref(self._h))
-        self._finish(rc)
+        self._adopt(self._l.dpfhe_polyeval_create_grouped(ctx._h, self.n_special, int(t_plain), C.c_void_p(cs.ctypes.data), len(cs) - 1,
+                                                          _hptr(relin_key), C.byref(self._h)))
 
     @classmethod
     def ckks(cls, ctx, n_special, coeffs, scale_in, relin_key, scale_out=None):
@@ -647,38 +664,17 @@ class PolyEval:
         which result_scale reports.  relin_key: the grouped key of the top level generated with t_plain = 0.  The result has
         result_limbs = Lq - ceil(log2 d) - 1 limbs and decodes with ckks_decode at result_scale."""
         self = cls.__new__(cls)
-        self._l, self.ctx = ctx._l, ctx
-        self._h = C.c_void_p()
-        self.n_special = int(n_special)
-        self.Lq = ctx.L - self.n_special
+        _ContextObject.__init__(self, ctx, n_special)
         cs = np.ascontiguousarray([float(c) for c in coeffs], dtype=np.float64)
         so = float(scale_in if scale_out is None else scale_out)
-        rc = self._l.dpfhe_polyeval_create_ckks(ctx._h, self.n_special, C.c_void_p(cs.ctypes.data), len(cs) - 1, float(scale_in), so,
-                                                _hptr(relin_key), C.byref(self._h))
-        self._finish(rc)
+        self._adopt(self._l.dpfhe_polyeval_create_ckks(ctx._h, self.n_special, C.c_void_p(cs.ctypes.data), len(cs) - 1, float(scale_in), so,
+                                                       _hptr(relin_key), C.byref(self._h)))
         return self
 
-    def _finish(self, rc):
-        if rc != 0:
-            self._h = C.c_void_p()
-            raise DpfheError(self._l.dpfhe_last_error().decode())
+    def _adopt(self, rc):
+        super()._adopt(rc)
         self.result_limbs = int(self._l.dpfhe_polyeval_result_limbs(self._h))
         self.result_scale = float(self._l.dpfhe_polyeval_result_scale(self._h))
-
-    def close(self):
-        """Close the evaluator before its context (as LinearLayer.close)."""
-        if getattr(self, "_h", None) and self._h.value:
-            if self.ctx._h.value:
-                self._l.dpfhe_polyeval_destroy(self._h)
-            self._h = C.c_void_p()
-
-    __del__ = close
-
-    def apply(self, ct, out, batch, stream=None):
-        self.ctx._chk(self._l.dpfhe_polyeval_apply(self._h, _ptr(ct), _ptr(out), batch, _stream(stream)))
-
-    def apply_host(self, ct, out):
-        self.ctx._chk(self._l.dpfhe_polyeval_apply_host(self._h, _hptr(ct), _hptr(out, True), ct.size // (2 * self.Lq * self.ctx.N)))
 
 
 def slotsum_steps(stride, radices):
@@ -695,44 +691,25 @@ def slotsum_steps(stride, radices):
     return [int(out[k]) for k in range(n.value)]
 
 
-class SlotSum:
+class SlotSum(_ContextObject):
     """Encrypted slot sums as a library object (dpfhe_slotsum_*, DESIGN.md section 2.17): slot i of the result is
     sum_{j < count} x[(i + j * stride) mod N/2] in every row, count = prod(radices), one summed-rotation call per radix.  Build it
     with SlotSum.grouped; apply / apply_host take ciphertexts [batch][2][Lq][N]."""
 
+    _prefix = "dpfhe_slotsum"
+
     def __init__(self, ctx, n_special, stride, radices, gks, t_plain=0):
-        self._l, self.ctx = ctx._l, ctx
-        self._h = C.c_void_p()
-        self.n_special = int(n_special)
-        self.Lq = ctx.L - self.n_special
+        super().__init__(ctx, n_special)
         self.stride, self.radices = int(stride), [int(r) for r in radices]
         rs = (C.c_uint * max(len(self.radices), 1))(*self.radices)
-        rc = self._l.dpfhe_slotsum_create_grouped(ctx._h, self.n_special, self.stride, rs, len(self.radices), _hptr(gks), int(t_plain),
-                                                  C.byref(self._h))
-        if rc != 0:
-            self._h = C.c_void_p()
-            raise DpfheError(self._l.dpfhe_last_error().decode())
+        self._adopt(self._l.dpfhe_slotsum_create_grouped(ctx._h, self.n_special, self.stride, rs, len(self.radices), _hptr(gks), int(t_plain),
+                                                         C.byref(self._h)))
 
     @classmethod
     def grouped(cls, ctx, n_special, stride, radices, gks, t_plain=0):
         """ctx's last n_special limbs are special primes; gks [n_steps][dnum][2][L][N] (C-contiguous numpy uint64): the grouped Galois
         keys of the rotations by slotsum_steps(stride, radices), in that order; t_plain as rotate_hoisted_grouped (0: CKKS)"""
         return cls(ctx, n_special, stride, radices, gks, t_plain)
-
-    def close(self):
-        """Close the object before its context (as LinearLayer.close)."""
-        if getattr(self, "_h", None) and self._h.value:
-            if self.ctx._h.value:
-                self._l.dpfhe_slotsum_destroy(self._h)
-            self._h = C.c_void_p()
-
-    __del__ = close
-
-    def apply(self, ct, out, batch, stream=None):
-        self.ctx._chk(self._l.dpfhe_slotsum_apply(self._h, _ptr(ct), _ptr(out), batch, _stream(stream)))
-
-    def apply_host(self, ct, out):
-        self.ctx._chk(self._l.dpfhe_slotsum_apply_host(self._h, _hptr(ct), _hptr(out, True), ct.size // (2 * self.Lq * self.ctx.N)))
 
 
 class MultiContext:

@@ -47,6 +47,13 @@ struct ConstCiphertextBatch {
     ConstCiphertextBatch(const CiphertextBatch &b) : data(b.data), count(b.count) {}
 };
 
+namespace detail {
+// the part the library objects built on an Evaluator share (below)
+template <class H, void (*Destroy)(H *), int (*Apply)(H *, const std::uint64_t *, std::uint64_t *, std::size_t, void *),
+          int (*ApplyHost)(H *, const std::uint64_t *, std::uint64_t *, std::size_t)>
+class ContextObject;
+}  // namespace detail
+
 class Evaluator {
 public:
     explicit Evaluator(const EncryptionParameters &parms, int device_id = 0) : log_n_(parms.log_n), limbs_(parms.n_limbs) {
@@ -342,10 +349,9 @@ public:
     dpfhe_ctx *native_handle() { return ctx_; }
 
 private:
-    friend class LinearLayer;
-    friend class PolyEval;
-    friend class SlotSum;
-    friend class CkksPolyEval;
+    template <class H, void (*)(H *), int (*)(H *, const std::uint64_t *, std::uint64_t *, std::size_t, void *),
+              int (*)(H *, const std::uint64_t *, std::uint64_t *, std::size_t)>
+    friend class detail::ContextObject;
     static void check(int status) {
         if (status != DPFHE_OK) throw std::runtime_error(dpfhe_last_error());
     }
@@ -404,122 +410,100 @@ private:
     std::uint64_t t_, next_;
 };
 
+namespace detail {
+
+// A non-copyable owner of the C handle H with the host-buffer and device-buffer applications.  The public classes derive from it and
+// add their constructors (which fill h_) and accessors.
+template <class H, void (*Destroy)(H *), int (*Apply)(H *, const std::uint64_t *, std::uint64_t *, std::size_t, void *),
+          int (*ApplyHost)(H *, const std::uint64_t *, std::uint64_t *, std::size_t)>
+class ContextObject {
+public:
+    ContextObject(const ContextObject &) = delete;
+    ContextObject &operator=(const ContextObject &) = delete;
+    void apply(ConstCiphertextBatch in, CiphertextBatch out) {   // host buffers, pipelined
+        if (in.count != out.count) throw std::runtime_error("ciphertext batches must have the same count");
+        check(ApplyHost(h_, in.data, out.data, in.count));
+    }
+    void apply_device(const std::uint64_t *in, std::uint64_t *out, std::size_t count, void *stream = nullptr) {
+        check(Apply(h_, in, out, count, stream));
+    }
+
+protected:
+    ContextObject() = default;
+    ~ContextObject() { Destroy(h_); }
+    static void check(int status) { Evaluator::check(status); }
+    H *h_ = nullptr;
+};
+using LinearObject = ContextObject<dpfhe_linear, dpfhe_linear_destroy, dpfhe_linear_apply, dpfhe_linear_apply_host>;
+using PolyEvalObject = ContextObject<dpfhe_polyeval, dpfhe_polyeval_destroy, dpfhe_polyeval_apply, dpfhe_polyeval_apply_host>;
+using SlotSumObject = ContextObject<dpfhe_slotsum, dpfhe_slotsum_destroy, dpfhe_slotsum_apply, dpfhe_slotsum_apply_host>;
+
+}  // namespace detail
+
 // An encrypted linear layer y = W x (baby-step/giant-step diagonals) whose weights and Galois keys live on the device.
 // diagonals: [n][L][N] plaintexts in evaluation form (diagonal g*baby + b pre-rotated by -g*baby), n a multiple of baby;
 // baby_keys: [baby-1][L][2][L][N] keys of the rotations by 1 .. baby-1 slots; giant_key: [L][2][L][N], rotation by `baby`.
-class LinearLayer {
+class LinearLayer : public detail::LinearObject {
 public:
     LinearLayer(Evaluator &ev, const std::uint64_t *diagonals, std::size_t n_diagonals, std::size_t baby, const std::uint64_t *baby_keys,
                 const std::uint64_t *giant_key) {
-        Evaluator::check(dpfhe_linear_create(ev.native_handle(), diagonals, n_diagonals, baby, baby_keys, giant_key, &h_));
+        check(dpfhe_linear_create(ev.native_handle(), diagonals, n_diagonals, baby, baby_keys, giant_key, &h_));
     }
     // with grouped special-prime keys: the evaluator's last `special` limbs are special primes, ciphertexts and diagonals carry
     // limbs()-special limbs, keys are [dnum][2][limbs()][N] (dpfhe_linear_create_grouped)
     LinearLayer(Evaluator &ev, unsigned special, const std::uint64_t *diagonals, std::size_t n_diagonals, std::size_t baby,
                 const std::uint64_t *baby_keys, const std::uint64_t *giant_key, std::uint64_t plain_modulus) {
-        Evaluator::check(dpfhe_linear_create_grouped(ev.native_handle(), special, diagonals, n_diagonals, baby, baby_keys, giant_key, plain_modulus,
+        check(dpfhe_linear_create_grouped(ev.native_handle(), special, diagonals, n_diagonals, baby, baby_keys, giant_key, plain_modulus,
                                                      &h_));
     }
-    ~LinearLayer() { dpfhe_linear_destroy(h_); }
-    LinearLayer(const LinearLayer &) = delete;
-    LinearLayer &operator=(const LinearLayer &) = delete;
-    void apply(ConstCiphertextBatch in, CiphertextBatch out) {   // host buffers, pipelined
-        if (in.count != out.count) throw std::runtime_error("ciphertext batches must have the same count");
-        Evaluator::check(dpfhe_linear_apply_host(h_, in.data, out.data, in.count));
-    }
-    void apply_device(const std::uint64_t *in, std::uint64_t *out, std::size_t count, void *stream = nullptr) {
-        Evaluator::check(dpfhe_linear_apply(h_, in, out, count, stream));
-    }
-
-private:
-    dpfhe_linear *h_ = nullptr;
 };
 
 // BGV polynomial evaluation on encrypted slots down the modulus chain (dpfhe_polyeval_*): p(x) = sum_k coeffs[k] x^k mod
 // plain_modulus, slot by slot.  The evaluator's last `special` limbs are special primes; relin_key is the grouped relinearisation key
 // [dnum][2][limbs()][N] of the top level (host memory).  Inputs carry limbs()-special limbs, results result_limbs().
-class PolyEval {
+class PolyEval : public detail::PolyEvalObject {
 public:
     PolyEval(Evaluator &ev, unsigned special, std::uint64_t plain_modulus, const std::vector<std::int64_t> &coeffs, const std::uint64_t *relin_key) {
         if (coeffs.size() < 2) throw std::runtime_error("a polynomial of degree at least 1");
-        Evaluator::check(dpfhe_polyeval_create_grouped(ev.native_handle(), special, plain_modulus, coeffs.data(), coeffs.size() - 1, relin_key, &h_));
+        check(dpfhe_polyeval_create_grouped(ev.native_handle(), special, plain_modulus, coeffs.data(), coeffs.size() - 1, relin_key, &h_));
     }
-    ~PolyEval() { dpfhe_polyeval_destroy(h_); }
-    PolyEval(const PolyEval &) = delete;
-    PolyEval &operator=(const PolyEval &) = delete;
     unsigned result_limbs() const { return dpfhe_polyeval_result_limbs(h_); }
-    void apply(ConstCiphertextBatch in, CiphertextBatch out) {   // host buffers, pipelined
-        if (in.count != out.count) throw std::runtime_error("ciphertext batches must have the same count");
-        Evaluator::check(dpfhe_polyeval_apply_host(h_, in.data, out.data, in.count));
-    }
-    void apply_device(const std::uint64_t *in, std::uint64_t *out, std::size_t count, void *stream = nullptr) {
-        Evaluator::check(dpfhe_polyeval_apply(h_, in, out, count, stream));
-    }
-
-private:
-    dpfhe_polyeval *h_ = nullptr;
 };
 
 // Slot sums (dpfhe_slotsum_*, DESIGN.md §2.17): slot i of the result is sum_{j < prod(radices)} x[(i + j * stride) mod N/2] in every
 // row.  galois_keys: the grouped Galois keys of the rotations by SlotSum::steps(stride, radices), in that order, back to back in host
 // memory (what Evaluator::generate_galois_keys writes); plain_modulus 0 for CKKS.
-class SlotSum {
+class SlotSum : public detail::SlotSumObject {
 public:
     SlotSum(Evaluator &ev, unsigned special, std::size_t stride, const std::vector<unsigned> &radices, const std::uint64_t *galois_keys,
             std::uint64_t plain_modulus = 0) {
-        Evaluator::check(dpfhe_slotsum_create_grouped(ev.native_handle(), special, stride, radices.data(), radices.size(), galois_keys, plain_modulus,
+        check(dpfhe_slotsum_create_grouped(ev.native_handle(), special, stride, radices.data(), radices.size(), galois_keys, plain_modulus,
                                                       &h_));
     }
-    ~SlotSum() { dpfhe_slotsum_destroy(h_); }
-    SlotSum(const SlotSum &) = delete;
-    SlotSum &operator=(const SlotSum &) = delete;
     // the rotation steps, stage by stage and ascending within a stage: the order of the keys
     static std::vector<long> steps(std::size_t stride, const std::vector<unsigned> &radices) {
         std::size_t n = 0;
-        Evaluator::check(dpfhe_slotsum_steps(stride, radices.data(), radices.size(), nullptr, &n));
+        check(dpfhe_slotsum_steps(stride, radices.data(), radices.size(), nullptr, &n));
         std::vector<int> s(n);
-        Evaluator::check(dpfhe_slotsum_steps(stride, radices.data(), radices.size(), s.data(), &n));
+        check(dpfhe_slotsum_steps(stride, radices.data(), radices.size(), s.data(), &n));
         return std::vector<long>(s.begin(), s.end());
     }
-    void apply(ConstCiphertextBatch in, CiphertextBatch out) {   // host buffers, pipelined
-        if (in.count != out.count) throw std::runtime_error("ciphertext batches must have the same count");
-        Evaluator::check(dpfhe_slotsum_apply_host(h_, in.data, out.data, in.count));
-    }
-    void apply_device(const std::uint64_t *in, std::uint64_t *out, std::size_t count, void *stream = nullptr) {
-        Evaluator::check(dpfhe_slotsum_apply(h_, in, out, count, stream));
-    }
-
-private:
-    dpfhe_slotsum *h_ = nullptr;
 };
 
 // CKKS polynomial evaluation on encrypted slots down the rescaling chain (dpfhe_polyeval_create_ckks, DESIGN.md §2.16): p(z) = sum_k
 // coeffs[k] z^k with real coefficients, slot by slot.  Inputs at scale scale_in carry limbs()-special limbs; results carry
 // result_limbs() limbs at result_scale() (scale_out, or scale_in when scale_out is 0).  relin_key: the grouped relinearisation key
 // of the top level generated with plain modulus 0 (host memory).
-class CkksPolyEval {
+class CkksPolyEval : public detail::PolyEvalObject {
 public:
     CkksPolyEval(Evaluator &ev, unsigned special, const std::vector<double> &coeffs, double scale_in, const std::uint64_t *relin_key,
                  double scale_out = 0) {
         if (coeffs.size() < 2) throw std::runtime_error("a polynomial of degree at least 1");
-        Evaluator::check(dpfhe_polyeval_create_ckks(ev.native_handle(), special, coeffs.data(), coeffs.size() - 1, scale_in,
+        check(dpfhe_polyeval_create_ckks(ev.native_handle(), special, coeffs.data(), coeffs.size() - 1, scale_in,
                                                     scale_out == 0 ? scale_in : scale_out, relin_key, &h_));
     }
-    ~CkksPolyEval() { dpfhe_polyeval_destroy(h_); }
-    CkksPolyEval(const CkksPolyEval &) = delete;
-    CkksPolyEval &operator=(const CkksPolyEval &) = delete;
     unsigned result_limbs() const { return dpfhe_polyeval_result_limbs(h_); }
     double result_scale() const { return dpfhe_polyeval_result_scale(h_); }
-    void apply(ConstCiphertextBatch in, CiphertextBatch out) {   // host buffers, pipelined
-        if (in.count != out.count) throw std::runtime_error("ciphertext batches must have the same count");
-        Evaluator::check(dpfhe_polyeval_apply_host(h_, in.data, out.data, in.count));
-    }
-    void apply_device(const std::uint64_t *in, std::uint64_t *out, std::size_t count, void *stream = nullptr) {
-        Evaluator::check(dpfhe_polyeval_apply(h_, in, out, count, stream));
-    }
-
-private:
-    dpfhe_polyeval *h_ = nullptr;
 };
 
 // Several GPUs behind one object (dpfhe_multi_*): contiguous shards of every batch, one context and host thread per device, no
