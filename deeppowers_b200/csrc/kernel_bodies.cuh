@@ -723,36 +723,68 @@ DPFHE_HD void ks_blk_phase2(CTA &cta, u64 *buf, U64x2 *acc, const KsArgs &A, con
     constexpr int B0 = 2 * SB + 1;
     const bool last = jj + 1 == A.L;
     const bool trim = !last && acc_trim_after(B0, (int)jj - 1);
+    // chunk lc with the key words b, a and their Shoup companions bs, as
+    auto mac = [&](int lc, const U64x2 &b, const U64x2 &a, const U64x2 &bs, const U64x2 &as) {
+        // u < 16q straight from the transform: Shoup multiplication accepts any 64-bit operand
+        const U64x2 u = reinterpret_cast<const U64x2 *>(buf)[swz_chunk(lc)];
+        U64x2 r0 = acc[lc], r1 = acc[HC + lc];
+        r0.x += shoup_lazy(u.x, b.x, bs.x, p);
+        r0.y += shoup_lazy(u.y, b.y, bs.y, p);
+        r1.x += shoup_lazy(u.x, a.x, as.x, p);
+        r1.y += shoup_lazy(u.y, a.y, as.y, p);
+        if (trim) {
+            r0.x = csub(r0.x, p.q8); r0.y = csub(r0.y, p.q8);
+            r1.x = csub(r1.x, p.q8); r1.y = csub(r1.y, p.q8);
+        }
+        if (last) {
+            r0.x = canon(r0.x, p); r0.y = canon(r0.y, p);
+            r1.x = canon(r1.x, p); r1.y = canon(r1.y, p);
+            st_stream(out0 + lc, r0);
+            st_stream(out1 + lc, r1);
+        } else {
+            acc[lc] = r0;
+            acc[HC + lc] = r1;
+        }
+    };
     cta.par([&](int tid) {
-        U64x2 vb = ld_keep(kb + tid), va = ld_keep(ka + tid), vbs = ld_keep(kbs + tid), vas = ld_keep(kas + tid);
+        if constexpr (DPFHE_FAST) {
+            // Only the companions are read and each key word is rebuilt from its own (shoup_w_from_companion, two IMAD.WIDE):
+            // half the key bytes.  Two chunks are in flight, in the registers one chunk of words and companions took: the loop
+            // takes the chunks two at a time, and each set is refilled as soon as its chunk's products have read it.
+            static_assert(HC % (2 * NT) == 0, "the key-column loop takes two chunks per iteration");
+            auto mac_s = [&](int lc, const U64x2 &bs, const U64x2 &as) {
+                U64x2 b, a;
+                b.x = shoup_w_from_companion(bs.x, p); b.y = shoup_w_from_companion(bs.y, p);
+                a.x = shoup_w_from_companion(as.x, p); a.y = shoup_w_from_companion(as.y, p);
+                mac(lc, b, a, bs, as);
+            };
+            U64x2 s0b = ld_keep(kbs + tid), s0a = ld_keep(kas + tid), s1b = ld_keep(kbs + tid + NT), s1a = ld_keep(kas + tid + NT);
 #pragma unroll 1
-        for (int lc = tid; lc < HC; lc += NT) {
-            const U64x2 b = vb, a = va, bs = vbs, as = vas;
-            if (lc + NT < HC) {   // the next chunk's key loads fly during this chunk's math
-                vb = ld_keep(kb + lc + NT);
-                va = ld_keep(ka + lc + NT);
-                vbs = ld_keep(kbs + lc + NT);
-                vas = ld_keep(kas + lc + NT);
+            for (int lc = tid; lc < HC; lc += 2 * NT) {
+                mac_s(lc, s0b, s0a);
+                if (lc + 2 * NT < HC) {
+                    s0b = ld_keep(kbs + lc + 2 * NT);
+                    s0a = ld_keep(kas + lc + 2 * NT);
+                }
+                mac_s(lc + NT, s1b, s1a);
+                if (lc + 3 * NT < HC) {
+                    s1b = ld_keep(kbs + lc + 3 * NT);
+                    s1a = ld_keep(kas + lc + 3 * NT);
+                }
             }
-            // u < 16q straight from the transform: Shoup multiplication accepts any 64-bit operand
-            const U64x2 u = reinterpret_cast<const U64x2 *>(buf)[swz_chunk(lc)];
-            U64x2 r0 = acc[lc], r1 = acc[HC + lc];
-            r0.x += shoup_lazy(u.x, b.x, bs.x, p);
-            r0.y += shoup_lazy(u.y, b.y, bs.y, p);
-            r1.x += shoup_lazy(u.x, a.x, as.x, p);
-            r1.y += shoup_lazy(u.y, a.y, as.y, p);
-            if (trim) {
-                r0.x = csub(r0.x, p.q8); r0.y = csub(r0.y, p.q8);
-                r1.x = csub(r1.x, p.q8); r1.y = csub(r1.y, p.q8);
-            }
-            if (last) {
-                r0.x = canon(r0.x, p); r0.y = canon(r0.y, p);
-                r1.x = canon(r1.x, p); r1.y = canon(r1.y, p);
-                st_stream(out0 + lc, r0);
-                st_stream(out1 + lc, r1);
-            } else {
-                acc[lc] = r0;
-                acc[HC + lc] = r1;
+        } else {
+            // gen: rebuilding a word would take a full 64 x 64 product, so both rows are read
+            U64x2 vb = ld_keep(kb + tid), va = ld_keep(ka + tid), vbs = ld_keep(kbs + tid), vas = ld_keep(kas + tid);
+#pragma unroll 1
+            for (int lc = tid; lc < HC; lc += NT) {
+                const U64x2 b = vb, a = va, bs = vbs, as = vas;
+                if (lc + NT < HC) {   // the next chunk's key loads fly during this chunk's math
+                    vb = ld_keep(kb + lc + NT);
+                    va = ld_keep(ka + lc + NT);
+                    vbs = ld_keep(kbs + lc + NT);
+                    vas = ld_keep(kas + lc + NT);
+                }
+                mac(lc, b, a, bs, as);
             }
         }
     });

@@ -202,6 +202,46 @@ DPFHE_HD u64 shoup_lazy(u64 x, u64 w, u64 ws, const LimbParams &p) { return shou
 // shoup_lazy with mulhi_approx_cc: the same value
 DPFHE_HD u64 shoup_lazy_cc(u64 x, u64 w, u64 ws, const LimbParams &p) { return shoup_tail(x, w, mulhi_approx_cc(x, ws), p); }
 
+// The Shoup factor w < q from its companion ws = floor(w * 2^64 / q) alone, exactly: ws*q lies in (w 2^64 - q, w 2^64], so
+// ws*q + q - 1 lies in [w 2^64, w 2^64 + q - 1] and w = hi64(ws*q + q - 1).  A kernel that reads only the companions of a key
+// row reads half the bytes (DESIGN.md §4.4).
+// fast: q - 1 = qh 2^32, so ws*q + q - 1 = wl + 2^32 (wh + qh + wl qh) + 2^64 wh qh (ws = wh:wl): two IMAD.WIDE (wl qh, wh qh)
+//       and a carry chain; of the middle sum only the carry out of its low word matters.
+// gen:  the full 128-bit product (not used on the device's hot path).
+DPFHE_HD u64 shoup_w_from_companion(u64 ws, const LimbParams &p) {
+#if defined(__CUDA_ARCH__)
+#if DPFHE_FAST
+    const u32 qh = 0u - p.nqh;
+    u64 w;
+    asm("{\n\t"
+        ".reg .u32 wl, wh, sl, sh, bl, bh;\n\t"
+        ".reg .u64 S, B;\n\t"
+        "mov.b64 {wl, wh}, %1;\n\t"
+        "mul.wide.u32 S, wl, %2;\n\t"
+        "mul.wide.u32 B, wh, %2;\n\t"
+        "mov.b64 {sl, sh}, S;\n\t"
+        "add.cc.u32 sl, sl, wh;\n\t"
+        "addc.u32 sh, sh, 0;\n\t"
+        "add.cc.u32 sl, sl, %2;\n\t"
+        "addc.u32 sh, sh, 0;\n\t"
+        "mov.b64 {bl, bh}, B;\n\t"
+        "add.cc.u32 bl, bl, sh;\n\t"
+        "addc.u32 bh, bh, 0;\n\t"
+        "mov.b64 %0, {bl, bh};\n\t"
+        "}"
+        : "=l"(w)
+        : "l"(ws), "r"(qh));
+    return w;
+#else
+    const u64 hi = umulhi64(ws, p.q), lo = ws * p.q;
+    const u64 s = lo + (p.q - 1);
+    return hi + (s < lo ? 1u : 0u);
+#endif
+#else
+    return (u64)(((unsigned __int128)ws * p.q + (p.q - 1)) >> 64);
+#endif
+}
+
 // 128-bit product (hi:lo) of two 64-bit words.  Device: four IMAD.WIDE partial products combined once
 // (nvcc's separate a*b and __umul64hi(a,b) would recompute the low partial product: 5 IMAD.WIDE + 2 IMAD).
 DPFHE_HD void mul128(u64 a, u64 b, u64 &hi, u64 &lo) {
