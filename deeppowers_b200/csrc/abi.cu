@@ -108,10 +108,12 @@ namespace {
 // Generic three-stage pipeline over `n_items` items split into chunks:
 //   upload(chunk -> stage_in[slot]) on s_h2d, compute on ctx->stream, download(stage_out[slot]) on s_d2h.
 // in_item_bytes / out_item_bytes are per item; h_in may be two arrays (a and b) laid out back to back in the stage.
+// n_slices > 1: each input is n_slices arrays of n_items items, slice_stride words apart (the operands of an inner product,
+// [n_terms][batch] ciphertexts); a chunk stages its items of every slice, [input][slice][chunk_items], slice after slice.
 template <class Compute>
 int run_pipeline_body(dpfhe_ctx *ctx, const u64 *h_in0, const u64 *h_in1, u64 *h_out, size_t n_items, size_t in_item_words,
-                      size_t out_item_words, size_t chunk_items, Compute compute) {
-    const size_t n_in = h_in1 ? 2 : 1;
+                      size_t out_item_words, size_t chunk_items, Compute compute, size_t n_slices, size_t slice_stride) {
+    const size_t n_in = (h_in1 ? 2 : 1) * n_slices;
     int rc = DPFHE_OK;
     for (int k = 0; k < PIPE_DEPTH && !rc; ++k) rc = ctx->stage_in[k].reserve(ctx, n_in * chunk_items * in_item_words * 8);
     for (int k = 0; k < PIPE_DEPTH && !rc; ++k) rc = ctx->stage_out[k].reserve(ctx, chunk_items * out_item_words * 8);
@@ -120,11 +122,13 @@ int run_pipeline_body(dpfhe_ctx *ctx, const u64 *h_in0, const u64 *h_in1, u64 *h
     for (size_t first = 0; first < n_items; first += chunk_items, ++k) {
         const size_t cnt = n_items - first < chunk_items ? n_items - first : chunk_items;
         const int slot = (int)(k % PIPE_DEPTH);
-        u64 *din0 = ctx->stage_in[slot].get(), *din1 = din0 + chunk_items * in_item_words, *dout = ctx->stage_out[slot].get();
+        u64 *din0 = ctx->stage_in[slot].get(), *din1 = din0 + n_slices * chunk_items * in_item_words, *dout = ctx->stage_out[slot].get();
         if (k >= PIPE_DEPTH) CU_TRY(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_comp[slot], 0));   // stage_in[slot] free again
-        CU_TRY(cudaMemcpyAsync(din0, h_in0 + first * in_item_words, cnt * in_item_words * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
-        if (h_in1)
-            CU_TRY(cudaMemcpyAsync(din1, h_in1 + first * in_item_words, cnt * in_item_words * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
+        for (size_t s = 0; s < n_slices; ++s) {
+            const size_t src = s * slice_stride + first * in_item_words, dst = s * chunk_items * in_item_words;
+            CU_TRY(cudaMemcpyAsync(din0 + dst, h_in0 + src, cnt * in_item_words * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
+            if (h_in1) CU_TRY(cudaMemcpyAsync(din1 + dst, h_in1 + src, cnt * in_item_words * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
+        }
         CU_TRY(cudaEventRecord(ctx->ev_h2d[slot], ctx->s_h2d));
         CU_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ev_h2d[slot], 0));
         if (k >= PIPE_DEPTH) CU_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ev_d2h[slot], 0));   // stage_out[slot] drained
@@ -144,8 +148,8 @@ int run_pipeline_body(dpfhe_ctx *ctx, const u64 *h_in0, const u64 *h_in1, u64 *h
 // the caller's host buffers (or the staging slots) when the error is reported
 template <class Compute>
 int run_pipeline(dpfhe_ctx *ctx, const u64 *h_in0, const u64 *h_in1, u64 *h_out, size_t n_items, size_t in_item_words,
-                 size_t out_item_words, size_t chunk_items, Compute compute) {
-    const int rc = run_pipeline_body(ctx, h_in0, h_in1, h_out, n_items, in_item_words, out_item_words, chunk_items, compute);
+                 size_t out_item_words, size_t chunk_items, Compute compute, size_t n_slices = 1, size_t slice_stride = 0) {
+    const int rc = run_pipeline_body(ctx, h_in0, h_in1, h_out, n_items, in_item_words, out_item_words, chunk_items, compute, n_slices, slice_stride);
     if (rc != DPFHE_OK) {
         const std::string why = g_err;   // the drains below must not replace the message of the failure
         cudaStreamSynchronize(ctx->s_h2d);
@@ -718,6 +722,35 @@ int dpfhe_rotate_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_c
                          size_t batch, uint64_t t_plain, void *stream) {
     return ks_hybrid_common(ctx, n_special, KS_ROTATE, d_ct, nullptr, d_gk, d_out, batch, galois_elt, t_plain, stream);
 }
+// Encrypted inner product (DESIGN.md §2.18): the tensor products of n_terms pairs summed before one relinearisation.  Every
+// n_special runs the grouped kernel (with one special prime its digits are single limbs and it computes what the hybrid kernel does).
+int dpfhe_ct_dot_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *const *d_as, const uint64_t *const *d_bs,
+                         const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (n_terms < 1 || n_terms > (size_t)DOT_MAX_TERMS) return fail(DPFHE_ERR_INVALID, "n_terms must be in [1, %d]", DOT_MAX_TERMS);
+    if (!d_as || !d_bs) return fail(DPFHE_ERR_INVALID, "null argument");
+    for (size_t i = 0; i < n_terms; ++i)
+        if (!d_as[i] || !d_bs[i] || !aligned16(d_as[i]) || !aligned16(d_bs[i])) return fail(DPFHE_ERR_INVALID, "null or misaligned operand of pair %zu", i);
+    CHECK_PTR(d_evk); CHECK_PTR(d_out);
+    rc = check_grouped(ctx, n_special, t_plain);
+    if (rc) return rc;
+    if (batch == 0) return DPFHE_OK;
+    // the output rows are written while other work items still read their inputs: no overlap at all
+    const size_t ct_bytes = batch * 2 * (size_t)(ctx->hp.L - n_special) * ctx->N() * 8;
+    for (size_t i = 0; i < n_terms; ++i)
+        if (overlaps(d_out, ct_bytes, d_as[i], ct_bytes) || overlaps(d_out, ct_bytes, d_bs[i], ct_bytes))
+            return fail(DPFHE_ERR_INVALID, "output must not overlap an operand (pair %zu)", i);
+    rc = ensure_hyb(ctx);
+    if (rc) return rc;
+    MsConsts K;
+    GroupConsts G;
+    build_group_consts(ctx->hp, n_special, t_plain, G, K);
+    CU_TRY(VCALL(launch_ct_dot_grouped, ctx->lc, d_as, d_bs, (u32)n_terms, d_evk, d_out, batch, K, G, pick(ctx, stream)));
+    note_launch(ctx, 2);   // key_prepare_kernel + ct_dot_grouped_kernel
+    return DPFHE_OK;
+}
+
 int dpfhe_grouped_digits(const dpfhe_ctx *ctx, unsigned n_special, unsigned *digits) {
     if (!ctx || !digits) return fail(DPFHE_ERR_INVALID, "null argument");
     int rc = check_special(ctx, n_special);
@@ -1114,6 +1147,38 @@ int dpfhe_ct_mul_relin_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const ui
                          return ks_hybrid_common(ctx, n_special, KS_MUL_RELIN, da, db, ctx->stage_key.get(), dout, cnt, 0, t_plain, st);
                      },
                      [&] { return check_special(ctx, n_special); });
+}
+
+// host form of the inner product: the key uploaded once, the batch pipelined in chunks, each chunk uploading its ciphertexts of
+// every pair.  A chunk stages 2 n_terms operands per ciphertext, so its size is budgeted on all of them; where the batch allows,
+// it is a whole number of rounds of the persistent grid.
+int dpfhe_ct_dot_grouped_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs, const uint64_t *h_evk,
+                              uint64_t *h_out, size_t batch, uint64_t t_plain) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (n_terms < 1 || n_terms > (size_t)DOT_MAX_TERMS) return fail(DPFHE_ERR_INVALID, "n_terms must be in [1, %d]", DOT_MAX_TERMS);
+    if (!h_as || !h_bs || !h_evk || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    rc = check_grouped(ctx, n_special, t_plain);
+    if (rc) return rc;
+    if (batch == 0) return DPFHE_OK;
+    const size_t ctw = 2 * (size_t)(ctx->hp.L - n_special) * ctx->N();   // words of a ciphertext
+    rc = upload_key(ctx, h_evk, 2 * key_digits(ctx, n_special) * ctx->P());
+    if (rc) return rc;
+    size_t chunk = std::max<size_t>(1, ((size_t)64 << 20) / (n_terms * ctw * 8));   // ~64 MiB per staged operand side, as pick_chunk
+    const size_t round = std::max<size_t>(1, (size_t)ctx->lc.num_sms * 3 / ctx->hp.L);   // ciphertexts per round of the grid (3 CTAs per SM)
+    if (chunk > round) chunk -= chunk % round;
+    if (chunk > batch) chunk = batch;
+    return run_pipeline(
+        ctx, h_as, h_bs, h_out, batch, ctw, ctw, chunk,
+        [&](u64 *da, u64 *db, u64 *dout, size_t cnt, cudaStream_t st) {
+            const u64 *as[DOT_MAX_TERMS], *bs[DOT_MAX_TERMS];
+            for (size_t t = 0; t < n_terms; ++t) {
+                as[t] = da + t * chunk * ctw;
+                bs[t] = db + t * chunk * ctw;
+            }
+            return dpfhe_ct_dot_grouped(ctx, n_special, n_terms, as, bs, ctx->stage_key.get(), dout, cnt, t_plain, st);
+        },
+        n_terms, batch * ctw);
 }
 
 int dpfhe_rotate_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_ct, uint64_t galois_elt, const uint64_t *h_gk,

@@ -366,14 +366,119 @@ DPFHE_HD void ks_p1_chunk(const KsP1Operands &o, const LimbParams &p, bool only,
     }
 }
 
+// ---- encrypted inner product (KS_DOT, DESIGN.md §2.18 / §4.15) ------------------------------------------------------------
+// The operand tables of one call: pair t is (a[t], b[t]), each [batch][2][Lq][N] canonical.  Passed by value in the kernel
+// parameter block, so a pair's pointers are constant-bank operands with a CTA-uniform index.
+struct DotArgs {
+    const u64 *a[DOT_MAX_TERMS];
+    const u64 *b[DOT_MAX_TERMS];
+    u32 n_terms;   // 1 .. DOT_MAX_TERMS
+};
+
+// Test hook (host builds with DPFHE_DOT_TRACK only): the largest 128-bit running sum in units of 2^(2b) (b = bit length of q; the
+// precondition of barrett_lazy_long is "below 16") and the largest reduced value in units of q (its result is below 15).
+#if defined(DPFHE_DOT_TRACK) && !defined(__CUDA_ARCH__)
+struct DotTrack {
+    double sum_over_q2 = 0, red_over_q = 0;
+};
+inline DotTrack &dot_track() {
+    static DotTrack t;
+    return t;
+}
+inline void dot_track_note(u64 hi, u64 lo, u64 r, const LimbParams &p) {
+    const double z = (double)hi * 18446744073709551616.0 + (double)lo, pb = (double)(1ull << (p.bar_shift + 2));
+    DotTrack &t = dot_track();
+    const double s = z / (pb * pb), d = (double)r / (double)p.q;
+    if (s > t.sum_over_q2) t.sum_over_q2 = s;
+    if (d > t.red_over_q) t.red_over_q = d;
+}
+#define DPFHE_DOT_NOTE(hi, lo, r, p) dot_track_note(hi, lo, r, p)
+#else
+#define DPFHE_DOT_NOTE(hi, lo, r, p)
+#endif
+
+// A running sum of 128-bit products folded to one word: (hi:lo) < 2^(2b+4)  ->  (0 : r), r < 15q
+DPFHE_HD void dot_fold(u64 &hi, u64 &lo, const LimbParams &p) {
+    const u64 r = barrett_lazy_long(hi, lo, p);
+    DPFHE_DOT_NOTE(hi, lo, r, p);
+    lo = r;
+    hi = 0;
+}
+
+// D_c = sum_t tensor(a_t, b_t)_c of one coefficient position `pos` (word offset into a ciphertext's c0 row; c1 is P words on),
+// congruent mod q and below 15q.  The four products of a pair are summed in 128 bits and reduced once per 16 products: a folded
+// sum r < 15q plus 16 products of canonical factors is 15q + 16 (q - 1)^2 < 16 q^2 < 2^(2b+4), the precondition of
+// barrett_lazy_long, so D_1 (two products per pair) folds every 8 pairs and D_0, D_2 every 16.
+DPFHE_HD void dot_coeff_pair(const DotArgs &D, size_t pos, size_t P, const LimbParams &p, U64x2 &d0, U64x2 &d1, U64x2 &d2) {
+    u64 h0x = 0, l0x = 0, h1x = 0, l1x = 0, h2x = 0, l2x = 0, h0y = 0, l0y = 0, h1y = 0, l1y = 0, h2y = 0, l2y = 0;
+    const u32 n = D.n_terms;
+#pragma unroll 1
+    for (u32 t = 0; t < n; ++t) {
+        if (t != 0 && (t & 7u) == 0) {
+            dot_fold(h1x, l1x, p);
+            dot_fold(h1y, l1y, p);
+            if ((t & 15u) == 0) {
+                dot_fold(h0x, l0x, p);
+                dot_fold(h0y, l0y, p);
+                dot_fold(h2x, l2x, p);
+                dot_fold(h2y, l2y, p);
+            }
+        }
+        const U64x2 *pa = reinterpret_cast<const U64x2 *>(D.a[t] + pos), *pb = reinterpret_cast<const U64x2 *>(D.b[t] + pos);
+        const U64x2 a0 = ld_stream(pa), a1 = ld_stream(pa + P / 2), b0 = ld_stream(pb), b1 = ld_stream(pb + P / 2);
+        mac128(h0x, l0x, a0.x, b0.x);
+        mac128(h0y, l0y, a0.y, b0.y);
+        mac128(h1x, l1x, a0.x, b1.x);
+        mac128(h1y, l1y, a0.y, b1.y);
+        mac128(h1x, l1x, a1.x, b0.x);
+        mac128(h1y, l1y, a1.y, b0.y);
+        mac128(h2x, l2x, a1.x, b1.x);
+        mac128(h2y, l2y, a1.y, b1.y);
+    }
+    dot_fold(h0x, l0x, p);
+    dot_fold(h0y, l0y, p);
+    dot_fold(h1x, l1x, p);
+    dot_fold(h1y, l1y, p);
+    dot_fold(h2x, l2x, p);
+    dot_fold(h2y, l2y, p);
+    d0.x = l0x; d0.y = l0y;
+    d1.x = l1x; d1.y = l1y;
+    d2.x = l2x; d2.y = l2y;
+}
+
+// One chunk position of a limb CTA's phase 1: what ks_p1_chunk<KS_MUL_RELIN, true> does with one pair's tensor, done with the sums.
+// D_2 enters the inverse transform below SB*q; P*D_0, P*D_1 (Shoup products accept any word) start the accumulators below SB*q each,
+// and the own-digit key terms add another SB*q: below (2 SB + 1) q as phase 2 expects.
+DPFHE_HD void ks_p1_dot_chunk(const DotArgs &D, size_t pos, size_t P, const KsP1Pointers &ptr, const LimbParams &p, u64 *buf, U64x2 *acc0,
+                              U64x2 *acc1, int c, int c_buf, u64 pm, u64 pm_s) {
+    U64x2 s0, s1, d;
+    dot_coeff_pair(D, pos, P, p, s0, s1, d);
+    d.x = word_reduce(d.x, p);   // < 3q
+    d.y = word_reduce(d.y, p);
+    if (SB < 3) {
+        d.x = csub(d.x, p.q);
+        d.y = csub(d.y, p.q);
+    }
+    reinterpret_cast<U64x2 *>(buf)[swz_chunk(c_buf)] = d;
+    const U64x2 kb = ld_keep(ptr.kb + c), ka = ld_keep(ptr.ka + c), kbs = ld_keep(ptr.kbs + c), kas = ld_keep(ptr.kas + c);
+    U64x2 r0, r1;
+    r0.x = shoup_lazy(s0.x, pm, pm_s, p) + shoup_lazy(d.x, kb.x, kbs.x, p);
+    r0.y = shoup_lazy(s0.y, pm, pm_s, p) + shoup_lazy(d.y, kb.y, kbs.y, p);
+    r1.x = shoup_lazy(s1.x, pm, pm_s, p) + shoup_lazy(d.x, ka.x, kas.x, p);
+    r1.y = shoup_lazy(s1.y, pm, pm_s, p) + shoup_lazy(d.y, ka.y, kas.y, p);
+    st_cg(acc0 + c, r0);
+    st_cg(acc1 + c, r1);
+}
+
 // slot_free / slot_free_target: when non-null, the digit slot is single-buffered and may only be overwritten once the counter has
 // reached the target (every reader of the previous digit has signalled); cta.wait_ge spins on it (a no-op in the host emulator,
 // whose sequential order already guarantees it).
 template <int LOGN, int NT, int MODE, bool HYB = false, class CTA>
 DPFHE_HD void ks_phase1(CTA &cta, u64 *buf, const KsArgs &A, const LimbParams &p, size_t ct, u32 i, u64 *t_slot, u64 *acc_rows, u64 pm = 0,
-                        u64 pm_s = 0, const u32 *slot_free = nullptr, u32 slot_free_target = 0, u32 key_digit = ~0u) {
+                        u64 pm_s = 0, const u32 *slot_free = nullptr, u32 slot_free_target = 0, u32 key_digit = ~0u, const DotArgs *dot = nullptr) {
     constexpr int N = 1 << LOGN, NC = N / 2;
     static_assert((NC / NT) % 2 == 0, "chunk loops may be unrolled by two (ping-pong operand buffers)");
+    static_assert(MODE != KS_DOT || HYB, "the inner product exists with special-prime keys only");
     const size_t P = (size_t)A.L * N, PK = HYB ? (size_t)A.Lk * N : P;
     U64x2 *acc0 = reinterpret_cast<U64x2 *>(acc_rows), *acc1 = reinterpret_cast<U64x2 *>(acc_rows + N);
     U64x2 *out0 = reinterpret_cast<U64x2 *>(A.out + ct * 2 * P + (size_t)i * N);
@@ -399,7 +504,13 @@ DPFHE_HD void ks_phase1(CTA &cta, u64 *buf, const KsArgs &A, const LimbParams &p
     // chunk range [c_lo, c_lo + n_c) of the limb goes to shared-memory chunks [0, n_c)
     auto build = [&](int c_lo, int n_c) {
         cta.par([&](int tid) {
-            if (MODE == KS_MUL_RELIN) {
+            if constexpr (MODE == KS_DOT) {
+                // the pair loop runs inside a chunk position: three 128-bit sums per coefficient stay in registers (§4.15)
+                const size_t pos0 = ct * 2 * P + (size_t)i * N;
+#pragma unroll 1
+                for (int lc = tid; lc < n_c; lc += NT)
+                    ks_p1_dot_chunk(*dot, pos0 + 2 * (size_t)(c_lo + lc), P, ptr, p, buf, acc0, acc1, c_lo + lc, lc, pm, pm_s);
+            } else if (MODE == KS_MUL_RELIN) {
                 // No software prefetch for the tensor product: three co-resident CTAs hide the load latency, and a
                 // second operand set (32 registers) would push the 80-register kernel into spills (+5% instructions).
 #pragma unroll 1

@@ -791,10 +791,11 @@ __global__ void __launch_bounds__(NT, MINB) ks_hybrid_kernel(KsArgs A, const __g
 // With Lq = 4, K = 2 every CTA runs four transforms per ciphertext (24 in all, against 30 for one special prime).
 // ADD (KS_ROTATE only): the division step adds addend [batch][2][Lq][N] (canonical) to the result before its one store, so that a
 // Horner step of a linear layer, out = rot(acc) + inner_g, is one launch (DESIGN.md §4.4b′).  out must not alias a or addend.
-template <int LOGN, int NT, int MINB, int MODE, bool ADD = false>
-__global__ void __launch_bounds__(NT, MINB) ks_grouped_kernel(KsArgs A, const __grid_constant__ LimbTable lt, const __grid_constant__ MsConsts K,
-                                                              const __grid_constant__ GroupConsts G, size_t batch, u32 *flags, u32 epoch,
-                                                              u32 *ticket, u64 *mail, const u64 *addend) {
+// KS_DOT (DESIGN.md §2.18, §4.15): the limb CTAs build their digit from the summed tensor products of dot's pairs; everything after
+// phase 1 is the same program.  The body is shared by the two kernels below, which differ in their parameter block only.
+template <int LOGN, int NT, int MODE, bool ADD>
+__device__ __forceinline__ void ks_grouped_body(const KsArgs &A, const LimbTable &lt, const MsConsts &K, const GroupConsts &G, size_t batch, u32 *flags,
+                                                u32 epoch, u32 *ticket, u64 *mail, const u64 *addend, const DotArgs *dot) {
     static_assert(!ADD || MODE == KS_ROTATE, "the fused addition is a Horner step of rotations");
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     constexpr size_t N = (size_t)1 << LOGN;
@@ -855,7 +856,7 @@ __global__ void __launch_bounds__(NT, MINB) ks_grouped_kernel(KsArgs A, const __
         if (!special) {
             const u32 g_own = i / Ks;
             ks_phase1<LOGN, NT, MODE, true>(cta, buf, A, G.lp_up[i], ct, i, A.scratch + ((size_t)slot * 2 + parity) * N, acc_of(parity), K.qlm[i],
-                                            K.qlm_s[i], nullptr, 0, g_own);
+                                            K.qlm_s[i], nullptr, 0, g_own, dot);
             publish(tag);
             for (u32 jj = 1; jj < dnum; ++jj) {
                 const u32 g = (g_own + jj) % dnum, lo = g * Ks, cnt = lo + Ks < Lq ? Ks : Lq - lo;
@@ -880,6 +881,21 @@ __global__ void __launch_bounds__(NT, MINB) ks_grouped_kernel(KsArgs A, const __
         }
     }
     if (pending) divide(prev_ct, prev_tag, prev_parity);   // the group's last ciphertext
+}
+
+template <int LOGN, int NT, int MINB, int MODE, bool ADD = false>
+__global__ void __launch_bounds__(NT, MINB) ks_grouped_kernel(KsArgs A, const __grid_constant__ LimbTable lt, const __grid_constant__ MsConsts K,
+                                                              const __grid_constant__ GroupConsts G, size_t batch, u32 *flags, u32 epoch,
+                                                              u32 *ticket, u64 *mail, const u64 *addend) {
+    ks_grouped_body<LOGN, NT, MODE, ADD>(A, lt, K, G, batch, flags, epoch, ticket, mail, addend, nullptr);
+}
+
+// the encrypted inner product: ks_grouped_kernel's program in mode KS_DOT, with the operand tables of the call in D
+template <int LOGN, int NT, int MINB>
+__global__ void __launch_bounds__(NT, MINB) ct_dot_grouped_kernel(KsArgs A, const __grid_constant__ LimbTable lt, const __grid_constant__ MsConsts K,
+                                                                  const __grid_constant__ GroupConsts G, const __grid_constant__ DotArgs D,
+                                                                  size_t batch, u32 *flags, u32 epoch, u32 *ticket, u64 *mail) {
+    ks_grouped_body<LOGN, NT, KS_DOT, false>(A, lt, K, G, batch, flags, epoch, ticket, mail, nullptr, &D);
 }
 
 // Hoisted rotations with grouped hybrid keys, step 1 (DESIGN.md §2.11b): groups of L CTAs (every limb of the context) build
@@ -1634,9 +1650,11 @@ cudaError_t launch_ks_hybrid(LaunchCtx &lc, int mode, const u64 *a, const u64 *b
 #if DPFHE_PART_GROUPED
 template <int LOGN, int MODE, bool ADD = false>
 static cudaError_t launch_ks_grouped_t(LaunchCtx &lc, const KsArgs &A, const MsConsts &K, const GroupConsts &Gc, size_t batch, cudaStream_t st,
-                                       const u64 *addend) {
+                                       const u64 *addend, const DotArgs *dot = nullptr) {
     constexpr int NT = 256, MINB = 3;
-    auto kern = ks_grouped_kernel<LOGN, NT, MINB, MODE, ADD>;
+    const void *kern;
+    if constexpr (MODE == KS_DOT) kern = (const void *)ct_dot_grouped_kernel<LOGN, NT, MINB>;
+    else kern = (const void *)ks_grouped_kernel<LOGN, NT, MINB, MODE, ADD>;
     const size_t smem = LOGN <= 13 ? Geometry<LOGN>::LIMB_BYTES : Geometry<13>::LIMB_BYTES;
     static ConfiguredMask configured;
     if (!configured.has(lc.device)) {
@@ -1671,7 +1689,8 @@ static cudaError_t launch_ks_grouped_t(LaunchCtx &lc, const KsArgs &A, const MsC
     u64 *mail = lc.ks_mail;
     const u64 *add = addend;
     void *params[] = {&args, &lt, &consts, &gc, &batch_arg, &flags, &epoch, &ticket, &mail, &add};
-    e = cudaLaunchCooperativeKernel((void *)kern, dim3((unsigned)G), dim3(NT), params, smem, st);
+    void *params_dot[] = {&args, &lt, &consts, &gc, const_cast<DotArgs *>(dot), &batch_arg, &flags, &epoch, &ticket, &mail};
+    e = cudaLaunchCooperativeKernel(kern, dim3((unsigned)G), dim3(NT), MODE == KS_DOT ? params_dot : params, smem, st);
     lc.ks_epoch += rounds;
     return e;
 }
@@ -1711,6 +1730,36 @@ cudaError_t launch_ks_grouped(LaunchCtx &lc, int mode, const u64 *a, const u64 *
         case 12: KS_GRP_DISPATCH(12)
         case 13: KS_GRP_DISPATCH(13)
         case 14: KS_GRP_DISPATCH(14)
+    }
+    return cudaErrorNotSupported;
+}
+
+// out = relinearised sum of the n_terms tensor products a[t] x b[t] (DESIGN.md §2.18): launch_ks_grouped's launches with the limb
+// CTAs' phase 1 in mode KS_DOT.  a, b: host arrays of device pointers.
+cudaError_t launch_ct_dot_grouped(LaunchCtx &lc, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, u64 *out, size_t batch,
+                                  const MsConsts &K, const GroupConsts &Gc, cudaStream_t st, const u64 *key_s) {
+    if (batch == 0) return cudaSuccess;
+    if (lc.L < 2 || !lc.ks_hyb || !lc.ks_acc_hyb || Gc.Lq + Gc.K != lc.L || Gc.K > Gc.Lq || Gc.K > (u32)KS_MAX_SPECIAL) return cudaErrorInvalidValue;
+    if (n_terms < 1 || n_terms > (u32)DOT_MAX_TERMS) return cudaErrorInvalidValue;
+    if (!key_s) {
+        cudaError_t e = launch_key_prepare_grouped(lc, key, lc.ks_key_s, Gc.dnum, st);
+        if (e != cudaSuccess) return e;
+        key_s = lc.ks_key_s;
+    }
+    KsArgs A;
+    A.a = nullptr; A.b = nullptr; A.key = key; A.key_s = key_s; A.out = out; A.scratch = lc.ks_scratch;
+    A.tw = lc.tw; A.itw = lc.itw; A.L = Gc.Lq; A.galois = 0; A.Lk = lc.L; A.hyb = lc.ks_hyb; A.only = nullptr;
+    A.acc = lc.ks_acc_hyb; A.acc_par = 2; A.lift_reduce = 0u;
+    DotArgs D{};
+    D.n_terms = n_terms;
+    for (u32 t = 0; t < n_terms; ++t) {
+        D.a[t] = a[t];
+        D.b[t] = b[t];
+    }
+    switch (lc.log_n) {
+        case 12: return launch_ks_grouped_t<12, KS_DOT>(lc, A, K, Gc, batch, st, nullptr, &D);
+        case 13: return launch_ks_grouped_t<13, KS_DOT>(lc, A, K, Gc, batch, st, nullptr, &D);
+        case 14: return launch_ks_grouped_t<14, KS_DOT>(lc, A, K, Gc, batch, st, nullptr, &D);
     }
     return cudaErrorNotSupported;
 }

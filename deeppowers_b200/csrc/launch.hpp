@@ -60,6 +60,8 @@ struct LaunchCtx {
     cudaError_t launch_ks_grouped(LaunchCtx &lc, int mode, const u64 *a, const u64 *b, const u64 *key, u64 *out, size_t batch, u32 galois, \
                                   const MsConsts &K, const GroupConsts &G, cudaStream_t st, const u64 *addend = nullptr, \
                                   const u64 *key_s = nullptr); \
+    cudaError_t launch_ct_dot_grouped(LaunchCtx &lc, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, u64 *out, size_t batch, \
+                                      const MsConsts &K, const GroupConsts &G, cudaStream_t st, const u64 *key_s = nullptr); \
     cudaError_t launch_hoist_grouped(LaunchCtx &lc, const u64 *ct, u64 *U, const GroupConsts &G, size_t batch, cudaStream_t st); \
     cudaError_t launch_key_prepare_grouped(const LaunchCtx &lc, const u64 *key, u64 *key_s, u32 dnum, cudaStream_t st); \
     cudaError_t launch_rot_apply_grouped(LaunchCtx &lc, const u64 *ct, const u64 *U, const u64 *key, const u64 *key_s, u32 galois, u64 *acc, \
@@ -104,6 +106,7 @@ DPFHE_DECLARE_LAUNCHERS
 // (or, with key_s == nullptr, in lc.ks_key_s).  launch_rot_prepare / launch_rot_apply: key_s(_out) == nullptr means lc.ks_key_s.
 // launch_ks_grouped: key_s == nullptr builds the companions into lc.ks_key_s (two launches), otherwise one launch; addend (KS_ROTATE
 // only) is added to the result in the kernel's final store.
+// launch_ct_dot_grouped: a[t] / b[t] of n_terms (1 .. DOT_MAX_TERMS) pairs, host arrays of device pointers; key_s as launch_ks_grouped.
 // launch_rot_sum_grouped: keys[m] / key_s[m] / galois[m] of n_rot (1 .. ROT_SUM_MAX) rotations; the companions are required.
 
 }  // namespace dpfhe

@@ -173,7 +173,9 @@ struct KeyArgs {
     u64 *out;                     // secret [L][N], keys [n_elts][ndig][2][L][N], public key [2][L][N], ciphertexts [n][2][L][N]
 };
 
-enum KsMode { KS_MUL_RELIN = 0, KS_PLAIN = 1, KS_ROTATE = 2 };
+// KS_DOT (grouped keys only, DESIGN.md §2.18): the digit is the third component of a SUM of tensor products
+enum KsMode { KS_MUL_RELIN = 0, KS_PLAIN = 1, KS_ROTATE = 2, KS_DOT = 3 };
+constexpr int DOT_MAX_TERMS = 64;   // pairs of one encrypted inner product
 // tau' rows of a hybrid key-switching group are double-buffered by round parity (the division step runs one round late)
 constexpr int KS_HYB_ROWS = 6;
 

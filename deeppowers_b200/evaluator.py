@@ -478,6 +478,24 @@ class Context:
         self._chk(self._l.dpfhe_rotate_sum_grouped_host(self._h, int(n_special), _hptr(ct), n, ge, _hptr(gks), _hptr(out, True), ct.size // pq,
                                                         int(t_plain)))
 
+    def ct_dot_grouped(self, n_special, a_list, b_list, evk, out, batch, t_plain=0, stream=None):
+        """out = the relinearised sum of the tensor products a_list[i] x b_list[i] (DESIGN.md section 2.18): 1 .. 64 pairs of device
+        tensors [batch][2][L-n_special][N], one key switch for the sum; a pair may name one tensor twice and a tensor may appear
+        in several pairs, out must not overlap any of them"""
+        n = len(a_list)
+        if len(b_list) != n:
+            raise ValueError("need as many right operands as left operands")
+        pa = (C.c_void_p * max(n, 1))(*[_ptr(x) for x in a_list])
+        pb = (C.c_void_p * max(n, 1))(*[_ptr(x) for x in b_list])
+        self._chk(self._l.dpfhe_ct_dot_grouped(self._h, int(n_special), n, pa, pb, _ptr(evk), _ptr(out), batch, int(t_plain), _stream(stream)))
+
+    def ct_dot_grouped_host(self, n_special, a, b, evk, out, t_plain=0):
+        """host form of ct_dot_grouped: a, b [n_terms][batch][2][L-n_special][N] (C-contiguous numpy uint64)"""
+        n = a.shape[0]
+        pq = 2 * (self.L - n_special) * self.N
+        self._chk(self._l.dpfhe_ct_dot_grouped_host(self._h, int(n_special), n, _hptr(a), _hptr(b), _hptr(evk), _hptr(out, True),
+                                                    a.size // (n * pq) if n else 0, int(t_plain)))
+
     def mod_down_special(self, n_special, polys, out, n_polys, t_plain=0, stream=None):
         self._chk(self._l.dpfhe_mod_down_special(self._h, int(n_special), _ptr(polys), _ptr(out), n_polys, int(t_plain), _stream(stream)))
 

@@ -256,6 +256,20 @@ public:
         for (std::size_t r = 0; r < steps.size(); ++r) elts[r] = galois_element(steps[r]);
         check(dpfhe_rotate_sum_grouped(ctx_, special, ct, steps.size(), elts.data(), galois_keys.data(), out, count, plain_modulus, stream));
     }
+    // out = the relinearised sum of the products a[i] x b[i] (1 .. 64 pairs, DESIGN.md §2.18): the tensor products are summed
+    // before ONE key switch and one division by P.  a[i] and b[i] may be the same batch, a batch may appear in several pairs; out
+    // must not overlap any of them.  One pair is multiply_relin_grouped, bit for bit.  Host buffers (pipelined) need the pairs back
+    // to back, so the host form takes the two operand arrays [n_terms][count] directly; the device form takes one batch per term.
+    void dot_relin_grouped(unsigned special, std::size_t n_terms, const std::uint64_t *a, const std::uint64_t *b, const std::uint64_t *relin_key,
+                           CiphertextBatch out, std::uint64_t plain_modulus = 0) {
+        check(dpfhe_ct_dot_grouped_host(ctx_, special, n_terms, a, b, relin_key, out.data, out.count, plain_modulus));
+    }
+    void dot_relin_grouped_device(unsigned special, const std::vector<const std::uint64_t *> &a, const std::vector<const std::uint64_t *> &b,
+                                  const std::uint64_t *relin_key, std::uint64_t *out, std::size_t count, std::uint64_t plain_modulus = 0,
+                                  void *stream = nullptr) {
+        if (a.size() != b.size()) throw std::invalid_argument("one right operand per left operand");
+        check(dpfhe_ct_dot_grouped(ctx_, special, a.size(), a.data(), b.data(), relin_key, out, count, plain_modulus, stream));
+    }
     // divide by the product of the last `special` limbs: in holds limbs() limbs per polynomial, out limbs()-special
     void mod_down_special_device(unsigned special, const std::uint64_t *ct, std::uint64_t *out, std::size_t count, std::uint64_t plain_modulus = 0,
                                  void *stream = nullptr) {

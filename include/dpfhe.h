@@ -264,6 +264,21 @@ int dpfhe_rotate_sum_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t 
 /* host-buffer form: h_gks [n_rot][dnum][2][L][N] back to back, uploaded once; the batch pipelined in chunks (synchronous) */
 int dpfhe_rotate_sum_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_ct, size_t n_rot, const uint64_t *galois_elts,
                                   const uint64_t *h_gks, uint64_t *h_out, size_t batch, uint64_t t_plain);
+/* Encrypted inner product (DESIGN.md §2.18): d_out = relinearise(sum_i d_as[i] x d_bs[i]) for n_terms = 1 .. 64 pairs of
+ * ciphertext batches [batch][2][L-K][N].  The three-component tensor products are summed exactly and key-switched ONCE: 24
+ * transforms, one pass over the key and one division by P per output ciphertext at Lq = 4, K = 2, whatever n_terms is.
+ * n_terms = 1 is dpfhe_ct_mul_relin_grouped, bit for bit; any n_terms is, bit for bit, dpfhe_ct_tensor per pair summed with
+ * dpfhe_poly_add, dpfhe_keyswitch_grouped of the third component, and dpfhe_poly_add of the first two.  It is not the bits of
+ * n_terms separate dpfhe_ct_mul_relin_grouped results summed (those round n_terms times) but decrypts to the same plaintext, with
+ * one key-switching noise term instead of n_terms.  d_as, d_bs: HOST arrays of n_terms device pointers; d_as[i] and d_bs[i] may be
+ * the same buffer (a sum of squares) and a buffer may appear in several pairs; d_out must not overlap any of them.  The sum of the
+ * products must still fit the plaintext space (t for BGV, the scale budget for CKKS); the library does not check it.  Argument
+ * checks of dpfhe_ct_mul_relin_grouped, plus n_terms and every table entry.  Two launches (key companions + kernel). */
+int dpfhe_ct_dot_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *const *d_as, const uint64_t *const *d_bs,
+                         const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream);
+/* host-buffer form: h_as, h_bs [n_terms][batch][2][L-K][N]; the key uploaded once, the batch pipelined in chunks (synchronous) */
+int dpfhe_ct_dot_grouped_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs,
+                              const uint64_t *h_evk, uint64_t *h_out, size_t batch, uint64_t t_plain);
 /* ---- slot sums (DESIGN.md §2.17): slot i of the result is sum_{j < count} x[(i + j * stride) mod N/2] in every row, count =
  *      prod radices[t], computed in n_stages (1 .. 16) summed-rotation stages; stage t rotates by m * stride * prod_{u<t} radices[u],
  *      m = 1 .. radices[t] - 1 (2 <= radices[t] <= 16), and stride * count must be at most N/2.
