@@ -513,6 +513,7 @@ void dpfhe_context_destroy(dpfhe_ctx *ctx) {
     cudaFree(ctx->lc.ks_mail);
     cudaFree(ctx->lc.ks_prof);
     cudaFree(ctx->lc.ks_hyb);
+    cudaFree(ctx->lc.ks_tau_drop);
     for (int k = 0; k < PIPE_DEPTH; ++k) {
         if (ctx->ev_h2d[k]) cudaEventDestroy(ctx->ev_h2d[k]);
         if (ctx->ev_comp[k]) cudaEventDestroy(ctx->ev_comp[k]);
@@ -722,25 +723,37 @@ int dpfhe_rotate_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_c
                          size_t batch, uint64_t t_plain, void *stream) {
     return ks_hybrid_common(ctx, n_special, KS_ROTATE, d_ct, nullptr, d_gk, d_out, batch, galois_elt, t_plain, stream);
 }
+// The argument checks of a call on n_terms operand pairs (d_as[i], d_bs[i]) [batch][2][Lq][N] with grouped keys, in this order: the
+// pair table, the key and output pointers, check() (the call's own checks of n_special and t_plain), then, for a non-empty batch, the
+// output [batch][2][Lq - drop][N] against every operand: the output rows are written while other work items still read their inputs,
+// so no overlap at all.  An empty batch passes once the checks before the overlap have.
+extern "C++" {   // a template inside the C entry points' linkage block
+template <class Check>
+static int check_pairs(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *const *d_as, const uint64_t *const *d_bs,
+                       const uint64_t *d_evk, uint64_t *d_out, size_t batch, unsigned drop, Check check) {
+    if (n_terms < 1 || n_terms > (size_t)DOT_MAX_TERMS) return fail(DPFHE_ERR_INVALID, "n_terms must be in [1, %d]", DOT_MAX_TERMS);
+    if (!d_as || !d_bs) return fail(DPFHE_ERR_INVALID, "null argument");
+    for (size_t i = 0; i < n_terms; ++i)
+        if (!d_as[i] || !d_bs[i] || !aligned16(d_as[i]) || !aligned16(d_bs[i])) return fail(DPFHE_ERR_INVALID, "null or misaligned operand of pair %zu", i);
+    CHECK_PTR(d_evk); CHECK_PTR(d_out);
+    const int rc = check();
+    if (rc || batch == 0) return rc;
+    const size_t Lq = ctx->hp.L - n_special, in_bytes = batch * 2 * Lq * ctx->N() * 8, out_bytes = batch * 2 * (Lq - drop) * ctx->N() * 8;
+    for (size_t i = 0; i < n_terms; ++i)
+        if (overlaps(d_out, out_bytes, d_as[i], in_bytes) || overlaps(d_out, out_bytes, d_bs[i], in_bytes))
+            return fail(DPFHE_ERR_INVALID, "output must not overlap an operand (pair %zu)", i);
+    return DPFHE_OK;
+}
+}
+
 // Encrypted inner product (DESIGN.md §2.18): the tensor products of n_terms pairs summed before one relinearisation.  Every
 // n_special runs the grouped kernel (with one special prime its digits are single limbs and it computes what the hybrid kernel does).
 int dpfhe_ct_dot_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *const *d_as, const uint64_t *const *d_bs,
                          const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
-    if (n_terms < 1 || n_terms > (size_t)DOT_MAX_TERMS) return fail(DPFHE_ERR_INVALID, "n_terms must be in [1, %d]", DOT_MAX_TERMS);
-    if (!d_as || !d_bs) return fail(DPFHE_ERR_INVALID, "null argument");
-    for (size_t i = 0; i < n_terms; ++i)
-        if (!d_as[i] || !d_bs[i] || !aligned16(d_as[i]) || !aligned16(d_bs[i])) return fail(DPFHE_ERR_INVALID, "null or misaligned operand of pair %zu", i);
-    CHECK_PTR(d_evk); CHECK_PTR(d_out);
-    rc = check_grouped(ctx, n_special, t_plain);
-    if (rc) return rc;
-    if (batch == 0) return DPFHE_OK;
-    // the output rows are written while other work items still read their inputs: no overlap at all
-    const size_t ct_bytes = batch * 2 * (size_t)(ctx->hp.L - n_special) * ctx->N() * 8;
-    for (size_t i = 0; i < n_terms; ++i)
-        if (overlaps(d_out, ct_bytes, d_as[i], ct_bytes) || overlaps(d_out, ct_bytes, d_bs[i], ct_bytes))
-            return fail(DPFHE_ERR_INVALID, "output must not overlap an operand (pair %zu)", i);
+    rc = check_pairs(ctx, n_special, n_terms, d_as, d_bs, d_evk, d_out, batch, 0, [&] { return check_grouped(ctx, n_special, t_plain); });
+    if (rc || batch == 0) return rc;
     rc = ensure_hyb(ctx);
     if (rc) return rc;
     MsConsts K;
@@ -749,6 +762,58 @@ int dpfhe_ct_dot_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, con
     CU_TRY(VCALL(launch_ct_dot_grouped, ctx->lc, d_as, d_bs, (u32)n_terms, d_evk, d_out, batch, K, G, pick(ctx, stream)));
     note_launch(ctx, 2);   // key_prepare_kernel + ct_dot_grouped_kernel
     return DPFHE_OK;
+}
+
+// the dropped limb's y_qbar rows of multiply-and-rescale (DESIGN.md §4.16), allocated at the first such call: one block of
+// [2 parities][2][N] per group of the grid, whose groups have L >= 3 CTAs
+static int ensure_tau_drop(dpfhe_ctx *ctx) {
+    if (ctx->lc.ks_tau_drop) return DPFHE_OK;
+    u64 *rows = nullptr;
+    const size_t bytes = (ctx->lc.ks_slots / 3 + 1) * 4 * ctx->N() * sizeof(u64);
+    CU_TRY(cudaMalloc(&rows, bytes));
+    ctx->lc.ks_tau_drop = rows;
+    ctx->device_bytes += bytes;
+    return DPFHE_OK;
+}
+
+// the checks of a multiply-and-rescale call beyond its operands: those of the grouped product, at least two ciphertext limbs (one
+// is kept) and t_plain below the dropped modulus as well as the special primes
+static int check_rescale(const dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain) {
+    int rc = check_grouped(ctx, n_special, t_plain);
+    if (rc) return rc;
+    if (ctx->hp.L - n_special < 2)
+        return fail(DPFHE_ERR_INVALID, "multiply-and-rescale needs at least two ciphertext limbs: the context has %u limbs, %u of them special",
+                    ctx->hp.L, n_special);
+    return check_t_below_special(ctx, n_special + 1, t_plain, "the special primes and the dropped modulus");
+}
+
+// Multiply-and-rescale (DESIGN.md §2.19): dot = false is the ct x ct product of d_as[0] and d_bs[0] (n_terms = 1), dot = true the
+// inner product of n_terms pairs; relinearised and divided by P * q_{Lq-1} in one kernel.  out: [batch][2][Lq-1][N].
+static int rescale_common(dpfhe_ctx *ctx, unsigned n_special, bool dot, size_t n_terms, const uint64_t *const *d_as, const uint64_t *const *d_bs,
+                          const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    rc = check_pairs(ctx, n_special, n_terms, d_as, d_bs, d_evk, d_out, batch, 1, [&] { return check_rescale(ctx, n_special, t_plain); });
+    if (rc || batch == 0) return rc;
+    rc = ensure_hyb(ctx);
+    if (rc) return rc;
+    rc = ensure_tau_drop(ctx);
+    if (rc) return rc;
+    MsConsts K;
+    GroupConsts G;
+    RescaleConsts R;
+    build_rescale_consts(ctx->hp, n_special, t_plain, G, K, R);
+    CU_TRY(VCALL(launch_ks_rescale_grouped, ctx->lc, dot, d_as, d_bs, (u32)n_terms, d_evk, d_out, batch, K, G, R, pick(ctx, stream)));
+    note_launch(ctx, 2);   // key_prepare_kernel + ks_rescale_grouped_kernel
+    return DPFHE_OK;
+}
+int dpfhe_ct_mul_relin_rescale_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_a, const uint64_t *d_b, const uint64_t *d_evk,
+                                       uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+    return rescale_common(ctx, n_special, false, 1, &d_a, &d_b, d_evk, d_out, batch, t_plain, stream);
+}
+int dpfhe_ct_dot_rescale_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *const *d_as, const uint64_t *const *d_bs,
+                                 const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+    return rescale_common(ctx, n_special, true, n_terms, d_as, d_bs, d_evk, d_out, batch, t_plain, stream);
 }
 
 int dpfhe_grouped_digits(const dpfhe_ctx *ctx, unsigned n_special, unsigned *digits) {
@@ -1149,19 +1214,23 @@ int dpfhe_ct_mul_relin_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const ui
                      [&] { return check_special(ctx, n_special); });
 }
 
-// host form of the inner product: the key uploaded once, the batch pipelined in chunks, each chunk uploading its ciphertexts of
-// every pair.  A chunk stages 2 n_terms operands per ciphertext, so its size is budgeted on all of them; where the batch allows,
-// it is a whole number of rounds of the persistent grid.
-int dpfhe_ct_dot_grouped_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs, const uint64_t *h_evk,
-                              uint64_t *h_out, size_t batch, uint64_t t_plain) {
+// Host form of a call on operand pairs (the inner product, multiply-and-rescale): h_as, h_bs [n_terms][batch][2][Lq][N], h_out
+// [batch][2][Lq - drop][N].  The key is uploaded once and the batch pipelined in chunks, each chunk uploading its ciphertexts of
+// every pair.  A chunk stages 2 n_terms operands per ciphertext, so its size is budgeted on all of them; where the batch allows, it
+// is a whole number of rounds of the persistent grid.  check(): the call's own checks of n_special and t_plain; call(as, bs, dout,
+// cnt, st): the device form on one chunk.
+extern "C++" {   // a template inside the C entry points' linkage block
+template <class Check, class Call>
+static int pairs_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs, const uint64_t *h_evk,
+                      uint64_t *h_out, size_t batch, unsigned drop, Check check, Call call) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (n_terms < 1 || n_terms > (size_t)DOT_MAX_TERMS) return fail(DPFHE_ERR_INVALID, "n_terms must be in [1, %d]", DOT_MAX_TERMS);
     if (!h_as || !h_bs || !h_evk || !h_out) return fail(DPFHE_ERR_INVALID, "null host pointer");
-    rc = check_grouped(ctx, n_special, t_plain);
+    rc = check();
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
-    const size_t ctw = 2 * (size_t)(ctx->hp.L - n_special) * ctx->N();   // words of a ciphertext
+    const size_t Lq = ctx->hp.L - n_special, ctw = 2 * Lq * ctx->N(), outw = 2 * (Lq - drop) * ctx->N();   // words of an operand / output
     rc = upload_key(ctx, h_evk, 2 * key_digits(ctx, n_special) * ctx->P());
     if (rc) return rc;
     size_t chunk = std::max<size_t>(1, ((size_t)64 << 20) / (n_terms * ctw * 8));   // ~64 MiB per staged operand side, as pick_chunk
@@ -1169,16 +1238,42 @@ int dpfhe_ct_dot_grouped_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms
     if (chunk > round) chunk -= chunk % round;
     if (chunk > batch) chunk = batch;
     return run_pipeline(
-        ctx, h_as, h_bs, h_out, batch, ctw, ctw, chunk,
+        ctx, h_as, h_bs, h_out, batch, ctw, outw, chunk,
         [&](u64 *da, u64 *db, u64 *dout, size_t cnt, cudaStream_t st) {
             const u64 *as[DOT_MAX_TERMS], *bs[DOT_MAX_TERMS];
             for (size_t t = 0; t < n_terms; ++t) {
                 as[t] = da + t * chunk * ctw;
                 bs[t] = db + t * chunk * ctw;
             }
-            return dpfhe_ct_dot_grouped(ctx, n_special, n_terms, as, bs, ctx->stage_key.get(), dout, cnt, t_plain, st);
+            return call(as, bs, dout, cnt, st);
         },
         n_terms, batch * ctw);
+}
+}
+
+int dpfhe_ct_dot_grouped_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs, const uint64_t *h_evk,
+                              uint64_t *h_out, size_t batch, uint64_t t_plain) {
+    return pairs_host(ctx, n_special, n_terms, h_as, h_bs, h_evk, h_out, batch, 0, [&] { return check_grouped(ctx, n_special, t_plain); },
+                      [&](const u64 *const *as, const u64 *const *bs, u64 *dout, size_t cnt, cudaStream_t st) {
+                          return dpfhe_ct_dot_grouped(ctx, n_special, n_terms, as, bs, ctx->stage_key.get(), dout, cnt, t_plain, st);
+                      });
+}
+
+// host forms of multiply-and-rescale: the pipeline of the inner product's, with Lq - 1 limbs per output ciphertext
+static int rescale_host(dpfhe_ctx *ctx, unsigned n_special, bool dot, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs, const uint64_t *h_evk,
+                        uint64_t *h_out, size_t batch, uint64_t t_plain) {
+    return pairs_host(ctx, n_special, n_terms, h_as, h_bs, h_evk, h_out, batch, 1, [&] { return check_rescale(ctx, n_special, t_plain); },
+                      [&](const u64 *const *as, const u64 *const *bs, u64 *dout, size_t cnt, cudaStream_t st) {
+                          return rescale_common(ctx, n_special, dot, n_terms, as, bs, ctx->stage_key.get(), dout, cnt, t_plain, st);
+                      });
+}
+int dpfhe_ct_mul_relin_rescale_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_a, const uint64_t *h_b, const uint64_t *h_evk,
+                                            uint64_t *h_out, size_t batch, uint64_t t_plain) {
+    return rescale_host(ctx, n_special, false, 1, h_a, h_b, h_evk, h_out, batch, t_plain);
+}
+int dpfhe_ct_dot_rescale_grouped_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs,
+                                      const uint64_t *h_evk, uint64_t *h_out, size_t batch, uint64_t t_plain) {
+    return rescale_host(ctx, n_special, true, n_terms, h_as, h_bs, h_evk, h_out, batch, t_plain);
 }
 
 int dpfhe_rotate_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_ct, uint64_t galois_elt, const uint64_t *h_gk,

@@ -254,6 +254,49 @@ void build_group_consts(const HostParams &hp, unsigned K, uint64_t t_plain, Grou
     }
 }
 
+void build_rescale_consts(const HostParams &hp, unsigned K, uint64_t t_plain, GroupConsts &G, MsConsts &Km, RescaleConsts &R) {
+    typedef unsigned __int128 u128;
+    auto shoup = [](uint64_t w, uint64_t q) { return (uint64_t)((((u128)w) << 64) / q); };
+    build_group_consts(hp, K, t_plain, G, Km);
+    const unsigned L = hp.L, Lq = L - K, d = Lq - 1;   // d: the dropped limb
+    const uint64_t qbar = hp.limbs[d].lp.q;
+    auto fold = [&](LimbParams p, uint64_t f) {   // N^-1 replaced by N^-1 * f
+        p.ninv = host_mulmod(p.ninv, f, p.q);
+        p.ninv_s = shoup(p.ninv, p.q);
+        p.wninv = host_mulmod(p.wninv, f, p.q);
+        p.wninv_s = shoup(p.wninv, p.q);
+        return p;
+    };
+    // special k: Phat'_k = Phat_k * qbar, so its N^-1 takes a further qbar^-1
+    for (unsigned k = 0; k < K; ++k) {
+        const uint64_t p = hp.limbs[Lq + k].lp.q;
+        G.lp_up[Lq + k] = fold(G.lp_up[Lq + k], host_powmod(qbar % p, p - 2, p));
+    }
+    // the dropped limb: Phat'_qbar = P, y_qbar = INTT(acc) * (t P)^-1 mod qbar
+    uint64_t P_qbar = 1;
+    for (unsigned k = 0; k < K; ++k) P_qbar = host_mulmod(P_qbar, hp.limbs[Lq + k].lp.q % qbar, qbar);
+    const uint64_t f = t_plain ? host_mulmod(P_qbar, t_plain % qbar, qbar) : P_qbar;
+    R = RescaleConsts();
+    R.lp_drop = fold(hp.limbs[d].lp, host_powmod(f, qbar - 2, qbar));
+    R.half = qbar >> 1;
+    for (unsigned i = 0; i < 16; ++i) G.neg_p[i] = 0, Km.inv[i] = Km.inv_s[i] = Km.sinv[i] = Km.sinv_s[i] = 0;
+    for (unsigned k = 0; k < K; ++k) G.dn[k][d] = G.dn_s[k][d] = 0;
+    for (unsigned i = 0; i < d; ++i) {
+        const uint64_t q = hp.limbs[i].lp.q, Pm = Km.qlm[i], Ppm = host_mulmod(Pm, qbar % q, q);   // P mod q_i, P' mod q_i
+        for (unsigned k = 0; k < K; ++k) {
+            G.dn[k][i] = host_mulmod(G.dn[k][i], qbar % q, q);
+            G.dn_s[k][i] = shoup(G.dn[k][i], q);
+        }
+        R.dn[i] = Pm;
+        R.dn_s[i] = shoup(Pm, q);
+        G.neg_p[i] = q - Ppm;
+        Km.inv[i] = host_powmod(Ppm, q - 2, q);
+        Km.inv_s[i] = shoup(Km.inv[i], q);
+        Km.sinv[i] = t_plain ? host_mulmod(t_plain % q, Km.inv[i], q) : Km.inv[i];
+        Km.sinv_s[i] = shoup(Km.sinv[i], q);
+    }
+}
+
 // ---- CKKS slot encoding (DESIGN.md §2.12) ----------------------------------------------------------------------
 // cos and sin of pi k / N in fixed point with 126 fractional bits (Taylor series, error below 2^-120), rounded once to double.
 namespace {

@@ -33,6 +33,10 @@ void build_ms_consts(const HostParams &hp, uint64_t t_plain, MsConsts &K);
 // constants of grouped hybrid key switching with the last K limbs of `hp` as special primes (types.hpp: GroupConsts); Km
 // receives the constants of the division by P.  Requires 1 <= K <= KS_MAX_SPECIAL, K < hp.L, t_plain < every special prime.
 void build_group_consts(const HostParams &hp, unsigned K, uint64_t t_plain, GroupConsts &G, MsConsts &Km);
+// multiply-and-rescale (DESIGN.md §2.19): the constants of the division by P' = P * qbar, qbar = q_{L-K-1} the last ciphertext modulus:
+// G and Km as build_group_consts would build them for P', and R the dropped limb's row (its pointers stay null: the launcher sets
+// them).  Requires what build_group_consts does, L - K >= 2 and t_plain < qbar.
+void build_rescale_consts(const HostParams &hp, unsigned K, uint64_t t_plain, GroupConsts &G, MsConsts &Km, RescaleConsts &R);
 
 // CKKS slot encoding (DESIGN.md §2.12): the twiddles (cos, sin)(pi k / N), k < N, each correctly rounded; the slot
 // permutation t_j, j < N/2; and 2^e mod q_l, [L][CKKS_POW2_E]

@@ -1045,14 +1045,18 @@ DPFHE_HD void ms_limb_body(CTA &cta, u64 *buf, const u64 *tau, const u64 *c_limb
 
 // division by the product P of K special primes (DESIGN.md §2.11): tau_rows + k * tau_stride is y_k = tau'_k * Phat_k^-1 of
 // special prime k; the value to subtract is sum_k centred(y_k) * Phat_k, converted term by term.  ADD / add_limb: as ms_limb_core.
-template <int LOGN, int NT, bool COHERENT = true, bool ADD = false, class CTA>
+// DROP (multiply-and-rescale, DESIGN.md §2.19 / §4.16): the divided set has a fifth row, y_qbar of the dropped limb in drop_row, with
+// its own constants in R (P mod q_i, floor(qbar / 2)); G and K then describe P' = P * qbar.  K + 1 terms: the per-term reduction
+// holds up to five (15q < 16q), and the slim form up to three.
+template <int LOGN, int NT, bool COHERENT = true, bool ADD = false, bool DROP = false, class CTA>
 DPFHE_HD void ms_limb_group(CTA &cta, u64 *buf, const u64 *tau_rows, size_t tau_stride, const u64 *c_limb, u64 *out_limb, const Twiddle *tw,
-                            const LimbParams &p, const MsConsts &K, const GroupConsts &G, u32 i, const u64 *add_limb = nullptr) {
+                            const LimbParams &p, const MsConsts &K, const GroupConsts &G, u32 i, const u64 *add_limb = nullptr,
+                            const u64 *drop_row = nullptr, const RescaleConsts *R = nullptr) {
     const u64 neg_p = G.neg_p[i];
     auto lift = [&](int c) {
         U64x2 r;
         r.x = r.y = 0;
-        const bool slim = G.K <= 3;   // terms below SB*q + q = 5q: three of them stay below 16q, four need the per-term reduction (3q each)
+        const bool slim = G.K + (DROP ? 1u : 0u) <= 3;   // terms below SB*q + q = 5q: three of them stay below 16q, four or five need the per-term reduction (3q each)
         for (u32 k = 0; k < G.K; ++k) {
             const U64x2 v = ld_cg(reinterpret_cast<const U64x2 *>(tau_rows + (size_t)k * tau_stride) + c);
             u64 tx = shoup_lazy(v.x, G.dn[k][i], G.dn_s[k][i], p), ty = shoup_lazy(v.y, G.dn[k][i], G.dn_s[k][i], p);
@@ -1062,6 +1066,16 @@ DPFHE_HD void ms_limb_group(CTA &cta, u64 *buf, const u64 *tau_rows, size_t tau_
             }
             r.x += tx + (v.x > G.half[k] ? neg_p : 0);
             r.y += ty + (v.y > G.half[k] ? neg_p : 0);
+        }
+        if constexpr (DROP) {   // the fifth row: the same term with the dropped limb's constants
+            const U64x2 v = ld_cg(reinterpret_cast<const U64x2 *>(drop_row) + c);
+            u64 tx = shoup_lazy(v.x, R->dn[i], R->dn_s[i], p), ty = shoup_lazy(v.y, R->dn[i], R->dn_s[i], p);
+            if (!slim) {
+                tx = csub(tx, p.q2);
+                ty = csub(ty, p.q2);
+            }
+            r.x += tx + (v.x > R->half ? neg_p : 0);
+            r.y += ty + (v.y > R->half ? neg_p : 0);
         }
         r.x = csub(csub(r.x, p.q8), p.q4);   // < 16q  ->  < 4q
         r.y = csub(csub(r.y, p.q8), p.q4);

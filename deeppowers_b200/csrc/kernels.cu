@@ -792,11 +792,17 @@ __global__ void __launch_bounds__(NT, MINB) ks_hybrid_kernel(KsArgs A, const __g
 // ADD (KS_ROTATE only): the division step adds addend [batch][2][Lq][N] (canonical) to the result before its one store, so that a
 // Horner step of a linear layer, out = rot(acc) + inner_g, is one launch (DESIGN.md §4.4b′).  out must not alias a or addend.
 // KS_DOT (DESIGN.md §2.18, §4.15): the limb CTAs build their digit from the summed tensor products of dot's pairs; everything after
-// phase 1 is the same program.  The body is shared by the two kernels below, which differ in their parameter block only.
-template <int LOGN, int NT, int MODE, bool ADD>
+// phase 1 is the same program.  The body is shared by the kernels below, which differ in their parameter block only.
+// RS (multiply-and-rescale, DESIGN.md §2.19, §4.16; modes KS_MUL_RELIN and KS_DOT): the division is by P' = P * qbar, qbar = q_{Lq-1}.
+// The dropped limb's CTA runs phases 1 and 2 as before, then turns its accumulator rows into y_qbar as a special CTA does (inverse
+// transform, (t P)^-1 folded into N^-1) and publishes them on its group's flag in R; it divides nothing and stores no output.  The
+// other limb CTAs divide one round late over K + 1 rows and write [batch][2][Lq-1][N].
+template <int LOGN, int NT, int MODE, bool ADD, bool RS = false>
 __device__ __forceinline__ void ks_grouped_body(const KsArgs &A, const LimbTable &lt, const MsConsts &K, const GroupConsts &G, size_t batch, u32 *flags,
-                                                u32 epoch, u32 *ticket, u64 *mail, const u64 *addend, const DotArgs *dot) {
+                                                u32 epoch, u32 *ticket, u64 *mail, const u64 *addend, const DotArgs *dot,
+                                                const RescaleConsts *R = nullptr) {
     static_assert(!ADD || MODE == KS_ROTATE, "the fused addition is a Horner step of rotations");
+    static_assert(!RS || (!ADD && (MODE == KS_MUL_RELIN || MODE == KS_DOT)), "multiply-and-rescale follows a product");
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     constexpr size_t N = (size_t)1 << LOGN;
     u64 *buf = reinterpret_cast<u64 *>(smem_raw);
@@ -820,8 +826,24 @@ __device__ __forceinline__ void ks_grouped_body(const KsArgs &A, const LimbTable
         if (threadIdx.x == 0) st_release_u32(flags + slot, tag);
     };
     auto acc_of = [&](u32 parity) { return A.acc + ((size_t)slot * 2 + parity) * 2 * N; };
+    // y_qbar row c of round parity `parity` (RS)
+    auto drop_of = [&](u32 parity, u32 c) { return R->tau + (((size_t)group * 2 + parity) * 2 + c) * N; };
     auto divide = [&](size_t ct, u32 tag, u32 parity) {
+        if constexpr (RS) {
+            if (threadIdx.x == 0) {
+                while ((int)(ld_acquire_u32(R->tau_flag + group) - tag) < 0) {
+                }
+            }
+        }
         wait_for(base + Lq, Ks, tag);
+        if constexpr (RS) {
+            const size_t P = (size_t)(Lq - 1) * N;
+            for (u32 c = 0; c < 2; ++c)
+                ms_limb_group<LOGN, NT, true, false, true>(cta, buf, hyb_of(0) + ks_hyb_tau_row(parity, c) * N, (size_t)KS_HYB_ROWS * N, acc_of(parity) + c * N,
+                                                           A.out + ct * 2 * P + c * P + (size_t)i * N, A.tw + (size_t)i * N, p, K, G, i, nullptr,
+                                                           drop_of(parity, c), R);
+            return;
+        }
         const size_t P = (size_t)Lq * N;
         for (u32 c = 0; c < 2; ++c) {
             u64 *row = A.out + ct * 2 * P + c * P + (size_t)i * N;
@@ -863,6 +885,21 @@ __device__ __forceinline__ void ks_grouped_body(const KsArgs &A, const LimbTable
                 wait_for(base + lo, cnt, tag);
                 ks_phase2_group<LOGN, NT, false>(cta, buf, A, G, p, ct, i, g, jj, t_rows, 2 * N, acc_of(parity));
             }
+            if constexpr (RS) if (i == Lq - 1) {
+                // the dropped limb.  Its y_qbar rows of this parity were last read by the divide() of round - 2, which every other
+                // limb CTA runs before its digit of this round: the foreign digits were awaited above, the digit mates (limbs lo ..
+                // Lq-2 of its own digit, never awaited by phase 2) are awaited here.  Its digit slot is protected by the mailbox:
+                // limb 0 posts this round only after its divide(round - 2), which waited for every special CTA of round - 2.
+                const u32 lo = g_own * Ks;
+                wait_for(base + lo, i - lo, tag);
+                for (u32 c = 0; c < 2; ++c)
+                    ms_tau_body<LOGN, NT, true>(cta, buf, acc_of(parity) + c * N, acc_of(parity) + c * N, A.itw + (size_t)i * N, R->lp_drop,
+                                                drop_of(parity, c), K);
+                __threadfence();
+                __syncthreads();
+                if (threadIdx.x == 0) st_release_u32(R->tau_flag + group, tag);
+                continue;
+            }
             if (pending) divide(prev_ct, prev_tag, prev_parity);
             pending = true;
             prev_ct = ct;
@@ -888,6 +925,16 @@ __global__ void __launch_bounds__(NT, MINB) ks_grouped_kernel(KsArgs A, const __
                                                               const __grid_constant__ GroupConsts G, size_t batch, u32 *flags, u32 epoch,
                                                               u32 *ticket, u64 *mail, const u64 *addend) {
     ks_grouped_body<LOGN, NT, MODE, ADD>(A, lt, K, G, batch, flags, epoch, ticket, mail, addend, nullptr);
+}
+
+// multiply-and-rescale (DESIGN.md §2.19): the program in mode MODE (KS_MUL_RELIN or KS_DOT, D unused by the former) with the division
+// by P * q_{Lq-1}; R carries the dropped limb's constants and rows
+template <int LOGN, int NT, int MINB, int MODE>
+__global__ void __launch_bounds__(NT, MINB) ks_rescale_grouped_kernel(KsArgs A, const __grid_constant__ LimbTable lt, const __grid_constant__ MsConsts K,
+                                                                      const __grid_constant__ GroupConsts G, const __grid_constant__ DotArgs D,
+                                                                      const __grid_constant__ RescaleConsts R, size_t batch, u32 *flags, u32 epoch,
+                                                                      u32 *ticket, u64 *mail) {
+    ks_grouped_body<LOGN, NT, MODE, false, true>(A, lt, K, G, batch, flags, epoch, ticket, mail, nullptr, MODE == KS_DOT ? &D : nullptr, &R);
 }
 
 // the encrypted inner product: ks_grouped_kernel's program in mode KS_DOT, with the operand tables of the call in D
@@ -1648,12 +1695,13 @@ cudaError_t launch_ks_hybrid(LaunchCtx &lc, int mode, const u64 *a, const u64 *b
 
 #endif
 #if DPFHE_PART_GROUPED
-template <int LOGN, int MODE, bool ADD = false>
+template <int LOGN, int MODE, bool ADD = false, bool RS = false>
 static cudaError_t launch_ks_grouped_t(LaunchCtx &lc, const KsArgs &A, const MsConsts &K, const GroupConsts &Gc, size_t batch, cudaStream_t st,
-                                       const u64 *addend, const DotArgs *dot = nullptr) {
+                                       const u64 *addend, const DotArgs *dot = nullptr, const RescaleConsts *rs = nullptr) {
     constexpr int NT = 256, MINB = 3;
     const void *kern;
-    if constexpr (MODE == KS_DOT) kern = (const void *)ct_dot_grouped_kernel<LOGN, NT, MINB>;
+    if constexpr (RS) kern = (const void *)ks_rescale_grouped_kernel<LOGN, NT, MINB, MODE>;
+    else if constexpr (MODE == KS_DOT) kern = (const void *)ct_dot_grouped_kernel<LOGN, NT, MINB>;
     else kern = (const void *)ks_grouped_kernel<LOGN, NT, MINB, MODE, ADD>;
     const size_t smem = LOGN <= 13 ? Geometry<LOGN>::LIMB_BYTES : Geometry<13>::LIMB_BYTES;
     static ConfiguredMask configured;
@@ -1690,7 +1738,11 @@ static cudaError_t launch_ks_grouped_t(LaunchCtx &lc, const KsArgs &A, const MsC
     const u64 *add = addend;
     void *params[] = {&args, &lt, &consts, &gc, &batch_arg, &flags, &epoch, &ticket, &mail, &add};
     void *params_dot[] = {&args, &lt, &consts, &gc, const_cast<DotArgs *>(dot), &batch_arg, &flags, &epoch, &ticket, &mail};
-    e = cudaLaunchCooperativeKernel(kern, dim3((unsigned)G), dim3(NT), MODE == KS_DOT ? params_dot : params, smem, st);
+    DotArgs no_dot{};
+    RescaleConsts rc{};
+    if (rs) rc = *rs;
+    void *params_rs[] = {&args, &lt, &consts, &gc, dot ? const_cast<DotArgs *>(dot) : &no_dot, &rc, &batch_arg, &flags, &epoch, &ticket, &mail};
+    e = cudaLaunchCooperativeKernel(kern, dim3((unsigned)G), dim3(NT), RS ? params_rs : MODE == KS_DOT ? params_dot : params, smem, st);
     lc.ks_epoch += rounds;
     return e;
 }
@@ -1761,6 +1813,48 @@ cudaError_t launch_ct_dot_grouped(LaunchCtx &lc, const u64 *const *a, const u64 
         case 13: return launch_ks_grouped_t<13, KS_DOT>(lc, A, K, Gc, batch, st, nullptr, &D);
         case 14: return launch_ks_grouped_t<14, KS_DOT>(lc, A, K, Gc, batch, st, nullptr, &D);
     }
+    return cudaErrorNotSupported;
+}
+
+// multiply-and-rescale (DESIGN.md §2.19): out [batch][2][Lq-1][N] = the product (dot: the summed products of the n_terms pairs a[t] x b[t];
+// otherwise the ct x ct product a[0] x b[0]) relinearised and divided by P * q_{Lq-1} in one launch (+ key_prepare without key_s).
+// R: the dropped limb's constants; its row and flag pointers are set here (lc.ks_tau_drop; one flag per group in the second half of
+// lc.ks_flags, whose words ks_hoistg_kernel uses as round marks in other launches: a tag is always above what an earlier launch left).  lc.ks_tau_drop must hold (ks_slots / 3 + 1) * 4 * N words: a group has L >= 3 CTAs.
+cudaError_t launch_ks_rescale_grouped(LaunchCtx &lc, bool dot, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, u64 *out,
+                                      size_t batch, const MsConsts &K, const GroupConsts &Gc, const RescaleConsts &R, cudaStream_t st,
+                                      const u64 *key_s) {
+    if (batch == 0) return cudaSuccess;
+    if (lc.L < 3 || !lc.ks_hyb || !lc.ks_acc_hyb || !lc.ks_tau_drop || Gc.Lq + Gc.K != lc.L || Gc.Lq < 2 || Gc.K > Gc.Lq ||
+        Gc.K > (u32)KS_MAX_SPECIAL)
+        return cudaErrorInvalidValue;
+    if (n_terms < 1 || n_terms > (u32)DOT_MAX_TERMS || (!dot && n_terms != 1)) return cudaErrorInvalidValue;
+    if (!key_s) {
+        cudaError_t e = launch_key_prepare_grouped(lc, key, lc.ks_key_s, Gc.dnum, st);
+        if (e != cudaSuccess) return e;
+        key_s = lc.ks_key_s;
+    }
+    KsArgs A;
+    A.a = dot ? nullptr : a[0]; A.b = dot ? nullptr : b[0]; A.key = key; A.key_s = key_s; A.out = out; A.scratch = lc.ks_scratch;
+    A.tw = lc.tw; A.itw = lc.itw; A.L = Gc.Lq; A.galois = 0; A.Lk = lc.L; A.hyb = lc.ks_hyb; A.only = nullptr;
+    A.acc = lc.ks_acc_hyb; A.acc_par = 2; A.lift_reduce = 0u;
+    RescaleConsts Rc = R;
+    Rc.tau = lc.ks_tau_drop;
+    Rc.tau_flag = lc.ks_flags + lc.ks_slots;
+    DotArgs D{};
+    D.n_terms = n_terms;
+    for (u32 t = 0; dot && t < n_terms; ++t) {
+        D.a[t] = a[t];
+        D.b[t] = b[t];
+    }
+#define KS_RS_DISPATCH(LOGN)                                                                                                     \
+    return dot ? launch_ks_grouped_t<LOGN, KS_DOT, false, true>(lc, A, K, Gc, batch, st, nullptr, &D, &Rc)                       \
+               : launch_ks_grouped_t<LOGN, KS_MUL_RELIN, false, true>(lc, A, K, Gc, batch, st, nullptr, nullptr, &Rc);
+    switch (lc.log_n) {
+        case 12: KS_RS_DISPATCH(12)
+        case 13: KS_RS_DISPATCH(13)
+        case 14: KS_RS_DISPATCH(14)
+    }
+#undef KS_RS_DISPATCH
     return cudaErrorNotSupported;
 }
 

@@ -36,6 +36,7 @@ struct LaunchCtx {
     u64 *ks_mail = nullptr;           // [ks_slots] per-group mailbox: (round tag << 32) | ciphertext index
     u64 *ks_key_s = nullptr;          // [L][2][L][N] Shoup companions of the current switch key
     u64 *ks_hyb = nullptr;            // hybrid key switching: [ks_slots / 2 + 1][KS_HYB_ROWS][N], allocated at the first hybrid call
+    u64 *ks_tau_drop = nullptr;       // multiply-and-rescale: [ks_slots / 3 + 1][2 parities][2][N] rows of the dropped limb, allocated at the first such call
     size_t ks_slots = 0;
     u32 ks_epoch = 0;                 // rounds consumed so far (flag values already used)
     unsigned long long ks_epoch_limit = 1ull << 30;   // the round numbering restarts before it gets here (DPFHE_EPOCH_LIMIT: tests)
@@ -62,6 +63,9 @@ struct LaunchCtx {
                                   const u64 *key_s = nullptr); \
     cudaError_t launch_ct_dot_grouped(LaunchCtx &lc, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, u64 *out, size_t batch, \
                                       const MsConsts &K, const GroupConsts &G, cudaStream_t st, const u64 *key_s = nullptr); \
+    cudaError_t launch_ks_rescale_grouped(LaunchCtx &lc, bool dot, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, \
+                                          u64 *out, size_t batch, const MsConsts &K, const GroupConsts &G, const RescaleConsts &R, \
+                                          cudaStream_t st, const u64 *key_s = nullptr); \
     cudaError_t launch_hoist_grouped(LaunchCtx &lc, const u64 *ct, u64 *U, const GroupConsts &G, size_t batch, cudaStream_t st); \
     cudaError_t launch_key_prepare_grouped(const LaunchCtx &lc, const u64 *key, u64 *key_s, u32 dnum, cudaStream_t st); \
     cudaError_t launch_rot_apply_grouped(LaunchCtx &lc, const u64 *ct, const u64 *U, const u64 *key, const u64 *key_s, u32 galois, u64 *acc, \
@@ -107,6 +111,8 @@ DPFHE_DECLARE_LAUNCHERS
 // launch_ks_grouped: key_s == nullptr builds the companions into lc.ks_key_s (two launches), otherwise one launch; addend (KS_ROTATE
 // only) is added to the result in the kernel's final store.
 // launch_ct_dot_grouped: a[t] / b[t] of n_terms (1 .. DOT_MAX_TERMS) pairs, host arrays of device pointers; key_s as launch_ks_grouped.
+// launch_ks_rescale_grouped: dot = false: a[0] x b[0] (n_terms = 1), dot = true: the pairs as launch_ct_dot_grouped; key_s as
+// launch_ks_grouped.
 // launch_rot_sum_grouped: keys[m] / key_s[m] / galois[m] of n_rot (1 .. ROT_SUM_MAX) rotations; the companions are required.
 
 }  // namespace dpfhe

@@ -101,6 +101,19 @@ struct GroupConsts {
     u64 half[KS_MAX_SPECIAL];                                    // floor(p_k / 2)
 };
 
+// Multiply-and-rescale (DESIGN.md §2.19, §4.16): the division by P' = P * qbar, qbar = q_{Lq-1} the dropped ciphertext limb.  The
+// GroupConsts of such a call describe P' for the K special rows (lp_up, dn, neg_p), its MsConsts divide by P'; this block is the
+// divided set's fifth row, kept apart so that the parameter blocks of the other grouped kernels keep their layout
+// (host_params.cpp:build_rescale_consts).
+struct RescaleConsts {
+    LimbParams lp_drop;   // limb Lq-1 with N^-1 scaled by (t * P)^-1 mod qbar: its inverse transform yields y_qbar
+    u64 dn[16], dn_s[16]; // [i]: P mod q_i (= P' / qbar), with its Shoup companion (i < Lq - 1)
+    u64 half;             // floor(qbar / 2)
+    u64 *tau;             // [groups][2 parities][2][N]: y_qbar of the dropped limb's CTA, double-buffered by round parity
+    u32 *tau_flag;        // [groups]: round tag of the last y_qbar published
+    u32 pad_[2];
+};
+
 // ---- twiddle table layout (host_params.cpp writes it, ntt_core.cuh reads it) -----------------------------
 // natural index of the twiddle of group i at stage s is 2^s + i.  Stages of the last
 // register pass (s >= LOGN-4) are stored transposed so that lane-consecutive rows read

@@ -496,6 +496,35 @@ class Context:
         self._chk(self._l.dpfhe_ct_dot_grouped_host(self._h, int(n_special), n, _hptr(a), _hptr(b), _hptr(evk), _hptr(out, True),
                                                     a.size // (n * pq) if n else 0, int(t_plain)))
 
+    def ct_mul_relin_rescale_grouped(self, n_special, a, b, evk, out, batch, t_plain=0, stream=None):
+        """ct_mul_relin_grouped followed by the rescale (BGV: modulus switch) to L - n_special - 1 limbs, in one division by P times
+        the last ciphertext modulus (DESIGN.md section 2.19); a, b: [batch][2][L-n_special][N], out: [batch][2][L-n_special-1][N]"""
+        self._chk(self._l.dpfhe_ct_mul_relin_rescale_grouped(self._h, int(n_special), _ptr(a), _ptr(b), _ptr(evk), _ptr(out), batch,
+                                                             int(t_plain), _stream(stream)))
+
+    def ct_mul_relin_rescale_grouped_host(self, n_special, a, b, evk, out, t_plain=0):
+        """host form of ct_mul_relin_rescale_grouped (C-contiguous numpy uint64)"""
+        pq = 2 * (self.L - n_special) * self.N
+        self._chk(self._l.dpfhe_ct_mul_relin_rescale_grouped_host(self._h, int(n_special), _hptr(a), _hptr(b), _hptr(evk), _hptr(out, True),
+                                                                  a.size // pq, int(t_plain)))
+
+    def ct_dot_rescale_grouped(self, n_special, a_list, b_list, evk, out, batch, t_plain=0, stream=None):
+        """ct_dot_grouped followed by the rescale, in one division (DESIGN.md section 2.19); out: [batch][2][L-n_special-1][N]"""
+        n = len(a_list)
+        if len(b_list) != n:
+            raise ValueError("need as many right operands as left operands")
+        pa = (C.c_void_p * max(n, 1))(*[_ptr(x) for x in a_list])
+        pb = (C.c_void_p * max(n, 1))(*[_ptr(x) for x in b_list])
+        self._chk(self._l.dpfhe_ct_dot_rescale_grouped(self._h, int(n_special), n, pa, pb, _ptr(evk), _ptr(out), batch, int(t_plain),
+                                                       _stream(stream)))
+
+    def ct_dot_rescale_grouped_host(self, n_special, a, b, evk, out, t_plain=0):
+        """host form of ct_dot_rescale_grouped: a, b [n_terms][batch][2][L-n_special][N] (C-contiguous numpy uint64)"""
+        n = a.shape[0]
+        pq = 2 * (self.L - n_special) * self.N
+        self._chk(self._l.dpfhe_ct_dot_rescale_grouped_host(self._h, int(n_special), n, _hptr(a), _hptr(b), _hptr(evk), _hptr(out, True),
+                                                            a.size // (n * pq) if n else 0, int(t_plain)))
+
     def mod_down_special(self, n_special, polys, out, n_polys, t_plain=0, stream=None):
         self._chk(self._l.dpfhe_mod_down_special(self._h, int(n_special), _ptr(polys), _ptr(out), n_polys, int(t_plain), _stream(stream)))
 

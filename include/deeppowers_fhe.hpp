@@ -270,6 +270,27 @@ public:
         if (a.size() != b.size()) throw std::invalid_argument("one right operand per left operand");
         check(dpfhe_ct_dot_grouped(ctx_, special, a.size(), a.data(), b.data(), relin_key, out, count, plain_modulus, stream));
     }
+    // multiply-and-rescale (DESIGN.md §2.19): multiply_relin_grouped / dot_relin_grouped followed by the rescale (BGV: modulus switch)
+    // that drops the last ciphertext limb, in one division.  The inputs hold limbs()-special limbs, out limbs()-special-1.
+    void multiply_relin_rescale_grouped(unsigned special, ConstCiphertextBatch a, ConstCiphertextBatch b, const std::uint64_t *relin_key,
+                                        CiphertextBatch out, std::uint64_t plain_modulus = 0) {
+        same(a.count, b.count, out.count);
+        check(dpfhe_ct_mul_relin_rescale_grouped_host(ctx_, special, a.data, b.data, relin_key, out.data, a.count, plain_modulus));
+    }
+    void multiply_relin_rescale_grouped_device(unsigned special, const std::uint64_t *a, const std::uint64_t *b, const std::uint64_t *relin_key,
+                                               std::uint64_t *out, std::size_t count, std::uint64_t plain_modulus = 0, void *stream = nullptr) {
+        check(dpfhe_ct_mul_relin_rescale_grouped(ctx_, special, a, b, relin_key, out, count, plain_modulus, stream));
+    }
+    void dot_relin_rescale_grouped(unsigned special, std::size_t n_terms, const std::uint64_t *a, const std::uint64_t *b,
+                                   const std::uint64_t *relin_key, CiphertextBatch out, std::uint64_t plain_modulus = 0) {
+        check(dpfhe_ct_dot_rescale_grouped_host(ctx_, special, n_terms, a, b, relin_key, out.data, out.count, plain_modulus));
+    }
+    void dot_relin_rescale_grouped_device(unsigned special, const std::vector<const std::uint64_t *> &a,
+                                          const std::vector<const std::uint64_t *> &b, const std::uint64_t *relin_key, std::uint64_t *out,
+                                          std::size_t count, std::uint64_t plain_modulus = 0, void *stream = nullptr) {
+        if (a.size() != b.size()) throw std::invalid_argument("one right operand per left operand");
+        check(dpfhe_ct_dot_rescale_grouped(ctx_, special, a.size(), a.data(), b.data(), relin_key, out, count, plain_modulus, stream));
+    }
     // divide by the product of the last `special` limbs: in holds limbs() limbs per polynomial, out limbs()-special
     void mod_down_special_device(unsigned special, const std::uint64_t *ct, std::uint64_t *out, std::size_t count, std::uint64_t plain_modulus = 0,
                                  void *stream = nullptr) {

@@ -279,6 +279,23 @@ int dpfhe_ct_dot_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, con
 /* host-buffer form: h_as, h_bs [n_terms][batch][2][L-K][N]; the key uploaded once, the batch pipelined in chunks (synchronous) */
 int dpfhe_ct_dot_grouped_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs,
                               const uint64_t *h_evk, uint64_t *h_out, size_t batch, uint64_t t_plain);
+/* Multiply-and-rescale (DESIGN.md §2.19): the product of dpfhe_ct_mul_relin_grouped (or the inner product of dpfhe_ct_dot_grouped)
+ * relinearised and divided by P * q_{Lq-1} in ONE division, Lq = L - K: d_out [batch][2][Lq-1][N] is the ciphertext one level down
+ * (the CKKS rescale; BGV's modulus switch, with its factor q_{Lq-1}^-1 mod t on the slots).  It decrypts, under the first Lq - 1 limbs
+ * of the secret, to what dpfhe_mod_switch_down of the unrescaled product decrypts to, but is not its bits (one rounding instead of
+ * two).  24 transforms per ciphertext at Lq = 4, K = 2, against 32 for the product and a separate rescale, and no round trip of the
+ * product through memory.  Same parameters and checks as the unrescaled calls, plus Lq >= 2 and t_plain below q_{Lq-1}; the output
+ * must not overlap any operand.  Two launches (key companions + kernel). */
+int dpfhe_ct_mul_relin_rescale_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_a, const uint64_t *d_b,
+                                       const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream);
+int dpfhe_ct_dot_rescale_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *const *d_as, const uint64_t *const *d_bs,
+                                 const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream);
+/* host-buffer forms: h_a, h_b [batch][2][Lq][N] (h_as, h_bs [n_terms][batch][2][Lq][N]), h_out [batch][2][Lq-1][N]; the key
+ * uploaded once, the batch pipelined in chunks (synchronous) */
+int dpfhe_ct_mul_relin_rescale_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_a, const uint64_t *h_b,
+                                            const uint64_t *h_evk, uint64_t *h_out, size_t batch, uint64_t t_plain);
+int dpfhe_ct_dot_rescale_grouped_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs,
+                                      const uint64_t *h_evk, uint64_t *h_out, size_t batch, uint64_t t_plain);
 /* ---- slot sums (DESIGN.md §2.17): slot i of the result is sum_{j < count} x[(i + j * stride) mod N/2] in every row, count =
  *      prod radices[t], computed in n_stages (1 .. 16) summed-rotation stages; stage t rotates by m * stride * prod_{u<t} radices[u],
  *      m = 1 .. radices[t] - 1 (2 <= radices[t] <= 16), and stride * count must be at most N/2.
