@@ -133,6 +133,22 @@ SYMBOLS = {
                                                C.c_uint64, C.c_void_p]),
     "dpfhe_ct_dot_rescale_grouped_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                                     C.c_uint64]),
+    "dpfhe_ct_mul_relin_grouped_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                   C.c_uint64, C.c_void_p]),
+    "dpfhe_ct_mul_relin_rescale_grouped_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                           C.c_size_t, C.c_uint64, C.c_void_p]),
+    "dpfhe_ct_dot_grouped_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_size_t, C.c_uint64, C.c_void_p]),
+    "dpfhe_ct_dot_rescale_grouped_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                     C.c_size_t, C.c_uint64, C.c_void_p]),
+    "dpfhe_rotate_grouped_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t,
+                                             C.c_uint64, C.c_void_p]),
+    "dpfhe_rotate_sum_grouped_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.c_size_t, C.c_uint64, C.c_void_p]),
+    "dpfhe_ct_mul_relin_rescale_grouped_level_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                                C.c_size_t, C.c_uint64]),
+    "dpfhe_ct_dot_rescale_grouped_level_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                          C.c_void_p, C.c_size_t, C.c_uint64]),
     "dpfhe_slotsum_steps": (C.c_int, [C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_size_t)]),
     "dpfhe_slotsum_create_grouped": (C.c_int, [C.c_void_p, C.c_uint, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint64, C.POINTER(C.c_void_p)]),
     "dpfhe_slotsum_apply": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

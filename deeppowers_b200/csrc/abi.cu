@@ -514,6 +514,7 @@ void dpfhe_context_destroy(dpfhe_ctx *ctx) {
     cudaFree(ctx->lc.ks_prof);
     cudaFree(ctx->lc.ks_hyb);
     cudaFree(ctx->lc.ks_tau_drop);
+    ctx->ks_levels.clear();
     for (int k = 0; k < PIPE_DEPTH; ++k) {
         if (ctx->ev_h2d[k]) cudaEventDestroy(ctx->ev_h2d[k]);
         if (ctx->ev_comp[k]) cudaEventDestroy(ctx->ev_comp[k]);
@@ -551,14 +552,16 @@ size_t dpfhe_context_device_bytes(const dpfhe_ctx *ctx) {
     return n;
 }
 
-// frees the scratch that grows with use (hoisted-rotation transforms, modulus-switch rows, encoding tables, host staging); it comes
-// back on demand
+// frees the scratch that grows with use (hoisted-rotation transforms, modulus-switch rows, encoding tables, host staging, the level
+// bases of the level calls); it comes back on demand
 int dpfhe_context_trim(dpfhe_ctx *ctx) {
     int rc = enter(ctx);
     if (rc) return rc;
     rc = dpfhe_synchronize(ctx);
     if (rc) return rc;
     dpfhe_ctx::each_trimmed(*ctx, [](DeviceScratch &s) { s.release(); });
+    for (const auto &v : ctx->ks_levels) ctx->device_bytes -= v->bytes;
+    ctx->ks_levels.clear();   // the level bases come back at the next level call
     ctx->ckks = CkksTables();
     ctx->bgv_t = 0;
     ctx->bgv = BgvTables();
@@ -726,11 +729,12 @@ int dpfhe_rotate_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_c
 // The argument checks of a call on n_terms operand pairs (d_as[i], d_bs[i]) [batch][2][Lq][N] with grouped keys, in this order: the
 // pair table, the key and output pointers, check() (the call's own checks of n_special and t_plain), then, for a non-empty batch, the
 // output [batch][2][Lq - drop][N] against every operand: the output rows are written while other work items still read their inputs,
-// so no overlap at all.  An empty batch passes once the checks before the overlap have.
+// so no overlap at all.  An empty batch passes once the checks before the overlap have.  level: the operands' limbs of a level call
+// (DESIGN.md §2.20), 0 for the top level Lq = L - n_special.
 extern "C++" {   // a template inside the C entry points' linkage block
 template <class Check>
 static int check_pairs(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *const *d_as, const uint64_t *const *d_bs,
-                       const uint64_t *d_evk, uint64_t *d_out, size_t batch, unsigned drop, Check check) {
+                       const uint64_t *d_evk, uint64_t *d_out, size_t batch, unsigned drop, Check check, unsigned level = 0) {
     if (n_terms < 1 || n_terms > (size_t)DOT_MAX_TERMS) return fail(DPFHE_ERR_INVALID, "n_terms must be in [1, %d]", DOT_MAX_TERMS);
     if (!d_as || !d_bs) return fail(DPFHE_ERR_INVALID, "null argument");
     for (size_t i = 0; i < n_terms; ++i)
@@ -738,7 +742,7 @@ static int check_pairs(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const
     CHECK_PTR(d_evk); CHECK_PTR(d_out);
     const int rc = check();
     if (rc || batch == 0) return rc;
-    const size_t Lq = ctx->hp.L - n_special, in_bytes = batch * 2 * Lq * ctx->N() * 8, out_bytes = batch * 2 * (Lq - drop) * ctx->N() * 8;
+    const size_t Lq = level ? level : ctx->hp.L - n_special, in_bytes = batch * 2 * Lq * ctx->N() * 8, out_bytes = batch * 2 * (Lq - drop) * ctx->N() * 8;
     for (size_t i = 0; i < n_terms; ++i)
         if (overlaps(d_out, out_bytes, d_as[i], in_bytes) || overlaps(d_out, out_bytes, d_bs[i], in_bytes))
             return fail(DPFHE_ERR_INVALID, "output must not overlap an operand (pair %zu)", i);
@@ -814,6 +818,168 @@ int dpfhe_ct_mul_relin_rescale_grouped(dpfhe_ctx *ctx, unsigned n_special, const
 int dpfhe_ct_dot_rescale_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *const *d_as, const uint64_t *const *d_bs,
                                  const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
     return rescale_common(ctx, n_special, true, n_terms, d_as, d_bs, d_evk, d_out, batch, t_plain, stream);
+}
+
+// ---- calls at level l on the top-level context (DESIGN.md §2.20, §4.17) ----------------------------------------------------------
+// A level-l call is the same call on a context over {q_0 .. q_{l-1}, p_0 .. p_{K-1}} with the top-level key restricted to the level's
+// digits and rows.  It runs on the level's view of this context: the level's own tables (KsLevel, built at the first call at (K, l)),
+// the context's scratch and round numbering, and the top-level key read in place through the kernels' key-row map.
+
+// the checks of a level call beyond those of the unrescaled top-level call (check_grouped), after them: K <= l <= Lq; with the
+// rescale also l >= 2 and t_plain below q_{l-1}
+static int check_level(const dpfhe_ctx *ctx, unsigned K, unsigned level, bool rescale, uint64_t t_plain) {
+    const unsigned Lq = ctx->hp.L - K;
+    if (level < K || level > Lq)
+        return fail(DPFHE_ERR_INVALID, "level %u is outside [%u, %u]: a level call needs at least n_special = %u ciphertext limbs and at most the "
+                    "context's %u", level, K, Lq, K, Lq);
+    if (!rescale) return DPFHE_OK;
+    if (level < 2) return fail(DPFHE_ERR_INVALID, "level %u: multiply-and-rescale needs at least two ciphertext limbs", level);
+    if (t_plain >= ctx->hp.limbs[level - 1].lp.q)
+        return fail(DPFHE_ERR_INVALID, "level %u: plaintext modulus must be below the dropped modulus q_%u", level, level - 1);
+    return DPFHE_OK;
+}
+
+// the level state of (K, l), l < Lq: found, or built and uploaded (its bytes counted in device_bytes until dpfhe_context_trim)
+static int level_state(dpfhe_ctx *ctx, unsigned K, unsigned l, const KsLevel *&out) {
+    for (const auto &v : ctx->ks_levels)
+        if (v->K == K && v->l == l) {
+            out = v.get();
+            return DPFHE_OK;
+        }
+    std::unique_ptr<KsLevel> v(new (std::nothrow) KsLevel());
+    if (!v) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    v->K = K;
+    v->l = l;
+    const unsigned Lq = ctx->hp.L - K;
+    std::vector<uint64_t> mod(l + K);
+    for (unsigned i = 0; i < l; ++i) mod[i] = ctx->hp.limbs[i].lp.q;
+    for (unsigned k = 0; k < K; ++k) mod[l + k] = ctx->hp.limbs[Lq + k].lp.q;
+    const std::string msg = build_host_params(ctx->hp.log_n, l + K, mod.data(), v->hp);
+    if (!msg.empty()) return fail(DPFHE_ERR_INVALID, "level %u: %s", l, msg.c_str());
+    const int rc = upload_basis(v->hp, v->d_lp, v->d_tw, v->d_itw, v->lt, v->lift_reduce, v->bytes);
+    if (rc) return rc;   // the destructor frees what was allocated
+    // the arithmetic variant a context over this basis picks (dpfhe_context_create)
+    v->fast = getenv("DPFHE_FORCE_GENERIC") == nullptr;
+    for (unsigned i = 0; i < l + K; ++i) v->fast = v->fast && v->lt.lp[i].nqh != 0;
+    ctx->device_bytes += v->bytes;
+    out = v.get();
+    ctx->ks_levels.push_back(std::move(v));
+    return DPFHE_OK;
+}
+
+// the launch state of a level: the context's, with the level's basis and tables
+static LaunchCtx level_ks_view(const dpfhe_ctx *ctx, const KsLevel &v) {
+    LaunchCtx lc = ctx->lc;
+    lc.L = v.l + v.K;
+    lc.lp = v.d_lp;
+    lc.lt = v.lt;
+    lc.tw = v.d_tw;
+    lc.itw = v.d_itw;
+    lc.lift_reduce = v.lift_reduce;
+    lc.fast = v.fast;
+    return lc;
+}
+
+// runs launch(lc) on the level's view and carries the round numbering back to the context: the next key switch on any view continues
+// from there
+extern "C++" {   // a template inside the C entry points' linkage block
+template <class Launch>
+static cudaError_t on_level_view(dpfhe_ctx *ctx, const KsLevel &v, Launch launch) {
+    LaunchCtx lc = level_ks_view(ctx, v);
+    const cudaError_t e = launch(lc);
+    ctx->lc.ks_epoch = lc.ks_epoch;
+    ctx->lc.ks_epoch_restarts = lc.ks_epoch_restarts;
+    return e;
+}
+}
+
+// A key-switching call at level l < Lq once its arguments are checked: the level state, the top-level key's companions over the
+// digits g < ceil(l / K) (the context's launch state, into lc.ks_key_s) and the kernel on the level's view.  mode KS_MUL_RELIN /
+// KS_ROTATE (as[0], bs[0]; galois) or KS_DOT (n_terms pairs); rescale: divided by P * q_{l-1}.  K = 1 without the pairs and the
+// rescale is the one-special-prime kernel, as at the top level.  Two launches.
+static int level_launch(dpfhe_ctx *ctx, unsigned K, unsigned l, int mode, bool rescale, size_t n_terms, const uint64_t *const *as,
+                        const uint64_t *const *bs, const uint64_t *key, uint64_t *out, size_t batch, uint64_t galois, uint64_t t_plain, void *stream) {
+    const KsLevel *v = nullptr;
+    int rc = level_state(ctx, K, l, v);
+    if (!rc) rc = ensure_hyb(ctx);
+    if (!rc && rescale) rc = ensure_tau_drop(ctx);
+    if (rc) return rc;
+    MsConsts Kc;
+    GroupConsts G;
+    RescaleConsts R;
+    const bool hybrid = K == 1 && mode != KS_DOT && !rescale;
+    if (hybrid) build_ms_consts(v->hp, t_plain, Kc);
+    else if (rescale) build_rescale_consts(v->hp, K, t_plain, G, Kc, R);
+    else build_group_consts(v->hp, K, t_plain, G, Kc);
+    cudaStream_t st = pick(ctx, stream);
+    CU_TRY(VCALL(launch_key_prepare_grouped, ctx->lc, key, ctx->lc.ks_key_s, (u32)((l + K - 1) / K), st));
+    const u32 key_L = ctx->hp.L;
+    CU_TRY(on_level_view(ctx, *v, [&](LaunchCtx &lc) {
+        if (hybrid) return VCALL(launch_ks_hybrid_level, lc, mode, as[0], bs ? bs[0] : nullptr, key, lc.ks_key_s, key_L, out, batch, (u32)galois, Kc, st);
+        return VCALL(launch_ks_grouped_level, lc, mode, as, bs, (u32)n_terms, key, lc.ks_key_s, key_L, out, batch, (u32)galois, Kc, G,
+                     rescale ? &R : nullptr, st);
+    }));
+    note_launch(ctx, 2);   // key_prepare_kernel + the kernel
+    return DPFHE_OK;
+}
+
+// ct x ct product and rotation at level l: ks_hybrid_common's checks, in its order, with the operands' sizes of the level
+static int level_single(dpfhe_ctx *ctx, unsigned n_special, unsigned level, int mode, const uint64_t *a, const uint64_t *b, const uint64_t *key,
+                        uint64_t *out, size_t batch, uint64_t galois, uint64_t t_plain, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (batch == 0) return DPFHE_OK;
+    CHECK_PTR(a); CHECK_PTR(key); CHECK_PTR(out);
+    if (mode == KS_MUL_RELIN) CHECK_PTR(b);
+    rc = check_grouped(ctx, n_special, t_plain);
+    if (!rc) rc = check_level(ctx, n_special, level, false, t_plain);
+    if (!rc && mode == KS_ROTATE) rc = check_galois(ctx, galois);
+    if (rc) return rc;
+    if (level == ctx->hp.L - n_special) return ks_hybrid_common(ctx, n_special, mode, a, b, key, out, batch, galois, t_plain, stream);
+    const size_t ct_bytes = 2 * (size_t)level * ctx->N() * 8;
+    if (overlaps(out, batch * ct_bytes, a, batch * ct_bytes) || overlaps(out, batch * ct_bytes, b, batch * ct_bytes))
+        return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+    return level_launch(ctx, n_special, level, mode, false, 1, &a, &b, key, out, batch, galois, t_plain, stream);
+}
+
+// the calls on operand pairs at level l: check_pairs with the level's checks and sizes, then the top-level call at l = Lq
+static int level_pairs(dpfhe_ctx *ctx, unsigned n_special, unsigned level, bool rescale, bool dot, size_t n_terms, const uint64_t *const *d_as,
+                       const uint64_t *const *d_bs, const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    rc = check_pairs(ctx, n_special, n_terms, d_as, d_bs, d_evk, d_out, batch, rescale ? 1 : 0, [&] {
+        const int r = check_grouped(ctx, n_special, t_plain);
+        return r ? r : check_level(ctx, n_special, level, rescale, t_plain);
+    }, level);
+    if (rc || batch == 0) return rc;
+    if (level == ctx->hp.L - n_special) {
+        if (rescale) return rescale_common(ctx, n_special, dot, n_terms, d_as, d_bs, d_evk, d_out, batch, t_plain, stream);
+        if (dot) return dpfhe_ct_dot_grouped(ctx, n_special, n_terms, d_as, d_bs, d_evk, d_out, batch, t_plain, stream);
+        return dpfhe_ct_mul_relin_grouped(ctx, n_special, d_as[0], d_bs[0], d_evk, d_out, batch, t_plain, stream);
+    }
+    return level_launch(ctx, n_special, level, dot ? KS_DOT : KS_MUL_RELIN, rescale, n_terms, d_as, d_bs, d_evk, d_out, batch, 0, t_plain, stream);
+}
+
+int dpfhe_ct_mul_relin_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *d_a, const uint64_t *d_b,
+                                     const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+    return level_single(ctx, n_special, level, KS_MUL_RELIN, d_a, d_b, d_evk, d_out, batch, 0, t_plain, stream);
+}
+int dpfhe_rotate_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *d_ct, uint64_t galois_elt, const uint64_t *d_gk,
+                               uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+    return level_single(ctx, n_special, level, KS_ROTATE, d_ct, nullptr, d_gk, d_out, batch, galois_elt, t_plain, stream);
+}
+int dpfhe_ct_dot_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, size_t n_terms, const uint64_t *const *d_as,
+                               const uint64_t *const *d_bs, const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+    return level_pairs(ctx, n_special, level, false, true, n_terms, d_as, d_bs, d_evk, d_out, batch, t_plain, stream);
+}
+int dpfhe_ct_mul_relin_rescale_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *d_a, const uint64_t *d_b,
+                                             const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+    return level_pairs(ctx, n_special, level, true, false, 1, &d_a, &d_b, d_evk, d_out, batch, t_plain, stream);
+}
+int dpfhe_ct_dot_rescale_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, size_t n_terms, const uint64_t *const *d_as,
+                                       const uint64_t *const *d_bs, const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain,
+                                       void *stream) {
+    return level_pairs(ctx, n_special, level, true, true, n_terms, d_as, d_bs, d_evk, d_out, batch, t_plain, stream);
 }
 
 int dpfhe_grouped_digits(const dpfhe_ctx *ctx, unsigned n_special, unsigned *digits) {
@@ -959,30 +1125,38 @@ int dpfhe_rotate_hoisted_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint6
 // Summed rotations (DESIGN.md §2.17).  Scratch in ctx->hoistg: `head` words first (the key companions of a dpfhe_rotate_sum_grouped
 // call; 0 for a slot-sum object, which keeps its own), then per ciphertext of a chunk the lifted digits [dnum][L][N], the summed
 // accumulators [2][L][N] and the tau' rows [2][K][N].
-static size_t rotate_sum_per_ct(const dpfhe_ctx *ctx, unsigned K) {
-    const size_t N = ctx->N(), L = ctx->hp.L;
-    return (key_digits(ctx, K) * L * N + 2 * L * N + 2 * (size_t)K * N) * sizeof(u64);
+// lv: a level call's basis (DESIGN.md §2.20), nullptr for the top level
+static size_t rotate_sum_per_ct(const dpfhe_ctx *ctx, unsigned K, const KsLevel *lv = nullptr) {
+    const size_t N = ctx->N(), L = lv ? lv->l + K : ctx->hp.L, dnum = (L - K + K - 1) / K;
+    return (dnum * L * N + 2 * L * N + 2 * (size_t)K * N) * sizeof(u64);
 }
 
-static int rotate_sum_reserve(dpfhe_ctx *ctx, unsigned K, size_t head, size_t batch) {
-    const size_t per_ct = rotate_sum_per_ct(ctx, K);
+static int rotate_sum_reserve(dpfhe_ctx *ctx, unsigned K, size_t head, size_t batch, const KsLevel *lv = nullptr) {
+    const size_t per_ct = rotate_sum_per_ct(ctx, K, lv);
     return ctx->hoistg.reserve(ctx, head * sizeof(u64) + hoist_chunk(per_ct, batch) * per_ct);
 }
 
 // one stage: per chunk of the batch the mod-up of c1 (ks_hoistg_kernel), the summed multiply-accumulate of every rotation
-// (rot_sum_grouped_kernel) and the division by P (md_tau, md_limb); 4 launches.  The scratch is reserved by the caller.
+// (rot_sum_grouped_kernel) and the division by P (md_tau, md_limb); 4 launches.  The scratch is reserved by the caller.  lv: the
+// stage at that level (DESIGN.md §2.20), on its view, with the top-level keys and their companions.
 static int rotate_sum_stage(dpfhe_ctx *ctx, unsigned K, size_t head, const u64 *d_ct, u32 n_rot, const u32 *galois, const u64 *const *keys,
-                            const u64 *const *key_s, u64 *d_out, size_t batch, const MsConsts &Kc, const GroupConsts &G, cudaStream_t st) {
-    const size_t N = ctx->N(), L = ctx->hp.L, Pq = (L - K) * N;
-    const size_t u_words = key_digits(ctx, K) * L * N, acc_words = 2 * L * N, per_ct = rotate_sum_per_ct(ctx, K), chunk = hoist_chunk(per_ct, batch);
+                            const u64 *const *key_s, u64 *d_out, size_t batch, const MsConsts &Kc, const GroupConsts &G, cudaStream_t st,
+                            const KsLevel *lv = nullptr) {
+    const size_t N = ctx->N(), L = lv ? lv->l + K : ctx->hp.L, Pq = (L - K) * N, dnum = (L - K + K - 1) / K;
+    const size_t u_words = dnum * L * N, acc_words = 2 * L * N, per_ct = rotate_sum_per_ct(ctx, K, lv), chunk = hoist_chunk(per_ct, batch);
     if (ctx->hoistg.bytes() < head * sizeof(u64) + chunk * per_ct) return fail(DPFHE_ERR_INVALID, "summed rotations: scratch not reserved");
     u64 *U = ctx->hoistg.get() + head, *acc = U + chunk * u_words, *tau = acc + chunk * acc_words;
+    const u32 key_shift = (u32)(ctx->hp.L - L);
     for (size_t first = 0; first < batch; first += chunk) {
         const size_t cnt = batch - first < chunk ? batch - first : chunk;
         const u64 *in = d_ct + first * 2 * Pq;
-        CU_TRY(VCALL(launch_hoist_grouped, ctx->lc, in, U, G, cnt, st));
-        CU_TRY(VCALL(launch_rot_sum_grouped, ctx->lc, in, U, n_rot, keys, key_s, galois, acc, Kc, G, cnt, st));
-        CU_TRY(VCALL(launch_mod_down_special, ctx->lc, acc, tau, d_out + first * 2 * Pq, Kc, G, 2 * cnt, st));
+        auto launch = [&](LaunchCtx &lc) {
+            cudaError_t e = VCALL(launch_hoist_grouped, lc, in, U, G, cnt, st);
+            if (e == cudaSuccess) e = VCALL(launch_rot_sum_grouped, lc, in, U, n_rot, keys, key_s, galois, acc, Kc, G, cnt, st, key_shift);
+            if (e == cudaSuccess) e = VCALL(launch_mod_down_special, lc, acc, tau, d_out + first * 2 * Pq, Kc, G, 2 * cnt, st);
+            return e;
+        };
+        CU_TRY(lv ? on_level_view(ctx, *lv, launch) : launch(ctx->lc));
         note_launch(ctx, 4);   // ks_hoistg, rot_sum_grouped, md_tau, md_limb
     }
     return DPFHE_OK;
@@ -1012,11 +1186,12 @@ struct RotSumPrep {
 };
 
 // reserves the scratch of chunks of up to `batch` ciphertexts and builds the companions (n_rot launches)
+// lv: at that level (DESIGN.md §2.20): the companions of the top-level keys' rows of the level's digits, the level's constants
 static int rotate_sum_prepare(dpfhe_ctx *ctx, unsigned n_special, size_t n_rot, const uint64_t *galois_elts, const uint64_t *const *d_gks,
-                              uint64_t t_plain, size_t batch, cudaStream_t st, RotSumPrep &pr) {
-    const size_t dnum = key_digits(ctx, n_special), key_words = dnum * 2 * ctx->P();
+                              uint64_t t_plain, size_t batch, cudaStream_t st, RotSumPrep &pr, const KsLevel *lv = nullptr) {
+    const size_t dnum = lv ? (lv->l + n_special - 1) / n_special : key_digits(ctx, n_special), key_words = dnum * 2 * ctx->P();
     pr.head = n_rot * key_words;
-    int rc = rotate_sum_reserve(ctx, n_special, pr.head, batch);
+    int rc = rotate_sum_reserve(ctx, n_special, pr.head, batch, lv);
     if (rc) return rc;
     u64 *key_s = ctx->hoistg.get();
     for (size_t r = 0; r < n_rot; ++r) {
@@ -1025,7 +1200,7 @@ static int rotate_sum_prepare(dpfhe_ctx *ctx, unsigned n_special, size_t n_rot, 
         pr.key_s[r] = key_s + r * key_words;
         pr.galois[r] = (u32)galois_elts[r];
     }
-    build_group_consts(ctx->hp, n_special, t_plain, pr.G, pr.K);
+    build_group_consts(lv ? lv->hp : ctx->hp, n_special, t_plain, pr.G, pr.K);
     return DPFHE_OK;
 }
 
@@ -1046,6 +1221,32 @@ int dpfhe_rotate_sum_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t 
     rc = rotate_sum_prepare(ctx, n_special, n_rot, galois_elts, d_gks, t_plain, batch, st, pr);
     if (rc) return rc;
     return rotate_sum_stage(ctx, n_special, pr.head, d_ct, (u32)n_rot, pr.galois, d_gks, pr.key_s, d_out, batch, pr.K, pr.G, st);
+}
+
+// summed rotations at level l (DESIGN.md §2.20): the checks of dpfhe_rotate_sum_grouped, then the level's; the level's scratch
+// and constants, the top-level keys' companions over its digits and the stage on its view
+int dpfhe_rotate_sum_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *d_ct, size_t n_rot, const uint64_t *galois_elts,
+                                   const uint64_t *const *d_gks, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (batch == 0) return DPFHE_OK;
+    CHECK_PTR(d_ct); CHECK_PTR(d_out);
+    if (!d_gks) return fail(DPFHE_ERR_INVALID, "null argument");
+    rc = check_rotate_sum(ctx, n_special, n_rot, galois_elts, t_plain);
+    if (!rc) rc = check_rotations(ctx, n_rot, galois_elts, d_gks);
+    if (!rc) rc = check_level(ctx, n_special, level, false, t_plain);
+    if (rc) return rc;
+    if (level == ctx->hp.L - n_special) return dpfhe_rotate_sum_grouped(ctx, n_special, d_ct, n_rot, galois_elts, d_gks, d_out, batch, t_plain, stream);
+    const size_t ct_bytes = batch * 2 * (size_t)level * ctx->N() * 8;
+    if (overlaps(d_out, ct_bytes, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    const KsLevel *lv = nullptr;
+    rc = level_state(ctx, n_special, level, lv);
+    if (rc) return rc;
+    cudaStream_t st = pick(ctx, stream);
+    RotSumPrep pr;
+    rc = rotate_sum_prepare(ctx, n_special, n_rot, galois_elts, d_gks, t_plain, batch, st, pr, lv);
+    if (rc) return rc;
+    return rotate_sum_stage(ctx, n_special, pr.head, d_ct, (u32)n_rot, pr.galois, d_gks, pr.key_s, d_out, batch, pr.K, pr.G, st, lv);
 }
 
 int dpfhe_rotate_sum_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_ct, size_t n_rot, const uint64_t *galois_elts,
@@ -1222,7 +1423,7 @@ int dpfhe_ct_mul_relin_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const ui
 extern "C++" {   // a template inside the C entry points' linkage block
 template <class Check, class Call>
 static int pairs_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs, const uint64_t *h_evk,
-                      uint64_t *h_out, size_t batch, unsigned drop, Check check, Call call) {
+                      uint64_t *h_out, size_t batch, unsigned drop, Check check, Call call, unsigned level = 0) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (n_terms < 1 || n_terms > (size_t)DOT_MAX_TERMS) return fail(DPFHE_ERR_INVALID, "n_terms must be in [1, %d]", DOT_MAX_TERMS);
@@ -1230,11 +1431,12 @@ static int pairs_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const 
     rc = check();
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
-    const size_t Lq = ctx->hp.L - n_special, ctw = 2 * Lq * ctx->N(), outw = 2 * (Lq - drop) * ctx->N();   // words of an operand / output
+    // words of an operand / output (level: the operands' limbs of a level call, whose key is still the top-level one)
+    const size_t Lq = level ? level : ctx->hp.L - n_special, ctw = 2 * Lq * ctx->N(), outw = 2 * (Lq - drop) * ctx->N();
     rc = upload_key(ctx, h_evk, 2 * key_digits(ctx, n_special) * ctx->P());
     if (rc) return rc;
     size_t chunk = std::max<size_t>(1, ((size_t)64 << 20) / (n_terms * ctw * 8));   // ~64 MiB per staged operand side, as pick_chunk
-    const size_t round = std::max<size_t>(1, (size_t)ctx->lc.num_sms * 3 / ctx->hp.L);   // ciphertexts per round of the grid (3 CTAs per SM)
+    const size_t round = std::max<size_t>(1, (size_t)ctx->lc.num_sms * 3 / (Lq + n_special));   // ciphertexts per round of the grid (3 CTAs per SM)
     if (chunk > round) chunk -= chunk % round;
     if (chunk > batch) chunk = batch;
     return run_pipeline(
@@ -1274,6 +1476,26 @@ int dpfhe_ct_mul_relin_rescale_grouped_host(dpfhe_ctx *ctx, unsigned n_special, 
 int dpfhe_ct_dot_rescale_grouped_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs,
                                       const uint64_t *h_evk, uint64_t *h_out, size_t batch, uint64_t t_plain) {
     return rescale_host(ctx, n_special, true, n_terms, h_as, h_bs, h_evk, h_out, batch, t_plain);
+}
+
+// host forms of multiply-and-rescale at level l (DESIGN.md §2.20): the top-level key uploaded once, operands of l limbs and outputs of
+// l - 1 limbs pipelined in chunks
+static int rescale_level_host(dpfhe_ctx *ctx, unsigned n_special, unsigned level, bool dot, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs,
+                              const uint64_t *h_evk, uint64_t *h_out, size_t batch, uint64_t t_plain) {
+    return pairs_host(ctx, n_special, n_terms, h_as, h_bs, h_evk, h_out, batch, 1, [&] {
+        const int rc = check_grouped(ctx, n_special, t_plain);
+        return rc ? rc : check_level(ctx, n_special, level, true, t_plain);
+    }, [&](const u64 *const *as, const u64 *const *bs, u64 *dout, size_t cnt, cudaStream_t st) {
+        return level_pairs(ctx, n_special, level, true, dot, n_terms, as, bs, ctx->stage_key.get(), dout, cnt, t_plain, st);
+    }, level);
+}
+int dpfhe_ct_mul_relin_rescale_grouped_level_host(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *h_a, const uint64_t *h_b,
+                                                  const uint64_t *h_evk, uint64_t *h_out, size_t batch, uint64_t t_plain) {
+    return rescale_level_host(ctx, n_special, level, false, 1, h_a, h_b, h_evk, h_out, batch, t_plain);
+}
+int dpfhe_ct_dot_rescale_grouped_level_host(dpfhe_ctx *ctx, unsigned n_special, unsigned level, size_t n_terms, const uint64_t *h_as,
+                                            const uint64_t *h_bs, const uint64_t *h_evk, uint64_t *h_out, size_t batch, uint64_t t_plain) {
+    return rescale_level_host(ctx, n_special, level, true, n_terms, h_as, h_bs, h_evk, h_out, batch, t_plain);
 }
 
 int dpfhe_rotate_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_ct, uint64_t galois_elt, const uint64_t *h_gk,

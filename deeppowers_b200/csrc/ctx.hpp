@@ -5,6 +5,8 @@
 #include <cstddef>
 #include <cstdint>
 #include <initializer_list>
+#include <memory>
+#include <vector>
 
 #include "host_params.hpp"
 #include "launch.hpp"
@@ -35,6 +37,27 @@ public:
 private:
     void *p_ = nullptr;
     size_t bytes_ = 0;
+};
+
+// The key-switching basis of level l with K special primes (DESIGN.md §2.20, §4.17): {q_0 .. q_{l-1}, p_0 .. p_{K-1}}, its host
+// parameters and device tables, and what a context over that basis would pick (arithmetic variant, lift_reduce).  No key: the level
+// calls read the context's top-level keys in place.
+struct KsLevel {
+    unsigned K = 0, l = 0;
+    dpfhe::HostParams hp;
+    dpfhe::LimbParams *d_lp = nullptr;
+    dpfhe::Twiddle *d_tw = nullptr, *d_itw = nullptr;
+    dpfhe::LimbTable lt;
+    bool lift_reduce = true, fast = false;
+    size_t bytes = 0;   // of the device tables
+    KsLevel() = default;
+    KsLevel(const KsLevel &) = delete;
+    KsLevel &operator=(const KsLevel &) = delete;
+    ~KsLevel() {
+        cudaFree(d_lp);
+        cudaFree(d_tw);
+        cudaFree(d_itw);
+    }
 };
 
 struct dpfhe_ctx {
@@ -68,6 +91,8 @@ struct dpfhe_ctx {
     // allocated on first use and kept: per-rotation constants of the hoisted rotations, M [L][N] and kprime [2][L][N], and the
     // table delta[j][i] = q_j mod q_i
     DeviceScratch hoist_M, hoist_kprime, hoist_delta;
+    // the level bases of the level calls, built at the first call at (K, l), counted in device_bytes, released by dpfhe_context_trim
+    std::vector<std::unique_ptr<KsLevel>> ks_levels;
     cudaEvent_t ev_h2d[DPFHE_PIPE_DEPTH] = {}, ev_comp[DPFHE_PIPE_DEPTH] = {}, ev_d2h[DPFHE_PIPE_DEPTH] = {};
     size_t N() const { return (size_t)1 << hp.log_n; }
     size_t P() const { return N() * hp.L; }

@@ -284,6 +284,12 @@ struct KsArgs {
 // tau' rows of a hybrid group are double-buffered by round parity (KS_HYB_ROWS, types.hpp)
 DPFHE_HD u32 ks_hyb_tau_row(u32 parity, u32 c) { return 2u + 2u * parity + c; }
 
+// The key row that limb i of a level view over lq ciphertext limbs reads (LV instances, DESIGN.md §4.17): the key is the top-level
+// one, restricted by the choice of rows alone.  Limbs below lq read their own row, the special limbs the row `shift` further down
+// (shift = Lq - l; the key's stride, A.Lk, is the top-level L).  The Shoup companions have the key's layout and use the same map.
+// Without LV the bodies keep their own expressions for the row, so that the instances that existed before compile as they did.
+DPFHE_HD size_t ks_key_row(u32 i, u32 lq, u32 shift) { return i >= lq ? (size_t)i + shift : (size_t)i; }
+
 // operands of one 16-byte chunk position of phase 1, fetched one iteration ahead of their use
 struct KsP1Operands {
     U64x2 a0, a1, b0, b1;   // MUL_RELIN: the four input chunks; PLAIN: a0 = digit; ROTATE: a0 = c0 gather, a1 = c1 gather
@@ -473,9 +479,10 @@ DPFHE_HD void ks_p1_dot_chunk(const DotArgs &D, size_t pos, size_t P, const KsP1
 // slot_free / slot_free_target: when non-null, the digit slot is single-buffered and may only be overwritten once the counter has
 // reached the target (every reader of the previous digit has signalled); cta.wait_ge spins on it (a no-op in the host emulator,
 // whose sequential order already guarantees it).
-template <int LOGN, int NT, int MODE, bool HYB = false, class CTA>
+template <int LOGN, int NT, int MODE, bool HYB = false, bool LV = false, class CTA>
 DPFHE_HD void ks_phase1(CTA &cta, u64 *buf, const KsArgs &A, const LimbParams &p, size_t ct, u32 i, u64 *t_slot, u64 *acc_rows, u64 pm = 0,
-                        u64 pm_s = 0, const u32 *slot_free = nullptr, u32 slot_free_target = 0, u32 key_digit = ~0u, const DotArgs *dot = nullptr) {
+                        u64 pm_s = 0, const u32 *slot_free = nullptr, u32 slot_free_target = 0, u32 key_digit = ~0u, const DotArgs *dot = nullptr,
+                        u32 key_shift = 0) {
     constexpr int N = 1 << LOGN, NC = N / 2;
     static_assert((NC / NT) % 2 == 0, "chunk loops may be unrolled by two (ping-pong operand buffers)");
     static_assert(MODE != KS_DOT || HYB, "the inner product exists with special-prime keys only");
@@ -487,7 +494,15 @@ DPFHE_HD void ks_phase1(CTA &cta, u64 *buf, const KsArgs &A, const LimbParams &p
     KsP1Pointers ptr;
     {
         const u32 kd = key_digit == ~0u ? i : key_digit;   // the key digit that limb i belongs to (grouped digits: i / K)
-        const size_t koff_b = ((size_t)kd * 2 + 0) * PK + (size_t)i * N, koff_a = ((size_t)kd * 2 + 1) * PK + (size_t)i * N;
+        size_t koff_b, koff_a;
+        if constexpr (LV) {
+            const size_t kr = ks_key_row(i, A.L, key_shift);
+            koff_b = ((size_t)kd * 2 + 0) * PK + kr * N;
+            koff_a = ((size_t)kd * 2 + 1) * PK + kr * N;
+        } else {
+            koff_b = ((size_t)kd * 2 + 0) * PK + (size_t)i * N;
+            koff_a = ((size_t)kd * 2 + 1) * PK + (size_t)i * N;
+        }
         ptr.kb = reinterpret_cast<const U64x2 *>(A.key + koff_b);
         ptr.ka = reinterpret_cast<const U64x2 *>(A.key + koff_a);
         ptr.kbs = reinterpret_cast<const U64x2 *>(A.key_s + koff_b);
@@ -573,14 +588,22 @@ DPFHE_HD void ks_phase1(CTA &cta, u64 *buf, const KsArgs &A, const LimbParams &p
 // SPECIAL (hybrid only): limb i = A.L is the special prime; jj = 0 .. L-1 counts its digits and its accumulators start from zero.
 // LOAD(h): fills the transform buffer with the first forward stage(s) of the lifted digit (h = half for N = 16384, else 0), from
 // values below BIN*q.  n_digits: how many digits the accumulation runs over (the last one finishes a non-hybrid result).
-template <int LOGN, int NT, bool HYB, bool SPECIAL, int BIN, class CTA, class LOAD>
+template <int LOGN, int NT, bool HYB, bool SPECIAL, int BIN, bool LV = false, class CTA, class LOAD>
 DPFHE_HD void ks_phase2_core(CTA &cta, u64 *buf, const KsArgs &A, const LimbParams &p, size_t ct, u32 i, u32 j, u32 jj, u32 n_digits, LOAD load,
-                             u64 *acc_rows) {
+                             u64 *acc_rows, u32 key_shift = 0) {
     constexpr int N = 1 << LOGN, NC = N / 2;
     static_assert(HYB || !SPECIAL, "the special limb exists only in hybrid key switching");
     const size_t P = (size_t)A.L * N, PK = HYB ? (size_t)A.Lk * N : P;
     const Twiddle *tw = A.tw + (size_t)i * N;
-    const size_t koff_b = ((size_t)j * 2 + 0) * PK + (size_t)i * N, koff_a = ((size_t)j * 2 + 1) * PK + (size_t)i * N;
+    size_t koff_b, koff_a;
+    if constexpr (LV) {
+        const size_t kr = ks_key_row(i, A.L, key_shift);
+        koff_b = ((size_t)j * 2 + 0) * PK + kr * N;
+        koff_a = ((size_t)j * 2 + 1) * PK + kr * N;
+    } else {
+        koff_b = ((size_t)j * 2 + 0) * PK + (size_t)i * N;
+        koff_a = ((size_t)j * 2 + 1) * PK + (size_t)i * N;
+    }
     const U64x2 *kb = reinterpret_cast<const U64x2 *>(A.key + koff_b), *ka = reinterpret_cast<const U64x2 *>(A.key + koff_a);
     const U64x2 *kbs = reinterpret_cast<const U64x2 *>(A.key_s + koff_b), *kas = reinterpret_cast<const U64x2 *>(A.key_s + koff_a);
     U64x2 *acc0 = reinterpret_cast<U64x2 *>(acc_rows), *acc1 = reinterpret_cast<U64x2 *>(acc_rows + N);
@@ -668,9 +691,9 @@ DPFHE_HD void ks_phase2_core(CTA &cta, u64 *buf, const KsArgs &A, const LimbPara
 }
 
 // one digit = one limb (BV-RNS, and hybrid key switching with one special prime): the lift is t_j itself
-template <int LOGN, int NT, bool HYB = false, bool SPECIAL = false, class CTA>
+template <int LOGN, int NT, bool HYB = false, bool SPECIAL = false, bool LV = false, class CTA>
 DPFHE_HD void ks_phase2_digit(CTA &cta, u64 *buf, const KsArgs &A, const LimbParams &p, size_t ct, u32 i, u32 j, u32 jj, const u64 *t_src,
-                              u64 *acc_rows) {
+                              u64 *acc_rows, u32 key_shift = 0) {
     const Twiddle *tw = A.tw + (size_t)i * ((size_t)1 << LOGN);
     const U64x2 *src = reinterpret_cast<const U64x2 *>(t_src);
     // lift of the digit into Z_{q_i}: t_j < q_j.  When every modulus of the basis is below twice every other one (the default
@@ -688,7 +711,7 @@ DPFHE_HD void ks_phase2_digit(CTA &cta, u64 *buf, const KsArgs &A, const LimbPar
             }
         });
     };
-    ks_phase2_core<LOGN, NT, HYB, SPECIAL, 3>(cta, buf, A, p, ct, i, j, jj, A.L, load, acc_rows);
+    ks_phase2_core<LOGN, NT, HYB, SPECIAL, 3, LV>(cta, buf, A, p, ct, i, j, jj, A.L, load, acc_rows, key_shift);
 }
 
 // ---- fused key switch at N <= 8192: one 4096-point block per CTA (DESIGN.md §4.4) -----------------------------------------
@@ -905,9 +928,9 @@ DPFHE_HD void ks_blk_phase2(CTA &cta, u64 *buf, U64x2 *acc, const KsArgs &A, con
 // a digit of several limbs (grouped hybrid key switching, DESIGN.md §2.11): the lift of group g into limb i is the fast basis
 // conversion sum_{j in g} y_j * (Qhat_j mod q_i), y_j = the scaled inverse transforms the members published.
 // t_rows + j * t_stride: the published row of limb j.
-template <int LOGN, int NT, bool SPECIAL, class CTA>
+template <int LOGN, int NT, bool SPECIAL, bool LV = false, class CTA>
 DPFHE_HD void ks_phase2_group(CTA &cta, u64 *buf, const KsArgs &A, const GroupConsts &G, const LimbParams &p, size_t ct, u32 i, u32 g, u32 jj,
-                              const u64 *t_rows, size_t t_stride, u64 *acc_rows) {
+                              const u64 *t_rows, size_t t_stride, u64 *acc_rows, u32 key_shift = 0) {
     const Twiddle *tw = A.tw + (size_t)i * ((size_t)1 << LOGN);
     const u32 lo = g * G.K, hi = lo + G.K < G.Lq ? lo + G.K : G.Lq;
     auto get = [&](int c) {
@@ -932,7 +955,7 @@ DPFHE_HD void ks_phase2_group(CTA &cta, u64 *buf, const KsArgs &A, const GroupCo
             else fwd_load_stage_half<LOGN, NT, false>(buf, tw, p, tid, get, h);
         });
     };
-    ks_phase2_core<LOGN, NT, true, SPECIAL, 4>(cta, buf, A, p, ct, i, g, jj, G.dnum, load, acc_rows);
+    ks_phase2_core<LOGN, NT, true, SPECIAL, 4, LV>(cta, buf, A, p, ct, i, g, jj, G.dnum, load, acc_rows, key_shift);
 }
 
 // ---- modulus switching: drop the last limb (DESIGN.md §2.9) -------------------------------------
@@ -1376,9 +1399,11 @@ struct LazyBound {
 // Lazy bound: both rows start below SB*q (P * c0 and P * c1, ciphertext limbs) and gain one Shoup product (< SB*q) per pair,
 // n_rot * (dnum + 1) <= 15 (dnum + 1) of them; a row takes csub(8q) after a pair whenever the next addition could pass 16q (the
 // rule of acc_trim_after, kept as a running bound), so every value stays below 16q, what canon accepts.
-template <int LOGN, int NT, int CB, class CTA>
+// LV (DESIGN.md §4.17): the keys are top-level keys, key_shift rows longer than the view's per (digit, component), read through
+// ks_key_row; the lifted digits U keep the view's layout.
+template <int LOGN, int NT, int CB, bool LV = false, class CTA>
 DPFHE_HD void rot_sum_grouped_rows(CTA &cta, const RotSumGArgs &A, const GroupConsts &G, const MsConsts &K, const LimbParams &p, size_t ct0,
-                                   u32 n_ct, u32 i, int c_lo = 0, int c_hi = 1 << (LOGN - 1)) {
+                                   u32 n_ct, u32 i, int c_lo = 0, int c_hi = 1 << (LOGN - 1), u32 key_shift = 0) {
     constexpr int N = 1 << LOGN;
     const u32 L = G.Lq + G.K, D = G.dnum;
     const size_t P = (size_t)L * N, Pq = (size_t)G.Lq * N;
@@ -1405,7 +1430,15 @@ DPFHE_HD void rot_sum_grouped_rows(CTA &cta, const RotSumGArgs &A, const GroupCo
                     return r;
                 };
                 if (d < D) {
-                    const size_t kb = ((size_t)d * 2 + 0) * P + (size_t)i * N, ka = ((size_t)d * 2 + 1) * P + (size_t)i * N;
+                    size_t kb, ka;
+                    if constexpr (LV) {
+                        const size_t PK = (size_t)(L + key_shift) * N, kr = ks_key_row(i, G.Lq, key_shift);
+                        kb = ((size_t)d * 2 + 0) * PK + kr * N;
+                        ka = ((size_t)d * 2 + 1) * PK + kr * N;
+                    } else {
+                        kb = ((size_t)d * 2 + 0) * P + (size_t)i * N;
+                        ka = ((size_t)d * 2 + 1) * P + (size_t)i * N;
+                    }
                     o.vb = ld_keep(reinterpret_cast<const U64x2 *>(A.key[m] + kb) + c);
                     o.vbs = ld_keep(reinterpret_cast<const U64x2 *>(A.key_s[m] + kb) + c);
                     o.va = ld_keep(reinterpret_cast<const U64x2 *>(A.key[m] + ka) + c);

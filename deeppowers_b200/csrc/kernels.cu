@@ -698,15 +698,18 @@ __global__ void __launch_bounds__(256) kprime_kernel(const u64 *__restrict__ key
 // so a limb CTA postpones the division step of ciphertext r until it has done the digit and multiply-accumulate
 // work of ciphertext r + 1 (software pipeline of depth one): tau' rows, like the digits and the mailbox, are
 // double-buffered by round parity, and the output rows keep the lazy accumulators in between (DESIGN.md §4.6).
-template <int LOGN, int NT, int MINB, int MODE>
-__global__ void __launch_bounds__(NT, MINB) ks_hybrid_kernel(KsArgs A, const __grid_constant__ LimbTable lt, const __grid_constant__ MsConsts K,
-                                                             size_t batch, u32 *flags, u32 epoch, u32 *ticket, u64 *mail) {
+// LV (DESIGN.md §4.17): a level view reading the top-level key through ks_key_row, its stride A.Lk the top-level L; the body is
+// shared by the two kernels below.
+template <int LOGN, int NT, int MODE, bool LV>
+__device__ __forceinline__ void ks_hybrid_body(const KsArgs &A, const LimbTable &lt, const MsConsts &K, size_t batch, u32 *flags, u32 epoch,
+                                               u32 *ticket, u64 *mail) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     constexpr size_t N = (size_t)1 << LOGN;
     u64 *buf = reinterpret_cast<u64 *>(smem_raw);
     DevCta<NT> cta;
     __shared__ u32 s_ct;
     const u32 L = A.L, GS = L + 1, slot = blockIdx.x, i = slot % GS, group = slot / GS, base = slot - i;
+    const u32 key_shift = LV ? A.Lk - GS : 0u;   // Lq - l
     const bool special = i == L;
     const LimbParams &p = lt.lp[i];
     u64 *hyb = A.hyb + (size_t)group * KS_HYB_ROWS * N;
@@ -754,12 +757,17 @@ __global__ void __launch_bounds__(NT, MINB) ks_hybrid_kernel(KsArgs A, const __g
         const size_t ct = s_ct;
         if (ct >= batch) break;
         if (!special) {
-            ks_phase1<LOGN, NT, MODE, true>(cta, buf, A, p, ct, i, A.scratch + ((size_t)slot * 2 + parity) * N, acc_of(parity), K.qlm[i], K.qlm_s[i]);
+            if constexpr (LV)
+                ks_phase1<LOGN, NT, MODE, true, true>(cta, buf, A, p, ct, i, A.scratch + ((size_t)slot * 2 + parity) * N, acc_of(parity), K.qlm[i],
+                                                      K.qlm_s[i], nullptr, 0, ~0u, nullptr, key_shift);
+            else
+                ks_phase1<LOGN, NT, MODE, true>(cta, buf, A, p, ct, i, A.scratch + ((size_t)slot * 2 + parity) * N, acc_of(parity), K.qlm[i], K.qlm_s[i]);
             publish(tag);
             for (u32 jj = 1; jj < L; ++jj) {
                 const u32 j = (i + jj) % L;
                 wait_for(base + j, tag);
-                ks_phase2_digit<LOGN, NT, true, false>(cta, buf, A, p, ct, i, j, jj, A.scratch + ((size_t)(base + j) * 2 + parity) * N, acc_of(parity));
+                ks_phase2_digit<LOGN, NT, true, false, LV>(cta, buf, A, p, ct, i, j, jj, A.scratch + ((size_t)(base + j) * 2 + parity) * N, acc_of(parity),
+                                                           key_shift);
             }
             if (pending) divide(prev_ct, prev_tag, prev_parity);
             pending = true;
@@ -770,7 +778,7 @@ __global__ void __launch_bounds__(NT, MINB) ks_hybrid_kernel(KsArgs A, const __g
             for (u32 jj = 0; jj < L; ++jj) {
                 const u32 j = (group + jj) % L;   // groups start at different digits: spreads the key-column reads
                 wait_for(base + j, tag);
-                ks_phase2_digit<LOGN, NT, true, true>(cta, buf, A, p, ct, i, j, jj, A.scratch + ((size_t)(base + j) * 2 + parity) * N, hyb);
+                ks_phase2_digit<LOGN, NT, true, true, LV>(cta, buf, A, p, ct, i, j, jj, A.scratch + ((size_t)(base + j) * 2 + parity) * N, hyb, key_shift);
             }
             for (u32 c = 0; c < 2; ++c)
                 ms_tau_body<LOGN, NT, true>(cta, buf, hyb + c * N, hyb + c * N, A.itw + (size_t)i * N, p, hyb + ks_hyb_tau_row(parity, c) * N, K);
@@ -778,6 +786,19 @@ __global__ void __launch_bounds__(NT, MINB) ks_hybrid_kernel(KsArgs A, const __g
         }
     }
     if (pending) divide(prev_ct, prev_tag, prev_parity);   // the group's last ciphertext
+}
+
+template <int LOGN, int NT, int MINB, int MODE>
+__global__ void __launch_bounds__(NT, MINB) ks_hybrid_kernel(KsArgs A, const __grid_constant__ LimbTable lt, const __grid_constant__ MsConsts K,
+                                                             size_t batch, u32 *flags, u32 epoch, u32 *ticket, u64 *mail) {
+    ks_hybrid_body<LOGN, NT, MODE, false>(A, lt, K, batch, flags, epoch, ticket, mail);
+}
+
+// one special prime at level l (DESIGN.md §2.20, §4.17): ks_hybrid_kernel's program on the level's view, reading the top-level key
+template <int LOGN, int NT, int MINB, int MODE>
+__global__ void __launch_bounds__(NT, MINB) ks_hybrid_level_kernel(KsArgs A, const __grid_constant__ LimbTable lt, const __grid_constant__ MsConsts K,
+                                                                   size_t batch, u32 *flags, u32 epoch, u32 *ticket, u64 *mail) {
+    ks_hybrid_body<LOGN, NT, MODE, true>(A, lt, K, batch, flags, epoch, ticket, mail);
 }
 
 #endif
@@ -797,7 +818,8 @@ __global__ void __launch_bounds__(NT, MINB) ks_hybrid_kernel(KsArgs A, const __g
 // The dropped limb's CTA runs phases 1 and 2 as before, then turns its accumulator rows into y_qbar as a special CTA does (inverse
 // transform, (t P)^-1 folded into N^-1) and publishes them on its group's flag in R; it divides nothing and stores no output.  The
 // other limb CTAs divide one round late over K + 1 rows and write [batch][2][Lq-1][N].
-template <int LOGN, int NT, int MODE, bool ADD, bool RS = false>
+// LV (DESIGN.md §4.17): a level view reading the top-level key through ks_key_row, its stride A.Lk the top-level L.
+template <int LOGN, int NT, int MODE, bool ADD, bool RS = false, bool LV = false>
 __device__ __forceinline__ void ks_grouped_body(const KsArgs &A, const LimbTable &lt, const MsConsts &K, const GroupConsts &G, size_t batch, u32 *flags,
                                                 u32 epoch, u32 *ticket, u64 *mail, const u64 *addend, const DotArgs *dot,
                                                 const RescaleConsts *R = nullptr) {
@@ -809,6 +831,7 @@ __device__ __forceinline__ void ks_grouped_body(const KsArgs &A, const LimbTable
     DevCta<NT> cta;
     __shared__ u32 s_ct;
     const u32 Lq = G.Lq, Ks = G.K, dnum = G.dnum, GS = Lq + Ks, slot = blockIdx.x, i = slot % GS, group = slot / GS, base = slot - i;
+    const u32 key_shift = LV ? A.Lk - GS : 0u;   // Lq - l of the top level
     const bool special = i >= Lq;
     const LimbParams &p = lt.lp[i];
     // rows of special prime k of this group: accumulators (0, 1) and tau' (double-buffered by round parity)
@@ -877,13 +900,13 @@ __device__ __forceinline__ void ks_grouped_body(const KsArgs &A, const LimbTable
         const u64 *t_rows = A.scratch + ((size_t)base * 2 + parity) * N;   // row of limb j: + j * 2N
         if (!special) {
             const u32 g_own = i / Ks;
-            ks_phase1<LOGN, NT, MODE, true>(cta, buf, A, G.lp_up[i], ct, i, A.scratch + ((size_t)slot * 2 + parity) * N, acc_of(parity), K.qlm[i],
-                                            K.qlm_s[i], nullptr, 0, g_own, dot);
+            ks_phase1<LOGN, NT, MODE, true, LV>(cta, buf, A, G.lp_up[i], ct, i, A.scratch + ((size_t)slot * 2 + parity) * N, acc_of(parity), K.qlm[i],
+                                                K.qlm_s[i], nullptr, 0, g_own, dot, key_shift);
             publish(tag);
             for (u32 jj = 1; jj < dnum; ++jj) {
                 const u32 g = (g_own + jj) % dnum, lo = g * Ks, cnt = lo + Ks < Lq ? Ks : Lq - lo;
                 wait_for(base + lo, cnt, tag);
-                ks_phase2_group<LOGN, NT, false>(cta, buf, A, G, p, ct, i, g, jj, t_rows, 2 * N, acc_of(parity));
+                ks_phase2_group<LOGN, NT, false, LV>(cta, buf, A, G, p, ct, i, g, jj, t_rows, 2 * N, acc_of(parity), key_shift);
             }
             if constexpr (RS) if (i == Lq - 1) {
                 // the dropped limb.  Its y_qbar rows of this parity were last read by the divide() of round - 2, which every other
@@ -910,7 +933,7 @@ __device__ __forceinline__ void ks_grouped_body(const KsArgs &A, const LimbTable
             for (u32 jj = 0; jj < dnum; ++jj) {
                 const u32 g = (group + jj) % dnum, lo = g * Ks, cnt = lo + Ks < Lq ? Ks : Lq - lo;
                 wait_for(base + lo, cnt, tag);
-                ks_phase2_group<LOGN, NT, true>(cta, buf, A, G, p, ct, i, g, jj, t_rows, 2 * N, hyb);
+                ks_phase2_group<LOGN, NT, true, LV>(cta, buf, A, G, p, ct, i, g, jj, t_rows, 2 * N, hyb, key_shift);
             }
             for (u32 c = 0; c < 2; ++c)
                 ms_tau_body<LOGN, NT, true>(cta, buf, hyb + c * N, hyb + c * N, A.itw + (size_t)i * N, G.lp_up[i], hyb + ks_hyb_tau_row(parity, c) * N, K);
@@ -935,6 +958,18 @@ __global__ void __launch_bounds__(NT, MINB) ks_rescale_grouped_kernel(KsArgs A, 
                                                                       const __grid_constant__ RescaleConsts R, size_t batch, u32 *flags, u32 epoch,
                                                                       u32 *ticket, u64 *mail) {
     ks_grouped_body<LOGN, NT, MODE, false, true>(A, lt, K, G, batch, flags, epoch, ticket, mail, nullptr, MODE == KS_DOT ? &D : nullptr, &R);
+}
+
+// every grouped call at level l (DESIGN.md §2.20, §4.17): the program in mode MODE (KS_MUL_RELIN, KS_ROTATE, KS_DOT) with the division
+// by P (RS = false) or by P * q_{l-1} (RS = true, ks_rescale_grouped_kernel's), on the level's view, reading the top-level key.  One
+// parameter block, that of ks_rescale_grouped_kernel, for all of them; D and R are unused where the mode has none.
+template <int LOGN, int NT, int MINB, int MODE, bool RS>
+__global__ void __launch_bounds__(NT, MINB) ks_level_grouped_kernel(KsArgs A, const __grid_constant__ LimbTable lt, const __grid_constant__ MsConsts K,
+                                                                    const __grid_constant__ GroupConsts G, const __grid_constant__ DotArgs D,
+                                                                    const __grid_constant__ RescaleConsts R, size_t batch, u32 *flags, u32 epoch,
+                                                                    u32 *ticket, u64 *mail) {
+    ks_grouped_body<LOGN, NT, MODE, false, RS, true>(A, lt, K, G, batch, flags, epoch, ticket, mail, nullptr, MODE == KS_DOT ? &D : nullptr,
+                                                     RS ? &R : nullptr);
 }
 
 // the encrypted inner product: ks_grouped_kernel's program in mode KS_DOT, with the operand tables of the call in D
@@ -1041,6 +1076,25 @@ __global__ void __launch_bounds__(NT, MINB) rot_sum_grouped_kernel(const __grid_
         const size_t ct0 = (w / nseg / L) * ROT_CB;
         const u32 n_ct = (u32)(batch - ct0 < (size_t)ROT_CB ? batch - ct0 : (size_t)ROT_CB);
         rot_sum_grouped_rows<LOGN, NT, ROT_CB>(cta, A, G, K, lt.lp[i], ct0, n_ct, i, (int)seg * seg_chunks, ((int)seg + 1) * seg_chunks);
+    }
+}
+
+// the same at level l (DESIGN.md §2.20, §4.17): the keys are top-level keys, key_shift = Lq - l rows longer per (digit, component)
+template <int LOGN, int NT, int MINB, int ROT_CB>
+__global__ void __launch_bounds__(NT, MINB) rot_sum_grouped_level_kernel(const __grid_constant__ RotSumGArgs A, const __grid_constant__ LimbTable lt,
+                                                                         const __grid_constant__ MsConsts K, const __grid_constant__ GroupConsts G,
+                                                                         size_t batch, u32 nseg, u32 key_shift) {
+    DevCta<NT> cta;
+    constexpr int NC = 1 << (LOGN - 1);
+    const u32 L = G.Lq + G.K;
+    const size_t n_blocks = (batch + ROT_CB - 1) / ROT_CB, n_items = n_blocks * L * nseg;
+    const int seg_chunks = NC / (int)nseg;
+    for (size_t w = blockIdx.x; w < n_items; w += gridDim.x) {
+        const u32 seg = (u32)(w % nseg), i = (u32)((w / nseg) % L);
+        const size_t ct0 = (w / nseg / L) * ROT_CB;
+        const u32 n_ct = (u32)(batch - ct0 < (size_t)ROT_CB ? batch - ct0 : (size_t)ROT_CB);
+        rot_sum_grouped_rows<LOGN, NT, ROT_CB, true>(cta, A, G, K, lt.lp[i], ct0, n_ct, i, (int)seg * seg_chunks, ((int)seg + 1) * seg_chunks,
+                                                     key_shift);
     }
 }
 
@@ -1618,10 +1672,11 @@ static cudaError_t launch_ks_t(LaunchCtx &lc, const KsArgs &A, size_t batch, cud
 
 #endif
 #if DPFHE_PART_HYBRID
-template <int LOGN, int MODE>
+template <int LOGN, int MODE, bool LV = false>
 static cudaError_t launch_ks_hybrid_t(LaunchCtx &lc, const KsArgs &A, const MsConsts &K, size_t batch, cudaStream_t st) {
     constexpr int NT = 256, MINB = 3;
     auto kern = ks_hybrid_kernel<LOGN, NT, MINB, MODE>;
+    if constexpr (LV) kern = ks_hybrid_level_kernel<LOGN, NT, MINB, MODE>;
     const size_t smem = LOGN <= 13 ? Geometry<LOGN>::LIMB_BYTES : Geometry<13>::LIMB_BYTES;
     static ConfiguredMask configured;
     if (!configured.has(lc.device)) {
@@ -1693,14 +1748,40 @@ cudaError_t launch_ks_hybrid(LaunchCtx &lc, int mode, const u64 *a, const u64 *b
     return cudaErrorNotSupported;
 }
 
+// one special prime at level l (DESIGN.md §4.17): lc is the level's view (L = l + 1 limbs, its own tables), key the top-level key
+// [Lq][2][key_L][N] with its companions key_s, built by the caller over the top-level rows.  Modes KS_MUL_RELIN and KS_ROTATE.
+cudaError_t launch_ks_hybrid_level(LaunchCtx &lc, int mode, const u64 *a, const u64 *b, const u64 *key, const u64 *key_s, u32 key_L, u64 *out,
+                                   size_t batch, u32 galois, const MsConsts &K, cudaStream_t st) {
+    if (batch == 0) return cudaSuccess;
+    if (lc.L < 2 || key_L < lc.L || !key_s || !lc.ks_hyb || !lc.ks_acc_hyb) return cudaErrorInvalidValue;
+    KsArgs A;
+    A.a = a; A.b = b; A.key = key; A.key_s = key_s; A.out = out; A.scratch = lc.ks_scratch;
+    A.tw = lc.tw; A.itw = lc.itw; A.L = lc.L - 1; A.galois = galois; A.Lk = key_L; A.hyb = lc.ks_hyb; A.only = nullptr;
+    A.acc = lc.ks_acc_hyb; A.acc_par = 2; A.lift_reduce = lc.lift_reduce ? 1u : 0u;
+#define KS_HYB_LV_DISPATCH(LOGN)                                                                      \
+    switch (mode) {                                                                                   \
+        case KS_MUL_RELIN: return launch_ks_hybrid_t<LOGN, KS_MUL_RELIN, true>(lc, A, K, batch, st);   \
+        case KS_ROTATE: return launch_ks_hybrid_t<LOGN, KS_ROTATE, true>(lc, A, K, batch, st);         \
+    }                                                                                                 \
+    return cudaErrorInvalidValue;
+    switch (lc.log_n) {
+        case 12: KS_HYB_LV_DISPATCH(12)
+        case 13: KS_HYB_LV_DISPATCH(13)
+        case 14: KS_HYB_LV_DISPATCH(14)
+    }
+#undef KS_HYB_LV_DISPATCH
+    return cudaErrorNotSupported;
+}
+
 #endif
 #if DPFHE_PART_GROUPED
-template <int LOGN, int MODE, bool ADD = false, bool RS = false>
+template <int LOGN, int MODE, bool ADD = false, bool RS = false, bool LV = false>
 static cudaError_t launch_ks_grouped_t(LaunchCtx &lc, const KsArgs &A, const MsConsts &K, const GroupConsts &Gc, size_t batch, cudaStream_t st,
                                        const u64 *addend, const DotArgs *dot = nullptr, const RescaleConsts *rs = nullptr) {
     constexpr int NT = 256, MINB = 3;
     const void *kern;
-    if constexpr (RS) kern = (const void *)ks_rescale_grouped_kernel<LOGN, NT, MINB, MODE>;
+    if constexpr (LV) kern = (const void *)ks_level_grouped_kernel<LOGN, NT, MINB, MODE, RS>;
+    else if constexpr (RS) kern = (const void *)ks_rescale_grouped_kernel<LOGN, NT, MINB, MODE>;
     else if constexpr (MODE == KS_DOT) kern = (const void *)ct_dot_grouped_kernel<LOGN, NT, MINB>;
     else kern = (const void *)ks_grouped_kernel<LOGN, NT, MINB, MODE, ADD>;
     const size_t smem = LOGN <= 13 ? Geometry<LOGN>::LIMB_BYTES : Geometry<13>::LIMB_BYTES;
@@ -1742,7 +1823,7 @@ static cudaError_t launch_ks_grouped_t(LaunchCtx &lc, const KsArgs &A, const MsC
     RescaleConsts rc{};
     if (rs) rc = *rs;
     void *params_rs[] = {&args, &lt, &consts, &gc, dot ? const_cast<DotArgs *>(dot) : &no_dot, &rc, &batch_arg, &flags, &epoch, &ticket, &mail};
-    e = cudaLaunchCooperativeKernel(kern, dim3((unsigned)G), dim3(NT), RS ? params_rs : MODE == KS_DOT ? params_dot : params, smem, st);
+    e = cudaLaunchCooperativeKernel(kern, dim3((unsigned)G), dim3(NT), RS || LV ? params_rs : MODE == KS_DOT ? params_dot : params, smem, st);
     lc.ks_epoch += rounds;
     return e;
 }
@@ -1855,6 +1936,51 @@ cudaError_t launch_ks_rescale_grouped(LaunchCtx &lc, bool dot, const u64 *const 
         case 14: KS_RS_DISPATCH(14)
     }
 #undef KS_RS_DISPATCH
+    return cudaErrorNotSupported;
+}
+
+// every grouped call at level l (DESIGN.md §2.20, §4.17): lc is the level's view (L = l + K limbs, its own tables and Gc built on them),
+// key the top-level key [dnum][2][key_L][N] with its companions key_s, built by the caller over the top-level rows of the level's
+// digits.  mode KS_MUL_RELIN / KS_ROTATE (a[0], b[0]; galois) or KS_DOT (the n_terms pairs); R non-null: multiply-and-rescale (modes
+// KS_MUL_RELIN, KS_DOT), its rows and flags as launch_ks_rescale_grouped's.  One launch.
+cudaError_t launch_ks_grouped_level(LaunchCtx &lc, int mode, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, const u64 *key_s,
+                                    u32 key_L, u64 *out, size_t batch, u32 galois, const MsConsts &K, const GroupConsts &Gc, const RescaleConsts *R,
+                                    cudaStream_t st) {
+    if (batch == 0) return cudaSuccess;
+    if (lc.L < 2 || key_L < lc.L || !key_s || !lc.ks_hyb || !lc.ks_acc_hyb || Gc.Lq + Gc.K != lc.L || Gc.K > Gc.Lq || Gc.K > (u32)KS_MAX_SPECIAL)
+        return cudaErrorInvalidValue;
+    if (R && (mode == KS_ROTATE || lc.L < 3 || Gc.Lq < 2 || !lc.ks_tau_drop)) return cudaErrorInvalidValue;
+    if (n_terms < 1 || n_terms > (u32)DOT_MAX_TERMS || (mode != KS_DOT && n_terms != 1)) return cudaErrorInvalidValue;
+    const bool dot = mode == KS_DOT;
+    KsArgs A;
+    A.a = dot ? nullptr : a[0]; A.b = dot || !b ? nullptr : b[0]; A.key = key; A.key_s = key_s; A.out = out; A.scratch = lc.ks_scratch;
+    A.tw = lc.tw; A.itw = lc.itw; A.L = Gc.Lq; A.galois = galois; A.Lk = key_L; A.hyb = lc.ks_hyb; A.only = nullptr;
+    A.acc = lc.ks_acc_hyb; A.acc_par = 2; A.lift_reduce = 0u;
+    RescaleConsts Rc{};
+    if (R) {
+        Rc = *R;
+        Rc.tau = lc.ks_tau_drop;
+        Rc.tau_flag = lc.ks_flags + lc.ks_slots;
+    }
+    DotArgs D{};
+    D.n_terms = n_terms;
+    for (u32 t = 0; dot && t < n_terms; ++t) {
+        D.a[t] = a[t];
+        D.b[t] = b[t];
+    }
+#define KS_LV_DISPATCH(LOGN)                                                                                                        \
+    if (mode == KS_ROTATE) return launch_ks_grouped_t<LOGN, KS_ROTATE, false, false, true>(lc, A, K, Gc, batch, st, nullptr, nullptr, &Rc); \
+    if (R) return dot ? launch_ks_grouped_t<LOGN, KS_DOT, false, true, true>(lc, A, K, Gc, batch, st, nullptr, &D, &Rc)                  \
+                      : launch_ks_grouped_t<LOGN, KS_MUL_RELIN, false, true, true>(lc, A, K, Gc, batch, st, nullptr, nullptr, &Rc);   \
+    return dot ? launch_ks_grouped_t<LOGN, KS_DOT, false, false, true>(lc, A, K, Gc, batch, st, nullptr, &D, &Rc)                        \
+               : launch_ks_grouped_t<LOGN, KS_MUL_RELIN, false, false, true>(lc, A, K, Gc, batch, st, nullptr, nullptr, &Rc);
+    if (mode != KS_MUL_RELIN && mode != KS_ROTATE && mode != KS_DOT) return cudaErrorInvalidValue;
+    switch (lc.log_n) {
+        case 12: KS_LV_DISPATCH(12)
+        case 13: KS_LV_DISPATCH(13)
+        case 14: KS_LV_DISPATCH(14)
+    }
+#undef KS_LV_DISPATCH
     return cudaErrorNotSupported;
 }
 
@@ -2062,8 +2188,9 @@ cudaError_t launch_rot_apply_grouped(LaunchCtx &lc, const u64 *ct, const u64 *U,
 }
 
 // summed rotations: acc [batch][2][L][N] of n_rot (1 .. ROT_SUM_MAX) rotations with their keys' Shoup companions key_s[m]
+// key_shift > 0: a level view reading top-level keys (rot_sum_grouped_level_kernel, DESIGN.md §4.17)
 cudaError_t launch_rot_sum_grouped(const LaunchCtx &lc, const u64 *ct, const u64 *U, u32 n_rot, const u64 *const *keys, const u64 *const *key_s,
-                                   const u32 *galois, u64 *acc, const MsConsts &K, const GroupConsts &G, size_t batch, cudaStream_t st) {
+                                   const u32 *galois, u64 *acc, const MsConsts &K, const GroupConsts &G, size_t batch, cudaStream_t st, u32 key_shift) {
     if (batch == 0) return cudaSuccess;
     if (n_rot < 1 || n_rot > (u32)ROT_SUM_MAX || G.Lq + G.K != lc.L) return cudaErrorInvalidValue;
     RotSumGArgs A;
@@ -2081,6 +2208,15 @@ cudaError_t launch_rot_sum_grouped(const LaunchCtx &lc, const u64 *ct, const u64
     while (nseg < max_seg && rows * nseg < want) nseg *= 2;
     const size_t n_items = rows * nseg, cap = (size_t)lc.num_sms * 8;
     const unsigned grid = (unsigned)(n_items < cap ? n_items : cap);
+    if (key_shift) {
+        switch (lc.log_n) {
+            case 12: rot_sum_grouped_level_kernel<12, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg, key_shift); break;
+            case 13: rot_sum_grouped_level_kernel<13, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg, key_shift); break;
+            case 14: rot_sum_grouped_level_kernel<14, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg, key_shift); break;
+            default: return cudaErrorInvalidValue;
+        }
+        return cudaGetLastError();
+    }
     switch (lc.log_n) {
         case 12: rot_sum_grouped_kernel<12, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
         case 13: rot_sum_grouped_kernel<13, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;

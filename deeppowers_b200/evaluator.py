@@ -525,6 +525,59 @@ class Context:
         self._chk(self._l.dpfhe_ct_dot_rescale_grouped_host(self._h, int(n_special), n, _hptr(a), _hptr(b), _hptr(evk), _hptr(out, True),
                                                             a.size // (n * pq) if n else 0, int(t_plain)))
 
+    # calls at level `level` on this (top-level) context (DESIGN.md section 2.20): ciphertexts [batch][2][level][N] over q_0 ..
+    # q_{level-1}, the keys the context's top-level grouped keys [dnum][2][L][N]; bit for bit the same call on a context over
+    # {q_0 .. q_{level-1}, p_0 .. p_{K-1}} with the key restricted to it.  n_special <= level <= L - n_special.
+    def ct_mul_relin_grouped_level(self, n_special, level, a, b, evk, out, batch, t_plain=0, stream=None):
+        self._chk(self._l.dpfhe_ct_mul_relin_grouped_level(self._h, int(n_special), int(level), _ptr(a), _ptr(b), _ptr(evk), _ptr(out), batch,
+                                                           int(t_plain), _stream(stream)))
+
+    def ct_mul_relin_rescale_grouped_level(self, n_special, level, a, b, evk, out, batch, t_plain=0, stream=None):
+        """out: [batch][2][level-1][N]"""
+        self._chk(self._l.dpfhe_ct_mul_relin_rescale_grouped_level(self._h, int(n_special), int(level), _ptr(a), _ptr(b), _ptr(evk), _ptr(out),
+                                                                   batch, int(t_plain), _stream(stream)))
+
+    def _pairs(self, a_list, b_list):
+        n = len(a_list)
+        if len(b_list) != n:
+            raise ValueError("need as many right operands as left operands")
+        return n, (C.c_void_p * max(n, 1))(*[_ptr(x) for x in a_list]), (C.c_void_p * max(n, 1))(*[_ptr(x) for x in b_list])
+
+    def ct_dot_grouped_level(self, n_special, level, a_list, b_list, evk, out, batch, t_plain=0, stream=None):
+        n, pa, pb = self._pairs(a_list, b_list)
+        self._chk(self._l.dpfhe_ct_dot_grouped_level(self._h, int(n_special), int(level), n, pa, pb, _ptr(evk), _ptr(out), batch, int(t_plain),
+                                                     _stream(stream)))
+
+    def ct_dot_rescale_grouped_level(self, n_special, level, a_list, b_list, evk, out, batch, t_plain=0, stream=None):
+        """out: [batch][2][level-1][N]"""
+        n, pa, pb = self._pairs(a_list, b_list)
+        self._chk(self._l.dpfhe_ct_dot_rescale_grouped_level(self._h, int(n_special), int(level), n, pa, pb, _ptr(evk), _ptr(out), batch,
+                                                             int(t_plain), _stream(stream)))
+
+    def rotate_grouped_level(self, n_special, level, ct, galois_elt, gk, out, batch, t_plain=0, stream=None):
+        self._chk(self._l.dpfhe_rotate_grouped_level(self._h, int(n_special), int(level), _ptr(ct), int(galois_elt), _ptr(gk), _ptr(out), batch,
+                                                     int(t_plain), _stream(stream)))
+
+    def rotate_sum_grouped_level(self, n_special, level, ct, galois_elts, gks, out, batch, t_plain=0, stream=None):
+        n = len(galois_elts)
+        if len(gks) != n:
+            raise ValueError("need one key per Galois element")
+        ge = (C.c_uint64 * max(n, 1))(*[int(g) for g in galois_elts])
+        kp = (C.c_void_p * max(n, 1))(*[_ptr(k) for k in gks])
+        self._chk(self._l.dpfhe_rotate_sum_grouped_level(self._h, int(n_special), int(level), _ptr(ct), n, ge, kp, _ptr(out), batch, int(t_plain),
+                                                         _stream(stream)))
+
+    def ct_mul_relin_rescale_grouped_level_host(self, n_special, level, a, b, evk, out, t_plain=0):
+        """host form of ct_mul_relin_rescale_grouped_level (C-contiguous numpy uint64)"""
+        self._chk(self._l.dpfhe_ct_mul_relin_rescale_grouped_level_host(self._h, int(n_special), int(level), _hptr(a), _hptr(b), _hptr(evk),
+                                                                        _hptr(out, True), a.size // (2 * level * self.N), int(t_plain)))
+
+    def ct_dot_rescale_grouped_level_host(self, n_special, level, a, b, evk, out, t_plain=0):
+        """host form of ct_dot_rescale_grouped_level: a, b [n_terms][batch][2][level][N] (C-contiguous numpy uint64)"""
+        n = a.shape[0]
+        self._chk(self._l.dpfhe_ct_dot_rescale_grouped_level_host(self._h, int(n_special), int(level), n, _hptr(a), _hptr(b), _hptr(evk),
+                                                                  _hptr(out, True), a.size // (n * 2 * level * self.N) if n else 0, int(t_plain)))
+
     def mod_down_special(self, n_special, polys, out, n_polys, t_plain=0, stream=None):
         self._chk(self._l.dpfhe_mod_down_special(self._h, int(n_special), _ptr(polys), _ptr(out), n_polys, int(t_plain), _stream(stream)))
 

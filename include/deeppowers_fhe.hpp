@@ -291,6 +291,53 @@ public:
         if (a.size() != b.size()) throw std::invalid_argument("one right operand per left operand");
         check(dpfhe_ct_dot_rescale_grouped(ctx_, special, a.size(), a.data(), b.data(), relin_key, out, count, plain_modulus, stream));
     }
+    // the calls above at level `level` on this evaluator (DESIGN.md §2.20): batches hold `level` limbs (the rescale forms' out
+    // level-1), the keys are this evaluator's top-level grouped keys, read in place; special <= level <= limbs()-special.  Bit for
+    // bit the same call on an evaluator over the first `level` limbs and the special primes, with the key restricted to it.
+    void multiply_relin_grouped_device(unsigned special, unsigned level, const std::uint64_t *a, const std::uint64_t *b,
+                                       const std::uint64_t *relin_key, std::uint64_t *out, std::size_t count, std::uint64_t plain_modulus = 0,
+                                       void *stream = nullptr) {
+        check(dpfhe_ct_mul_relin_grouped_level(ctx_, special, level, a, b, relin_key, out, count, plain_modulus, stream));
+    }
+    void multiply_relin_rescale_grouped(unsigned special, unsigned level, ConstCiphertextBatch a, ConstCiphertextBatch b,
+                                        const std::uint64_t *relin_key, CiphertextBatch out, std::uint64_t plain_modulus = 0) {
+        same(a.count, b.count, out.count);
+        check(dpfhe_ct_mul_relin_rescale_grouped_level_host(ctx_, special, level, a.data, b.data, relin_key, out.data, a.count, plain_modulus));
+    }
+    void multiply_relin_rescale_grouped_device(unsigned special, unsigned level, const std::uint64_t *a, const std::uint64_t *b,
+                                               const std::uint64_t *relin_key, std::uint64_t *out, std::size_t count,
+                                               std::uint64_t plain_modulus = 0, void *stream = nullptr) {
+        check(dpfhe_ct_mul_relin_rescale_grouped_level(ctx_, special, level, a, b, relin_key, out, count, plain_modulus, stream));
+    }
+    void dot_relin_grouped_device(unsigned special, unsigned level, const std::vector<const std::uint64_t *> &a,
+                                  const std::vector<const std::uint64_t *> &b, const std::uint64_t *relin_key, std::uint64_t *out,
+                                  std::size_t count, std::uint64_t plain_modulus = 0, void *stream = nullptr) {
+        if (a.size() != b.size()) throw std::invalid_argument("one right operand per left operand");
+        check(dpfhe_ct_dot_grouped_level(ctx_, special, level, a.size(), a.data(), b.data(), relin_key, out, count, plain_modulus, stream));
+    }
+    void dot_relin_rescale_grouped(unsigned special, unsigned level, std::size_t n_terms, const std::uint64_t *a, const std::uint64_t *b,
+                                   const std::uint64_t *relin_key, CiphertextBatch out, std::uint64_t plain_modulus = 0) {
+        check(dpfhe_ct_dot_rescale_grouped_level_host(ctx_, special, level, n_terms, a, b, relin_key, out.data, out.count, plain_modulus));
+    }
+    void dot_relin_rescale_grouped_device(unsigned special, unsigned level, const std::vector<const std::uint64_t *> &a,
+                                          const std::vector<const std::uint64_t *> &b, const std::uint64_t *relin_key, std::uint64_t *out,
+                                          std::size_t count, std::uint64_t plain_modulus = 0, void *stream = nullptr) {
+        if (a.size() != b.size()) throw std::invalid_argument("one right operand per left operand");
+        check(dpfhe_ct_dot_rescale_grouped_level(ctx_, special, level, a.size(), a.data(), b.data(), relin_key, out, count, plain_modulus, stream));
+    }
+    void rotate_grouped_device(unsigned special, unsigned level, const std::uint64_t *ct, long steps, const std::uint64_t *galois_key,
+                               std::uint64_t *out, std::size_t count, std::uint64_t plain_modulus = 0, void *stream = nullptr) {
+        check(dpfhe_rotate_grouped_level(ctx_, special, level, ct, galois_element(steps), galois_key, out, count, plain_modulus, stream));
+    }
+    void rotate_sum_grouped_device(unsigned special, unsigned level, const std::uint64_t *ct, const std::vector<long> &steps,
+                                   const std::vector<const std::uint64_t *> &galois_keys, std::uint64_t *out, std::size_t count,
+                                   std::uint64_t plain_modulus = 0, void *stream = nullptr) {
+        if (steps.size() != galois_keys.size()) throw std::invalid_argument("one Galois key per rotation");
+        std::vector<std::uint64_t> elts(steps.size());
+        for (std::size_t r = 0; r < steps.size(); ++r) elts[r] = galois_element(steps[r]);
+        check(dpfhe_rotate_sum_grouped_level(ctx_, special, level, ct, steps.size(), elts.data(), galois_keys.data(), out, count, plain_modulus,
+                                             stream));
+    }
     // divide by the product of the last `special` limbs: in holds limbs() limbs per polynomial, out limbs()-special
     void mod_down_special_device(unsigned special, const std::uint64_t *ct, std::uint64_t *out, std::size_t count, std::uint64_t plain_modulus = 0,
                                  void *stream = nullptr) {

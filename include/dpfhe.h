@@ -296,6 +296,38 @@ int dpfhe_ct_mul_relin_rescale_grouped_host(dpfhe_ctx *ctx, unsigned n_special, 
                                             const uint64_t *h_evk, uint64_t *h_out, size_t batch, uint64_t t_plain);
 int dpfhe_ct_dot_rescale_grouped_host(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const uint64_t *h_as, const uint64_t *h_bs,
                                       const uint64_t *h_evk, uint64_t *h_out, size_t batch, uint64_t t_plain);
+/* ---- calls at level l on the top-level context (DESIGN.md §2.20).  The context's last K = n_special limbs are special primes and
+ *      Lq = L - K; a level-l ciphertext lies over q_0 .. q_{l-1}, [batch][2][level][N].  Each call below takes the arguments of the
+ *      call it is named after plus `level`, and is, bit for bit, that call on a context over {q_0 .. q_{l-1}, p_0 .. p_{K-1}} with
+ *      the key restricted to that basis: digits g < ceil(l / K), rows 0 .. l-1 and Lq .. Lq+K-1 (the last digit is shorter when K
+ *      does not divide l).  The keys are the context's TOP-LEVEL grouped keys [dnum][2][L][N], as dpfhe_relin_keygen /
+ *      dpfhe_galois_keygen write them; they are read in place, never copied or restricted.  level = Lq is the call itself.
+ *      Valid levels: K <= level <= Lq; the rescale forms also need level >= 2 and t_plain below q_{level-1} (their output is
+ *      [batch][2][level-1][N]); t_plain below every special prime as always.  A failed check leaves the output untouched and names
+ *      the level.  The first call at a (K, level) builds that level's tables on the context (counted in
+ *      dpfhe_context_device_bytes, released by dpfhe_context_trim); after that a level call launches what the top-level call
+ *      launches and allocates nothing.  Level calls and top-level calls share the context's round numbering and call order. ---- */
+int dpfhe_ct_mul_relin_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *d_a, const uint64_t *d_b,
+                                     const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream);
+int dpfhe_ct_mul_relin_rescale_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *d_a, const uint64_t *d_b,
+                                             const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream);
+int dpfhe_ct_dot_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, size_t n_terms, const uint64_t *const *d_as,
+                               const uint64_t *const *d_bs, const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream);
+int dpfhe_ct_dot_rescale_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, size_t n_terms, const uint64_t *const *d_as,
+                                       const uint64_t *const *d_bs, const uint64_t *d_evk, uint64_t *d_out, size_t batch, uint64_t t_plain,
+                                       void *stream);
+int dpfhe_rotate_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *d_ct, uint64_t galois_elt,
+                               const uint64_t *d_gk, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream);
+int dpfhe_rotate_sum_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *d_ct, size_t n_rot,
+                                   const uint64_t *galois_elts, const uint64_t *const *d_gks, uint64_t *d_out, size_t batch,
+                                   uint64_t t_plain, void *stream);
+/* host-buffer forms of the rescale calls: operands [batch][2][level][N] ([n_terms][batch][2][level][N]), h_out
+ * [batch][2][level-1][N]; the top-level key uploaded once, the batch pipelined in chunks (synchronous) */
+int dpfhe_ct_mul_relin_rescale_grouped_level_host(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *h_a,
+                                                  const uint64_t *h_b, const uint64_t *h_evk, uint64_t *h_out, size_t batch,
+                                                  uint64_t t_plain);
+int dpfhe_ct_dot_rescale_grouped_level_host(dpfhe_ctx *ctx, unsigned n_special, unsigned level, size_t n_terms, const uint64_t *h_as,
+                                            const uint64_t *h_bs, const uint64_t *h_evk, uint64_t *h_out, size_t batch, uint64_t t_plain);
 /* ---- slot sums (DESIGN.md §2.17): slot i of the result is sum_{j < count} x[(i + j * stride) mod N/2] in every row, count =
  *      prod radices[t], computed in n_stages (1 .. 16) summed-rotation stages; stage t rotates by m * stride * prod_{u<t} radices[u],
  *      m = 1 .. radices[t] - 1 (2 <= radices[t] <= 16), and stride * count must be at most N/2.
