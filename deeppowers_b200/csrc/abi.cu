@@ -285,7 +285,7 @@ int prepare_keys(dpfhe_ctx *ctx, const LaunchCtx &lc, size_t n, size_t dnum, cud
     for (size_t k = 0; k < n && e == cudaSuccess; ++k) {
         pk.keys.push_back(pk.d_keys + k * key_words);
         pk.key_s.push_back(pk.d_key_s + k * key_words);
-        e = VCALL(launch_key_prepare_grouped, lc, pk.keys[k], pk.d_key_s + k * key_words, (u32)dnum, st);
+        e = VCALL(launch_key_prepare, lc, pk.keys[k], pk.d_key_s + k * key_words, (u32)dnum, st);
         note_launch(ctx, 1);
     }
     if (e != cudaSuccess) {
@@ -912,10 +912,10 @@ static int level_launch(dpfhe_ctx *ctx, unsigned K, unsigned l, int mode, bool r
     else if (rescale) build_rescale_consts(v->hp, K, t_plain, G, Kc, R);
     else build_group_consts(v->hp, K, t_plain, G, Kc);
     cudaStream_t st = pick(ctx, stream);
-    CU_TRY(VCALL(launch_key_prepare_grouped, ctx->lc, key, ctx->lc.ks_key_s, (u32)((l + K - 1) / K), st));
+    CU_TRY(VCALL(launch_key_prepare, ctx->lc, key, ctx->lc.ks_key_s, (u32)((l + K - 1) / K), st));
     const u32 key_L = ctx->hp.L;
     CU_TRY(on_level_view(ctx, *v, [&](LaunchCtx &lc) {
-        if (hybrid) return VCALL(launch_ks_hybrid_level, lc, mode, as[0], bs ? bs[0] : nullptr, key, lc.ks_key_s, key_L, out, batch, (u32)galois, Kc, st);
+        if (hybrid) return VCALL(launch_ks_hybrid, lc, mode, as[0], bs ? bs[0] : nullptr, key, out, batch, (u32)galois, Kc, st, lc.ks_key_s, key_L);
         return VCALL(launch_ks_grouped_level, lc, mode, as, bs, (u32)n_terms, key, lc.ks_key_s, key_L, out, batch, (u32)galois, Kc, G,
                      rescale ? &R : nullptr, st);
     }));
@@ -1195,7 +1195,7 @@ static int rotate_sum_prepare(dpfhe_ctx *ctx, unsigned n_special, size_t n_rot, 
     if (rc) return rc;
     u64 *key_s = ctx->hoistg.get();
     for (size_t r = 0; r < n_rot; ++r) {
-        CU_TRY(VCALL(launch_key_prepare_grouped, ctx->lc, d_gks[r], key_s + r * key_words, (u32)dnum, st));
+        CU_TRY(VCALL(launch_key_prepare, ctx->lc, d_gks[r], key_s + r * key_words, (u32)dnum, st));
         note_launch(ctx, 1);
         pr.key_s[r] = key_s + r * key_words;
         pr.galois[r] = (u32)galois_elts[r];

@@ -4,10 +4,8 @@
 // separate compilation unit: no kernel of kernels.cu or keys.cu shares a body with it.
 #include <cuda_runtime.h>
 
-#include <atomic>
-
 #include "eval.cuh"
-#include "launch.hpp"
+#include "launch_util.hpp"
 
 namespace dpfhe {
 namespace DPFHE_VNS {
@@ -33,10 +31,7 @@ cudaError_t launch_lincomb_t(const LaunchCtx &lc, const u64 *const *in, const in
     A.pt = reinterpret_cast<const U64x2 *>(pt);
     A.log_half = lc.log_n - 1;
     A.n_chunks = batch * 2 * lc.L * ((size_t)1 << (lc.log_n - 1));
-    size_t blocks = (A.n_chunks + 255) / 256;
-    const size_t cap = (size_t)lc.num_sms * 32;   // as the element-wise kernels of kernels.cu
-    if (blocks > cap) blocks = cap;
-    ct_lincomb_kernel<MAXT><<<(unsigned)blocks, 256, 0, st>>>(A, lc.lp);
+    ct_lincomb_kernel<MAXT><<<ew_grid(lc, A.n_chunks), 256, 0, st>>>(A, lc.lp);
     return cudaGetLastError();
 }
 
@@ -109,25 +104,15 @@ __global__ void __launch_bounds__(NT, MINB) ckks_comb_limb_kernel(const __grid_c
 
 namespace {
 
-struct CombConfigured {
-    std::atomic<unsigned long long> bits{0};
-    bool has(int device) const { return (bits.load(std::memory_order_acquire) >> (device & 63)) & 1ull; }
-    void set(int device) { bits.fetch_or(1ull << (device & 63), std::memory_order_release); }
-};
-
 template <int LOGN, int NT, int MINB, int MAXT>
 cudaError_t launch_ckks_comb_t(const LaunchCtx &lc, const u64 *const *in, const u32 *levels, const double *coeffs, u32 n_terms, double constant,
                                const MsConsts &K, u64 *tau, u64 *out, size_t batch, cudaStream_t st) {
     auto k1 = ckks_comb_tau_kernel<LOGN, NT, MINB, MAXT>;
     auto k2 = ckks_comb_limb_kernel<LOGN, NT, MINB, MAXT>;
     const size_t smem = (size_t)8 << LOGN;
-    static CombConfigured configured;
-    if (!configured.has(lc.device)) {
-        cudaError_t e = cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        configured.set(lc.device);
-    }
+    static ConfiguredMask configured;
+    cudaError_t e = set_smem_once(configured, lc.device, smem, k1, k2);
+    if (e != cudaSuccess) return e;
     CkksCombArgs<MAXT> A;
     build_ckks_comb_coeffs(lc.lt.lp, lc.L, coeffs, n_terms, constant, A);
     for (u32 i = 0; i < n_terms; ++i) {
@@ -138,7 +123,7 @@ cudaError_t launch_ckks_comb_t(const LaunchCtx &lc, const u64 *const *in, const 
     A.K = K;
     const size_t n_polys = 2 * batch, n_items = n_polys * (lc.L - 1);
     k1<<<(unsigned)(n_polys < 0x7fffffffull ? n_polys : 0x7fffffffull), NT, smem, st>>>(A, lc.lt, lc.itw, tau, n_polys);
-    cudaError_t e = cudaGetLastError();
+    e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     k2<<<(unsigned)(n_items < 0x7fffffffull ? n_items : 0x7fffffffull), NT, smem, st>>>(A, lc.lt, lc.tw, tau, out, n_items);
     return cudaGetLastError();
@@ -162,12 +147,10 @@ cudaError_t launch_ckks_comb(const LaunchCtx &lc, const u64 *const *in, const u3
     if (n_terms < 1 || n_terms > (u32)CKKS_COMB_MAX_TERMS || lc.L < 2 || lc.L > 16) return cudaErrorInvalidValue;
     for (u32 i = 0; i < n_terms; ++i)
         if (levels[i] < lc.L) return cudaErrorInvalidValue;
-    switch (lc.log_n) {
-        case 12: return launch_ckks_comb_n<12, 256, 2>(lc, in, levels, coeffs, n_terms, constant, K, tau, out, batch, st);
-        case 13: return launch_ckks_comb_n<13, 256, 3>(lc, in, levels, coeffs, n_terms, constant, K, tau, out, batch, st);
-        case 14: return launch_ckks_comb_n<14, 512, 1>(lc, in, levels, coeffs, n_terms, constant, K, tau, out, batch, st);
-    }
-    return cudaErrorInvalidValue;
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value, NT = LOGN == 14 ? 512 : 256, MINB = LOGN == 12 ? 2 : LOGN == 13 ? 3 : 1;
+        return launch_ckks_comb_n<LOGN, NT, MINB>(lc, in, levels, coeffs, n_terms, constant, K, tau, out, batch, st);
+    });
 }
 
 }  // namespace DPFHE_VNS

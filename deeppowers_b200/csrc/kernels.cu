@@ -12,7 +12,7 @@
 #include <atomic>
 
 #include "kernel_bodies.cuh"
-#include "launch.hpp"
+#include "launch_util.hpp"
 
 // The file is large (every kernel x three ring degrees x three modes); the build compiles it in two parts per variant, in parallel:
 // -DDPFHE_PART=1 everything but the special-prime key-switch family, 2 its one-special-prime kernel, 3 the grouped kernels; no flag = all.
@@ -1224,22 +1224,8 @@ template <int LOGN>
 struct Geometry {
     static constexpr int NT = LOGN == 12 ? 256 : 512;
     static constexpr size_t LIMB_BYTES = (size_t)8 << LOGN;
+    static constexpr size_t KS_SMEM = (size_t)8 << (LOGN <= 13 ? LOGN : 13);   // persistent key-switch kernels: a limb, half a limb at N = 16384
 };
-
-// "already configured on this device" bits of one kernel (a function-local static per launcher instantiation).  Several
-// host threads may drive different devices at once (dpfhe_multi_*): the attribute call is idempotent, the bit set atomic.
-struct ConfiguredMask {
-    std::atomic<unsigned long long> bits{0};
-    bool has(int device) const { return (bits.load(std::memory_order_acquire) >> (device & 63)) & 1ull; }
-    void set(int device) { bits.fetch_or(1ull << (device & 63), std::memory_order_release); }
-};
-
-static unsigned ew_grid(const LaunchCtx &lc, size_t work_items) {
-    size_t blocks = (work_items + 255) / 256;
-    const size_t cap = (size_t)lc.num_sms * 32;   // 8 resident CTAs of 256 threads per SM, 4 waves
-    if (blocks > cap) blocks = cap;
-    return (unsigned)(blocks ? blocks : 1);
-}
 
 #if DPFHE_PART_MAIN
 template <int LOGN, int NT, int MINB, bool INV>
@@ -1247,11 +1233,8 @@ static cudaError_t launch_ntt_t(const LaunchCtx &lc, u64 *data, size_t n_limbs, 
     auto kern = ntt_kernel<LOGN, NT, MINB, INV>;
     const size_t smem = Geometry<LOGN>::LIMB_BYTES;
     static ConfiguredMask configured;
-    if (!configured.has(lc.device)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        configured.set(lc.device);
-    }
+    cudaError_t e = set_smem_once(configured, lc.device, smem, kern);
+    if (e != cudaSuccess) return e;
     // one CTA per limb transform; the grid-stride loop only matters beyond 2^31-1 limbs
     const size_t grid = n_limbs < 0x7fffffffull ? n_limbs : 0x7fffffffull;
     kern<<<(unsigned)grid, NT, smem, st>>>(data, INV ? lc.itw : lc.tw, lc.lt, lc.L, n_limbs);
@@ -1291,11 +1274,8 @@ static cudaError_t launch_ntt_inv_tma(const LaunchCtx &lc, u64 *data, size_t n_l
     auto kern = ntt_inv_tma_kernel<LOGN, NT, MINB>;
     const size_t smem = Geometry<LOGN>::LIMB_BYTES;
     static ConfiguredMask configured;
-    if (!configured.has(lc.device)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        configured.set(lc.device);
-    }
+    cudaError_t e = set_smem_once(configured, lc.device, smem, kern);
+    if (e != cudaSuccess) return e;
     kern<<<(unsigned)n_limbs, NT, smem, st>>>(tm, data, lc.itw, lc.lt, lc.L);
     return cudaGetLastError();
 }
@@ -1317,87 +1297,52 @@ static cudaError_t launch_ntt_pair_t(const LaunchCtx &lc, u64 *data, size_t n_li
     auto kern = ntt_pair_kernel<NT, MINB, INV>;
     const size_t smem = Geometry<13>::LIMB_BYTES;   // half a limb
     static ConfiguredMask configured;
-    if (!configured.has(lc.device)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        configured.set(lc.device);
-    }
+    cudaError_t e = set_smem_once(configured, lc.device, smem, kern);
+    if (e != cudaSuccess) return e;
     const size_t pairs = n_limbs < 0x3fffffffull ? n_limbs : 0x3fffffffull;
     kern<<<(unsigned)(2 * pairs), NT, smem, st>>>(data, INV ? lc.itw : lc.tw, lc.lt, lc.L, n_limbs);
     return cudaGetLastError();
-}
-static cudaError_t launch_ntt_pair(const LaunchCtx &lc, u64 *data, size_t n_limbs, bool inverse, cudaStream_t st) {
-    return inverse ? launch_ntt_pair_t<true>(lc, data, n_limbs, st) : launch_ntt_pair_t<false>(lc, data, n_limbs, st);
 }
 
 cudaError_t launch_ntt(const LaunchCtx &lc, u64 *data, size_t n_polys, bool inverse, cudaStream_t st) {
     const size_t n_limbs = n_polys * lc.L;
     if (n_limbs == 0) return cudaSuccess;
-    switch (lc.log_n) {
-        case 12: return launch_ntt_dir<12, 256, 2>(lc, data, n_limbs, inverse, st);
-        case 13:
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value;
+        if constexpr (LOGN == 12) {
+            return launch_ntt_dir<12, 256, 2>(lc, data, n_limbs, inverse, st);
+        } else if constexpr (LOGN == 13) {
             switch (lc.ntt_cfg) {   // tuning variants (DPFHE_NTT_CFG), default 0
                 case 1: return launch_ntt_dir<13, 512, 1>(lc, data, n_limbs, inverse, st);   //  9.9 M NTT/s
                 case 2: return launch_ntt_dir<13, 512, 2>(lc, data, n_limbs, inverse, st);   // 12.6 M (64 regs, spills)
                 case 3: return launch_ntt_dir<13, 256, 2>(lc, data, n_limbs, inverse, st);   // 12.3 M
                 default: return launch_ntt_dir<13, 256, 3>(lc, data, n_limbs, inverse, st);  // 13.2 M: 3 CTAs/SM (smem-limited), 80 regs
             }
-        case 14:
+        } else {
             if (lc.ntt_cfg == 1) return launch_ntt_dir<14, 512, 1>(lc, data, n_limbs, inverse, st);   // whole limb per CTA, 1 CTA/SM
-            return launch_ntt_pair(lc, data, n_limbs, inverse, st);                                   // CTA pair per limb, 3 CTAs/SM
-    }
-    return cudaErrorInvalidValue;
-}
-
-template <int LOGN, int NT, int MINB>
-static cudaError_t launch_ms_t(const LaunchCtx &lc, const u64 *in, u64 *tau, u64 *out, const MsConsts &K, size_t n_polys, cudaStream_t st) {
-    auto k1 = ms_tau_kernel<LOGN, NT, MINB>;
-    auto k2 = ms_limb_kernel<LOGN, NT, MINB>;
-    const size_t smem = Geometry<LOGN>::LIMB_BYTES;
-    static ConfiguredMask configured;
-    if (!configured.has(lc.device)) {
-        cudaError_t e = cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        configured.set(lc.device);
-    }
-    const size_t n_items = n_polys * (lc.L - 1);
-    k1<<<(unsigned)(n_polys < 0x7fffffffull ? n_polys : 0x7fffffffull), NT, smem, st>>>(in, tau, lc.itw, lc.lt, K, lc.L, n_polys);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    k2<<<(unsigned)(n_items < 0x7fffffffull ? n_items : 0x7fffffffull), NT, smem, st>>>(in, tau, out, lc.tw, lc.lt, K, lc.L, n_items);
-    return cudaGetLastError();
+            // CTA pair per limb, 3 CTAs/SM
+            return inverse ? launch_ntt_pair_t<true>(lc, data, n_limbs, st) : launch_ntt_pair_t<false>(lc, data, n_limbs, st);
+        }
+    });
 }
 
 cudaError_t launch_mod_switch(const LaunchCtx &lc, const u64 *in, u64 *tau, u64 *out, const MsConsts &K, size_t n_polys, cudaStream_t st) {
     if (n_polys == 0) return cudaSuccess;
-    switch (lc.log_n) {
-        case 12: return launch_ms_t<12, 256, 2>(lc, in, tau, out, K, n_polys, st);
-        case 13: return launch_ms_t<13, 256, 3>(lc, in, tau, out, K, n_polys, st);
-        case 14: return launch_ms_t<14, 512, 1>(lc, in, tau, out, K, n_polys, st);
-    }
-    return cudaErrorInvalidValue;
-}
-
-template <int LOGN, int NT, int MINB>
-static cudaError_t launch_md_t(const LaunchCtx &lc, const u64 *in, u64 *tau, u64 *out, const MsConsts &K, const GroupConsts &G, size_t n_polys,
-                               cudaStream_t st) {
-    auto k1 = md_tau_kernel<LOGN, NT, MINB>;
-    auto k2 = md_limb_kernel<LOGN, NT, MINB>;
-    const size_t smem = Geometry<LOGN>::LIMB_BYTES;
-    static ConfiguredMask configured;
-    if (!configured.has(lc.device)) {
-        cudaError_t e = cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value, NT = LOGN == 14 ? 512 : 256, MINB = LOGN == 12 ? 2 : LOGN == 13 ? 3 : 1;
+        const size_t smem = Geometry<LOGN>::LIMB_BYTES;
+        auto k1 = ms_tau_kernel<LOGN, NT, MINB>;
+        auto k2 = ms_limb_kernel<LOGN, NT, MINB>;
+        static ConfiguredMask configured;
+        cudaError_t e = set_smem_once(configured, lc.device, smem, k1, k2);
         if (e != cudaSuccess) return e;
-        configured.set(lc.device);
-    }
-    const size_t n_tau = n_polys * G.K, n_items = n_polys * G.Lq;
-    k1<<<(unsigned)(n_tau < 0x7fffffffull ? n_tau : 0x7fffffffull), NT, smem, st>>>(in, tau, lc.itw, K, G, n_tau);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    k2<<<(unsigned)(n_items < 0x7fffffffull ? n_items : 0x7fffffffull), NT, smem, st>>>(in, tau, out, lc.tw, lc.lt, K, G, n_items);
-    return cudaGetLastError();
+        const size_t n_items = n_polys * (lc.L - 1);
+        k1<<<(unsigned)(n_polys < 0x7fffffffull ? n_polys : 0x7fffffffull), NT, smem, st>>>(in, tau, lc.itw, lc.lt, K, lc.L, n_polys);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+        k2<<<(unsigned)(n_items < 0x7fffffffull ? n_items : 0x7fffffffull), NT, smem, st>>>(in, tau, out, lc.tw, lc.lt, K, lc.L, n_items);
+        return cudaGetLastError();
+    });
 }
 
 // in [n_polys][L][N] -> out [n_polys][L-K][N]; tau: n_polys * K * N words of scratch
@@ -1405,156 +1350,125 @@ cudaError_t launch_mod_down_special(const LaunchCtx &lc, const u64 *in, u64 *tau
                                     cudaStream_t st) {
     if (n_polys == 0) return cudaSuccess;
     if (G.Lq + G.K != lc.L) return cudaErrorInvalidValue;
-    switch (lc.log_n) {
-        case 12: return launch_md_t<12, 256, 2>(lc, in, tau, out, K, G, n_polys, st);
-        case 13: return launch_md_t<13, 256, 3>(lc, in, tau, out, K, G, n_polys, st);
-        case 14: return launch_md_t<14, 512, 1>(lc, in, tau, out, K, G, n_polys, st);
-    }
-    return cudaErrorInvalidValue;
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value, NT = LOGN == 14 ? 512 : 256, MINB = LOGN == 12 ? 2 : LOGN == 13 ? 3 : 1;
+        const size_t smem = Geometry<LOGN>::LIMB_BYTES;
+        auto k1 = md_tau_kernel<LOGN, NT, MINB>;
+        auto k2 = md_limb_kernel<LOGN, NT, MINB>;
+        static ConfiguredMask configured;
+        cudaError_t e = set_smem_once(configured, lc.device, smem, k1, k2);
+        if (e != cudaSuccess) return e;
+        const size_t n_tau = n_polys * G.K, n_items = n_polys * G.Lq;
+        k1<<<(unsigned)(n_tau < 0x7fffffffull ? n_tau : 0x7fffffffull), NT, smem, st>>>(in, tau, lc.itw, K, G, n_tau);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+        k2<<<(unsigned)(n_items < 0x7fffffffull ? n_items : 0x7fffffffull), NT, smem, st>>>(in, tau, out, lc.tw, lc.lt, K, G, n_items);
+        return cudaGetLastError();
+    });
 }
 
 // ---- CKKS slot encoding
 constexpr int CKKS_FFT_NT = 512;
 
-template <class K>
-static cudaError_t set_smem_once(K kern, size_t smem, ConfiguredMask &configured, int device) {
-    if (configured.has(device)) return cudaSuccess;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) configured.set(device);
-    return e;
-}
-
-template <int LOGN>
-static cudaError_t launch_ckks_encode_t(const LaunchCtx &lc, const Cplx *slots, double *coeffs, u64 *pt, const CkksTables &T, double sc,
-                                        size_t n_vec, cudaStream_t st) {
-    auto kf = ckks_enc_fft_kernel<LOGN, CKKS_FFT_NT>;
-    const size_t smem_fft = ((size_t)1 << (LOGN - 1)) * sizeof(Cplx);
-    static ConfiguredMask conf_fft, conf_ntt;
-    cudaError_t e = set_smem_once(kf, smem_fft, conf_fft, lc.device);
-    if (e != cudaSuccess) return e;
-    kf<<<(unsigned)n_vec, CKKS_FFT_NT, smem_fft, st>>>(slots, coeffs, T.tw, T.tj, sc);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    const size_t n_limbs = n_vec * lc.L;
-    if constexpr (LOGN == NTT_PAIR_LOGN) {
-        auto kn = ckks_enc_ntt_pair_kernel<256, 2>;   // at 3 CTAs per SM (80 registers) the reducing load stage spills
-        const size_t smem = Geometry<13>::LIMB_BYTES;   // half a limb
-        e = set_smem_once(kn, smem, conf_ntt, lc.device);
-        if (e != cudaSuccess) return e;
-        kn<<<(unsigned)(2 * n_limbs), 256, smem, st>>>(coeffs, pt, lc.tw, T.pow2, lc.lt, lc.L);
-    } else {
-        constexpr int MINB = LOGN == 12 ? 2 : 3;
-        auto kn = ckks_enc_ntt_kernel<LOGN, 256, MINB>;
-        const size_t smem = Geometry<LOGN>::LIMB_BYTES;
-        e = set_smem_once(kn, smem, conf_ntt, lc.device);
-        if (e != cudaSuccess) return e;
-        kn<<<(unsigned)n_limbs, 256, smem, st>>>(coeffs, pt, lc.tw, T.pow2, lc.lt, lc.L);
-    }
-    return cudaGetLastError();
-}
-
 cudaError_t launch_ckks_encode(const LaunchCtx &lc, const Cplx *slots, double *coeffs, u64 *pt, const CkksTables &T, double sc, size_t n_vec,
                                cudaStream_t st) {
     if (n_vec == 0) return cudaSuccess;
     if (n_vec * lc.L * 2 > 0x7fffffffull) return cudaErrorInvalidValue;
-    switch (lc.log_n) {
-        case 12: return launch_ckks_encode_t<12>(lc, slots, coeffs, pt, T, sc, n_vec, st);
-        case 13: return launch_ckks_encode_t<13>(lc, slots, coeffs, pt, T, sc, n_vec, st);
-        case 14: return launch_ckks_encode_t<14>(lc, slots, coeffs, pt, T, sc, n_vec, st);
-    }
-    return cudaErrorInvalidValue;
-}
-
-template <int LOGN>
-static cudaError_t launch_ckks_decode_t(const LaunchCtx &lc, u64 *work, Cplx *slots, const CkksTables &T, const CkksConsts &K, size_t n_vec,
-                                        cudaStream_t st) {
-    auto kd = ckks_dec_kernel<LOGN, CKKS_FFT_NT>;
-    const size_t smem = ((size_t)1 << (LOGN - 1)) * sizeof(Cplx);
-    static ConfiguredMask conf;
-    cudaError_t e = set_smem_once(kd, smem, conf, lc.device);
-    if (e != cudaSuccess) return e;
-    kd<<<(unsigned)n_vec, CKKS_FFT_NT, smem, st>>>(work, slots, T.tw, T.tj, lc.lt, K, lc.L);
-    return cudaGetLastError();
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value;
+        auto kf = ckks_enc_fft_kernel<LOGN, CKKS_FFT_NT>;
+        const size_t smem_fft = ((size_t)1 << (LOGN - 1)) * sizeof(Cplx);
+        static ConfiguredMask conf_fft, conf_ntt;
+        cudaError_t e = set_smem_once(conf_fft, lc.device, smem_fft, kf);
+        if (e != cudaSuccess) return e;
+        kf<<<(unsigned)n_vec, CKKS_FFT_NT, smem_fft, st>>>(slots, coeffs, T.tw, T.tj, sc);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+        const size_t n_limbs = n_vec * lc.L;
+        if constexpr (LOGN == NTT_PAIR_LOGN) {
+            auto kn = ckks_enc_ntt_pair_kernel<256, 2>;   // at 3 CTAs per SM (80 registers) the reducing load stage spills
+            const size_t smem = Geometry<13>::LIMB_BYTES;   // half a limb
+            e = set_smem_once(conf_ntt, lc.device, smem, kn);
+            if (e != cudaSuccess) return e;
+            kn<<<(unsigned)(2 * n_limbs), 256, smem, st>>>(coeffs, pt, lc.tw, T.pow2, lc.lt, lc.L);
+        } else {
+            constexpr int MINB = LOGN == 12 ? 2 : 3;
+            auto kn = ckks_enc_ntt_kernel<LOGN, 256, MINB>;
+            const size_t smem = Geometry<LOGN>::LIMB_BYTES;
+            e = set_smem_once(conf_ntt, lc.device, smem, kn);
+            if (e != cudaSuccess) return e;
+            kn<<<(unsigned)n_limbs, 256, smem, st>>>(coeffs, pt, lc.tw, T.pow2, lc.lt, lc.L);
+        }
+        return cudaGetLastError();
+    });
 }
 
 // work: [n_vec][L][N] inverse transforms of the plaintexts (overwritten)
 cudaError_t launch_ckks_decode(const LaunchCtx &lc, u64 *work, Cplx *slots, const CkksTables &T, const CkksConsts &K, size_t n_vec, cudaStream_t st) {
     if (n_vec == 0) return cudaSuccess;
     if (n_vec > 0x7fffffffull) return cudaErrorInvalidValue;
-    switch (lc.log_n) {
-        case 12: return launch_ckks_decode_t<12>(lc, work, slots, T, K, n_vec, st);
-        case 13: return launch_ckks_decode_t<13>(lc, work, slots, T, K, n_vec, st);
-        case 14: return launch_ckks_decode_t<14>(lc, work, slots, T, K, n_vec, st);
-    }
-    return cudaErrorInvalidValue;
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value;
+        auto kd = ckks_dec_kernel<LOGN, CKKS_FFT_NT>;
+        const size_t smem = ((size_t)1 << (LOGN - 1)) * sizeof(Cplx);
+        static ConfiguredMask conf;
+        cudaError_t e = set_smem_once(conf, lc.device, smem, kd);
+        if (e != cudaSuccess) return e;
+        kd<<<(unsigned)n_vec, CKKS_FFT_NT, smem, st>>>(work, slots, T.tw, T.tj, lc.lt, K, lc.L);
+        return cudaGetLastError();
+    });
 }
 
 // ---- BGV slot encoding
 constexpr int BGV_NT = 512;
 
-template <int LOGN>
-static cudaError_t launch_bgv_encode_t(const LaunchCtx &lc, const int64_t *slots, u32 *coeffs, u64 *pt, const BgvTables &T, size_t n_vec,
-                                       cudaStream_t st) {
-    auto ke = bgv_enc_kernel<LOGN, BGV_NT>;
-    const size_t smem_t = ((size_t)1 << LOGN) * sizeof(u32);
-    static ConfiguredMask conf_enc, conf_ntt;
-    cudaError_t e = set_smem_once(ke, smem_t, conf_enc, lc.device);
-    if (e != cudaSuccess) return e;
-    ke<<<(unsigned)n_vec, BGV_NT, smem_t, st>>>(slots, coeffs, T);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    const size_t n_limbs = n_vec * lc.L;
-    if constexpr (LOGN == NTT_PAIR_LOGN) {
-        auto kn = bgv_enc_ntt_pair_kernel<256, 2>;
-        const size_t smem = Geometry<13>::LIMB_BYTES;   // half a limb
-        e = set_smem_once(kn, smem, conf_ntt, lc.device);
-        if (e != cudaSuccess) return e;
-        kn<<<(unsigned)(2 * n_limbs), 256, smem, st>>>(coeffs, pt, lc.tw, T.m.t, lc.lt, lc.L);
-    } else {
-        constexpr int MINB = LOGN == 12 ? 2 : 3;
-        auto kn = bgv_enc_ntt_kernel<LOGN, 256, MINB>;
-        const size_t smem = Geometry<LOGN>::LIMB_BYTES;
-        e = set_smem_once(kn, smem, conf_ntt, lc.device);
-        if (e != cudaSuccess) return e;
-        kn<<<(unsigned)n_limbs, 256, smem, st>>>(coeffs, pt, lc.tw, T.m.t, lc.lt, lc.L);
-    }
-    return cudaGetLastError();
-}
-
 // coeffs: [n_vec][N] words of scratch
 cudaError_t launch_bgv_encode(const LaunchCtx &lc, const int64_t *slots, u32 *coeffs, u64 *pt, const BgvTables &T, size_t n_vec, cudaStream_t st) {
     if (n_vec == 0) return cudaSuccess;
     if (n_vec * lc.L * 2 > 0x7fffffffull) return cudaErrorInvalidValue;
-    switch (lc.log_n) {
-        case 12: return launch_bgv_encode_t<12>(lc, slots, coeffs, pt, T, n_vec, st);
-        case 13: return launch_bgv_encode_t<13>(lc, slots, coeffs, pt, T, n_vec, st);
-        case 14: return launch_bgv_encode_t<14>(lc, slots, coeffs, pt, T, n_vec, st);
-    }
-    return cudaErrorInvalidValue;
-}
-
-template <int LOGN>
-static cudaError_t launch_bgv_decode_t(const LaunchCtx &lc, u64 *work, u64 *slots, const BgvTables &T, const BgvConsts &K, size_t n_vec,
-                                       cudaStream_t st) {
-    auto kd = bgv_dec_kernel<LOGN, BGV_NT>;
-    const size_t smem = ((size_t)1 << LOGN) * sizeof(u32);
-    static ConfiguredMask conf;
-    cudaError_t e = set_smem_once(kd, smem, conf, lc.device);
-    if (e != cudaSuccess) return e;
-    kd<<<(unsigned)n_vec, BGV_NT, smem, st>>>(work, slots, T, lc.lt, K, lc.L);
-    return cudaGetLastError();
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value;
+        auto ke = bgv_enc_kernel<LOGN, BGV_NT>;
+        const size_t smem_t = ((size_t)1 << LOGN) * sizeof(u32);
+        static ConfiguredMask conf_enc, conf_ntt;
+        cudaError_t e = set_smem_once(conf_enc, lc.device, smem_t, ke);
+        if (e != cudaSuccess) return e;
+        ke<<<(unsigned)n_vec, BGV_NT, smem_t, st>>>(slots, coeffs, T);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+        const size_t n_limbs = n_vec * lc.L;
+        if constexpr (LOGN == NTT_PAIR_LOGN) {
+            auto kn = bgv_enc_ntt_pair_kernel<256, 2>;
+            const size_t smem = Geometry<13>::LIMB_BYTES;   // half a limb
+            e = set_smem_once(conf_ntt, lc.device, smem, kn);
+            if (e != cudaSuccess) return e;
+            kn<<<(unsigned)(2 * n_limbs), 256, smem, st>>>(coeffs, pt, lc.tw, T.m.t, lc.lt, lc.L);
+        } else {
+            constexpr int MINB = LOGN == 12 ? 2 : 3;
+            auto kn = bgv_enc_ntt_kernel<LOGN, 256, MINB>;
+            const size_t smem = Geometry<LOGN>::LIMB_BYTES;
+            e = set_smem_once(conf_ntt, lc.device, smem, kn);
+            if (e != cudaSuccess) return e;
+            kn<<<(unsigned)n_limbs, 256, smem, st>>>(coeffs, pt, lc.tw, T.m.t, lc.lt, lc.L);
+        }
+        return cudaGetLastError();
+    });
 }
 
 // work: [n_vec][L][N] inverse transforms of the plaintexts (overwritten)
 cudaError_t launch_bgv_decode(const LaunchCtx &lc, u64 *work, u64 *slots, const BgvTables &T, const BgvConsts &K, size_t n_vec, cudaStream_t st) {
     if (n_vec == 0) return cudaSuccess;
     if (n_vec > 0x7fffffffull) return cudaErrorInvalidValue;
-    switch (lc.log_n) {
-        case 12: return launch_bgv_decode_t<12>(lc, work, slots, T, K, n_vec, st);
-        case 13: return launch_bgv_decode_t<13>(lc, work, slots, T, K, n_vec, st);
-        case 14: return launch_bgv_decode_t<14>(lc, work, slots, T, K, n_vec, st);
-    }
-    return cudaErrorInvalidValue;
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value;
+        auto kd = bgv_dec_kernel<LOGN, BGV_NT>;
+        const size_t smem = ((size_t)1 << LOGN) * sizeof(u32);
+        static ConfiguredMask conf;
+        cudaError_t e = set_smem_once(conf, lc.device, smem, kd);
+        if (e != cudaSuccess) return e;
+        kd<<<(unsigned)n_vec, BGV_NT, smem, st>>>(work, slots, T, lc.lt, K, lc.L);
+        return cudaGetLastError();
+    });
 }
 
 #endif
@@ -1574,7 +1488,125 @@ static cudaError_t epoch_guard(LaunchCtx &lc, size_t batch, cudaStream_t st) {
     return cudaSuccess;
 }
 
+// the round state every persistent kernel takes (batch, flags, epoch, ticket, mailboxes): its parameter array points here, and
+// launch_persistent fills it once the round numbering is settled
+struct Rounds {
+    size_t batch;
+    u32 *flags;
+    u32 epoch;
+    u32 *ticket;
+    u64 *mail;
+};
+
+// One launch of a persistent key-switch kernel (256 threads per CTA).  The spin-waits need every CTA of the grid resident, so the
+// grid is what fits at once: the resident CTAs (occupancy per SM, or with cluster > 1 whole clusters of that many CTAs), capped by
+// DPFHE_KS_OCC per SM when occ_cap, then by lc.ks_slots, rounded down to whole groups of `group` CTAs and to at most `batch`
+// groups.  Clears the ticket, and advances the round numbering by the batch + 1 rounds a launch may consume, whether or not the
+// launch call succeeded.  cluster == 0: cudaLaunchCooperativeKernel; cluster >= 1 (ks_fused_kernel): cudaLaunchKernelExC,
+// cooperative, with the cluster dimension when > 1 and the DPFHE_L2_PERSIST window.
+template <class Kern>
+static cudaError_t launch_persistent(LaunchCtx &lc, Kern kern, ConfiguredMask &configured, size_t group, size_t smem, size_t batch, Rounds &r,
+                                     void **params, cudaStream_t st, bool occ_cap = true, int cluster = 0) {
+    constexpr int NT = 256;
+    cudaError_t e = set_smem_once(configured, lc.device, smem, kern);
+    if (e != cudaSuccess) return e;
+    cudaLaunchConfig_t cfg = {};
+    cfg.blockDim = dim3(NT);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[3];
+    attr[0].id = cudaLaunchAttributeCooperative;
+    attr[0].val.cooperative = 1;
+    attr[1].id = cudaLaunchAttributeClusterDimension;
+    attr[1].val.clusterDim.x = cluster;
+    attr[1].val.clusterDim.y = 1;
+    attr[1].val.clusterDim.z = 1;
+    int n_attr = cluster > 1 ? 2 : 1;
+    size_t G = 0;   // resident CTAs
+    if (cluster > 1) {
+        cfg.gridDim = dim3(cluster);
+        cfg.attrs = attr + 1;
+        cfg.numAttrs = 1;
+        int clusters = 0;
+        e = cudaOccupancyMaxActiveClusters(&clusters, (const void *)kern, &cfg);
+        if (e != cudaSuccess) return e;
+        G = (size_t)clusters * cluster;
+    } else {
+        int occ = 0;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, NT, smem);
+        if (e != cudaSuccess) return e;
+        G = (size_t)lc.num_sms * occ;
+    }
+    if (G == 0) return cudaErrorLaunchOutOfResources;
+    if (occ_cap && lc.ks_occ_cap > 0 && G > (size_t)lc.num_sms * lc.ks_occ_cap) G = (size_t)lc.num_sms * lc.ks_occ_cap;
+    if (G > lc.ks_slots) G = lc.ks_slots;
+    G = (G / group) * group;
+    if (G > batch * group) G = batch * group;
+    if (G == 0) return cudaErrorInvalidConfiguration;
+    e = epoch_guard(lc, batch, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(lc.ks_ticket, 0, sizeof(u32), st);
+    if (e != cudaSuccess) return e;
+    r = Rounds{batch, lc.ks_flags, lc.ks_epoch, lc.ks_ticket, lc.ks_mail};
+    if (cluster == 0) {
+        e = cudaLaunchCooperativeKernel((const void *)kern, dim3((unsigned)G), dim3(NT), params, smem, st);
+    } else {
+        if (lc.l2_persist && lc.l2_persist_max && lc.ks_window_bytes) {
+            // tuning (DPFHE_L2_PERSIST): the digit slots (and at N = 16384 the accumulator rows) are re-read within microseconds,
+            // the ciphertext streams never; a persisting access-policy window over the scratch keeps the streams from evicting it
+            attr[n_attr].id = cudaLaunchAttributeAccessPolicyWindow;
+            attr[n_attr].val.accessPolicyWindow.base_ptr = lc.ks_scratch;
+            attr[n_attr].val.accessPolicyWindow.num_bytes = lc.ks_window_bytes;
+            const double ratio = (double)lc.l2_persist_max / (double)lc.ks_window_bytes;
+            attr[n_attr].val.accessPolicyWindow.hitRatio = (float)(ratio > 1.0 ? 1.0 : ratio);
+            attr[n_attr].val.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
+            attr[n_attr].val.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
+            ++n_attr;
+        }
+        // never launched without the co-residency guarantee: if the runtime refuses the combination, the call returns its error
+        cfg.gridDim = dim3((unsigned)G);
+        cfg.attrs = attr;
+        cfg.numAttrs = (unsigned)n_attr;
+        e = cudaLaunchKernelExC(&cfg, (const void *)kern, params);
+    }
+    lc.ks_epoch += (u32)(batch + 1);
+    return e;
+}
+
+// the key-switch arguments of the fused, hybrid and grouped kernels: L ciphertext limbs (digits), key rows of Lk limbs.  Set for the
+// special-prime kernels (their digit rows and double accumulators); launch_ks resets the fields the fused kernel uses otherwise.
+static KsArgs ks_args(const LaunchCtx &lc, const u64 *a, const u64 *b, const u64 *key, const u64 *key_s, u64 *out, u32 L, u32 galois, u32 Lk,
+                      bool lift_reduce) {
+    KsArgs A;
+    A.a = a; A.b = b; A.key = key; A.key_s = key_s; A.out = out; A.scratch = lc.ks_scratch;
+    A.tw = lc.tw; A.itw = lc.itw; A.L = L; A.galois = galois; A.Lk = Lk; A.hyb = lc.ks_hyb; A.only = nullptr;
+    A.acc = lc.ks_acc_hyb; A.acc_par = 2; A.lift_reduce = lift_reduce ? 1u : 0u;
+    return A;
+}
+
+// Shoup companions of the first `rows` rows of a switch key [rows][2][L][N] into key_s (same layout)
+template <int LOGN>
+static cudaError_t launch_key_prepare_t(const LaunchCtx &lc, const u64 *key, u64 *key_s, size_t rows, cudaStream_t st) {
+    const size_t n = (size_t)2 * rows * lc.L << LOGN;
+    key_prepare_kernel<LOGN><<<ew_grid(lc, n), 256, 0, st>>>(key, key_s, lc.lp, lc.L, n);
+    return cudaGetLastError();
+}
+
+// grid of the gather kernels (rot_apply, rot_apply_grouped, rot_sum_grouped): `rows` work rows, cut into up to NC / 256 segments
+// (nseg) so that small batches still fill the machine several times over, at most 8 CTAs per SM
+static inline unsigned gather_grid(const LaunchCtx &lc, size_t rows, u32 &nseg) {
+    const size_t want = (size_t)lc.num_sms * 12;
+    const u32 max_seg = (1u << (lc.log_n - 1)) / 256;
+    nseg = 1;
+    while (nseg < max_seg && rows * nseg < want) nseg *= 2;
+    const size_t n_items = rows * nseg, cap = (size_t)lc.num_sms * 8;
+    return (unsigned)(n_items < cap ? n_items : cap);
+}
+
 #if DPFHE_PART_MAIN
+cudaError_t launch_key_prepare(const LaunchCtx &lc, const u64 *key, u64 *key_s, u32 rows, cudaStream_t st) {
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) { return launch_key_prepare_t<decltype(lg)::value>(lc, key, key_s, rows, st); });
+}
+
 template <int LOGN, int MODE>
 static cudaError_t launch_ks_t(LaunchCtx &lc, const KsArgs &A, size_t batch, cudaStream_t st) {
     // N <= 8192: a 4096-point block and two accumulator half-rows, 96 KiB of shared memory -> two CTAs per SM, CTA pairs of a
@@ -1591,397 +1623,200 @@ static cudaError_t launch_ks_t(LaunchCtx &lc, const KsArgs &A, size_t batch, cud
     const size_t smem = BLK ? 3 * Geometry<KS_BLK_LOGN>::LIMB_BYTES : Geometry<13>::LIMB_BYTES;
     static ConfiguredMask configured[3];
     const int variant = filter ? 2 : (lc.ks_prof && MODE == KS_MUL_RELIN ? 1 : 0);
-    if (!configured[variant].has(lc.device)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        configured[variant].set(lc.device);
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.blockDim = dim3(NT);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[3];
-    attr[0].id = cudaLaunchAttributeCooperative;   // the spin-waits need every CTA of the grid resident
-    attr[0].val.cooperative = 1;
-    attr[1].id = cudaLaunchAttributeClusterDimension;
-    attr[1].val.clusterDim.x = PAIR;
-    attr[1].val.clusterDim.y = 1;
-    attr[1].val.clusterDim.z = 1;
-    int n_attr = PAIR > 1 ? 2 : 1;
-    size_t G = 0;   // resident CTAs
-    cudaError_t e;
-    if (PAIR > 1) {
-        cfg.gridDim = dim3(PAIR);
-        cfg.attrs = attr + 1;
-        cfg.numAttrs = 1;
-        int clusters = 0;
-        e = cudaOccupancyMaxActiveClusters(&clusters, (const void *)kern, &cfg);
-        if (e != cudaSuccess) return e;
-        G = (size_t)clusters * PAIR;
-    } else {
-        int occ = 0;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, NT, smem);
-        if (e != cudaSuccess) return e;
-        G = (size_t)lc.num_sms * occ;
-    }
-    if (G == 0) return cudaErrorLaunchOutOfResources;
-    if (lc.ks_occ_cap > 0 && G > (size_t)lc.num_sms * lc.ks_occ_cap) G = (size_t)lc.num_sms * lc.ks_occ_cap;
-    if (G > lc.ks_slots) G = lc.ks_slots;
-    const size_t GS = (size_t)lc.L * PAIR;   // CTAs of a group
-    G = (G / GS) * GS;
-    if (G > batch * GS) G = batch * GS;
-    if (G == 0) return cudaErrorInvalidConfiguration;
-    // flag / mailbox tags this launch may consume: one per round, and a group runs at most batch + 1 rounds
-    const u32 rounds = (u32)(batch + 1);
-    cudaError_t em = epoch_guard(lc, batch, st);
-    if (em != cudaSuccess) return em;
-    em = cudaMemsetAsync(lc.ks_ticket, 0, sizeof(u32), st);
-    if (em != cudaSuccess) return em;
     KsArgs args = A;
-    size_t batch_arg = batch;
-    u32 *flags = lc.ks_flags;
-    u32 epoch = lc.ks_epoch;
     LimbTable lt = lc.lt;
     unsigned long long *prof = lc.ks_prof;
-    u32 *ticket = lc.ks_ticket;
-    u64 *mail = lc.ks_mail;
     u32 pf_dist = (u32)lc.ks_prefetch;
     u32 *consumed = !BLK && lc.ks_single ? lc.ks_consumed : nullptr;   // single-buffered digit slots: N = 16384 only
-    void *params[] = {&args, &lt, &batch_arg, &flags, &epoch, &ticket, &mail, &prof, &pf_dist, &consumed};
-    if (lc.l2_persist && lc.l2_persist_max && lc.ks_window_bytes) {
-        // tuning (DPFHE_L2_PERSIST): the digit slots (and at N = 16384 the accumulator rows) are re-read within microseconds,
-        // the ciphertext streams never; a persisting access-policy window over the scratch keeps the streams from evicting it
-        attr[n_attr].id = cudaLaunchAttributeAccessPolicyWindow;
-        attr[n_attr].val.accessPolicyWindow.base_ptr = lc.ks_scratch;
-        attr[n_attr].val.accessPolicyWindow.num_bytes = lc.ks_window_bytes;
-        const double ratio = (double)lc.l2_persist_max / (double)lc.ks_window_bytes;
-        attr[n_attr].val.accessPolicyWindow.hitRatio = (float)(ratio > 1.0 ? 1.0 : ratio);
-        attr[n_attr].val.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-        attr[n_attr].val.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-        ++n_attr;
-    }
-    // Cooperative and, at N = 8192, a cluster dimension of two.  Never launched without the co-residency guarantee: if the
-    // runtime refuses the combination, the call returns its error.
-    cfg.gridDim = dim3((unsigned)G);
-    cfg.attrs = attr;
-    cfg.numAttrs = (unsigned)n_attr;
-    e = cudaLaunchKernelExC(&cfg, (const void *)kern, params);
-    lc.ks_epoch += rounds;
-    return e;
+    Rounds r;
+    void *params[] = {&args, &lt, &r.batch, &r.flags, &r.epoch, &r.ticket, &r.mail, &prof, &pf_dist, &consumed};
+    return launch_persistent(lc, kern, configured[variant], (size_t)lc.L * PAIR, smem, batch, r, params, st, true, PAIR);
+}
+
+cudaError_t launch_ks(LaunchCtx &lc, int mode, const u64 *a, const u64 *b, const u64 *key, u64 *out, size_t batch,
+                      u32 galois, cudaStream_t st, const u32 *only, bool key_ready, const u64 *key_s) {
+    if (batch == 0) return cudaSuccess;
+    return with_log_n(lc.log_n, cudaErrorNotSupported, [&](auto lg) -> cudaError_t {
+        constexpr int LOGN = decltype(lg)::value;
+        // Shoup companions of the key for this launch (2*L*P words, a few microseconds; batch-amortised)
+        if (!key_ready) {
+            cudaError_t e = launch_key_prepare_t<LOGN>(lc, key, lc.ks_key_s, lc.L, st);
+            if (e != cudaSuccess) return e;
+        }
+        KsArgs A = ks_args(lc, a, b, key, key_ready && key_s ? key_s : lc.ks_key_s, out, lc.L, galois, lc.L, lc.lift_reduce);
+        A.hyb = nullptr; A.only = only; A.acc = lc.ks_acc; A.acc_par = 1;
+        switch (mode) {
+            case KS_MUL_RELIN: return launch_ks_t<LOGN, KS_MUL_RELIN>(lc, A, batch, st);
+            case KS_PLAIN: return launch_ks_t<LOGN, KS_PLAIN>(lc, A, batch, st);
+            case KS_ROTATE: return launch_ks_t<LOGN, KS_ROTATE>(lc, A, batch, st);
+        }
+        return cudaErrorInvalidValue;
+    });
 }
 
 #endif
 #if DPFHE_PART_HYBRID
-template <int LOGN, int MODE, bool LV = false>
+template <int LOGN, int MODE, bool LV>
 static cudaError_t launch_ks_hybrid_t(LaunchCtx &lc, const KsArgs &A, const MsConsts &K, size_t batch, cudaStream_t st) {
     constexpr int NT = 256, MINB = 3;
     auto kern = ks_hybrid_kernel<LOGN, NT, MINB, MODE>;
     if constexpr (LV) kern = ks_hybrid_level_kernel<LOGN, NT, MINB, MODE>;
-    const size_t smem = LOGN <= 13 ? Geometry<LOGN>::LIMB_BYTES : Geometry<13>::LIMB_BYTES;
     static ConfiguredMask configured;
-    if (!configured.has(lc.device)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        configured.set(lc.device);
-    }
-    int occ = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, NT, smem);
-    if (e != cudaSuccess) return e;
-    if (occ < 1) return cudaErrorLaunchOutOfResources;
-    if (lc.ks_occ_cap > 0 && occ > lc.ks_occ_cap) occ = lc.ks_occ_cap;
-    const size_t GS = lc.L;   // group size: L-1 ciphertext limbs + the special limb
-    size_t G = (size_t)lc.num_sms * occ;
-    if (G > lc.ks_slots) G = lc.ks_slots;
-    G = (G / GS) * GS;
-    if (G > batch * GS) G = batch * GS;
-    if (G == 0) return cudaErrorInvalidConfiguration;
-    const u32 rounds = (u32)(batch + 1);
-    cudaError_t em = epoch_guard(lc, batch, st);
-    if (em != cudaSuccess) return em;
-    em = cudaMemsetAsync(lc.ks_ticket, 0, sizeof(u32), st);
-    if (em != cudaSuccess) return em;
     KsArgs args = A;
     LimbTable lt = lc.lt;
     MsConsts consts = K;
-    size_t batch_arg = batch;
-    u32 *flags = lc.ks_flags;
-    u32 epoch = lc.ks_epoch;
-    u32 *ticket = lc.ks_ticket;
-    u64 *mail = lc.ks_mail;
-    void *params[] = {&args, &lt, &consts, &batch_arg, &flags, &epoch, &ticket, &mail};
-    e = cudaLaunchCooperativeKernel((void *)kern, dim3((unsigned)G), dim3(NT), params, smem, st);
-    lc.ks_epoch += rounds;
-    return e;
+    Rounds r;
+    void *params[] = {&args, &lt, &consts, &r.batch, &r.flags, &r.epoch, &r.ticket, &r.mail};
+    // group: L-1 ciphertext limbs + the special limb
+    return launch_persistent(lc, kern, configured, lc.L, Geometry<LOGN>::KS_SMEM, batch, r, params, st);
 }
 
-// data has L-1 limbs, the key [L-1][2][L][N]; lc.ks_hyb must hold (ks_slots / 2 + 1) * KS_HYB_ROWS * N words and
-// lc.ks_acc_hyb ks_slots * 2 * 2 * N words
+// data has L-1 limbs, the key [L-1][2][key_L][N]; lc.ks_hyb must hold (ks_slots / 2 + 1) * KS_HYB_ROWS * N words and lc.ks_acc_hyb
+// ks_slots * 2 * 2 * N words.  key_s == nullptr: the top-level call, modes KS_MUL_RELIN, KS_PLAIN and KS_ROTATE, the key's companions
+// built here into lc.ks_key_s.  key_s given: the call at level l (DESIGN.md §4.17), modes KS_MUL_RELIN and KS_ROTATE: lc is the level's
+// view (L = l + 1 limbs, its own tables), key the top-level key with key_L limbs per row and its companions key_s, built by the caller
+// over the top-level rows.
 cudaError_t launch_ks_hybrid(LaunchCtx &lc, int mode, const u64 *a, const u64 *b, const u64 *key, u64 *out, size_t batch, u32 galois,
-                             const MsConsts &K, cudaStream_t st) {
+                             const MsConsts &K, cudaStream_t st, const u64 *key_s, u32 key_L) {
     if (batch == 0) return cudaSuccess;
-    if (lc.L < 2 || !lc.ks_hyb || !lc.ks_acc_hyb) return cudaErrorInvalidValue;
-    {
-        const size_t n = (size_t)2 * (lc.L - 1) * lc.L << lc.log_n;
-        const unsigned grid = ew_grid(lc, n);
-        if (lc.log_n == 12) key_prepare_kernel<12><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
-        else if (lc.log_n == 13) key_prepare_kernel<13><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
-        else key_prepare_kernel<14><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return e;
-    }
-    KsArgs A;
-    A.a = a; A.b = b; A.key = key; A.key_s = lc.ks_key_s; A.out = out; A.scratch = lc.ks_scratch;
-    A.tw = lc.tw; A.itw = lc.itw; A.L = lc.L - 1; A.galois = galois; A.Lk = lc.L; A.hyb = lc.ks_hyb; A.only = nullptr;
-    A.acc = lc.ks_acc_hyb; A.acc_par = 2; A.lift_reduce = lc.lift_reduce ? 1u : 0u;
-#define KS_HYB_DISPATCH(LOGN)                                                                   \
-    switch (mode) {                                                                             \
-        case KS_MUL_RELIN: return launch_ks_hybrid_t<LOGN, KS_MUL_RELIN>(lc, A, K, batch, st);   \
-        case KS_PLAIN: return launch_ks_hybrid_t<LOGN, KS_PLAIN>(lc, A, K, batch, st);           \
-        case KS_ROTATE: return launch_ks_hybrid_t<LOGN, KS_ROTATE>(lc, A, K, batch, st);         \
-    }                                                                                           \
-    return cudaErrorInvalidValue;
-    switch (lc.log_n) {
-        case 12: KS_HYB_DISPATCH(12)
-        case 13: KS_HYB_DISPATCH(13)
-        case 14: KS_HYB_DISPATCH(14)
-    }
-    return cudaErrorNotSupported;
-}
-
-// one special prime at level l (DESIGN.md §4.17): lc is the level's view (L = l + 1 limbs, its own tables), key the top-level key
-// [Lq][2][key_L][N] with its companions key_s, built by the caller over the top-level rows.  Modes KS_MUL_RELIN and KS_ROTATE.
-cudaError_t launch_ks_hybrid_level(LaunchCtx &lc, int mode, const u64 *a, const u64 *b, const u64 *key, const u64 *key_s, u32 key_L, u64 *out,
-                                   size_t batch, u32 galois, const MsConsts &K, cudaStream_t st) {
-    if (batch == 0) return cudaSuccess;
-    if (lc.L < 2 || key_L < lc.L || !key_s || !lc.ks_hyb || !lc.ks_acc_hyb) return cudaErrorInvalidValue;
-    KsArgs A;
-    A.a = a; A.b = b; A.key = key; A.key_s = key_s; A.out = out; A.scratch = lc.ks_scratch;
-    A.tw = lc.tw; A.itw = lc.itw; A.L = lc.L - 1; A.galois = galois; A.Lk = key_L; A.hyb = lc.ks_hyb; A.only = nullptr;
-    A.acc = lc.ks_acc_hyb; A.acc_par = 2; A.lift_reduce = lc.lift_reduce ? 1u : 0u;
-#define KS_HYB_LV_DISPATCH(LOGN)                                                                      \
-    switch (mode) {                                                                                   \
-        case KS_MUL_RELIN: return launch_ks_hybrid_t<LOGN, KS_MUL_RELIN, true>(lc, A, K, batch, st);   \
-        case KS_ROTATE: return launch_ks_hybrid_t<LOGN, KS_ROTATE, true>(lc, A, K, batch, st);         \
-    }                                                                                                 \
-    return cudaErrorInvalidValue;
-    switch (lc.log_n) {
-        case 12: KS_HYB_LV_DISPATCH(12)
-        case 13: KS_HYB_LV_DISPATCH(13)
-        case 14: KS_HYB_LV_DISPATCH(14)
-    }
-#undef KS_HYB_LV_DISPATCH
-    return cudaErrorNotSupported;
+    const bool level = key_s != nullptr;
+    if (lc.L < 2 || (level && key_L < lc.L) || !lc.ks_hyb || !lc.ks_acc_hyb) return cudaErrorInvalidValue;
+    return with_log_n(lc.log_n, cudaErrorNotSupported, [&](auto lg) -> cudaError_t {
+        constexpr int LOGN = decltype(lg)::value;
+        if (!level) {
+            cudaError_t e = launch_key_prepare_t<LOGN>(lc, key, lc.ks_key_s, lc.L - 1, st);
+            if (e != cudaSuccess) return e;
+        }
+        const KsArgs A = ks_args(lc, a, b, key, level ? key_s : lc.ks_key_s, out, lc.L - 1, galois, level ? key_L : lc.L, lc.lift_reduce);
+        switch (mode) {
+            case KS_MUL_RELIN:
+                return level ? launch_ks_hybrid_t<LOGN, KS_MUL_RELIN, true>(lc, A, K, batch, st) : launch_ks_hybrid_t<LOGN, KS_MUL_RELIN, false>(lc, A, K, batch, st);
+            case KS_PLAIN:
+                if (!level) return launch_ks_hybrid_t<LOGN, KS_PLAIN, false>(lc, A, K, batch, st);
+                break;
+            case KS_ROTATE:
+                return level ? launch_ks_hybrid_t<LOGN, KS_ROTATE, true>(lc, A, K, batch, st) : launch_ks_hybrid_t<LOGN, KS_ROTATE, false>(lc, A, K, batch, st);
+        }
+        return cudaErrorInvalidValue;
+    });
 }
 
 #endif
 #if DPFHE_PART_GROUPED
+// one launch of a grouped kernel: ks_grouped_kernel (ADD: with the addend), ct_dot_grouped_kernel (MODE = KS_DOT),
+// ks_rescale_grouped_kernel (RS) or ks_level_grouped_kernel (LV; RS: with the division by the dropped limb).  Groups of L CTAs:
+// every limb of the context, ciphertext and special.
 template <int LOGN, int MODE, bool ADD = false, bool RS = false, bool LV = false>
-static cudaError_t launch_ks_grouped_t(LaunchCtx &lc, const KsArgs &A, const MsConsts &K, const GroupConsts &Gc, size_t batch, cudaStream_t st,
-                                       const u64 *addend, const DotArgs *dot = nullptr, const RescaleConsts *rs = nullptr) {
+static cudaError_t launch_ks_grouped_t(LaunchCtx &lc, KsArgs A, MsConsts K, GroupConsts G, DotArgs D, RescaleConsts R, const u64 *addend,
+                                       size_t batch, cudaStream_t st) {
     constexpr int NT = 256, MINB = 3;
-    const void *kern;
-    if constexpr (LV) kern = (const void *)ks_level_grouped_kernel<LOGN, NT, MINB, MODE, RS>;
-    else if constexpr (RS) kern = (const void *)ks_rescale_grouped_kernel<LOGN, NT, MINB, MODE>;
-    else if constexpr (MODE == KS_DOT) kern = (const void *)ct_dot_grouped_kernel<LOGN, NT, MINB>;
-    else kern = (const void *)ks_grouped_kernel<LOGN, NT, MINB, MODE, ADD>;
-    const size_t smem = LOGN <= 13 ? Geometry<LOGN>::LIMB_BYTES : Geometry<13>::LIMB_BYTES;
+    constexpr size_t smem = Geometry<LOGN>::KS_SMEM;
     static ConfiguredMask configured;
-    if (!configured.has(lc.device)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        configured.set(lc.device);
-    }
-    int occ = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, NT, smem);
-    if (e != cudaSuccess) return e;
-    if (occ < 1) return cudaErrorLaunchOutOfResources;
-    if (lc.ks_occ_cap > 0 && occ > lc.ks_occ_cap) occ = lc.ks_occ_cap;
-    const size_t GS = lc.L;   // group size: every limb of the context, ciphertext and special
-    size_t G = (size_t)lc.num_sms * occ;
-    if (G > lc.ks_slots) G = lc.ks_slots;
-    G = (G / GS) * GS;
-    if (G > batch * GS) G = batch * GS;
-    if (G == 0) return cudaErrorInvalidConfiguration;
-    const u32 rounds = (u32)(batch + 1);
-    cudaError_t em = epoch_guard(lc, batch, st);
-    if (em != cudaSuccess) return em;
-    em = cudaMemsetAsync(lc.ks_ticket, 0, sizeof(u32), st);
-    if (em != cudaSuccess) return em;
-    KsArgs args = A;
     LimbTable lt = lc.lt;
-    MsConsts consts = K;
-    GroupConsts gc = Gc;
-    size_t batch_arg = batch;
-    u32 *flags = lc.ks_flags;
-    u32 epoch = lc.ks_epoch;
-    u32 *ticket = lc.ks_ticket;
-    u64 *mail = lc.ks_mail;
-    const u64 *add = addend;
-    void *params[] = {&args, &lt, &consts, &gc, &batch_arg, &flags, &epoch, &ticket, &mail, &add};
-    void *params_dot[] = {&args, &lt, &consts, &gc, const_cast<DotArgs *>(dot), &batch_arg, &flags, &epoch, &ticket, &mail};
-    DotArgs no_dot{};
-    RescaleConsts rc{};
-    if (rs) rc = *rs;
-    void *params_rs[] = {&args, &lt, &consts, &gc, dot ? const_cast<DotArgs *>(dot) : &no_dot, &rc, &batch_arg, &flags, &epoch, &ticket, &mail};
-    e = cudaLaunchCooperativeKernel(kern, dim3((unsigned)G), dim3(NT), RS || LV ? params_rs : MODE == KS_DOT ? params_dot : params, smem, st);
-    lc.ks_epoch += rounds;
-    return e;
+    Rounds r;
+    if constexpr (LV || RS) {
+        void *params[] = {&A, &lt, &K, &G, &D, &R, &r.batch, &r.flags, &r.epoch, &r.ticket, &r.mail};
+        if constexpr (LV) return launch_persistent(lc, ks_level_grouped_kernel<LOGN, NT, MINB, MODE, RS>, configured, lc.L, smem, batch, r, params, st);
+        else return launch_persistent(lc, ks_rescale_grouped_kernel<LOGN, NT, MINB, MODE>, configured, lc.L, smem, batch, r, params, st);
+    } else if constexpr (MODE == KS_DOT) {
+        void *params[] = {&A, &lt, &K, &G, &D, &r.batch, &r.flags, &r.epoch, &r.ticket, &r.mail};
+        return launch_persistent(lc, ct_dot_grouped_kernel<LOGN, NT, MINB>, configured, lc.L, smem, batch, r, params, st);
+    } else {
+        void *params[] = {&A, &lt, &K, &G, &r.batch, &r.flags, &r.epoch, &r.ticket, &r.mail, &addend};
+        return launch_persistent(lc, ks_grouped_kernel<LOGN, NT, MINB, MODE, ADD>, configured, lc.L, smem, batch, r, params, st);
+    }
 }
 
-// data has Lq = L - K limbs, the key [dnum][2][L][N]; scratch requirements as launch_ks_hybrid (K <= Lq keeps the special
-// CTAs' rows within lc.ks_hyb).  addend (KS_ROTATE only): out = rotation + addend, one launch.  key_s: the key's Shoup companions,
-// built by the caller once (a linear layer); nullptr = built here into lc.ks_key_s (one more launch).
-cudaError_t launch_ks_grouped(LaunchCtx &lc, int mode, const u64 *a, const u64 *b, const u64 *key, u64 *out, size_t batch, u32 galois,
-                              const MsConsts &K, const GroupConsts &Gc, cudaStream_t st, const u64 *addend, const u64 *key_s) {
+// Every grouped key-switching call (data of Gc.Lq = L - K limbs, the key [dnum][2][key rows][N]; scratch requirements as
+// launch_ks_hybrid, K <= Lq keeping the special CTAs' rows within lc.ks_hyb):
+//   mode KS_MUL_RELIN / KS_PLAIN / KS_ROTATE on a[0], b[0] (galois; addend, KS_ROTATE only: out = rotation + addend), or KS_DOT on
+//   the n_terms (1 .. DOT_MAX_TERMS) pairs a[t], b[t] (DESIGN.md §2.18); host arrays of device pointers;
+//   R non-null: multiply-and-rescale (DESIGN.md §2.19, modes KS_MUL_RELIN and KS_DOT): out [batch][2][Lq-1][N], divided by
+//   P * q_{Lq-1}; the dropped limb's rows and flags are lc.ks_tau_drop, which must hold (ks_slots / 3 + 1) * 4 * N words (a group has
+//   L >= 3 CTAs), and one flag per group in the second half of lc.ks_flags, whose words ks_hoistg_kernel uses as round marks in
+//   other launches: a tag is always above what an earlier launch left;
+//   key_L > 0: the call at level l (DESIGN.md §2.20, §4.17, modes KS_MUL_RELIN, KS_ROTATE, KS_DOT): lc is the level's view (L = l + K
+//   limbs, its own tables and Gc built on them), key the top-level key with key_L limbs per row and its companions key_s, built by
+//   the caller over the top-level rows of the level's digits.
+// key_s == nullptr (top level only): the companions are built here into lc.ks_key_s, one more launch.
+static cudaError_t ks_grouped(LaunchCtx &lc, int mode, const u64 *const *a, const u64 *const *b, u32 n_terms, u32 galois, const u64 *addend,
+                              const u64 *key, const u64 *key_s, u32 key_L, const RescaleConsts *R, u64 *out, size_t batch, const MsConsts &K,
+                              const GroupConsts &Gc, cudaStream_t st) {
     if (batch == 0) return cudaSuccess;
+    const bool level = key_L != 0, dot = mode == KS_DOT;
     if (lc.L < 2 || !lc.ks_hyb || !lc.ks_acc_hyb || Gc.Lq + Gc.K != lc.L || Gc.K > Gc.Lq || Gc.K > (u32)KS_MAX_SPECIAL) return cudaErrorInvalidValue;
-    if (addend && mode != KS_ROTATE) return cudaErrorInvalidValue;
-    if (!key_s) {
-        const size_t n = (size_t)2 * Gc.dnum * lc.L << lc.log_n;
-        const unsigned grid = ew_grid(lc, n);
-        if (lc.log_n == 12) key_prepare_kernel<12><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
-        else if (lc.log_n == 13) key_prepare_kernel<13><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
-        else key_prepare_kernel<14><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return e;
-        key_s = lc.ks_key_s;
-    }
-    KsArgs A;
-    A.a = a; A.b = b; A.key = key; A.key_s = key_s; A.out = out; A.scratch = lc.ks_scratch;
-    A.tw = lc.tw; A.itw = lc.itw; A.L = Gc.Lq; A.galois = galois; A.Lk = lc.L; A.hyb = lc.ks_hyb; A.only = nullptr;
-    A.acc = lc.ks_acc_hyb; A.acc_par = 2; A.lift_reduce = 0u;
-#define KS_GRP_DISPATCH(LOGN)                                                                                          \
-    switch (mode) {                                                                                                    \
-        case KS_MUL_RELIN: return launch_ks_grouped_t<LOGN, KS_MUL_RELIN>(lc, A, K, Gc, batch, st, nullptr);            \
-        case KS_PLAIN: return launch_ks_grouped_t<LOGN, KS_PLAIN>(lc, A, K, Gc, batch, st, nullptr);                    \
-        case KS_ROTATE:                                                                                                \
-            if (addend) return launch_ks_grouped_t<LOGN, KS_ROTATE, true>(lc, A, K, Gc, batch, st, addend);            \
-            return launch_ks_grouped_t<LOGN, KS_ROTATE>(lc, A, K, Gc, batch, st, nullptr);                              \
-    }                                                                                                                  \
-    return cudaErrorInvalidValue;
-    switch (lc.log_n) {
-        case 12: KS_GRP_DISPATCH(12)
-        case 13: KS_GRP_DISPATCH(13)
-        case 14: KS_GRP_DISPATCH(14)
-    }
-    return cudaErrorNotSupported;
-}
-
-// out = relinearised sum of the n_terms tensor products a[t] x b[t] (DESIGN.md §2.18): launch_ks_grouped's launches with the limb
-// CTAs' phase 1 in mode KS_DOT.  a, b: host arrays of device pointers.
-cudaError_t launch_ct_dot_grouped(LaunchCtx &lc, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, u64 *out, size_t batch,
-                                  const MsConsts &K, const GroupConsts &Gc, cudaStream_t st, const u64 *key_s) {
-    if (batch == 0) return cudaSuccess;
-    if (lc.L < 2 || !lc.ks_hyb || !lc.ks_acc_hyb || Gc.Lq + Gc.K != lc.L || Gc.K > Gc.Lq || Gc.K > (u32)KS_MAX_SPECIAL) return cudaErrorInvalidValue;
-    if (n_terms < 1 || n_terms > (u32)DOT_MAX_TERMS) return cudaErrorInvalidValue;
-    if (!key_s) {
-        cudaError_t e = launch_key_prepare_grouped(lc, key, lc.ks_key_s, Gc.dnum, st);
-        if (e != cudaSuccess) return e;
-        key_s = lc.ks_key_s;
-    }
-    KsArgs A;
-    A.a = nullptr; A.b = nullptr; A.key = key; A.key_s = key_s; A.out = out; A.scratch = lc.ks_scratch;
-    A.tw = lc.tw; A.itw = lc.itw; A.L = Gc.Lq; A.galois = 0; A.Lk = lc.L; A.hyb = lc.ks_hyb; A.only = nullptr;
-    A.acc = lc.ks_acc_hyb; A.acc_par = 2; A.lift_reduce = 0u;
-    DotArgs D{};
-    D.n_terms = n_terms;
-    for (u32 t = 0; t < n_terms; ++t) {
-        D.a[t] = a[t];
-        D.b[t] = b[t];
-    }
-    switch (lc.log_n) {
-        case 12: return launch_ks_grouped_t<12, KS_DOT>(lc, A, K, Gc, batch, st, nullptr, &D);
-        case 13: return launch_ks_grouped_t<13, KS_DOT>(lc, A, K, Gc, batch, st, nullptr, &D);
-        case 14: return launch_ks_grouped_t<14, KS_DOT>(lc, A, K, Gc, batch, st, nullptr, &D);
-    }
-    return cudaErrorNotSupported;
-}
-
-// multiply-and-rescale (DESIGN.md §2.19): out [batch][2][Lq-1][N] = the product (dot: the summed products of the n_terms pairs a[t] x b[t];
-// otherwise the ct x ct product a[0] x b[0]) relinearised and divided by P * q_{Lq-1} in one launch (+ key_prepare without key_s).
-// R: the dropped limb's constants; its row and flag pointers are set here (lc.ks_tau_drop; one flag per group in the second half of
-// lc.ks_flags, whose words ks_hoistg_kernel uses as round marks in other launches: a tag is always above what an earlier launch left).  lc.ks_tau_drop must hold (ks_slots / 3 + 1) * 4 * N words: a group has L >= 3 CTAs.
-cudaError_t launch_ks_rescale_grouped(LaunchCtx &lc, bool dot, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, u64 *out,
-                                      size_t batch, const MsConsts &K, const GroupConsts &Gc, const RescaleConsts &R, cudaStream_t st,
-                                      const u64 *key_s) {
-    if (batch == 0) return cudaSuccess;
-    if (lc.L < 3 || !lc.ks_hyb || !lc.ks_acc_hyb || !lc.ks_tau_drop || Gc.Lq + Gc.K != lc.L || Gc.Lq < 2 || Gc.K > Gc.Lq ||
-        Gc.K > (u32)KS_MAX_SPECIAL)
-        return cudaErrorInvalidValue;
+    if ((level && (key_L < lc.L || !key_s)) || (addend && mode != KS_ROTATE)) return cudaErrorInvalidValue;
+    if (R && (mode == KS_ROTATE || lc.L < 3 || Gc.Lq < 2 || !lc.ks_tau_drop)) return cudaErrorInvalidValue;
     if (n_terms < 1 || n_terms > (u32)DOT_MAX_TERMS || (!dot && n_terms != 1)) return cudaErrorInvalidValue;
-    if (!key_s) {
-        cudaError_t e = launch_key_prepare_grouped(lc, key, lc.ks_key_s, Gc.dnum, st);
-        if (e != cudaSuccess) return e;
-        key_s = lc.ks_key_s;
-    }
-    KsArgs A;
-    A.a = dot ? nullptr : a[0]; A.b = dot ? nullptr : b[0]; A.key = key; A.key_s = key_s; A.out = out; A.scratch = lc.ks_scratch;
-    A.tw = lc.tw; A.itw = lc.itw; A.L = Gc.Lq; A.galois = 0; A.Lk = lc.L; A.hyb = lc.ks_hyb; A.only = nullptr;
-    A.acc = lc.ks_acc_hyb; A.acc_par = 2; A.lift_reduce = 0u;
-    RescaleConsts Rc = R;
-    Rc.tau = lc.ks_tau_drop;
-    Rc.tau_flag = lc.ks_flags + lc.ks_slots;
     DotArgs D{};
-    D.n_terms = n_terms;
     for (u32 t = 0; dot && t < n_terms; ++t) {
         D.a[t] = a[t];
         D.b[t] = b[t];
     }
-#define KS_RS_DISPATCH(LOGN)                                                                                                     \
-    return dot ? launch_ks_grouped_t<LOGN, KS_DOT, false, true>(lc, A, K, Gc, batch, st, nullptr, &D, &Rc)                       \
-               : launch_ks_grouped_t<LOGN, KS_MUL_RELIN, false, true>(lc, A, K, Gc, batch, st, nullptr, nullptr, &Rc);
-    switch (lc.log_n) {
-        case 12: KS_RS_DISPATCH(12)
-        case 13: KS_RS_DISPATCH(13)
-        case 14: KS_RS_DISPATCH(14)
-    }
-#undef KS_RS_DISPATCH
-    return cudaErrorNotSupported;
-}
-
-// every grouped call at level l (DESIGN.md §2.20, §4.17): lc is the level's view (L = l + K limbs, its own tables and Gc built on them),
-// key the top-level key [dnum][2][key_L][N] with its companions key_s, built by the caller over the top-level rows of the level's
-// digits.  mode KS_MUL_RELIN / KS_ROTATE (a[0], b[0]; galois) or KS_DOT (the n_terms pairs); R non-null: multiply-and-rescale (modes
-// KS_MUL_RELIN, KS_DOT), its rows and flags as launch_ks_rescale_grouped's.  One launch.
-cudaError_t launch_ks_grouped_level(LaunchCtx &lc, int mode, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, const u64 *key_s,
-                                    u32 key_L, u64 *out, size_t batch, u32 galois, const MsConsts &K, const GroupConsts &Gc, const RescaleConsts *R,
-                                    cudaStream_t st) {
-    if (batch == 0) return cudaSuccess;
-    if (lc.L < 2 || key_L < lc.L || !key_s || !lc.ks_hyb || !lc.ks_acc_hyb || Gc.Lq + Gc.K != lc.L || Gc.K > Gc.Lq || Gc.K > (u32)KS_MAX_SPECIAL)
-        return cudaErrorInvalidValue;
-    if (R && (mode == KS_ROTATE || lc.L < 3 || Gc.Lq < 2 || !lc.ks_tau_drop)) return cudaErrorInvalidValue;
-    if (n_terms < 1 || n_terms > (u32)DOT_MAX_TERMS || (mode != KS_DOT && n_terms != 1)) return cudaErrorInvalidValue;
-    const bool dot = mode == KS_DOT;
-    KsArgs A;
-    A.a = dot ? nullptr : a[0]; A.b = dot || !b ? nullptr : b[0]; A.key = key; A.key_s = key_s; A.out = out; A.scratch = lc.ks_scratch;
-    A.tw = lc.tw; A.itw = lc.itw; A.L = Gc.Lq; A.galois = galois; A.Lk = key_L; A.hyb = lc.ks_hyb; A.only = nullptr;
-    A.acc = lc.ks_acc_hyb; A.acc_par = 2; A.lift_reduce = 0u;
+    if (dot) D.n_terms = n_terms;
     RescaleConsts Rc{};
     if (R) {
         Rc = *R;
         Rc.tau = lc.ks_tau_drop;
         Rc.tau_flag = lc.ks_flags + lc.ks_slots;
     }
-    DotArgs D{};
-    D.n_terms = n_terms;
-    for (u32 t = 0; dot && t < n_terms; ++t) {
-        D.a[t] = a[t];
-        D.b[t] = b[t];
-    }
-#define KS_LV_DISPATCH(LOGN)                                                                                                        \
-    if (mode == KS_ROTATE) return launch_ks_grouped_t<LOGN, KS_ROTATE, false, false, true>(lc, A, K, Gc, batch, st, nullptr, nullptr, &Rc); \
-    if (R) return dot ? launch_ks_grouped_t<LOGN, KS_DOT, false, true, true>(lc, A, K, Gc, batch, st, nullptr, &D, &Rc)                  \
-                      : launch_ks_grouped_t<LOGN, KS_MUL_RELIN, false, true, true>(lc, A, K, Gc, batch, st, nullptr, nullptr, &Rc);   \
-    return dot ? launch_ks_grouped_t<LOGN, KS_DOT, false, false, true>(lc, A, K, Gc, batch, st, nullptr, &D, &Rc)                        \
-               : launch_ks_grouped_t<LOGN, KS_MUL_RELIN, false, false, true>(lc, A, K, Gc, batch, st, nullptr, nullptr, &Rc);
-    if (mode != KS_MUL_RELIN && mode != KS_ROTATE && mode != KS_DOT) return cudaErrorInvalidValue;
-    switch (lc.log_n) {
-        case 12: KS_LV_DISPATCH(12)
-        case 13: KS_LV_DISPATCH(13)
-        case 14: KS_LV_DISPATCH(14)
-    }
-#undef KS_LV_DISPATCH
-    return cudaErrorNotSupported;
+    return with_log_n(lc.log_n, cudaErrorNotSupported, [&](auto lg) -> cudaError_t {
+        constexpr int LOGN = decltype(lg)::value;
+        if (!key_s) {
+            cudaError_t e = launch_key_prepare_t<LOGN>(lc, key, lc.ks_key_s, Gc.dnum, st);
+            if (e != cudaSuccess) return e;
+            key_s = lc.ks_key_s;
+        }
+        const KsArgs A = ks_args(lc, dot ? nullptr : a[0], dot || !b ? nullptr : b[0], key, key_s, out, Gc.Lq, galois, level ? key_L : lc.L, false);
+        if (level) {
+            switch (mode) {
+                case KS_ROTATE: return launch_ks_grouped_t<LOGN, KS_ROTATE, false, false, true>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
+                case KS_MUL_RELIN:
+                    if (R) return launch_ks_grouped_t<LOGN, KS_MUL_RELIN, false, true, true>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
+                    return launch_ks_grouped_t<LOGN, KS_MUL_RELIN, false, false, true>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
+                case KS_DOT:
+                    if (R) return launch_ks_grouped_t<LOGN, KS_DOT, false, true, true>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
+                    return launch_ks_grouped_t<LOGN, KS_DOT, false, false, true>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
+            }
+            return cudaErrorInvalidValue;
+        }
+        if (R) return dot ? launch_ks_grouped_t<LOGN, KS_DOT, false, true>(lc, A, K, Gc, D, Rc, nullptr, batch, st)
+                          : launch_ks_grouped_t<LOGN, KS_MUL_RELIN, false, true>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
+        switch (mode) {
+            case KS_MUL_RELIN: return launch_ks_grouped_t<LOGN, KS_MUL_RELIN>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
+            case KS_PLAIN: return launch_ks_grouped_t<LOGN, KS_PLAIN>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
+            case KS_ROTATE:
+                if (addend) return launch_ks_grouped_t<LOGN, KS_ROTATE, true>(lc, A, K, Gc, D, Rc, addend, batch, st);
+                return launch_ks_grouped_t<LOGN, KS_ROTATE>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
+            case KS_DOT: return launch_ks_grouped_t<LOGN, KS_DOT>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
+        }
+        return cudaErrorInvalidValue;
+    });
+}
+
+// the entry points of ks_grouped: one ct x ct product, plain switch or rotation; the inner product; multiply-and-rescale; level calls
+cudaError_t launch_ks_grouped(LaunchCtx &lc, int mode, const u64 *a, const u64 *b, const u64 *key, u64 *out, size_t batch, u32 galois,
+                              const MsConsts &K, const GroupConsts &Gc, cudaStream_t st, const u64 *addend, const u64 *key_s) {
+    if (batch && mode == KS_DOT) return cudaErrorInvalidValue;
+    return ks_grouped(lc, mode, &a, &b, 1, galois, addend, key, key_s, 0, nullptr, out, batch, K, Gc, st);
+}
+
+cudaError_t launch_ct_dot_grouped(LaunchCtx &lc, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, u64 *out, size_t batch,
+                                  const MsConsts &K, const GroupConsts &Gc, cudaStream_t st, const u64 *key_s) {
+    return ks_grouped(lc, KS_DOT, a, b, n_terms, 0, nullptr, key, key_s, 0, nullptr, out, batch, K, Gc, st);
+}
+
+cudaError_t launch_ks_rescale_grouped(LaunchCtx &lc, bool dot, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, u64 *out,
+                                      size_t batch, const MsConsts &K, const GroupConsts &Gc, const RescaleConsts &R, cudaStream_t st,
+                                      const u64 *key_s) {
+    return ks_grouped(lc, dot ? KS_DOT : KS_MUL_RELIN, a, b, n_terms, 0, nullptr, key, key_s, 0, &R, out, batch, K, Gc, st);
+}
+
+cudaError_t launch_ks_grouped_level(LaunchCtx &lc, int mode, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, const u64 *key_s,
+                                    u32 key_L, u64 *out, size_t batch, u32 galois, const MsConsts &K, const GroupConsts &Gc, const RescaleConsts *R,
+                                    cudaStream_t st) {
+    if (batch && !key_L) return cudaErrorInvalidValue;
+    return ks_grouped(lc, mode, a, b, n_terms, galois, nullptr, key, key_s, key_L, R, out, batch, K, Gc, st);
 }
 
 #endif
@@ -1997,27 +1832,6 @@ static u32 pt_inner_gmax(u32 nb) {
     return gmax;
 }
 
-template <int LOGN>
-static cudaError_t launch_pt_inner_t(const LaunchCtx &lc, const PtInnerArgs &A, u32 gmax, cudaStream_t st) {
-    constexpr int NT = 256, MINB = 2;
-    auto kern = pt_inner_kernel<LOGN, NT, MINB>;
-    static ConfiguredMask configured;
-    if (!configured.has(lc.device)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PTI_SMEM_BUDGET);
-        if (e != cudaSuccess) return e;
-        configured.set(lc.device);
-    }
-    const size_t row = (size_t)A.nb * PTI_COEFFS * 8;
-    const unsigned grid = (unsigned)(lc.L * (((size_t)1 << LOGN) / PTI_COEFFS));
-    for (u32 g0 = 0; g0 < A.ng; g0 += gmax) {
-        const u32 gcnt = A.ng - g0 < gmax ? A.ng - g0 : gmax;
-        kern<<<grid, NT, ((size_t)gcnt + 4) * row, st>>>(A, lc.lt, g0, gcnt);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return e;
-    }
-    return cudaSuccess;
-}
-
 // out[g] = sum_b steps[b] o pts[g][b]; returns the number of kernel launches through *launches
 cudaError_t launch_pt_inner(const LaunchCtx &lc, const u64 *steps, u32 nb, const u64 *pts, u32 ng, u64 *out, size_t batch, cudaStream_t st,
                             unsigned *launches) {
@@ -2028,49 +1842,22 @@ cudaError_t launch_pt_inner(const LaunchCtx &lc, const u64 *steps, u32 nb, const
     const u32 gmax = pt_inner_gmax(nb);
     if (gmax == 0) return cudaErrorInvalidValue;
     *launches = (ng + gmax - 1) / gmax;
-    switch (lc.log_n) {
-        case 12: return launch_pt_inner_t<12>(lc, A, gmax, st);
-        case 13: return launch_pt_inner_t<13>(lc, A, gmax, st);
-        case 14: return launch_pt_inner_t<14>(lc, A, gmax, st);
-    }
-    return cudaErrorInvalidValue;
-}
-
-template <int LOGN>
-static cudaError_t launch_hoist_t(LaunchCtx &lc, const HoistArgs &A, size_t batch, cudaStream_t st) {
-    constexpr int NT = 256, MINB = 3;
-    auto kern = ks_hoist_kernel<LOGN, NT, MINB>;
-    const size_t smem = LOGN <= 13 ? Geometry<LOGN>::LIMB_BYTES : Geometry<13>::LIMB_BYTES;
-    static ConfiguredMask configured;
-    if (!configured.has(lc.device)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value, NT = 256, MINB = 2;
+        auto kern = pt_inner_kernel<LOGN, NT, MINB>;
+        static ConfiguredMask configured;
+        cudaError_t e = set_smem_once(configured, lc.device, PTI_SMEM_BUDGET, kern);
         if (e != cudaSuccess) return e;
-        configured.set(lc.device);
-    }
-    int occ = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, NT, smem);
-    if (e != cudaSuccess) return e;
-    if (occ < 1) return cudaErrorLaunchOutOfResources;
-    size_t G = (size_t)lc.num_sms * occ;
-    if (G > lc.ks_slots) G = lc.ks_slots;
-    G = (G / lc.L) * lc.L;
-    if (G > batch * lc.L) G = batch * lc.L;
-    if (G == 0) return cudaErrorInvalidConfiguration;
-    cudaError_t em = epoch_guard(lc, batch, st);
-    if (em != cudaSuccess) return em;
-    em = cudaMemsetAsync(lc.ks_ticket, 0, sizeof(u32), st);
-    if (em != cudaSuccess) return em;
-    HoistArgs args = A;
-    LimbTable lt = lc.lt;
-    size_t batch_arg = batch;
-    u32 *flags = lc.ks_flags;
-    u32 epoch = lc.ks_epoch;
-    u32 *ticket = lc.ks_ticket;
-    u64 *mail = lc.ks_mail;
-    void *params[] = {&args, &lt, &batch_arg, &flags, &epoch, &ticket, &mail};
-    e = cudaLaunchCooperativeKernel((void *)kern, dim3((unsigned)G), dim3(NT), params, smem, st);
-    lc.ks_epoch += (u32)(batch + 1);
-    return e;
+        const size_t row = (size_t)A.nb * PTI_COEFFS * 8;
+        const unsigned grid = (unsigned)(lc.L * (((size_t)1 << LOGN) / PTI_COEFFS));
+        for (u32 g0 = 0; g0 < A.ng; g0 += gmax) {
+            const u32 gcnt = A.ng - g0 < gmax ? A.ng - g0 : gmax;
+            kern<<<grid, NT, ((size_t)gcnt + 4) * row, st>>>(A, lc.lt, g0, gcnt);
+            e = cudaGetLastError();
+            if (e != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+    });
 }
 
 // hoisted rotations, step 1: U[ct][j][i] and the zero flags of `batch` ciphertexts (L >= 2)
@@ -2078,113 +1865,56 @@ cudaError_t launch_hoist(LaunchCtx &lc, const u64 *ct, u64 *U, u32 *zero, size_t
     if (batch == 0) return cudaSuccess;
     HoistArgs A;
     A.ct = ct; A.U = U; A.scratch = lc.ks_scratch; A.zero = zero; A.tw = lc.tw; A.itw = lc.itw; A.L = lc.L;
-    switch (lc.log_n) {
-        case 12: return launch_hoist_t<12>(lc, A, batch, st);
-        case 13: return launch_hoist_t<13>(lc, A, batch, st);
-        case 14: return launch_hoist_t<14>(lc, A, batch, st);
-    }
-    return cudaErrorInvalidValue;
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value;
+        static ConfiguredMask configured;
+        LimbTable lt = lc.lt;
+        Rounds r;
+        void *params[] = {&A, &lt, &r.batch, &r.flags, &r.epoch, &r.ticket, &r.mail};
+        // groups of L CTAs; DPFHE_KS_OCC does not apply
+        return launch_persistent(lc, ks_hoist_kernel<LOGN, 256, 3>, configured, lc.L, Geometry<LOGN>::KS_SMEM, batch, r, params, st, false);
+    });
 }
 
 #endif
 #if DPFHE_PART_GROUPED
-template <int LOGN>
-static cudaError_t launch_hoistg_t(LaunchCtx &lc, const HoistGArgs &A, const GroupConsts &Gc, size_t batch, cudaStream_t st) {
-    constexpr int NT = 256, MINB = 3;
-    auto kern = ks_hoistg_kernel<LOGN, NT, MINB>;
-    const size_t smem = LOGN <= 13 ? Geometry<LOGN>::LIMB_BYTES : Geometry<13>::LIMB_BYTES;
-    static ConfiguredMask configured;
-    if (!configured.has(lc.device)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        configured.set(lc.device);
-    }
-    int occ = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, NT, smem);
-    if (e != cudaSuccess) return e;
-    if (occ < 1) return cudaErrorLaunchOutOfResources;
-    size_t G = (size_t)lc.num_sms * occ;
-    if (G > lc.ks_slots) G = lc.ks_slots;
-    G = (G / lc.L) * lc.L;
-    if (G > batch * lc.L) G = batch * lc.L;
-    if (G == 0) return cudaErrorInvalidConfiguration;
-    cudaError_t em = epoch_guard(lc, batch, st);
-    if (em != cudaSuccess) return em;
-    em = cudaMemsetAsync(lc.ks_ticket, 0, sizeof(u32), st);
-    if (em != cudaSuccess) return em;
-    HoistGArgs args = A;
-    LimbTable lt = lc.lt;
-    GroupConsts gc = Gc;
-    size_t batch_arg = batch;
-    u32 *flags = lc.ks_flags;
-    u32 *done = lc.ks_flags + lc.ks_slots;   // second half of the flag array: "round finished" marks
-    u32 epoch = lc.ks_epoch;
-    u32 *ticket = lc.ks_ticket;
-    u64 *mail = lc.ks_mail;
-    void *params[] = {&args, &lt, &gc, &batch_arg, &flags, &done, &epoch, &ticket, &mail};
-    e = cudaLaunchCooperativeKernel((void *)kern, dim3((unsigned)G), dim3(NT), params, smem, st);
-    lc.ks_epoch += (u32)(batch + 1);
-    return e;
-}
-
 // hoisted rotations with grouped hybrid keys, step 1: U [batch][dnum][L][N]
 cudaError_t launch_hoist_grouped(LaunchCtx &lc, const u64 *ct, u64 *U, const GroupConsts &G, size_t batch, cudaStream_t st) {
     if (batch == 0) return cudaSuccess;
     if (G.Lq + G.K != lc.L) return cudaErrorInvalidValue;
     HoistGArgs A;
     A.ct = ct; A.U = U; A.scratch = lc.ks_scratch; A.tw = lc.tw; A.itw = lc.itw;
-    switch (lc.log_n) {
-        case 12: return launch_hoistg_t<12>(lc, A, G, batch, st);
-        case 13: return launch_hoistg_t<13>(lc, A, G, batch, st);
-        case 14: return launch_hoistg_t<14>(lc, A, G, batch, st);
-    }
-    return cudaErrorInvalidValue;
-}
-
-// Shoup companions of a grouped key [dnum][2][L][N] into key_s (same layout): what launch_ks_grouped and launch_rot_apply_grouped
-// build per call when they are not given them
-cudaError_t launch_key_prepare_grouped(const LaunchCtx &lc, const u64 *key, u64 *key_s, u32 dnum, cudaStream_t st) {
-    const size_t n = (size_t)2 * dnum * lc.L << lc.log_n;
-    const unsigned grid = ew_grid(lc, n);
-    switch (lc.log_n) {
-        case 12: key_prepare_kernel<12><<<grid, 256, 0, st>>>(key, key_s, lc.lp, lc.L, n); break;
-        case 13: key_prepare_kernel<13><<<grid, 256, 0, st>>>(key, key_s, lc.lp, lc.L, n); break;
-        case 14: key_prepare_kernel<14><<<grid, 256, 0, st>>>(key, key_s, lc.lp, lc.L, n); break;
-        default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value;
+        static ConfiguredMask configured;
+        LimbTable lt = lc.lt;
+        GroupConsts gc = G;
+        u32 *done = lc.ks_flags + lc.ks_slots;   // second half of the flag array: "round finished" marks
+        Rounds r;
+        void *params[] = {&A, &lt, &gc, &r.batch, &r.flags, &done, &r.epoch, &r.ticket, &r.mail};
+        // groups of L CTAs; DPFHE_KS_OCC does not apply
+        return launch_persistent(lc, ks_hoistg_kernel<LOGN, 256, 3>, configured, lc.L, Geometry<LOGN>::KS_SMEM, batch, r, params, st, false);
+    });
 }
 
 // step 2: acc [batch][2][L][N] of one rotation (key companions built here into lc.ks_key_s unless the caller supplies them)
 cudaError_t launch_rot_apply_grouped(LaunchCtx &lc, const u64 *ct, const u64 *U, const u64 *key, const u64 *key_s, u32 galois, u64 *acc,
                                      const MsConsts &K, const GroupConsts &G, size_t batch, cudaStream_t st) {
     if (batch == 0) return cudaSuccess;
-    if (!key_s) {
-        const size_t n = (size_t)2 * G.dnum * lc.L << lc.log_n;
-        const unsigned grid = ew_grid(lc, n);
-        if (lc.log_n == 12) key_prepare_kernel<12><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
-        else if (lc.log_n == 13) key_prepare_kernel<13><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
-        else key_prepare_kernel<14><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return e;
-        key_s = lc.ks_key_s;
-    }
-    RotApplyGArgs A;
-    A.ct = ct; A.U = U; A.key = key; A.key_s = key_s; A.acc = acc; A.galois = galois;
-    constexpr size_t cb = 2;
-    const size_t rows = ((batch + cb - 1) / cb) * lc.L, want = (size_t)lc.num_sms * 12;
-    u32 nseg = 1;
-    const u32 max_seg = (1u << (lc.log_n - 1)) / 256;
-    while (nseg < max_seg && rows * nseg < want) nseg *= 2;
-    const size_t n_items = rows * nseg, cap = (size_t)lc.num_sms * 8;
-    const unsigned grid = (unsigned)(n_items < cap ? n_items : cap);
-    switch (lc.log_n) {
-        case 12: rot_apply_grouped_kernel<12, 256, 3, 2><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
-        case 13: rot_apply_grouped_kernel<13, 256, 3, 2><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
-        case 14: rot_apply_grouped_kernel<14, 256, 3, 2><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
-        default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
+    u32 nseg;
+    const unsigned grid = gather_grid(lc, ((batch + 1) / 2) * lc.L, nseg);   // two ciphertexts per work item
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value;
+        if (!key_s) {
+            cudaError_t e = launch_key_prepare_t<LOGN>(lc, key, lc.ks_key_s, G.dnum, st);
+            if (e != cudaSuccess) return e;
+            key_s = lc.ks_key_s;
+        }
+        RotApplyGArgs A;
+        A.ct = ct; A.U = U; A.key = key; A.key_s = key_s; A.acc = acc; A.galois = galois;
+        rot_apply_grouped_kernel<LOGN, 256, 3, 2><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg);
+        return cudaGetLastError();
+    });
 }
 
 // summed rotations: acc [batch][2][L][N] of n_rot (1 .. ROT_SUM_MAX) rotations with their keys' Shoup companions key_s[m]
@@ -2202,28 +1932,14 @@ cudaError_t launch_rot_sum_grouped(const LaunchCtx &lc, const u64 *ct, const u64
         A.galois[m] = galois[m];
     }
     // one ciphertext per work item: with two (the rot_apply_grouped split) the 80 registers of three CTAs per SM spill
-    const size_t rows = batch * lc.L, want = (size_t)lc.num_sms * 12;
-    u32 nseg = 1;
-    const u32 max_seg = (1u << (lc.log_n - 1)) / 256;
-    while (nseg < max_seg && rows * nseg < want) nseg *= 2;
-    const size_t n_items = rows * nseg, cap = (size_t)lc.num_sms * 8;
-    const unsigned grid = (unsigned)(n_items < cap ? n_items : cap);
-    if (key_shift) {
-        switch (lc.log_n) {
-            case 12: rot_sum_grouped_level_kernel<12, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg, key_shift); break;
-            case 13: rot_sum_grouped_level_kernel<13, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg, key_shift); break;
-            case 14: rot_sum_grouped_level_kernel<14, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg, key_shift); break;
-            default: return cudaErrorInvalidValue;
-        }
+    u32 nseg;
+    const unsigned grid = gather_grid(lc, batch * lc.L, nseg);
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value;
+        if (key_shift) rot_sum_grouped_level_kernel<LOGN, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg, key_shift);
+        else rot_sum_grouped_kernel<LOGN, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg);
         return cudaGetLastError();
-    }
-    switch (lc.log_n) {
-        case 12: rot_sum_grouped_kernel<12, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
-        case 13: rot_sum_grouped_kernel<13, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
-        case 14: rot_sum_grouped_kernel<14, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg); break;
-        default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
+    });
 }
 
 #endif
@@ -2231,27 +1947,18 @@ cudaError_t launch_rot_sum_grouped(const LaunchCtx &lc, const u64 *ct, const u64
 // per-rotation constants: Shoup companions of the key (lc.ks_key_s), M = NTT(negmask_g) (in `M`, [L][N]) and kprime [2][L][N]
 cudaError_t launch_rot_prepare(LaunchCtx &lc, const u64 *key, u32 galois, const u64 *delta, u64 *M, u64 *kprime, cudaStream_t st, u64 *key_s_out) {
     u64 *key_s = key_s_out ? key_s_out : lc.ks_key_s;   // a caller that keeps the constants of a rotation supplies its own buffer
-    const size_t n = (size_t)2 * lc.L * lc.L << lc.log_n;
-    const unsigned grid = ew_grid(lc, n), gsmall = ew_grid(lc, (size_t)2 * lc.L << lc.log_n);
-#define ROT_PREP(LOGN)                                                                              \
-    key_prepare_kernel<LOGN><<<grid, 256, 0, st>>>(key, key_s, lc.lp, lc.L, n);                      \
-    negmask_kernel<LOGN><<<(1u << LOGN) / 256, 256, 0, st>>>(M, galois, lc.L);
-    switch (lc.log_n) {
-        case 12: ROT_PREP(12) break;
-        case 13: ROT_PREP(13) break;
-        case 14: ROT_PREP(14) break;
-        default: return cudaErrorInvalidValue;
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    e = launch_ntt(lc, M, 1, false, st);
-    if (e != cudaSuccess) return e;
-    switch (lc.log_n) {
-        case 12: kprime_kernel<12><<<gsmall, 256, 0, st>>>(key, M, delta, kprime, lc.lp, lc.L); break;
-        case 13: kprime_kernel<13><<<gsmall, 256, 0, st>>>(key, M, delta, kprime, lc.lp, lc.L); break;
-        case 14: kprime_kernel<14><<<gsmall, 256, 0, st>>>(key, M, delta, kprime, lc.lp, lc.L); break;
-    }
-    return cudaGetLastError();
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value;
+        cudaError_t e = launch_key_prepare_t<LOGN>(lc, key, key_s, lc.L, st);
+        if (e != cudaSuccess) return e;
+        negmask_kernel<LOGN><<<(1u << LOGN) / 256, 256, 0, st>>>(M, galois, lc.L);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+        e = launch_ntt(lc, M, 1, false, st);
+        if (e != cudaSuccess) return e;
+        kprime_kernel<LOGN><<<ew_grid(lc, (size_t)2 * lc.L << LOGN), 256, 0, st>>>(key, M, delta, kprime, lc.lp, lc.L);
+        return cudaGetLastError();
+    });
 }
 
 // hoisted rotations, step 2: one rotation of `batch` ciphertexts from the shared transforms (constants from launch_rot_prepare)
@@ -2260,141 +1967,86 @@ cudaError_t launch_rot_apply(const LaunchCtx &lc, const u64 *ct, const u64 *U, c
     if (batch == 0) return cudaSuccess;
     RotApplyArgs A;
     A.ct = ct; A.U = U; A.key = key; A.key_s = key_s ? key_s : lc.ks_key_s; A.kprime = kprime; A.out = out; A.L = lc.L; A.galois = galois;
-    // rows are cut into up to NC / 256 segments so that small batches still fill the machine several times over
     // tuning variant (DPFHE_ROT_CFG): 0 (default) = two ciphertexts share each key chunk, next digit prefetched;
     // 1 = one ciphertext per item, prefetched; 2 = one ciphertext, no prefetch.
     const int cfg = lc.rot_cfg;
     const size_t cb = cfg == 0 ? 2 : 1;
-    const size_t rows = ((batch + cb - 1) / cb) * lc.L, want = (size_t)lc.num_sms * 12;
-    u32 nseg = 1;
-    const u32 max_seg = (1u << (lc.log_n - 1)) / 256;
-    while (nseg < max_seg && rows * nseg < want) nseg *= 2;
-    const size_t n_items = rows * nseg, cap = (size_t)lc.num_sms * 8;
-    const unsigned grid = (unsigned)(n_items < cap ? n_items : cap);
-#define ROT_APPLY(LOGN)                                                                                          \
-    if (cfg == 1) rot_apply_kernel<LOGN, 256, 3, 1, true><<<grid, 256, 0, st>>>(A, lc.lt, batch, nseg);           \
-    else if (cfg == 2) rot_apply_kernel<LOGN, 256, 3, 1, false><<<grid, 256, 0, st>>>(A, lc.lt, batch, nseg);     \
-    else rot_apply_kernel<LOGN, 256, 3, 2, true><<<grid, 256, 0, st>>>(A, lc.lt, batch, nseg);
-    switch (lc.log_n) {
-        case 12: ROT_APPLY(12) break;
-        case 13: ROT_APPLY(13) break;
-        case 14: ROT_APPLY(14) break;
-        default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
+    u32 nseg;
+    const unsigned grid = gather_grid(lc, ((batch + cb - 1) / cb) * lc.L, nseg);
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value;
+        if (cfg == 1) rot_apply_kernel<LOGN, 256, 3, 1, true><<<grid, 256, 0, st>>>(A, lc.lt, batch, nseg);
+        else if (cfg == 2) rot_apply_kernel<LOGN, 256, 3, 1, false><<<grid, 256, 0, st>>>(A, lc.lt, batch, nseg);
+        else rot_apply_kernel<LOGN, 256, 3, 2, true><<<grid, 256, 0, st>>>(A, lc.lt, batch, nseg);
+        return cudaGetLastError();
+    });
 }
-
-cudaError_t launch_ks(LaunchCtx &lc, int mode, const u64 *a, const u64 *b, const u64 *key, u64 *out, size_t batch,
-                      u32 galois, cudaStream_t st, const u32 *only, bool key_ready, const u64 *key_s) {
-    if (batch == 0) return cudaSuccess;
-    // Shoup companions of the key for this launch (2*L*P words, a few microseconds; batch-amortised)
-    if (!key_ready) {
-        const size_t n = (size_t)2 * lc.L * lc.L << lc.log_n;
-        const unsigned grid = ew_grid(lc, n);
-        if (lc.log_n == 12) key_prepare_kernel<12><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
-        else if (lc.log_n == 13) key_prepare_kernel<13><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
-        else key_prepare_kernel<14><<<grid, 256, 0, st>>>(key, lc.ks_key_s, lc.lp, lc.L, n);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return e;
-    }
-    KsArgs A;
-    A.a = a; A.b = b; A.key = key; A.key_s = key_ready && key_s ? key_s : lc.ks_key_s; A.out = out; A.scratch = lc.ks_scratch;
-    A.tw = lc.tw; A.itw = lc.itw; A.L = lc.L; A.galois = galois; A.Lk = lc.L; A.hyb = nullptr; A.only = only;
-    A.acc = lc.ks_acc; A.acc_par = 1; A.lift_reduce = lc.lift_reduce ? 1u : 0u;
-#define KS_DISPATCH(LOGN)                                                              \
-    switch (mode) {                                                                    \
-        case KS_MUL_RELIN: return launch_ks_t<LOGN, KS_MUL_RELIN>(lc, A, batch, st);   \
-        case KS_PLAIN: return launch_ks_t<LOGN, KS_PLAIN>(lc, A, batch, st);           \
-        case KS_ROTATE: return launch_ks_t<LOGN, KS_ROTATE>(lc, A, batch, st);         \
-    }                                                                                  \
-    return cudaErrorInvalidValue;
-    switch (lc.log_n) {
-        case 12: KS_DISPATCH(12)
-        case 13: KS_DISPATCH(13)
-        case 14: KS_DISPATCH(14)
-    }
-    return cudaErrorNotSupported;
-}
-
-#define LOGN_SWITCH(call12, call13, call14)  \
-    switch (lc.log_n) {                      \
-        case 12: call12; break;              \
-        case 13: call13; break;              \
-        case 14: call14; break;              \
-        default: return cudaErrorInvalidValue; \
-    }
 
 cudaError_t launch_pointwise_mul(const LaunchCtx &lc, const u64 *a, const u64 *b, u64 *out, size_t n_polys, cudaStream_t st) {
     const size_t n_chunks = n_polys * lc.L * ((size_t)1 << (lc.log_n - 1));
     if (!n_chunks) return cudaSuccess;
-    const unsigned grid = ew_grid(lc, n_chunks);
     auto A = reinterpret_cast<const U64x2 *>(a), B = reinterpret_cast<const U64x2 *>(b);
     auto O = reinterpret_cast<U64x2 *>(out);
-    LOGN_SWITCH((pointwise_mul_kernel<12><<<grid, 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks)),
-                (pointwise_mul_kernel<13><<<grid, 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks)),
-                (pointwise_mul_kernel<14><<<grid, 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks)))
-    return cudaGetLastError();
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        pointwise_mul_kernel<decltype(lg)::value><<<ew_grid(lc, n_chunks), 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t launch_poly_add(const LaunchCtx &lc, const u64 *a, const u64 *b, u64 *out, size_t n_polys, cudaStream_t st) {
     const size_t n_chunks = n_polys * lc.L * ((size_t)1 << (lc.log_n - 1));
     if (!n_chunks) return cudaSuccess;
-    const unsigned grid = ew_grid(lc, n_chunks);
     auto A = reinterpret_cast<const U64x2 *>(a), B = reinterpret_cast<const U64x2 *>(b);
     auto O = reinterpret_cast<U64x2 *>(out);
-    LOGN_SWITCH((poly_add_kernel<12><<<grid, 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks)),
-                (poly_add_kernel<13><<<grid, 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks)),
-                (poly_add_kernel<14><<<grid, 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks)))
-    return cudaGetLastError();
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        poly_add_kernel<decltype(lg)::value><<<ew_grid(lc, n_chunks), 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t launch_ct_mul_plain(const LaunchCtx &lc, const u64 *ct, const u64 *pt, u64 *out, size_t batch, cudaStream_t st) {
     const size_t n_chunks = batch * 2 * lc.L * ((size_t)1 << (lc.log_n - 1));
     if (!n_chunks) return cudaSuccess;
-    const unsigned grid = ew_grid(lc, n_chunks);
     auto A = reinterpret_cast<const U64x2 *>(ct), B = reinterpret_cast<const U64x2 *>(pt);
     auto O = reinterpret_cast<U64x2 *>(out);
-    LOGN_SWITCH((ct_mul_plain_kernel<12><<<grid, 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks)),
-                (ct_mul_plain_kernel<13><<<grid, 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks)),
-                (ct_mul_plain_kernel<14><<<grid, 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks)))
-    return cudaGetLastError();
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        ct_mul_plain_kernel<decltype(lg)::value><<<ew_grid(lc, n_chunks), 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t launch_ct_mul_plain_acc(const LaunchCtx &lc, const u64 *ct, const u64 *pt, u64 *acc, size_t batch, cudaStream_t st) {
     const size_t n_chunks = batch * 2 * lc.L * ((size_t)1 << (lc.log_n - 1));
     if (!n_chunks) return cudaSuccess;
-    const unsigned grid = ew_grid(lc, n_chunks);
     auto A = reinterpret_cast<const U64x2 *>(ct), B = reinterpret_cast<const U64x2 *>(pt);
     auto O = reinterpret_cast<U64x2 *>(acc);
-    LOGN_SWITCH((ct_mul_plain_acc_kernel<12><<<grid, 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks)),
-                (ct_mul_plain_acc_kernel<13><<<grid, 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks)),
-                (ct_mul_plain_acc_kernel<14><<<grid, 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks)))
-    return cudaGetLastError();
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        ct_mul_plain_acc_kernel<decltype(lg)::value><<<ew_grid(lc, n_chunks), 256, 0, st>>>(A, B, O, lc.lp, lc.L, n_chunks);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t launch_ct_tensor(const LaunchCtx &lc, const u64 *a, const u64 *b, u64 *d, size_t batch, cudaStream_t st) {
     const size_t items = batch * lc.L * ((size_t)1 << (lc.log_n - 1));
     if (!items) return cudaSuccess;
-    const unsigned grid = ew_grid(lc, items);
     auto A = reinterpret_cast<const U64x2 *>(a), B = reinterpret_cast<const U64x2 *>(b);
     auto D = reinterpret_cast<U64x2 *>(d);
-    LOGN_SWITCH((ct_tensor_kernel<12><<<grid, 256, 0, st>>>(A, B, D, lc.lp, lc.L, batch)),
-                (ct_tensor_kernel<13><<<grid, 256, 0, st>>>(A, B, D, lc.lp, lc.L, batch)),
-                (ct_tensor_kernel<14><<<grid, 256, 0, st>>>(A, B, D, lc.lp, lc.L, batch)))
-    return cudaGetLastError();
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        ct_tensor_kernel<decltype(lg)::value><<<ew_grid(lc, items), 256, 0, st>>>(A, B, D, lc.lp, lc.L, batch);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t launch_fill_uniform(const LaunchCtx &lc, u64 seed, u64 first_poly, u64 *data, size_t n_polys, cudaStream_t st) {
     const size_t P = (size_t)lc.L << lc.log_n;
     const size_t n_chunks = n_polys * P / 2;
     if (!n_chunks) return cudaSuccess;
-    const unsigned grid = ew_grid(lc, n_chunks);
     auto O = reinterpret_cast<U64x2 *>(data);
     const u64 first_elem = first_poly * P;
-    LOGN_SWITCH((fill_uniform_kernel<12><<<grid, 256, 0, st>>>(O, lc.lp, lc.L, seed, first_elem, n_chunks)),
-                (fill_uniform_kernel<13><<<grid, 256, 0, st>>>(O, lc.lp, lc.L, seed, first_elem, n_chunks)),
-                (fill_uniform_kernel<14><<<grid, 256, 0, st>>>(O, lc.lp, lc.L, seed, first_elem, n_chunks)))
-    return cudaGetLastError();
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        fill_uniform_kernel<decltype(lg)::value><<<ew_grid(lc, n_chunks), 256, 0, st>>>(O, lc.lp, lc.L, seed, first_elem, n_chunks);
+        return cudaGetLastError();
+    });
 }
 
 #endif

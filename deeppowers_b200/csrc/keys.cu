@@ -4,10 +4,8 @@
 // compilation unit: no kernel of kernels.cu shares a body with these.
 #include <cuda_runtime.h>
 
-#include <atomic>
-
 #include "keys.cuh"
-#include "launch.hpp"
+#include "launch_util.hpp"
 
 namespace dpfhe {
 namespace DPFHE_VNS {
@@ -77,20 +75,6 @@ __global__ void __launch_bounds__(256) decrypt_kernel(const U64x2 *__restrict__ 
 
 namespace {
 
-struct ConfiguredMask {
-    std::atomic<unsigned long long> bits{0};
-    bool has(int device) const { return (bits.load(std::memory_order_acquire) >> (device & 63)) & 1ull; }
-    void set(int device) { bits.fetch_or(1ull << (device & 63), std::memory_order_release); }
-};
-
-template <class Kern>
-cudaError_t set_smem_once(Kern kern, size_t smem, ConfiguredMask &configured, int device) {
-    if (configured.has(device)) return cudaSuccess;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) configured.set(device);
-    return e;
-}
-
 template <int LOGN, int MODE>
 cudaError_t launch_keys_mode(const LaunchCtx &lc, const KeyArgs &A, size_t n_items, cudaStream_t st) {
     constexpr size_t N = (size_t)1 << LOGN;
@@ -99,13 +83,13 @@ cudaError_t launch_keys_mode(const LaunchCtx &lc, const KeyArgs &A, size_t n_ite
     if constexpr (LOGN == NTT_PAIR_LOGN) {
         auto k = keys_ntt_pair_kernel<256, 2, MODE>;
         const size_t smem = N * 4 + N;   // half a limb + the small row
-        cudaError_t e = set_smem_once(k, smem, conf, lc.device);
+        cudaError_t e = set_smem_once(conf, lc.device, smem, k);
         if (e != cudaSuccess) return e;
         k<<<(unsigned)(2 * n_limbs), 256, smem, st>>>(A, lc.tw, lc.lt, lc.L);
     } else {
         auto k = keys_ntt_kernel<LOGN, 256, 2, MODE>;   // at 3 CTAs per SM (80 registers) the generic variant's store stage spills
         const size_t smem = N * 8 + N;
-        cudaError_t e = set_smem_once(k, smem, conf, lc.device);
+        cudaError_t e = set_smem_once(conf, lc.device, smem, k);
         if (e != cudaSuccess) return e;
         k<<<(unsigned)n_limbs, 256, smem, st>>>(A, lc.tw, lc.lt, lc.L);
     }
@@ -131,29 +115,18 @@ cudaError_t launch_keys_n(const LaunchCtx &lc, int mode, const KeyArgs &A, size_
 cudaError_t launch_keys(const LaunchCtx &lc, int mode, const KeyArgs &A, size_t n_items, cudaStream_t st) {
     if (n_items == 0) return cudaSuccess;
     if (n_items * lc.L * 2 > 0x7fffffffull) return cudaErrorInvalidValue;
-    switch (lc.log_n) {
-        case 12: return launch_keys_n<12>(lc, mode, A, n_items, st);
-        case 13: return launch_keys_n<13>(lc, mode, A, n_items, st);
-        case 14: return launch_keys_n<14>(lc, mode, A, n_items, st);
-    }
-    return cudaErrorInvalidValue;
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) { return launch_keys_n<decltype(lg)::value>(lc, mode, A, n_items, st); });
 }
 
 cudaError_t launch_decrypt(const LaunchCtx &lc, const u64 *ct, const u64 *s, u64 *pt, u32 n_comp, size_t n, cudaStream_t st) {
     const size_t n_chunks = n * lc.L * ((size_t)1 << (lc.log_n - 1));
     if (!n_chunks) return cudaSuccess;
-    size_t blocks = (n_chunks + 255) / 256;
-    const size_t cap = (size_t)lc.num_sms * 32;   // as the element-wise kernels of kernels.cu
-    if (blocks > cap) blocks = cap;
     auto C = reinterpret_cast<const U64x2 *>(ct), S = reinterpret_cast<const U64x2 *>(s);
     auto O = reinterpret_cast<U64x2 *>(pt);
-    switch (lc.log_n) {
-        case 12: decrypt_kernel<12><<<(unsigned)blocks, 256, 0, st>>>(C, S, O, lc.lp, lc.L, n_comp, n_chunks); break;
-        case 13: decrypt_kernel<13><<<(unsigned)blocks, 256, 0, st>>>(C, S, O, lc.lp, lc.L, n_comp, n_chunks); break;
-        case 14: decrypt_kernel<14><<<(unsigned)blocks, 256, 0, st>>>(C, S, O, lc.lp, lc.L, n_comp, n_chunks); break;
-        default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        decrypt_kernel<decltype(lg)::value><<<ew_grid(lc, n_chunks), 256, 0, st>>>(C, S, O, lc.lp, lc.L, n_comp, n_chunks);
+        return cudaGetLastError();
+    });
 }
 
 }  // namespace DPFHE_VNS
