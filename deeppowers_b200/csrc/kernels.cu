@@ -27,12 +27,85 @@
 namespace dpfhe {
 namespace DPFHE_VNS {
 
+// The protocol of the persistent kernels (DESIGN.md §4.4, §4.7): tickets, mailboxes and flags carry 32-bit round numbers.
+__device__ __forceinline__ u32 ld_acquire_u32(const u32 *p) {
+    u32 v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_release_u32(u32 *p, u32 v) {
+    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ u64 ld_acquire_u64(const u64 *p) {
+    u64 v;
+    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_release_u64(u64 *p, u64 v) {
+    asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+// the calling thread waits until *flag has reached round `tag`; the signed difference keeps the comparison right across wrap-around
+__device__ __forceinline__ void spin_until(const u32 *flag, u32 tag) {
+    while ((int)(ld_acquire_u32(flag) - tag) < 0) {
+    }
+}
+// thread k < count waits for flags[k], then the CTA meets at a barrier
+__device__ __forceinline__ void wait_flags(const u32 *flags, u32 count, u32 tag) {
+    if (threadIdx.x < count) spin_until(flags + threadIdx.x, tag);
+    __syncthreads();
+}
+// makes the CTA's global stores visible, then thread 0 release-stores round `tag` to *flag
+__device__ __forceinline__ void publish_flag(u32 *flag, u32 tag) {
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) st_release_u32(flag, tag);
+}
+// the ciphertext of round `tag`, returned to every thread: the group's leader draws it from the global ticket counter and, if
+// `post`, posts it tagged with the round in the mailbox box(); the other members spin until that tag appears there.  Only thread 0
+// evaluates box(), so the mailbox address is not held in a register through the rest of the round.
+template <class Box>
+__device__ __forceinline__ u32 draw_ticket(u32 *ticket, Box box, u32 tag, bool leader, bool post) {
+    __shared__ u32 s_ct;
+    if (threadIdx.x == 0) {
+        u64 *const mb = box();
+        if (leader) {
+            const u32 t = atomicAdd(ticket, 1u);
+            if (post) st_release_u64(mb, ((u64)tag << 32) | t);
+            s_ct = t;
+        } else {
+            u64 m;
+            do m = ld_acquire_u64(mb);
+            while ((u32)(m >> 32) != tag);
+            s_ct = (u32)m;
+        }
+    }
+    __syncthreads();
+    return s_ct;
+}
+
 // barrier scopes of the CTA policy (ntt_core.cuh): CTA, 256-thread domain, warp.
 // PROF: thread 0 accumulates clock64() deltas per phase id into prof[blockIdx][id] (diagnostics only).
 template <int NT, bool PROF = false>
 struct DevCta {
     unsigned long long *prof = nullptr;
     long long last = 0;
+    unsigned long long t_start = 0, c_start = 0;
+    __device__ __forceinline__ void prof_begin(unsigned long long *all) {
+        if (PROF) {
+            prof = all + (size_t)blockIdx.x * 16;
+            last = clock64();
+            c_start = (unsigned long long)last;
+            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_start));
+        }
+    }
+    __device__ __forceinline__ void prof_end() {
+        if (PROF && threadIdx.x == 0) {   // CTA lifetime in nanoseconds (globaltimer) and in SM cycles
+            unsigned long long t_end;
+            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_end));
+            prof[14] += t_end - t_start;
+            prof[15] += (unsigned long long)clock64() - c_start;
+        }
+    }
     __device__ __forceinline__ void mark(int id) {
         if (PROF && threadIdx.x == 0) {
             const long long now = clock64();
@@ -46,14 +119,7 @@ struct DevCta {
         __syncthreads();
     }
     // blocks the CTA until the monotone counter *flag has reached `target` (wrap-safe comparison)
-    __device__ __forceinline__ void wait_ge(const u32 *flag, u32 target) {
-        if (threadIdx.x == 0) {
-            u32 v;
-            do asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(flag) : "memory");
-            while ((int)(v - target) < 0);
-        }
-        __syncthreads();
-    }
+    __device__ __forceinline__ void wait_ge(const u32 *flag, u32 target) { wait_flags(flag, 1, target); }
     template <class F>
     __device__ __forceinline__ void par_dom(F f) {
         f((int)threadIdx.x);
@@ -366,23 +432,6 @@ __global__ void __launch_bounds__(NT, 1) bgv_dec_kernel(u64 *work, u64 *slots, c
 
 #endif
 // ------------------------------------------------------------------ fused key-switch family
-__device__ __forceinline__ u32 ld_acquire_u32(const u32 *p) {
-    u32 v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_release_u32(u32 *p, u32 v) {
-    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ u64 ld_acquire_u64(const u64 *p) {
-    u64 v;
-    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_release_u64(u64 *p, u64 v) {
-    asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-
 // TMA-unit bulk prefetch of a contiguous region into L2 (SASS: UBLKPF.L2); bytes must be a multiple of 16
 __device__ __forceinline__ void bulk_prefetch_l2(const void *p, u32 bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
@@ -399,6 +448,26 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void *p, u32 bytes) {
 //             pair a cluster of two CTAs) or L CTAs (N = 4096); pair `slot` owns limb i = slot % L and digit slot `slot`.
 //   N = 16384 (else branch of ks_fused_kernel): one limb per CTA in two halves, accumulators in L2-resident scratch rows; a group is L CTAs.
 
+// Tickets are drawn in order, so ciphertext ct + pf_dist will be started by some group a few microseconds from now: thread 0
+// pulls this CTA's share of its inputs (`bytes` at offset `off` of every input polynomial of ciphertext nc = ct + pf_dist) from HBM
+// into L2 with the TMA unit's bulk prefetch, so the tensor phase that consumes them is L2- rather than HBM-latency bound.  The
+// callers test that condition themselves, so that only thread 0 evaluates the offset.
+template <int LOGN, int MODE>
+__device__ __forceinline__ void prefetch_inputs(const KsArgs &A, size_t nc, size_t off, u32 bytes) {
+    constexpr size_t N = (size_t)1 << LOGN;
+    const size_t P = (size_t)A.L * N;
+    if (MODE == KS_PLAIN) {
+        bulk_prefetch_l2(A.a + nc * P + off, bytes);
+    } else {
+        bulk_prefetch_l2(A.a + nc * 2 * P + off, bytes);
+        bulk_prefetch_l2(A.a + nc * 2 * P + P + off, bytes);
+        if (MODE == KS_MUL_RELIN) {
+            bulk_prefetch_l2(A.b + nc * 2 * P + off, bytes);
+            bulk_prefetch_l2(A.b + nc * 2 * P + P + off, bytes);
+        }
+    }
+}
+
 template <int LOGN, int NT, int MODE, bool PROF, bool FILTER>
 __device__ __forceinline__ void ks_fused_blk(const KsArgs &A, const LimbTable &lt, size_t batch, u32 *flags, u32 epoch, u32 *ticket, u64 *mail,
                                              unsigned long long *prof, u32 pf_dist) {
@@ -408,15 +477,8 @@ __device__ __forceinline__ void ks_fused_blk(const KsArgs &A, const LimbTable &l
     u64 *buf = reinterpret_cast<u64 *>(smem_raw);
     U64x2 *acc = reinterpret_cast<U64x2 *>(smem_raw + ((size_t)8 << KS_BLK_LOGN));
     DevCta<NT, PROF> cta;
-    unsigned long long t_start = 0, c_start = 0;
-    if (PROF) {
-        cta.prof = prof + (size_t)blockIdx.x * 16;
-        cta.last = clock64();
-        c_start = (unsigned long long)cta.last;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_start));
-    }
+    cta.prof_begin(prof);
     namespace cg = cooperative_groups;
-    __shared__ u32 s_ct;
     const u32 L = A.L, h = blockIdx.x % PAIR, slot = blockIdx.x / PAIR, i = slot % L, group = slot / L;
     const u64 *peer = buf;
     if constexpr (PAIR == 2) peer = cg::this_cluster().map_shared_rank(buf, (int)h ^ 1);
@@ -427,39 +489,16 @@ __device__ __forceinline__ void ks_fused_blk(const KsArgs &A, const LimbTable &l
     const LimbParams &p = lt.lp[i];
     u32 executed = 0;
     for (u32 round = 0;; ++round) {
-        if (!FILTER && threadIdx.x == 0) {
-            const u32 tag = epoch + round + 1;
-            if (i == 0 && h == 0) {
-                const u32 t = atomicAdd(ticket, 1u);
-                if (L * PAIR > 1) st_release_u64(mail + group, ((u64)tag << 32) | t);
-                s_ct = t;
-            } else {
-                u64 m;
-                do m = ld_acquire_u64(mail + group);
-                while ((u32)(m >> 32) != tag);
-                s_ct = (u32)m;
-            }
-        }
-        __syncthreads();
-        // FILTER: static assignment computed by every thread (see the N = 16384 branch below)
-        const size_t ct = FILTER ? (size_t)round * (gridDim.x / (L * PAIR)) + group : (size_t)s_ct;
+        if (FILTER) __syncthreads();
+        // FILTER: static assignment computed by every thread (see the N = 16384 branch below).  The round tag epoch + round + 1 is
+        // written out at each use in both fused loops: held in a register through the round, it spills at N = 16384.
+        const size_t ct = FILTER ? (size_t)round * (gridDim.x / (L * PAIR)) + group
+                                 : (size_t)draw_ticket(ticket, [&] { return mail + group; }, epoch + round + 1, i == 0 && h == 0,
+                                                       L * PAIR > 1);
         if (ct >= batch) break;   // every member of the group reads the same ticket, so they leave together
         if (FILTER && A.only[ct] == 0u) continue;
-        // bulk prefetch of this CTA's block of the inputs of ciphertext ct + pf_dist (see the N = 16384 branch below)
-        if (pf_dist && threadIdx.x == 0 && ct + pf_dist < batch) {
-            const size_t nc = ct + pf_dist, P = (size_t)L * N, off = (size_t)i * N + ((size_t)h << KS_BLK_LOGN);
-            constexpr u32 BB = 8u << KS_BLK_LOGN;
-            if (MODE == KS_PLAIN) {
-                bulk_prefetch_l2(A.a + nc * P + off, BB);
-            } else {
-                bulk_prefetch_l2(A.a + nc * 2 * P + off, BB);
-                bulk_prefetch_l2(A.a + nc * 2 * P + P + off, BB);
-                if (MODE == KS_MUL_RELIN) {
-                    bulk_prefetch_l2(A.b + nc * 2 * P + off, BB);
-                    bulk_prefetch_l2(A.b + nc * 2 * P + P + off, BB);
-                }
-            }
-        }
+        if (pf_dist && threadIdx.x == 0 && ct + pf_dist < batch)
+            prefetch_inputs<LOGN, MODE>(A, ct + pf_dist, (size_t)i * N + ((size_t)h << KS_BLK_LOGN), 8u << KS_BLK_LOGN);
         const u32 parity = (FILTER ? executed++ : round) & 1u;
         ks_blk_phase1_local<LOGN, NT, MODE>(cta, buf, acc, A, p, ct, i, (int)h);
         // the partner's block has been through the inverse passes, and the partner has read this round's mailbox (with L = 1 this
@@ -472,22 +511,13 @@ __device__ __forceinline__ void ks_fused_blk(const KsArgs &A, const LimbTable &l
             if (h == 0 && threadIdx.x == 0) st_release_u32(flags + slot, epoch + round + 1);
             for (u32 jj = 1; jj < L; ++jj) {
                 const u32 j = (i + jj) % L, sib = slot - i + j;
-                if (threadIdx.x == 0) {
-                    while ((int)(ld_acquire_u32(flags + sib) - (epoch + round + 1)) < 0) {
-                    }
-                }
-                __syncthreads();
+                wait_flags(flags + sib, 1, epoch + round + 1);
                 cta.mark(3);   // waiting for the sibling's digit
                 ks_blk_phase2<LOGN, NT>(cta, buf, acc, A, p, ct, i, j, jj, (int)h, A.scratch + ((size_t)sib * 2 + parity) * N);
             }
         }
     }
-    if (PROF && threadIdx.x == 0) {   // CTA lifetime in nanoseconds (globaltimer) and in SM cycles
-        unsigned long long t_end;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_end));
-        cta.prof[14] += t_end - t_start;
-        cta.prof[15] += (unsigned long long)clock64() - c_start;
-    }
+    cta.prof_end();
 }
 
 template <int LOGN, int NT, int MINB, int MODE, bool PROF, bool FILTER = false>
@@ -501,14 +531,7 @@ __global__ void __launch_bounds__(NT, MINB) ks_fused_kernel(KsArgs A, const __gr
         constexpr size_t N = (size_t)1 << LOGN;
         u64 *buf = reinterpret_cast<u64 *>(smem_raw);
         DevCta<NT, PROF> cta;
-        unsigned long long t_start = 0, c_start = 0;
-        if (PROF) {
-            cta.prof = prof + (size_t)blockIdx.x * 16;
-            cta.last = clock64();
-            c_start = (unsigned long long)cta.last;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_start));
-        }
-        __shared__ u32 s_ct;
+        cta.prof_begin(prof);
         const u32 L = A.L, slot = blockIdx.x, i = slot % L, group = slot / L;
         const LimbParams &p = lt.lp[i];
         u32 executed = 0;
@@ -522,42 +545,15 @@ __global__ void __launch_bounds__(NT, MINB) ks_fused_kernel(KsArgs A, const __gr
         const u32 consumed_base = consumed ? s_base : 0u;
         u32 published = 0;   // digits this CTA has published in this launch
         for (u32 round = 0;; ++round) {
-            if (!FILTER && threadIdx.x == 0) {
-                const u32 tag = epoch + round + 1;
-                if (i == 0) {
-                    const u32 t = atomicAdd(ticket, 1u);
-                    if (L > 1) st_release_u64(mail + group, ((u64)tag << 32) | t);
-                    s_ct = t;
-                } else {
-                    u64 m;
-                    do m = ld_acquire_u64(mail + group);
-                    while ((u32)(m >> 32) != tag);
-                    s_ct = (u32)m;
-                }
-            }
-            __syncthreads();
+            if (FILTER) __syncthreads();
             // FILTER: static assignment computed by every thread.  Skipped rounds involve no exchange between the members of
-            // a group, so a leader handing out tickets could run ahead and overwrite a mailbox tag (or s_ct) before it was read.
-            const size_t ct = FILTER ? (size_t)round * (gridDim.x / L) + group : (size_t)s_ct;
+            // a group, so a leader handing out tickets could run ahead and overwrite a mailbox tag (or the posted ticket in
+            // shared memory) before it was read.
+            const size_t ct = FILTER ? (size_t)round * (gridDim.x / L) + group
+                                     : (size_t)draw_ticket(ticket, [&] { return mail + group; }, epoch + round + 1, i == 0, L > 1);
             if (ct >= batch) break;   // every member of the group reads the same ticket, so they leave together
             if (FILTER && A.only[ct] == 0u) continue;
-            // Tickets are drawn in order, so ciphertext ct + pf_dist will be started by some group a few microseconds
-            // from now: pull this CTA's limb of its inputs from HBM into L2 with the TMA unit's bulk prefetch, so the
-            // tensor phase that consumes them is L2- rather than HBM-latency bound.
-            if (pf_dist && threadIdx.x == 0 && ct + pf_dist < batch) {
-                const size_t nc = ct + pf_dist, P = (size_t)L * N;
-                constexpr u32 LB = (u32)(N * 8);
-                if (MODE == KS_PLAIN) {
-                    bulk_prefetch_l2(A.a + nc * P + (size_t)i * N, LB);
-                } else {
-                    bulk_prefetch_l2(A.a + nc * 2 * P + (size_t)i * N, LB);
-                    bulk_prefetch_l2(A.a + nc * 2 * P + P + (size_t)i * N, LB);
-                    if (MODE == KS_MUL_RELIN) {
-                        bulk_prefetch_l2(A.b + nc * 2 * P + (size_t)i * N, LB);
-                        bulk_prefetch_l2(A.b + nc * 2 * P + P + (size_t)i * N, LB);
-                    }
-                }
-            }
+            if (pf_dist && threadIdx.x == 0 && ct + pf_dist < batch) prefetch_inputs<LOGN, MODE>(A, ct + pf_dist, (size_t)i * N, (u32)(N * 8));
             const u32 parity = consumed ? 0u : (FILTER ? executed++ : round) & 1u;
             const size_t slot_stride = consumed ? 1 : 2;      // digit slots per CTA
             u64 *acc_rows = A.acc + (size_t)slot * 2 * N;   // this CTA's two lazy accumulator rows (L2 resident, reused every round)
@@ -565,16 +561,10 @@ __global__ void __launch_bounds__(NT, MINB) ks_fused_kernel(KsArgs A, const __gr
                                       consumed && L > 1 ? consumed + slot : nullptr, consumed_base + published * (L - 1));
             ++published;
             if (L > 1) {
-                __threadfence();
-                __syncthreads();
-                if (threadIdx.x == 0) st_release_u32(flags + slot, epoch + round + 1);
+                publish_flag(flags + slot, epoch + round + 1);
                 for (u32 jj = 1; jj < L; ++jj) {
                     const u32 j = (i + jj) % L, sib = slot - i + j;
-                    if (threadIdx.x == 0) {
-                        while ((int)(ld_acquire_u32(flags + sib) - (epoch + round + 1)) < 0) {
-                        }
-                    }
-                    __syncthreads();
+                    wait_flags(flags + sib, 1, epoch + round + 1);
                     cta.mark(3);   // waiting for the sibling's digit
                     ks_phase2_digit<LOGN, NT>(cta, buf, A, p, ct, i, j, jj, A.scratch + ((size_t)sib * slot_stride + parity) * N, acc_rows);
                     // every thread is past its last read of the sibling's digit (the body ends with a CTA barrier): hand the slot back
@@ -585,13 +575,7 @@ __global__ void __launch_bounds__(NT, MINB) ks_fused_kernel(KsArgs A, const __gr
                 }
             }
         }
-        if (PROF && threadIdx.x == 0) {   // CTA lifetime in nanoseconds (globaltimer) and in SM cycles
-            unsigned long long t_end;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_end));
-            cta.prof[14] += t_end - t_start;
-            cta.prof[15] += (unsigned long long)clock64() - c_start;
-        }
-
+        cta.prof_end();
     }
 }
 
@@ -604,38 +588,18 @@ __global__ void __launch_bounds__(NT, MINB) ks_hoist_kernel(HoistArgs A, const _
     constexpr size_t N = (size_t)1 << LOGN;
     u64 *buf = reinterpret_cast<u64 *>(smem_raw);
     DevCta<NT> cta;
-    __shared__ u32 s_ct;
     const u32 L = A.L, slot = blockIdx.x, i = slot % L, group = slot / L;
     const LimbParams &p = lt.lp[i];
     for (u32 round = 0;; ++round) {
         const u32 tag = epoch + round + 1;
-        if (threadIdx.x == 0) {
-            if (i == 0) {
-                const u32 t = atomicAdd(ticket, 1u);
-                st_release_u64(mail + group, ((u64)tag << 32) | t);
-                s_ct = t;
-            } else {
-                u64 m;
-                do m = ld_acquire_u64(mail + group);
-                while ((u32)(m >> 32) != tag);
-                s_ct = (u32)m;
-            }
-        }
-        __syncthreads();
-        const size_t ct = s_ct;
+        const size_t ct = draw_ticket(ticket, [&] { return mail + group; }, tag, i == 0, true);
         if (ct >= batch) break;
         const u32 parity = round & 1u;
         hoist_phase1<LOGN, NT>(cta, buf, A, p, ct, i, A.scratch + ((size_t)slot * 2 + parity) * N);
-        __threadfence();
-        __syncthreads();
-        if (threadIdx.x == 0) st_release_u32(flags + slot, tag);
+        publish_flag(flags + slot, tag);
         for (u32 jj = 1; jj < L; ++jj) {
             const u32 j = (i + jj) % L, sib = slot - i + j;
-            if (threadIdx.x == 0) {
-                while ((int)(ld_acquire_u32(flags + sib) - tag) < 0) {
-                }
-            }
-            __syncthreads();
+            wait_flags(flags + sib, 1, tag);
             hoist_phase2<LOGN, NT>(cta, buf, A, p, ct, i, j, A.scratch + ((size_t)sib * 2 + parity) * N);
         }
     }
@@ -707,28 +671,15 @@ __device__ __forceinline__ void ks_hybrid_body(const KsArgs &A, const LimbTable 
     constexpr size_t N = (size_t)1 << LOGN;
     u64 *buf = reinterpret_cast<u64 *>(smem_raw);
     DevCta<NT> cta;
-    __shared__ u32 s_ct;
     const u32 L = A.L, GS = L + 1, slot = blockIdx.x, i = slot % GS, group = slot / GS, base = slot - i;
     const u32 key_shift = LV ? A.Lk - GS : 0u;   // Lq - l
     const bool special = i == L;
     const LimbParams &p = lt.lp[i];
     u64 *hyb = A.hyb + (size_t)group * KS_HYB_ROWS * N;
-    auto wait_for = [&](u32 sib, u32 tag) {
-        if (threadIdx.x == 0) {
-            while ((int)(ld_acquire_u32(flags + sib) - tag) < 0) {
-            }
-        }
-        __syncthreads();
-    };
-    auto publish = [&](u32 tag) {
-        __threadfence();
-        __syncthreads();
-        if (threadIdx.x == 0) st_release_u32(flags + slot, tag);
-    };
     // the postponed division of one ciphertext (limb CTAs): needs tau' of that round
     auto acc_of = [&](u32 parity) { return A.acc + ((size_t)slot * 2 + parity) * 2 * N; };   // accumulator rows, double-buffered by round parity
     auto divide = [&](size_t ct, u32 tag, u32 parity) {
-        wait_for(base + L, tag);
+        wait_flags(flags + (base + L), 1, tag);
         const size_t P = (size_t)L * N;
         for (u32 c = 0; c < 2; ++c) {
             u64 *row = A.out + ct * 2 * P + c * P + (size_t)i * N;   // lazy accumulator -> final value in the output row
@@ -740,21 +691,7 @@ __device__ __forceinline__ void ks_hybrid_body(const KsArgs &A, const LimbTable 
     u32 prev_tag = 0, prev_parity = 0;
     for (u32 round = 0;; ++round) {
         const u32 tag = epoch + round + 1, parity = round & 1u;
-        if (threadIdx.x == 0) {
-            u64 *box = mail + (size_t)group * 2 + parity;
-            if (i == 0) {
-                const u32 t = atomicAdd(ticket, 1u);
-                st_release_u64(box, ((u64)tag << 32) | t);
-                s_ct = t;
-            } else {
-                u64 m;
-                do m = ld_acquire_u64(box);
-                while ((u32)(m >> 32) != tag);
-                s_ct = (u32)m;
-            }
-        }
-        __syncthreads();
-        const size_t ct = s_ct;
+        const size_t ct = draw_ticket(ticket, [&] { return mail + (size_t)group * 2 + parity; }, tag, i == 0, true);
         if (ct >= batch) break;
         if (!special) {
             if constexpr (LV)
@@ -762,10 +699,10 @@ __device__ __forceinline__ void ks_hybrid_body(const KsArgs &A, const LimbTable 
                                                       K.qlm_s[i], nullptr, 0, ~0u, nullptr, key_shift);
             else
                 ks_phase1<LOGN, NT, MODE, true>(cta, buf, A, p, ct, i, A.scratch + ((size_t)slot * 2 + parity) * N, acc_of(parity), K.qlm[i], K.qlm_s[i]);
-            publish(tag);
+            publish_flag(flags + slot, tag);
             for (u32 jj = 1; jj < L; ++jj) {
                 const u32 j = (i + jj) % L;
-                wait_for(base + j, tag);
+                wait_flags(flags + (base + j), 1, tag);
                 ks_phase2_digit<LOGN, NT, true, false, LV>(cta, buf, A, p, ct, i, j, jj, A.scratch + ((size_t)(base + j) * 2 + parity) * N, acc_of(parity),
                                                            key_shift);
             }
@@ -777,12 +714,12 @@ __device__ __forceinline__ void ks_hybrid_body(const KsArgs &A, const LimbTable 
         } else {
             for (u32 jj = 0; jj < L; ++jj) {
                 const u32 j = (group + jj) % L;   // groups start at different digits: spreads the key-column reads
-                wait_for(base + j, tag);
+                wait_flags(flags + (base + j), 1, tag);
                 ks_phase2_digit<LOGN, NT, true, true, LV>(cta, buf, A, p, ct, i, j, jj, A.scratch + ((size_t)(base + j) * 2 + parity) * N, hyb, key_shift);
             }
             for (u32 c = 0; c < 2; ++c)
                 ms_tau_body<LOGN, NT, true>(cta, buf, hyb + c * N, hyb + c * N, A.itw + (size_t)i * N, p, hyb + ks_hyb_tau_row(parity, c) * N, K);
-            publish(tag);
+            publish_flag(flags + slot, tag);
         }
     }
     if (pending) divide(prev_ct, prev_tag, prev_parity);   // the group's last ciphertext
@@ -829,36 +766,18 @@ __device__ __forceinline__ void ks_grouped_body(const KsArgs &A, const LimbTable
     constexpr size_t N = (size_t)1 << LOGN;
     u64 *buf = reinterpret_cast<u64 *>(smem_raw);
     DevCta<NT> cta;
-    __shared__ u32 s_ct;
     const u32 Lq = G.Lq, Ks = G.K, dnum = G.dnum, GS = Lq + Ks, slot = blockIdx.x, i = slot % GS, group = slot / GS, base = slot - i;
     const u32 key_shift = LV ? A.Lk - GS : 0u;   // Lq - l of the top level
     const bool special = i >= Lq;
     const LimbParams &p = lt.lp[i];
     // rows of special prime k of this group: accumulators (0, 1) and tau' (double-buffered by round parity)
     auto hyb_of = [&](u32 k) { return A.hyb + ((size_t)group * Ks + k) * KS_HYB_ROWS * N; };
-    auto wait_for = [&](u32 first, u32 count, u32 tag) {
-        if (threadIdx.x < count) {
-            while ((int)(ld_acquire_u32(flags + first + threadIdx.x) - tag) < 0) {
-            }
-        }
-        __syncthreads();
-    };
-    auto publish = [&](u32 tag) {
-        __threadfence();
-        __syncthreads();
-        if (threadIdx.x == 0) st_release_u32(flags + slot, tag);
-    };
     auto acc_of = [&](u32 parity) { return A.acc + ((size_t)slot * 2 + parity) * 2 * N; };
     // y_qbar row c of round parity `parity` (RS)
     auto drop_of = [&](u32 parity, u32 c) { return R->tau + (((size_t)group * 2 + parity) * 2 + c) * N; };
     auto divide = [&](size_t ct, u32 tag, u32 parity) {
-        if constexpr (RS) {
-            if (threadIdx.x == 0) {
-                while ((int)(ld_acquire_u32(R->tau_flag + group) - tag) < 0) {
-                }
-            }
-        }
-        wait_for(base + Lq, Ks, tag);
+        if constexpr (RS) if (threadIdx.x == 0) spin_until(R->tau_flag + group, tag);   // the barrier of the next wait covers it
+        wait_flags(flags + (base + Lq), Ks, tag);
         if constexpr (RS) {
             const size_t P = (size_t)(Lq - 1) * N;
             for (u32 c = 0; c < 2; ++c)
@@ -881,31 +800,17 @@ __device__ __forceinline__ void ks_grouped_body(const KsArgs &A, const LimbTable
     u32 prev_tag = 0, prev_parity = 0;
     for (u32 round = 0;; ++round) {
         const u32 tag = epoch + round + 1, parity = round & 1u;
-        if (threadIdx.x == 0) {
-            u64 *box = mail + (size_t)group * 2 + parity;
-            if (i == 0) {
-                const u32 t = atomicAdd(ticket, 1u);
-                st_release_u64(box, ((u64)tag << 32) | t);
-                s_ct = t;
-            } else {
-                u64 m;
-                do m = ld_acquire_u64(box);
-                while ((u32)(m >> 32) != tag);
-                s_ct = (u32)m;
-            }
-        }
-        __syncthreads();
-        const size_t ct = s_ct;
+        const size_t ct = draw_ticket(ticket, [&] { return mail + (size_t)group * 2 + parity; }, tag, i == 0, true);
         if (ct >= batch) break;
         const u64 *t_rows = A.scratch + ((size_t)base * 2 + parity) * N;   // row of limb j: + j * 2N
         if (!special) {
             const u32 g_own = i / Ks;
             ks_phase1<LOGN, NT, MODE, true, LV>(cta, buf, A, G.lp_up[i], ct, i, A.scratch + ((size_t)slot * 2 + parity) * N, acc_of(parity), K.qlm[i],
                                                 K.qlm_s[i], nullptr, 0, g_own, dot, key_shift);
-            publish(tag);
+            publish_flag(flags + slot, tag);
             for (u32 jj = 1; jj < dnum; ++jj) {
                 const u32 g = (g_own + jj) % dnum, lo = g * Ks, cnt = lo + Ks < Lq ? Ks : Lq - lo;
-                wait_for(base + lo, cnt, tag);
+                wait_flags(flags + (base + lo), cnt, tag);
                 ks_phase2_group<LOGN, NT, false, LV>(cta, buf, A, G, p, ct, i, g, jj, t_rows, 2 * N, acc_of(parity), key_shift);
             }
             if constexpr (RS) if (i == Lq - 1) {
@@ -914,13 +819,11 @@ __device__ __forceinline__ void ks_grouped_body(const KsArgs &A, const LimbTable
                 // Lq-2 of its own digit, never awaited by phase 2) are awaited here.  Its digit slot is protected by the mailbox:
                 // limb 0 posts this round only after its divide(round - 2), which waited for every special CTA of round - 2.
                 const u32 lo = g_own * Ks;
-                wait_for(base + lo, i - lo, tag);
+                wait_flags(flags + (base + lo), i - lo, tag);
                 for (u32 c = 0; c < 2; ++c)
                     ms_tau_body<LOGN, NT, true>(cta, buf, acc_of(parity) + c * N, acc_of(parity) + c * N, A.itw + (size_t)i * N, R->lp_drop,
                                                 drop_of(parity, c), K);
-                __threadfence();
-                __syncthreads();
-                if (threadIdx.x == 0) st_release_u32(R->tau_flag + group, tag);
+                publish_flag(R->tau_flag + group, tag);
                 continue;
             }
             if (pending) divide(prev_ct, prev_tag, prev_parity);
@@ -932,12 +835,12 @@ __device__ __forceinline__ void ks_grouped_body(const KsArgs &A, const LimbTable
             u64 *hyb = hyb_of(i - Lq);
             for (u32 jj = 0; jj < dnum; ++jj) {
                 const u32 g = (group + jj) % dnum, lo = g * Ks, cnt = lo + Ks < Lq ? Ks : Lq - lo;
-                wait_for(base + lo, cnt, tag);
+                wait_flags(flags + (base + lo), cnt, tag);
                 ks_phase2_group<LOGN, NT, true, LV>(cta, buf, A, G, p, ct, i, g, jj, t_rows, 2 * N, hyb, key_shift);
             }
             for (u32 c = 0; c < 2; ++c)
                 ms_tau_body<LOGN, NT, true>(cta, buf, hyb + c * N, hyb + c * N, A.itw + (size_t)i * N, G.lp_up[i], hyb + ks_hyb_tau_row(parity, c) * N, K);
-            publish(tag);
+            publish_flag(flags + slot, tag);
         }
     }
     if (pending) divide(prev_ct, prev_tag, prev_parity);   // the group's last ciphertext
@@ -993,49 +896,25 @@ __global__ void __launch_bounds__(NT, MINB) ks_hoistg_kernel(HoistGArgs A, const
     constexpr size_t N = (size_t)1 << LOGN;
     u64 *buf = reinterpret_cast<u64 *>(smem_raw);
     DevCta<NT> cta;
-    __shared__ u32 s_ct;
     const u32 Lq = G.Lq, Ks = G.K, dnum = G.dnum, GS = Lq + Ks, slot = blockIdx.x, i = slot % GS, group = slot / GS, base = slot - i;
     const LimbParams &p = lt.lp[i];
-    auto wait_for = [&](const u32 *f, u32 first, u32 count, u32 tag) {
-        if (threadIdx.x < count) {
-            while ((int)(ld_acquire_u32(f + first + threadIdx.x) - tag) < 0) {
-            }
-        }
-        __syncthreads();
-    };
     for (u32 round = 0;; ++round) {
         const u32 tag = epoch + round + 1, parity = round & 1u;
-        if (round >= 2) wait_for(done, base, GS, tag - 2);
-        if (threadIdx.x == 0) {
-            u64 *box = mail + (size_t)group * 2 + parity;
-            if (i == 0) {
-                const u32 t = atomicAdd(ticket, 1u);
-                st_release_u64(box, ((u64)tag << 32) | t);
-                s_ct = t;
-            } else {
-                u64 m;
-                do m = ld_acquire_u64(box);
-                while ((u32)(m >> 32) != tag);
-                s_ct = (u32)m;
-            }
-        }
-        __syncthreads();
-        const size_t ct = s_ct;
+        if (round >= 2) wait_flags(done + base, GS, tag - 2);
+        const size_t ct = draw_ticket(ticket, [&] { return mail + (size_t)group * 2 + parity; }, tag, i == 0, true);
         if (ct >= batch) break;
         const u64 *t_rows = A.scratch + ((size_t)base * 2 + parity) * N;
         u32 g_own = dnum;   // a special limb belongs to no digit
         if (i < Lq) {
             g_own = i / Ks;
             hoistg_phase1<LOGN, NT>(cta, buf, A, G, ct, i, A.scratch + ((size_t)slot * 2 + parity) * N);
-            __threadfence();
-            __syncthreads();
-            if (threadIdx.x == 0) st_release_u32(flags + slot, tag);
+            publish_flag(flags + slot, tag);
         }
         for (u32 jj = 0; jj < dnum; ++jj) {
             const u32 g = (group + i + jj) % dnum;
             if (g == g_own) continue;
             const u32 lo = g * Ks, cnt = lo + Ks < Lq ? Ks : Lq - lo;
-            wait_for(flags, base + lo, cnt, tag);
+            wait_flags(flags + (base + lo), cnt, tag);
             hoistg_phase2<LOGN, NT>(cta, buf, A, G, p, ct, i, g, t_rows, 2 * N);
         }
         __syncthreads();   // every thread is past its last read of the group's digit slots
