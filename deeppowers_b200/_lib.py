@@ -145,6 +145,12 @@ SYMBOLS = {
                                              C.c_uint64, C.c_void_p]),
     "dpfhe_rotate_sum_grouped_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.c_size_t, C.c_uint64, C.c_void_p]),
+    "dpfhe_rotate_hoisted_grouped_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                     C.c_size_t, C.c_uint64, C.c_void_p]),
+    "dpfhe_linear_create_grouped_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p,
+                                                    C.c_uint64, C.POINTER(C.c_void_p)]),
+    "dpfhe_slotsum_create_grouped_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint64,
+                                                     C.POINTER(C.c_void_p)]),
     "dpfhe_ct_mul_relin_rescale_grouped_level_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                                 C.c_size_t, C.c_uint64]),
     "dpfhe_ct_dot_rescale_grouped_level_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -1078,9 +1078,11 @@ int dpfhe_rotate_hoisted(dpfhe_ctx *ctx, const uint64_t *d_ct, size_t n_rot, con
 // the division by P (md_tau / md_limb kernels).  Same plaintexts as n_rot calls of dpfhe_rotate_grouped, not the same bits.
 // key_s: optional Shoup companions of every key, kept by the caller (a linear layer applies the same rotations to every batch);
 // nullptr = built per rotation into the context's scratch (one more launch each).
+// lv: the rotations at that level (DESIGN.md §2.21), on its view, reading top-level keys; companions the caller does not give are
+// built with the context's launch state over the level's ceil(l / K) digits, as level_launch builds them.
 static int rotate_hoisted_grouped_impl(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_ct, size_t n_rot, const uint64_t *galois_elts,
                                        const uint64_t *const *d_gks, const uint64_t *const *key_s, uint64_t *d_out, size_t batch, uint64_t t_plain,
-                                       void *stream) {
+                                       void *stream, const KsLevel *lv = nullptr) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (batch == 0 || n_rot == 0) return DPFHE_OK;
@@ -1088,7 +1090,7 @@ static int rotate_hoisted_grouped_impl(dpfhe_ctx *ctx, unsigned n_special, const
     if (!galois_elts || !d_gks) return fail(DPFHE_ERR_INVALID, "null argument");
     rc = check_grouped(ctx, n_special, t_plain);
     if (rc) return rc;
-    const size_t N = ctx->N(), L = ctx->hp.L, Lq = L - n_special, Pq = Lq * N, dnum = (Lq + n_special - 1) / n_special;
+    const size_t N = ctx->N(), L = lv ? lv->l + n_special : ctx->hp.L, Lq = L - n_special, Pq = Lq * N, dnum = (Lq + n_special - 1) / n_special;
     rc = check_rotations(ctx, n_rot, galois_elts, d_gks);
     if (rc) return rc;
     if (overlaps(d_out, n_rot * batch * 2 * Pq * 8, d_ct, batch * 2 * Pq * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
@@ -1101,16 +1103,26 @@ static int rotate_hoisted_grouped_impl(dpfhe_ctx *ctx, unsigned n_special, const
     u64 *U = ctx->hoistg.get(), *acc = U + chunk * u_words, *tau = acc + chunk * acc_words;
     MsConsts K;
     GroupConsts G;
-    build_group_consts(ctx->hp, n_special, t_plain, G, K);
+    build_group_consts(lv ? lv->hp : ctx->hp, n_special, t_plain, G, K);
+    const u32 key_shift = (u32)(ctx->hp.L - L);
+    auto on_view = [&](auto launch) { return lv ? on_level_view(ctx, *lv, launch) : launch(ctx->lc); };
     for (size_t first = 0; first < batch; first += chunk) {
         const size_t cnt = batch - first < chunk ? batch - first : chunk;
         const u64 *in = d_ct + first * 2 * Pq;
-        CU_TRY(VCALL(launch_hoist_grouped, ctx->lc, in, U, G, cnt, st));
+        CU_TRY(on_view([&](LaunchCtx &lc) { return VCALL(launch_hoist_grouped, lc, in, U, G, cnt, st); }));
         note_launch(ctx, 1);
         for (size_t r = 0; r < n_rot; ++r) {
             u64 *out = d_out + (r * batch + first) * 2 * Pq;
-            CU_TRY(VCALL(launch_rot_apply_grouped, ctx->lc, in, U, d_gks[r], key_s ? key_s[r] : nullptr, (u32)galois_elts[r], acc, K, G, cnt, st));
-            CU_TRY(VCALL(launch_mod_down_special, ctx->lc, acc, tau, out, K, G, 2 * cnt, st));
+            const u64 *ks = key_s ? key_s[r] : nullptr;
+            if (lv && !ks) {
+                CU_TRY(VCALL(launch_key_prepare, ctx->lc, d_gks[r], ctx->lc.ks_key_s, (u32)dnum, st));
+                ks = ctx->lc.ks_key_s;
+            }
+            CU_TRY(on_view([&](LaunchCtx &lc) {
+                cudaError_t e = VCALL(launch_rot_apply_grouped, lc, in, U, d_gks[r], ks, (u32)galois_elts[r], acc, K, G, cnt, st, key_shift);
+                if (e == cudaSuccess) e = VCALL(launch_mod_down_special, lc, acc, tau, out, K, G, 2 * cnt, st);
+                return e;
+            }));
             note_launch(ctx, key_s ? 3 : 4);   // (key_prepare,) rot_apply_grouped, md_tau, md_limb
         }
     }
@@ -1120,6 +1132,28 @@ static int rotate_hoisted_grouped_impl(dpfhe_ctx *ctx, unsigned n_special, const
 int dpfhe_rotate_hoisted_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_ct, size_t n_rot, const uint64_t *galois_elts,
                                  const uint64_t *const *d_gks, uint64_t *d_out, size_t batch, uint64_t t_plain, void *stream) {
     return rotate_hoisted_grouped_impl(ctx, n_special, d_ct, n_rot, galois_elts, d_gks, nullptr, d_out, batch, t_plain, stream);
+}
+
+// hoisted rotations at level l (DESIGN.md §2.21): the checks of dpfhe_rotate_hoisted_grouped with the level's sizes, then the level's;
+// l = Lq is the top-level call
+int dpfhe_rotate_hoisted_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *d_ct, size_t n_rot,
+                                       const uint64_t *galois_elts, const uint64_t *const *d_gks, uint64_t *d_out, size_t batch, uint64_t t_plain,
+                                       void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (batch == 0 || n_rot == 0) return DPFHE_OK;
+    CHECK_PTR(d_ct); CHECK_PTR(d_out);
+    if (!galois_elts || !d_gks) return fail(DPFHE_ERR_INVALID, "null argument");
+    rc = check_grouped(ctx, n_special, t_plain);
+    if (!rc) rc = check_level(ctx, n_special, level, false, t_plain);
+    if (!rc) rc = check_rotations(ctx, n_rot, galois_elts, d_gks);
+    if (rc) return rc;
+    const size_t ct_bytes = batch * 2 * (size_t)level * ctx->N() * 8;
+    if (overlaps(d_out, n_rot * ct_bytes, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "level %u: output must not overlap the input", level);
+    const KsLevel *lv = nullptr;
+    if (level < ctx->hp.L - n_special) rc = level_state(ctx, n_special, level, lv);
+    if (rc) return rc;
+    return rotate_hoisted_grouped_impl(ctx, n_special, d_ct, n_rot, galois_elts, d_gks, nullptr, d_out, batch, t_plain, stream, lv);
 }
 
 // Summed rotations (DESIGN.md §2.17).  Scratch in ctx->hoistg: `head` words first (the key companions of a dpfhe_rotate_sum_grouped
@@ -2138,7 +2172,8 @@ struct dpfhe_linear {
     dpfhe_ctx *const ctx;
     size_t baby = 0, giant = 0;
     unsigned n_special = 0;                 // 0: per-limb-digit keys; K > 0: grouped keys with K special primes
-    size_t Lq = 0;                          // limbs of a ciphertext polynomial: L, or L - K with grouped keys
+    size_t Lq = 0;                          // limbs of a ciphertext polynomial: L, or L - K with grouped keys, or the level
+    unsigned level = 0;                     // grouped keys below the top level (DESIGN.md §2.21): Lq = level < L - K; 0 at the top
     u64 *d_diags = nullptr;                 // [n][Lq][N]
     std::vector<uint64_t> g_baby;           // Galois elements 5^b, b = 1 .. baby-1
     uint64_t g_giant = 0;
@@ -2179,10 +2214,13 @@ static int linear_check_shape(size_t n_diags, size_t baby, const uint64_t *h_gk_
 }
 
 // The start of both constructors: a layer with its diagonals on the device, and the Galois elements of its rotations.
-static int linear_new(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *h_diags, size_t n_diags, size_t baby, dpfhe_linear **out) {
+// level: the layer's level below the top (its diagonals have `level` rows), 0 at the top.
+static int linear_new(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *h_diags, size_t n_diags, size_t baby, dpfhe_linear **out,
+                      unsigned level = 0) {
     dpfhe_linear *lin = new (std::nothrow) dpfhe_linear(ctx);
     if (!lin) return fail(DPFHE_ERR_NOMEM, "out of host memory");
-    lin->baby = baby; lin->giant = n_diags / baby; lin->n_special = n_special; lin->Lq = ctx->hp.L - n_special; lin->t_plain = t_plain;
+    lin->baby = baby; lin->giant = n_diags / baby; lin->n_special = n_special; lin->Lq = level ? level : ctx->hp.L - n_special; lin->t_plain = t_plain;
+    lin->level = level;
     const size_t diag_bytes = n_diags * lin->Lq * ctx->N() * 8;
     cudaError_t e = cudaMalloc(&lin->d_diags, diag_bytes);
     if (e == cudaSuccess) e = cudaMemcpy(lin->d_diags, h_diags, diag_bytes, cudaMemcpyHostToDevice);
@@ -2241,20 +2279,18 @@ int dpfhe_linear_create(dpfhe_ctx *ctx, const uint64_t *h_diags, size_t n_diags,
     return object_finish(lin, rc, st, "linear layer constants", out);
 }
 
-int dpfhe_linear_create_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_diags, size_t n_diags, size_t baby,
-                                const uint64_t *h_gk_baby, const uint64_t *h_gk_giant, uint64_t t_plain, dpfhe_linear **out) {
-    int rc = enter(ctx);
-    if (rc) return rc;
-    if (!out || !h_diags) return fail(DPFHE_ERR_INVALID, "null argument");
-    *out = nullptr;
-    rc = check_grouped(ctx, n_special, t_plain);
-    if (rc) return rc;
-    rc = linear_check_shape(n_diags, baby, h_gk_baby, h_gk_giant);
+// the grouped layer once its arguments are checked; level: below the top level (DESIGN.md §2.21), 0 at the top.  A level layer builds
+// the level's state here, so that its first application allocates no level tables; its keys and their companions are the top-level
+// ones, which serve every level.
+static int linear_grouped_new(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *h_diags, size_t n_diags, size_t baby,
+                              const uint64_t *h_gk_baby, const uint64_t *h_gk_giant, uint64_t t_plain, dpfhe_linear **out) {
+    const KsLevel *lv = nullptr;
+    int rc = level ? level_state(ctx, n_special, level, lv) : DPFHE_OK;
     if (rc) return rc;
     dpfhe_linear *lin = nullptr;
-    rc = linear_new(ctx, n_special, t_plain, h_diags, n_diags, baby, &lin);
+    rc = linear_new(ctx, n_special, t_plain, h_diags, n_diags, baby, &lin, level);
     if (rc) return rc;
-    build_group_consts(ctx->hp, n_special, t_plain, lin->G, lin->K);
+    build_group_consts(lv ? lv->hp : ctx->hp, n_special, t_plain, lin->G, lin->K);
     rc = lin->giant > 1 ? ensure_hyb(ctx) : DPFHE_OK;   // the special-prime rows of the giant steps' kernel
     cudaStream_t st = pick(ctx, nullptr);
     // the Shoup companions of every key, once: each application would otherwise rebuild them for every rotation
@@ -2265,20 +2301,50 @@ int dpfhe_linear_create_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64
     return object_finish(lin, rc, st, "linear layer constants", out);
 }
 
+int dpfhe_linear_create_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *h_diags, size_t n_diags, size_t baby,
+                                const uint64_t *h_gk_baby, const uint64_t *h_gk_giant, uint64_t t_plain, dpfhe_linear **out) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!out || !h_diags) return fail(DPFHE_ERR_INVALID, "null argument");
+    *out = nullptr;
+    rc = check_grouped(ctx, n_special, t_plain);
+    if (rc) return rc;
+    rc = linear_check_shape(n_diags, baby, h_gk_baby, h_gk_giant);
+    if (rc) return rc;
+    return linear_grouped_new(ctx, n_special, 0, h_diags, n_diags, baby, h_gk_baby, h_gk_giant, t_plain, out);
+}
+
+// the grouped layer at level l (DESIGN.md §2.21): the checks of dpfhe_linear_create_grouped, then the level's; l = Lq is that call
+int dpfhe_linear_create_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *h_diags, size_t n_diags, size_t baby,
+                                      const uint64_t *h_gk_baby, const uint64_t *h_gk_giant, uint64_t t_plain, dpfhe_linear **out) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!out || !h_diags) return fail(DPFHE_ERR_INVALID, "level %u: null argument", level);
+    *out = nullptr;
+    rc = check_grouped(ctx, n_special, t_plain);
+    if (!rc) rc = check_level(ctx, n_special, level, false, t_plain);
+    if (!rc) rc = linear_check_shape(n_diags, baby, h_gk_baby, h_gk_giant);
+    if (rc) return rc;
+    return linear_grouped_new(ctx, n_special, level == ctx->hp.L - n_special ? 0 : level, h_diags, n_diags, baby, h_gk_baby, h_gk_giant, t_plain, out);
+}
+
 void dpfhe_linear_destroy(dpfhe_linear *lin) { object_destroy(lin); }
 
 // grouped keys: hoisted baby steps, the inner sums on the ciphertext moduli, giant - 1 fused Horner steps.  Launches per application
 // (a batch within one chunk of the hoisted-rotation scratch): [baby > 1] * (1 + 3 (baby-1)) + ceil(giant / gmax(baby)) + (giant - 1),
-// gmax = the giant steps one inner-product launch holds.
+// gmax = the giant steps one inner-product launch holds; the same at a level.  A level layer looks its level's state up at every
+// application rather than keeping it: dpfhe_context_trim frees it (the lookup then builds it again).
 int dpfhe_linear::apply_grouped_on(const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
+    const KsLevel *lv = nullptr;
+    int rc = level ? level_state(ctx, n_special, level, lv) : DPFHE_OK;
+    if (rc) return rc;
     const size_t ctb = batch * in_words();                      // words of one ciphertext batch
     u64 *steps = scratch.get(), *inner = steps + baby * ctb, *tmp = inner + giant * ctb;
     cudaStream_t st = pick(ctx, stream);
     CU_TRY(cudaMemcpyAsync(steps, d_ct, ctb * 8, cudaMemcpyDeviceToDevice, st));
-    int rc = DPFHE_OK;
     if (baby > 1)
         rc = rotate_hoisted_grouped_impl(ctx, n_special, steps, baby - 1, g_baby.data(), gk.keys.data(), gk.key_s.data(), steps + ctb, batch, t_plain,
-                                         stream);
+                                         stream, lv);
     if (rc) return rc;
     // every inner sum in one pass, on the ciphertext moduli
     st = pick(ctx, stream);
@@ -2295,8 +2361,14 @@ int dpfhe_linear::apply_grouped_on(const uint64_t *d_ct, uint64_t *d_out, size_t
     const u64 *acc = inner + (giant - 1) * ctb;
     for (size_t g = giant - 1; g-- > 0;) {
         u64 *dst = g % 2 == 0 ? d_out : tmp;
-        CU_TRY(VCALL(launch_ks_grouped, ctx->lc, KS_ROTATE, acc, nullptr, gk.keys[baby - 1], dst, batch, (u32)g_giant, K, G, st, inner + g * ctb,
-                     gk.key_s[baby - 1]));
+        if (lv)
+            CU_TRY(on_level_view(ctx, *lv, [&](LaunchCtx &lc) {
+                return VCALL(launch_ks_grouped_level, lc, KS_ROTATE, &acc, nullptr, 1, gk.keys[baby - 1], gk.key_s[baby - 1], (u32)ctx->hp.L, dst, batch,
+                             (u32)g_giant, K, G, nullptr, st, inner + g * ctb);
+            }));
+        else
+            CU_TRY(VCALL(launch_ks_grouped, ctx->lc, KS_ROTATE, acc, nullptr, gk.keys[baby - 1], dst, batch, (u32)g_giant, K, G, st, inner + g * ctb,
+                         gk.key_s[baby - 1]));
         note_launch(ctx, 1);
         acc = dst;
     }
@@ -2854,6 +2926,7 @@ struct dpfhe_slotsum {
     dpfhe_ctx *const ctx;
     unsigned K = 0;
     size_t Lq = 0;
+    unsigned level = 0;                  // below the top level (DESIGN.md §2.21): Lq = level < L - K, its state looked up at each use; 0 at the top
     std::vector<u32> n_rot;              // rotations of each stage
     std::vector<u32> galois;             // Galois elements of every step, stage by stage
     PreparedKeys gk;                     // the keys of every step, in the same order
@@ -2866,10 +2939,17 @@ struct dpfhe_slotsum {
     ~dpfhe_slotsum() { gk.release(); }
     size_t in_words() const { return 2 * Lq * ctx->N(); }
     size_t out_words() const { return in_words(); }
+    // the level's state (nullptr at the top): never kept, dpfhe_context_trim frees it
+    int level_of(const KsLevel *&lv) const {
+        lv = nullptr;
+        return level ? level_state(ctx, K, level, lv) : DPFHE_OK;
+    }
     // the object's intermediate batch and the context's hoisted-rotation scratch
     int reserve(size_t batch) {
-        const int rc = n_rot.size() > 1 ? mem.reserve(batch * in_words() * 8) : DPFHE_OK;
-        return rc ? rc : rotate_sum_reserve(ctx, K, 0, batch);
+        const KsLevel *lv = nullptr;
+        int rc = n_rot.size() > 1 ? mem.reserve(batch * in_words() * 8) : DPFHE_OK;
+        if (!rc) rc = level_of(lv);
+        return rc ? rc : rotate_sum_reserve(ctx, K, 0, batch, lv);
     }
     size_t host_chunk(size_t batch) const { return item_chunk(ctx, batch, "DPFHE_SLOTSUM_CHUNK"); }
     int apply_on(const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream);
@@ -2877,18 +2957,56 @@ struct dpfhe_slotsum {
 
 // S stages, alternating between the scratch batch and d_out so that the last one writes d_out; 4 launches per stage and chunk
 int dpfhe_slotsum::apply_on(const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream) {
+    const KsLevel *lv = nullptr;
+    const int rc = level_of(lv);
+    if (rc) return rc;
     cudaStream_t st = pick(ctx, stream);
     const size_t S = n_rot.size();
     const u64 *in = d_ct;
     size_t first = 0;
     for (size_t t = 0; t < S; ++t) {
         u64 *dst = (S - 1 - t) % 2 == 0 ? d_out : mem.get();
-        const int rc = rotate_sum_stage(ctx, K, 0, in, n_rot[t], galois.data() + first, gk.keys.data() + first, gk.key_s.data() + first, dst, batch, Kc, G, st);
+        const int rc = rotate_sum_stage(ctx, K, 0, in, n_rot[t], galois.data() + first, gk.keys.data() + first, gk.key_s.data() + first, dst, batch, Kc, G, st,
+                                        lv);
         if (rc) return rc;
         first += n_rot[t];
         in = dst;
     }
     return DPFHE_OK;
+}
+
+// the slot sum at `level` (0: the top level) once the context, the pointers, n_special and t_plain are checked; a level slot sum builds
+// its level's state here, so that its first application allocates no level tables; its keys are the top-level keys
+static int slotsum_new(dpfhe_ctx *ctx, unsigned n_special, unsigned level, size_t stride, const unsigned *radices, size_t n_stages,
+                       const uint64_t *h_gks, uint64_t t_plain, dpfhe_slotsum **out) {
+    int rc = DPFHE_OK;
+    int steps[16 * 15];   // the most dpfhe_slotsum_steps accepts: 16 stages of radix 16
+    size_t n_steps = 0;
+    rc = dpfhe_slotsum_steps(stride, radices, n_stages, steps, &n_steps);
+    if (rc) return rc;
+    // stride * prod(radices) is the last stage's span, its first step, times its radix
+    const unsigned r_last = radices[n_stages - 1];
+    const size_t total = (size_t)steps[n_steps - (r_last - 1)] * r_last;
+    if (total > ctx->N() / 2) return fail(DPFHE_ERR_INVALID, "stride * prod(radices) = %zu exceeds N/2 = %zu", total, ctx->N() / 2);
+    const KsLevel *lv = nullptr;
+    rc = level ? level_state(ctx, n_special, level, lv) : DPFHE_OK;
+    if (rc) return rc;
+    dpfhe_slotsum *ss = new (std::nothrow) dpfhe_slotsum(ctx);
+    if (!ss) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    ss->K = n_special; ss->Lq = level ? level : ctx->hp.L - n_special; ss->level = level;
+    for (size_t t = 0; t < n_stages; ++t) ss->n_rot.push_back(radices[t] - 1);
+    for (size_t k = 0; k < n_steps; ++k) {
+        uint64_t g = 0;
+        dpfhe_galois_element(ctx, steps[k], &g);
+        ss->galois.push_back((u32)g);
+    }
+    build_group_consts(lv ? lv->hp : ctx->hp, n_special, t_plain, ss->G, ss->Kc);
+    const size_t dnum = key_digits(ctx, n_special);
+    cudaStream_t st = pick(ctx, nullptr);
+    rc = prepare_keys(ctx, ctx->lc, n_steps, dnum, st, "slot sum keys",
+                      [&](u64 *d_keys) { return cudaMemcpyAsync(d_keys, h_gks, n_steps * dnum * 2 * ctx->P() * 8, cudaMemcpyHostToDevice, st); }, ss->gk);
+    if (rc == DPFHE_OK) ss->mem.count_fixed(ss->gk.bytes);
+    return object_finish(ss, rc, st, "slot sum keys", out);
 }
 
 int dpfhe_slotsum_create_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t stride, const unsigned *radices, size_t n_stages,
@@ -2899,30 +3017,20 @@ int dpfhe_slotsum_create_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t stri
     *out = nullptr;
     rc = check_grouped(ctx, n_special, t_plain);
     if (rc) return rc;
-    int steps[16 * 15];   // the most dpfhe_slotsum_steps accepts: 16 stages of radix 16
-    size_t n_steps = 0;
-    rc = dpfhe_slotsum_steps(stride, radices, n_stages, steps, &n_steps);
+    return slotsum_new(ctx, n_special, 0, stride, radices, n_stages, h_gks, t_plain, out);
+}
+
+// the slot sum at level l (DESIGN.md §2.21): the checks of dpfhe_slotsum_create_grouped, then the level's; l = Lq is that call
+int dpfhe_slotsum_create_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, size_t stride, const unsigned *radices, size_t n_stages,
+                                       const uint64_t *h_gks, uint64_t t_plain, dpfhe_slotsum **out) {
+    int rc = enter(ctx);
     if (rc) return rc;
-    // stride * prod(radices) is the last stage's span, its first step, times its radix
-    const unsigned r_last = radices[n_stages - 1];
-    const size_t total = (size_t)steps[n_steps - (r_last - 1)] * r_last;
-    if (total > ctx->N() / 2) return fail(DPFHE_ERR_INVALID, "stride * prod(radices) = %zu exceeds N/2 = %zu", total, ctx->N() / 2);
-    dpfhe_slotsum *ss = new (std::nothrow) dpfhe_slotsum(ctx);
-    if (!ss) return fail(DPFHE_ERR_NOMEM, "out of host memory");
-    ss->K = n_special; ss->Lq = ctx->hp.L - n_special;
-    for (size_t t = 0; t < n_stages; ++t) ss->n_rot.push_back(radices[t] - 1);
-    for (size_t k = 0; k < n_steps; ++k) {
-        uint64_t g = 0;
-        dpfhe_galois_element(ctx, steps[k], &g);
-        ss->galois.push_back((u32)g);
-    }
-    build_group_consts(ctx->hp, n_special, t_plain, ss->G, ss->Kc);
-    const size_t dnum = key_digits(ctx, n_special);
-    cudaStream_t st = pick(ctx, nullptr);
-    rc = prepare_keys(ctx, ctx->lc, n_steps, dnum, st, "slot sum keys",
-                      [&](u64 *d_keys) { return cudaMemcpyAsync(d_keys, h_gks, n_steps * dnum * 2 * ctx->P() * 8, cudaMemcpyHostToDevice, st); }, ss->gk);
-    if (rc == DPFHE_OK) ss->mem.count_fixed(ss->gk.bytes);
-    return object_finish(ss, rc, st, "slot sum keys", out);
+    if (!out || !h_gks) return fail(DPFHE_ERR_INVALID, "level %u: null argument", level);
+    *out = nullptr;
+    rc = check_grouped(ctx, n_special, t_plain);
+    if (!rc) rc = check_level(ctx, n_special, level, false, t_plain);
+    if (rc) return rc;
+    return slotsum_new(ctx, n_special, level == ctx->hp.L - n_special ? 0 : level, stride, radices, n_stages, h_gks, t_plain, out);
 }
 
 void dpfhe_slotsum_destroy(dpfhe_slotsum *ss) { object_destroy(ss); }

@@ -1281,9 +1281,11 @@ struct RotApplyGArgs {
     u32 galois;
 };
 
-template <int LOGN, int NT, int CB, class CTA>
+// LV (DESIGN.md §4.18): the key is a top-level key, key_shift rows longer than the view's per (digit, component), read through
+// ks_key_row with its companions, as in rot_sum_grouped_rows; the lifted digits U keep the view's layout.
+template <int LOGN, int NT, int CB, bool LV = false, class CTA>
 DPFHE_HD void rot_apply_grouped_rows(CTA &cta, const RotApplyGArgs &A, const GroupConsts &G, const MsConsts &K, const LimbParams &p, size_t ct0,
-                                     u32 n_ct, u32 i, int c_lo = 0, int c_hi = 1 << (LOGN - 1)) {
+                                     u32 n_ct, u32 i, int c_lo = 0, int c_hi = 1 << (LOGN - 1), u32 key_shift = 0) {
     constexpr int N = 1 << LOGN;
     const u32 L = G.Lq + G.K, D = G.dnum, g = A.galois;
     const size_t P = (size_t)L * N, Pq = (size_t)G.Lq * N;
@@ -1305,7 +1307,15 @@ DPFHE_HD void rot_apply_grouped_rows(CTA &cta, const RotApplyGArgs &A, const Gro
             // the operands of digit d + 1 (key chunks and gathered rows) are requested before the arithmetic of digit d: the loop
             // is bound by the latency of the gathers (ncu: long-scoreboard stalls), as in rot_apply_rows
             auto fetch = [&](u32 d, RotOperands<CB> &o) {
-                const size_t kb = ((size_t)d * 2 + 0) * P + (size_t)i * N, ka = ((size_t)d * 2 + 1) * P + (size_t)i * N;
+                size_t kb, ka;
+                if constexpr (LV) {
+                    const size_t PK = (size_t)(L + key_shift) * N, kr = ks_key_row(i, G.Lq, key_shift);
+                    kb = ((size_t)d * 2 + 0) * PK + kr * N;
+                    ka = ((size_t)d * 2 + 1) * PK + kr * N;
+                } else {
+                    kb = ((size_t)d * 2 + 0) * P + (size_t)i * N;
+                    ka = ((size_t)d * 2 + 1) * P + (size_t)i * N;
+                }
                 o.vb = ld_keep(reinterpret_cast<const U64x2 *>(A.key + kb) + c);
                 o.vbs = ld_keep(reinterpret_cast<const U64x2 *>(A.key_s + kb) + c);
                 o.va = ld_keep(reinterpret_cast<const U64x2 *>(A.key + ka) + c);
@@ -1338,8 +1348,11 @@ DPFHE_HD void rot_apply_grouped_rows(CTA &cta, const RotApplyGArgs &A, const Gro
                 if (limb) {
                     const size_t ct = ct0 + ((u32)b < n_ct ? (u32)b : n_ct - 1);
                     const U64x2 s0 = gather(A.ct + ct * 2 * Pq + (size_t)i * N);
-                    r0[b].x = shoup_lazy(s0.x, pm, pm_s, p);   // < SB*q
-                    r0[b].y = shoup_lazy(s0.y, pm, pm_s, p);
+                    // LV: read from the parameter block here rather than held across the loop, as rot_sum_grouped_rows does: the
+                    // generic variant's level instance fits its 80 registers that way
+                    const u64 m = LV ? K.qlm[i] : pm, m_s = LV ? K.qlm_s[i] : pm_s;
+                    r0[b].x = shoup_lazy(s0.x, m, m_s, p);   // < SB*q
+                    r0[b].y = shoup_lazy(s0.y, m, m_s, p);
                 }
             }
             for (u32 d = 0; d < D; d += 2) {

@@ -875,6 +875,16 @@ __global__ void __launch_bounds__(NT, MINB) ks_level_grouped_kernel(KsArgs A, co
                                                      RS ? &R : nullptr);
 }
 
+// the fused Horner step of a linear layer at level l (DESIGN.md §2.21, §4.18): ks_grouped_kernel's rotation with the addend
+// [batch][2][l][N] (ADD), on the level's view, reading the top-level key.  ks_level_grouped_kernel's parameter block plus the addend.
+template <int LOGN, int NT, int MINB>
+__global__ void __launch_bounds__(NT, MINB) ks_level_horner_kernel(KsArgs A, const __grid_constant__ LimbTable lt, const __grid_constant__ MsConsts K,
+                                                                   const __grid_constant__ GroupConsts G, const __grid_constant__ DotArgs D,
+                                                                   const __grid_constant__ RescaleConsts R, size_t batch, u32 *flags, u32 epoch,
+                                                                   u32 *ticket, u64 *mail, const u64 *addend) {
+    ks_grouped_body<LOGN, NT, KS_ROTATE, true, false, true>(A, lt, K, G, batch, flags, epoch, ticket, mail, addend, nullptr, nullptr);
+}
+
 // the encrypted inner product: ks_grouped_kernel's program in mode KS_DOT, with the operand tables of the call in D
 template <int LOGN, int NT, int MINB>
 __global__ void __launch_bounds__(NT, MINB) ct_dot_grouped_kernel(KsArgs A, const __grid_constant__ LimbTable lt, const __grid_constant__ MsConsts K,
@@ -936,6 +946,25 @@ __global__ void __launch_bounds__(NT, MINB) rot_apply_grouped_kernel(RotApplyGAr
         const size_t ct0 = (w / nseg / L) * ROT_CB;
         const u32 n_ct = (u32)(batch - ct0 < (size_t)ROT_CB ? batch - ct0 : (size_t)ROT_CB);
         rot_apply_grouped_rows<LOGN, NT, ROT_CB>(cta, A, G, K, lt.lp[i], ct0, n_ct, i, (int)seg * seg_chunks, ((int)seg + 1) * seg_chunks);
+    }
+}
+
+// the same at level l (DESIGN.md §2.21, §4.18): the key is a top-level key, key_shift = Lq - l rows longer per (digit, component)
+template <int LOGN, int NT, int MINB, int ROT_CB>
+__global__ void __launch_bounds__(NT, MINB) rot_apply_grouped_level_kernel(RotApplyGArgs A, const __grid_constant__ LimbTable lt,
+                                                                           const __grid_constant__ MsConsts K, const __grid_constant__ GroupConsts G,
+                                                                           size_t batch, u32 nseg, u32 key_shift) {
+    DevCta<NT> cta;
+    constexpr int NC = 1 << (LOGN - 1);
+    const u32 L = G.Lq + G.K;
+    const size_t n_blocks = (batch + ROT_CB - 1) / ROT_CB, n_items = n_blocks * L * nseg;
+    const int seg_chunks = NC / (int)nseg;
+    for (size_t w = blockIdx.x; w < n_items; w += gridDim.x) {
+        const u32 seg = (u32)(w % nseg), i = (u32)((w / nseg) % L);
+        const size_t ct0 = (w / nseg / L) * ROT_CB;
+        const u32 n_ct = (u32)(batch - ct0 < (size_t)ROT_CB ? batch - ct0 : (size_t)ROT_CB);
+        rot_apply_grouped_rows<LOGN, NT, ROT_CB, true>(cta, A, G, K, lt.lp[i], ct0, n_ct, i, (int)seg * seg_chunks, ((int)seg + 1) * seg_chunks,
+                                                       key_shift);
     }
 }
 
@@ -1593,7 +1622,10 @@ static cudaError_t launch_ks_grouped_t(LaunchCtx &lc, KsArgs A, MsConsts K, Grou
     static ConfiguredMask configured;
     LimbTable lt = lc.lt;
     Rounds r;
-    if constexpr (LV || RS) {
+    if constexpr (LV && ADD) {
+        void *params[] = {&A, &lt, &K, &G, &D, &R, &r.batch, &r.flags, &r.epoch, &r.ticket, &r.mail, &addend};
+        return launch_persistent(lc, ks_level_horner_kernel<LOGN, NT, MINB>, configured, lc.L, smem, batch, r, params, st);
+    } else if constexpr (LV || RS) {
         void *params[] = {&A, &lt, &K, &G, &D, &R, &r.batch, &r.flags, &r.epoch, &r.ticket, &r.mail};
         if constexpr (LV) return launch_persistent(lc, ks_level_grouped_kernel<LOGN, NT, MINB, MODE, RS>, configured, lc.L, smem, batch, r, params, st);
         else return launch_persistent(lc, ks_rescale_grouped_kernel<LOGN, NT, MINB, MODE>, configured, lc.L, smem, batch, r, params, st);
@@ -1649,7 +1681,9 @@ static cudaError_t ks_grouped(LaunchCtx &lc, int mode, const u64 *const *a, cons
         const KsArgs A = ks_args(lc, dot ? nullptr : a[0], dot || !b ? nullptr : b[0], key, key_s, out, Gc.Lq, galois, level ? key_L : lc.L, false);
         if (level) {
             switch (mode) {
-                case KS_ROTATE: return launch_ks_grouped_t<LOGN, KS_ROTATE, false, false, true>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
+                case KS_ROTATE:
+                    if (addend) return launch_ks_grouped_t<LOGN, KS_ROTATE, true, false, true>(lc, A, K, Gc, D, Rc, addend, batch, st);
+                    return launch_ks_grouped_t<LOGN, KS_ROTATE, false, false, true>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
                 case KS_MUL_RELIN:
                     if (R) return launch_ks_grouped_t<LOGN, KS_MUL_RELIN, false, true, true>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
                     return launch_ks_grouped_t<LOGN, KS_MUL_RELIN, false, false, true>(lc, A, K, Gc, D, Rc, nullptr, batch, st);
@@ -1693,9 +1727,9 @@ cudaError_t launch_ks_rescale_grouped(LaunchCtx &lc, bool dot, const u64 *const 
 
 cudaError_t launch_ks_grouped_level(LaunchCtx &lc, int mode, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, const u64 *key_s,
                                     u32 key_L, u64 *out, size_t batch, u32 galois, const MsConsts &K, const GroupConsts &Gc, const RescaleConsts *R,
-                                    cudaStream_t st) {
+                                    cudaStream_t st, const u64 *addend) {
     if (batch && !key_L) return cudaErrorInvalidValue;
-    return ks_grouped(lc, mode, a, b, n_terms, galois, nullptr, key, key_s, key_L, R, out, batch, K, Gc, st);
+    return ks_grouped(lc, mode, a, b, n_terms, galois, addend, key, key_s, key_L, R, out, batch, K, Gc, st);
 }
 
 #endif
@@ -1777,11 +1811,14 @@ cudaError_t launch_hoist_grouped(LaunchCtx &lc, const u64 *ct, u64 *U, const Gro
 }
 
 // step 2: acc [batch][2][L][N] of one rotation (key companions built here into lc.ks_key_s unless the caller supplies them)
+// key_shift > 0: a level view reading a top-level key (rot_apply_grouped_level_kernel, DESIGN.md §4.18), its companions required
 cudaError_t launch_rot_apply_grouped(LaunchCtx &lc, const u64 *ct, const u64 *U, const u64 *key, const u64 *key_s, u32 galois, u64 *acc,
-                                     const MsConsts &K, const GroupConsts &G, size_t batch, cudaStream_t st) {
+                                     const MsConsts &K, const GroupConsts &G, size_t batch, cudaStream_t st, u32 key_shift) {
     if (batch == 0) return cudaSuccess;
+    if (key_shift && !key_s) return cudaErrorInvalidValue;
+    // two ciphertexts per work item; one at a level, where two spill (the key-row map's registers, DESIGN.md §4.18)
     u32 nseg;
-    const unsigned grid = gather_grid(lc, ((batch + 1) / 2) * lc.L, nseg);   // two ciphertexts per work item
+    const unsigned grid = gather_grid(lc, (key_shift ? batch : (batch + 1) / 2) * lc.L, nseg);
     return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
         constexpr int LOGN = decltype(lg)::value;
         if (!key_s) {
@@ -1791,7 +1828,8 @@ cudaError_t launch_rot_apply_grouped(LaunchCtx &lc, const u64 *ct, const u64 *U,
         }
         RotApplyGArgs A;
         A.ct = ct; A.U = U; A.key = key; A.key_s = key_s; A.acc = acc; A.galois = galois;
-        rot_apply_grouped_kernel<LOGN, 256, 3, 2><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg);
+        if (key_shift) rot_apply_grouped_level_kernel<LOGN, 256, 3, 1><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg, key_shift);
+        else rot_apply_grouped_kernel<LOGN, 256, 3, 2><<<grid, 256, 0, st>>>(A, lc.lt, K, G, batch, nseg);
         return cudaGetLastError();
     });
 }

@@ -69,13 +69,13 @@ struct LaunchCtx {
     cudaError_t launch_hoist_grouped(LaunchCtx &lc, const u64 *ct, u64 *U, const GroupConsts &G, size_t batch, cudaStream_t st); \
     cudaError_t launch_key_prepare(const LaunchCtx &lc, const u64 *key, u64 *key_s, u32 rows, cudaStream_t st); \
     cudaError_t launch_rot_apply_grouped(LaunchCtx &lc, const u64 *ct, const u64 *U, const u64 *key, const u64 *key_s, u32 galois, u64 *acc, \
-                                         const MsConsts &K, const GroupConsts &G, size_t batch, cudaStream_t st); \
+                                         const MsConsts &K, const GroupConsts &G, size_t batch, cudaStream_t st, u32 key_shift = 0); \
     cudaError_t launch_rot_sum_grouped(const LaunchCtx &lc, const u64 *ct, const u64 *U, u32 n_rot, const u64 *const *keys, \
                                        const u64 *const *key_s, const u32 *galois, u64 *acc, const MsConsts &K, const GroupConsts &G, \
                                        size_t batch, cudaStream_t st, u32 key_shift = 0); \
     cudaError_t launch_ks_grouped_level(LaunchCtx &lc, int mode, const u64 *const *a, const u64 *const *b, u32 n_terms, const u64 *key, \
                                         const u64 *key_s, u32 key_L, u64 *out, size_t batch, u32 galois, const MsConsts &K, \
-                                        const GroupConsts &G, const RescaleConsts *R, cudaStream_t st); \
+                                        const GroupConsts &G, const RescaleConsts *R, cudaStream_t st, const u64 *addend = nullptr); \
     cudaError_t launch_pt_inner(const LaunchCtx &lc, const u64 *steps, u32 nb, const u64 *pts, u32 ng, u64 *out, size_t batch, cudaStream_t st, \
                                 unsigned *launches); \
     cudaError_t launch_pointwise_mul(const LaunchCtx &lc, const u64 *a, const u64 *b, u64 *out, size_t n_polys, cudaStream_t st); \
@@ -118,8 +118,10 @@ DPFHE_DECLARE_LAUNCHERS
 // launch_ks_grouped.
 // launch_rot_sum_grouped: keys[m] / key_s[m] / galois[m] of n_rot (1 .. ROT_SUM_MAX) rotations; the companions are required;
 // key_shift > 0: lc is a level view and the keys are top-level keys (DESIGN.md §4.17).
+// launch_rot_apply_grouped: key_shift > 0 as launch_rot_sum_grouped's, the companions then required (DESIGN.md §4.18).
 // launch_ks_hybrid with key_s / launch_ks_grouped_level: the calls at level l on the level's view lc (DESIGN.md §2.20, §4.17), reading
-// the top-level key (key_L limbs per row) and its companions key_s, which the caller builds with the context's own launch state.
+// the top-level key (key_L limbs per row) and its companions key_s, which the caller builds with the context's own launch state;
+// launch_ks_grouped_level's addend (KS_ROTATE only) as launch_ks_grouped's: the fused Horner step of a layer at level l (§4.18).
 // launch_key_prepare: the Shoup companions of the first `rows` rows [rows][2][L][N] of a switch key into key_s (same layout).
 
 }  // namespace dpfhe

@@ -567,6 +567,17 @@ class Context:
         self._chk(self._l.dpfhe_rotate_sum_grouped_level(self._h, int(n_special), int(level), _ptr(ct), n, ge, kp, _ptr(out), batch, int(t_plain),
                                                          _stream(stream)))
 
+    def rotate_hoisted_grouped_level(self, n_special, level, ct, galois_elts, gks, out, batch, t_plain=0, stream=None):
+        """rotate_hoisted_grouped at level `level` (DESIGN.md section 2.21): ct [batch][2][level][N], out [n_rot][batch][2][level][N],
+        gks the top-level keys [dnum][2][L][N]"""
+        n = len(galois_elts)
+        if len(gks) != n:
+            raise ValueError("need one key per Galois element")
+        ge = (C.c_uint64 * max(n, 1))(*[int(g) for g in galois_elts])
+        kp = (C.c_void_p * max(n, 1))(*[_ptr(k) for k in gks])
+        self._chk(self._l.dpfhe_rotate_hoisted_grouped_level(self._h, int(n_special), int(level), _ptr(ct), n, ge, kp, _ptr(out), batch,
+                                                             int(t_plain), _stream(stream)))
+
     def ct_mul_relin_rescale_grouped_level_host(self, n_special, level, a, b, evk, out, t_plain=0):
         """host form of ct_mul_relin_rescale_grouped_level (C-contiguous numpy uint64)"""
         self._chk(self._l.dpfhe_ct_mul_relin_rescale_grouped_level_host(self._h, int(n_special), int(level), _hptr(a), _hptr(b), _hptr(evk),
@@ -722,25 +733,31 @@ class LinearLayer(_ContextObject):
 
     _prefix = "dpfhe_linear"
 
-    def __init__(self, ctx, diags, baby, gk_baby, gk_giant, _n_special=0, _t_plain=0):
+    def __init__(self, ctx, diags, baby, gk_baby, gk_giant, _n_special=0, _t_plain=0, _level=None):
         super().__init__(ctx, _n_special)
         n = diags.shape[0]
         kb = _hptr(gk_baby) if gk_baby is not None else None
         kg = _hptr(gk_giant) if gk_giant is not None else None
-        if self.n_special:
+        if _level is not None:
+            self.Lq = int(_level)
+            rc = self._l.dpfhe_linear_create_grouped_level(ctx._h, self.n_special, self.Lq, _hptr(diags), n, int(baby), kb, kg, int(_t_plain),
+                                                           C.byref(self._h))
+        elif self.n_special:
             rc = self._l.dpfhe_linear_create_grouped(ctx._h, self.n_special, _hptr(diags), n, int(baby), kb, kg, int(_t_plain), C.byref(self._h))
         else:
             rc = self._l.dpfhe_linear_create(ctx._h, _hptr(diags), n, int(baby), kb, kg, C.byref(self._h))
         self._adopt(rc)
 
     @classmethod
-    def grouped(cls, ctx, n_special, diags, baby, gk_baby, gk_giant, t_plain=0):
+    def grouped(cls, ctx, n_special, diags, baby, gk_baby, gk_giant, t_plain=0, level=None):
         """The layer with grouped special-prime Galois keys (dpfhe_linear_create_grouped): ctx's last n_special limbs are special primes,
         Lq = L - n_special.  diags [n][Lq][N] (pre-rotated as for linear_bsgs_grouped), gk_baby [baby-1][dnum][2][L][N], gk_giant
-        [dnum][2][L][N]; apply / apply_host take ciphertexts [batch][2][Lq][N].  Bit-identical to linear_bsgs_grouped."""
+        [dnum][2][L][N]; apply / apply_host take ciphertexts [batch][2][Lq][N].  Bit-identical to linear_bsgs_grouped.
+        level: the layer at that level of the chain (dpfhe_linear_create_grouped_level, DESIGN.md section 2.21) with the same top-level
+        keys, diags [n][level][N] (the first `level` rows of the top-level encoding), ciphertexts [batch][2][level][N]; None: the top."""
         if int(n_special) < 1:
             raise ValueError("n_special must be at least 1")
-        return cls(ctx, diags, baby, gk_baby, gk_giant, _n_special=n_special, _t_plain=t_plain)
+        return cls(ctx, diags, baby, gk_baby, gk_giant, _n_special=n_special, _t_plain=t_plain, _level=level)
 
 
 class PolyEval(_ContextObject):
@@ -798,18 +815,25 @@ class SlotSum(_ContextObject):
 
     _prefix = "dpfhe_slotsum"
 
-    def __init__(self, ctx, n_special, stride, radices, gks, t_plain=0):
+    def __init__(self, ctx, n_special, stride, radices, gks, t_plain=0, level=None):
         super().__init__(ctx, n_special)
         self.stride, self.radices = int(stride), [int(r) for r in radices]
         rs = (C.c_uint * max(len(self.radices), 1))(*self.radices)
-        self._adopt(self._l.dpfhe_slotsum_create_grouped(ctx._h, self.n_special, self.stride, rs, len(self.radices), _hptr(gks), int(t_plain),
-                                                         C.byref(self._h)))
+        if level is None:
+            self._adopt(self._l.dpfhe_slotsum_create_grouped(ctx._h, self.n_special, self.stride, rs, len(self.radices), _hptr(gks), int(t_plain),
+                                                             C.byref(self._h)))
+        else:
+            self.Lq = int(level)
+            self._adopt(self._l.dpfhe_slotsum_create_grouped_level(ctx._h, self.n_special, self.Lq, self.stride, rs, len(self.radices), _hptr(gks),
+                                                                   int(t_plain), C.byref(self._h)))
 
     @classmethod
-    def grouped(cls, ctx, n_special, stride, radices, gks, t_plain=0):
+    def grouped(cls, ctx, n_special, stride, radices, gks, t_plain=0, level=None):
         """ctx's last n_special limbs are special primes; gks [n_steps][dnum][2][L][N] (C-contiguous numpy uint64): the grouped Galois
-        keys of the rotations by slotsum_steps(stride, radices), in that order; t_plain as rotate_hoisted_grouped (0: CKKS)"""
-        return cls(ctx, n_special, stride, radices, gks, t_plain)
+        keys of the rotations by slotsum_steps(stride, radices), in that order; t_plain as rotate_hoisted_grouped (0: CKKS).
+        level: the slot sum at that level of the chain (dpfhe_slotsum_create_grouped_level, DESIGN.md section 2.21) with the same
+        top-level keys, ciphertexts [batch][2][level][N]; None: the top."""
+        return cls(ctx, n_special, stride, radices, gks, t_plain, level)
 
 
 class MultiContext:

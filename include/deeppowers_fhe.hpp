@@ -338,6 +338,16 @@ public:
         check(dpfhe_rotate_sum_grouped_level(ctx_, special, level, ct, steps.size(), elts.data(), galois_keys.data(), out, count, plain_modulus,
                                              stream));
     }
+    // the hoisted rotations at level `level` (DESIGN.md §2.21): ct holds `level` limbs, out n_rot * count such ciphertexts
+    void rotate_hoisted_grouped_device(unsigned special, unsigned level, const std::uint64_t *ct, const std::vector<long> &steps,
+                                       const std::vector<const std::uint64_t *> &galois_keys, std::uint64_t *out, std::size_t count,
+                                       std::uint64_t plain_modulus = 0, void *stream = nullptr) {
+        if (steps.size() != galois_keys.size()) throw std::invalid_argument("one Galois key per rotation");
+        std::vector<std::uint64_t> elts(steps.size());
+        for (std::size_t r = 0; r < steps.size(); ++r) elts[r] = galois_element(steps[r]);
+        check(dpfhe_rotate_hoisted_grouped_level(ctx_, special, level, ct, steps.size(), elts.data(), galois_keys.data(), out, count, plain_modulus,
+                                                 stream));
+    }
     // divide by the product of the last `special` limbs: in holds limbs() limbs per polynomial, out limbs()-special
     void mod_down_special_device(unsigned special, const std::uint64_t *ct, std::uint64_t *out, std::size_t count, std::uint64_t plain_modulus = 0,
                                  void *stream = nullptr) {
@@ -538,6 +548,13 @@ public:
         check(dpfhe_linear_create_grouped(ev.native_handle(), special, diagonals, n_diagonals, baby, baby_keys, giant_key, plain_modulus,
                                                      &h_));
     }
+    // the same layer at level `level` of the chain (DESIGN.md §2.21): ciphertexts and diagonals carry `level` limbs (a diagonal is the
+    // first `level` rows of its top-level encoding), the keys are the top-level ones (dpfhe_linear_create_grouped_level)
+    LinearLayer(Evaluator &ev, unsigned special, unsigned level, const std::uint64_t *diagonals, std::size_t n_diagonals, std::size_t baby,
+                const std::uint64_t *baby_keys, const std::uint64_t *giant_key, std::uint64_t plain_modulus) {
+        check(dpfhe_linear_create_grouped_level(ev.native_handle(), special, level, diagonals, n_diagonals, baby, baby_keys, giant_key,
+                                                plain_modulus, &h_));
+    }
 };
 
 // BGV polynomial evaluation on encrypted slots down the modulus chain (dpfhe_polyeval_*): p(x) = sum_k coeffs[k] x^k mod
@@ -561,6 +578,12 @@ public:
             std::uint64_t plain_modulus = 0) {
         check(dpfhe_slotsum_create_grouped(ev.native_handle(), special, stride, radices.data(), radices.size(), galois_keys, plain_modulus,
                                                       &h_));
+    }
+    // the slot sum at level `level` of the chain (DESIGN.md §2.21): ciphertexts carry `level` limbs, the keys are the top-level ones
+    SlotSum(Evaluator &ev, unsigned special, unsigned level, std::size_t stride, const std::vector<unsigned> &radices,
+            const std::uint64_t *galois_keys, std::uint64_t plain_modulus = 0) {
+        check(dpfhe_slotsum_create_grouped_level(ev.native_handle(), special, level, stride, radices.data(), radices.size(), galois_keys,
+                                                 plain_modulus, &h_));
     }
     // the rotation steps, stage by stage and ascending within a stage: the order of the keys
     static std::vector<long> steps(std::size_t stride, const std::vector<unsigned> &radices) {

@@ -346,6 +346,29 @@ int dpfhe_slotsum_create_grouped(dpfhe_ctx *ctx, unsigned n_special, size_t stri
 int dpfhe_slotsum_apply(dpfhe_slotsum *ss, const uint64_t *d_ct, uint64_t *d_out, size_t batch, void *stream);
 int dpfhe_slotsum_apply_host(dpfhe_slotsum *ss, const uint64_t *h_ct, uint64_t *h_out, size_t batch);
 void dpfhe_slotsum_destroy(dpfhe_slotsum *ss);
+/* ---- the objects of a network layer at level l on the top-level context (DESIGN.md §2.21), in the sense of the level calls above:
+ *      each is, bit for bit, the same call or object on a context over {q_0 .. q_{l-1}, p_0 .. p_{K-1}} with the keys restricted to
+ *      that basis, and level = Lq is the top-level call or object itself.  The keys are the context's TOP-LEVEL grouped keys, read in
+ *      place; their Shoup companions are built once at creation and serve every level.  Valid levels K <= level <= Lq; every other
+ *      check is that of the top-level form; a failed check creates nothing and leaves the output untouched.  A level object builds
+ *      its level's tables on the context at creation (shared with the level calls at the same (K, level)); after
+ *      dpfhe_context_trim its next application builds them again.  An application launches what the top-level object's does.
+ *      dpfhe_rotate_hoisted_grouped_level: n_rot hoisted rotations of level-l ciphertexts [batch][2][level][N] with the top-level
+ *      keys d_gks[r] [dnum][2][L][N]; d_out [n_rot][batch][2][level][N]. */
+int dpfhe_rotate_hoisted_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *d_ct, size_t n_rot,
+                                       const uint64_t *galois_elts, const uint64_t *const *d_gks, uint64_t *d_out, size_t batch,
+                                       uint64_t t_plain, void *stream);
+/*      the grouped linear layer at level l: h_diags [n_diags][level][N]; keys top-level as dpfhe_linear_create_grouped takes them.
+ *      dpfhe_linear_apply / _apply_host / _destroy unchanged, their buffers [batch][2][level][N].  The level is the layer's, fixed at
+ *      creation: a layer sits at a fixed depth of a network, and its diagonals take level / Lq of the top-level memory.  Both
+ *      encoders (dpfhe_bgv_encode, dpfhe_ckks_encode) put the same integer in every limb, so a diagonal at level l is the first
+ *      `level` rows of its top-level encoding: slice it rather than encoding again. */
+int dpfhe_linear_create_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const uint64_t *h_diags, size_t n_diags,
+                                      size_t baby, const uint64_t *h_gk_baby, const uint64_t *h_gk_giant, uint64_t t_plain,
+                                      dpfhe_linear **out);
+/*      the slot sum at level l: h_gks top-level keys in the order of dpfhe_slotsum_steps; apply buffers [batch][2][level][N] */
+int dpfhe_slotsum_create_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, size_t stride, const unsigned *radices,
+                                       size_t n_stages, const uint64_t *h_gks, uint64_t t_plain, dpfhe_slotsum **out);
 /* division by the product of the last n_special limbs alone (the mod-down half of the calls above; n_special = 1 is
  * dpfhe_mod_switch_down): in [n_polys][L][N] -> out [n_polys][L - n_special][N], 1 <= n_special <= 4, n_special < L */
 int dpfhe_mod_down_special(dpfhe_ctx *ctx, unsigned n_special, const uint64_t *d_in, uint64_t *d_out, size_t n_polys,
