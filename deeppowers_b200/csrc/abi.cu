@@ -64,6 +64,9 @@ bool overlaps(const void *a, size_t na, const void *b, size_t nb) {
     return a0 < b0 + nb && b0 < a0 + na;
 }
 
+// an element-wise output: it may BE the input (each thread reads its words, then writes them), but not overlap it at another offset
+bool overlaps_shifted(const void *out, const void *in, size_t bytes) { return out != in && overlaps(out, bytes, in, bytes); }
+
 int enter(const dpfhe_ctx *ctx) {
     if (!ctx) return fail(DPFHE_ERR_INVALID, "null context");
     CU_TRY(cudaSetDevice(ctx->lc.device));
@@ -211,6 +214,13 @@ int check_rotations(const dpfhe_ctx *ctx, size_t n_rot, const uint64_t *galois_e
         if (rc) return rc;
         if (!d_gks[r] || !aligned16(d_gks[r])) return fail(DPFHE_ERR_INVALID, "null or misaligned Galois key");
     }
+    return DPFHE_OK;
+}
+
+// the output of n_rot rotations (out_bytes) against their Galois keys of key_bytes each, which the launches read throughout
+int check_keys_apart(const void *out, size_t out_bytes, size_t n_rot, const uint64_t *const *d_gks, size_t key_bytes) {
+    for (size_t r = 0; r < n_rot; ++r)
+        if (overlaps(out, out_bytes, d_gks[r], key_bytes)) return fail(DPFHE_ERR_INVALID, "output must not overlap a Galois key (rotation %zu)", r);
     return DPFHE_OK;
 }
 
@@ -593,6 +603,9 @@ int dpfhe_poly_mul_pointwise(dpfhe_ctx *ctx, const uint64_t *d_a, const uint64_t
     if (rc) return rc;
     if (n_polys == 0) return DPFHE_OK;
     CHECK_PTR(d_a); CHECK_PTR(d_b); CHECK_PTR(d_out);
+    const size_t bytes = n_polys * ctx->P() * 8;
+    if (overlaps_shifted(d_out, d_a, bytes) || overlaps_shifted(d_out, d_b, bytes))
+        return fail(DPFHE_ERR_INVALID, "output must be an input or not overlap it");
     CU_TRY(VCALL(launch_pointwise_mul, ctx->lc, d_a, d_b, d_out, n_polys, pick(ctx, stream)));
     note_launch(ctx, 1);
     return DPFHE_OK;
@@ -603,6 +616,9 @@ int dpfhe_poly_add(dpfhe_ctx *ctx, const uint64_t *d_a, const uint64_t *d_b, uin
     if (rc) return rc;
     if (n_polys == 0) return DPFHE_OK;
     CHECK_PTR(d_a); CHECK_PTR(d_b); CHECK_PTR(d_out);
+    const size_t bytes = n_polys * ctx->P() * 8;
+    if (overlaps_shifted(d_out, d_a, bytes) || overlaps_shifted(d_out, d_b, bytes))
+        return fail(DPFHE_ERR_INVALID, "output must be an input or not overlap it");
     CU_TRY(VCALL(launch_poly_add, ctx->lc, d_a, d_b, d_out, n_polys, pick(ctx, stream)));
     note_launch(ctx, 1);
     return DPFHE_OK;
@@ -613,6 +629,9 @@ int dpfhe_ct_tensor(dpfhe_ctx *ctx, const uint64_t *d_a, const uint64_t *d_b, ui
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
     CHECK_PTR(d_a); CHECK_PTR(d_b); CHECK_PTR(d_d);
+    const size_t in_bytes = batch * 2 * ctx->P() * 8, out_bytes = batch * 3 * ctx->P() * 8;
+    if (overlaps(d_d, out_bytes, d_a, in_bytes) || overlaps(d_d, out_bytes, d_b, in_bytes))
+        return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
     CU_TRY(VCALL(launch_ct_tensor, ctx->lc, d_a, d_b, d_d, batch, pick(ctx, stream)));
     note_launch(ctx, 1);
     return DPFHE_OK;
@@ -627,10 +646,12 @@ static int ks_common(dpfhe_ctx *ctx, int mode, const uint64_t *a, const uint64_t
     if (mode == KS_MUL_RELIN) CHECK_PTR(b);
     rc = mode == KS_ROTATE ? check_galois(ctx, galois) : DPFHE_OK;
     if (rc) return rc;
-    {   // the output rows are written while other work items still read their inputs: no overlap at all, not only out == in
+    {   // the output rows are written while other work items still read their inputs: no overlap at all, not only out == in;
+        // every work item reads the key [L][2][L][N]
         const size_t ct_bytes = 2 * ctx->P() * 8, in_bytes = batch * (mode == KS_PLAIN ? ct_bytes / 2 : ct_bytes);
         if (overlaps(out, batch * ct_bytes, a, in_bytes) || overlaps(out, batch * ct_bytes, b, in_bytes))
             return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+        if (overlaps(out, batch * ct_bytes, key, ctx->hp.L * ct_bytes)) return fail(DPFHE_ERR_INVALID, "output must not overlap the key");
     }
     CU_TRY(VCALL(launch_ks, ctx->lc, mode, a, b, key, out, batch, (u32)galois, pick(ctx, stream)));
     note_launch(ctx, 2);   // key_prepare_kernel + ks_fused_kernel
@@ -671,6 +692,9 @@ static size_t key_digits(const dpfhe_ctx *ctx, unsigned n_special) {
     return n_special ? (L - n_special + n_special - 1) / n_special : L;
 }
 
+// bytes of one switch key [digits][2][L][N] of the context: what every work item of a key-switching launch reads
+static size_t grouped_key_bytes(const dpfhe_ctx *ctx, unsigned n_special) { return key_digits(ctx, n_special) * 2 * ctx->P() * 8; }
+
 // the special-prime accumulator and tau' rows of the hybrid / grouped key-switch kernels, allocated at the first call that needs them
 static int ensure_hyb(dpfhe_ctx *ctx) {
     if (ctx->lc.ks_hyb) return DPFHE_OK;
@@ -699,6 +723,7 @@ static int ks_hybrid_common(dpfhe_ctx *ctx, unsigned n_special, int mode, const 
         const size_t ct_bytes = 2 * (size_t)(L - n_special) * ctx->N() * 8, in_bytes = batch * (mode == KS_PLAIN ? ct_bytes / 2 : ct_bytes);
         if (overlaps(out, batch * ct_bytes, a, in_bytes) || overlaps(out, batch * ct_bytes, b, in_bytes))
             return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+        if (overlaps(out, batch * ct_bytes, key, grouped_key_bytes(ctx, n_special))) return fail(DPFHE_ERR_INVALID, "output must not overlap the key");
     }
     rc = ensure_hyb(ctx);
     if (rc) return rc;
@@ -746,6 +771,7 @@ static int check_pairs(dpfhe_ctx *ctx, unsigned n_special, size_t n_terms, const
     for (size_t i = 0; i < n_terms; ++i)
         if (overlaps(d_out, out_bytes, d_as[i], in_bytes) || overlaps(d_out, out_bytes, d_bs[i], in_bytes))
             return fail(DPFHE_ERR_INVALID, "output must not overlap an operand (pair %zu)", i);
+    if (overlaps(d_out, out_bytes, d_evk, grouped_key_bytes(ctx, n_special))) return fail(DPFHE_ERR_INVALID, "output must not overlap the key");
     return DPFHE_OK;
 }
 }
@@ -939,6 +965,7 @@ static int level_single(dpfhe_ctx *ctx, unsigned n_special, unsigned level, int 
     const size_t ct_bytes = 2 * (size_t)level * ctx->N() * 8;
     if (overlaps(out, batch * ct_bytes, a, batch * ct_bytes) || overlaps(out, batch * ct_bytes, b, batch * ct_bytes))
         return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+    if (overlaps(out, batch * ct_bytes, key, grouped_key_bytes(ctx, n_special))) return fail(DPFHE_ERR_INVALID, "output must not overlap the key");
     return level_launch(ctx, n_special, level, mode, false, 1, &a, &b, key, out, batch, galois, t_plain, stream);
 }
 
@@ -1033,6 +1060,8 @@ static int rotate_hoisted_impl(dpfhe_ctx *ctx, const uint64_t *d_ct, size_t n_ro
     rc = check_rotations(ctx, n_rot, galois_elts, d_gks);
     if (rc) return rc;
     if (overlaps(d_out, n_rot * batch * 2 * P * 8, d_ct, batch * 2 * P * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    rc = check_keys_apart(d_out, n_rot * batch * 2 * P * 8, n_rot, d_gks, L * 2 * P * 8);
+    if (rc) return rc;
     cudaStream_t st = pick(ctx, stream);
     // scratch: the shared transforms and zero flags of a chunk of the batch
     const size_t per_ct = L * L * N * sizeof(u64), chunk = hoist_chunk(per_ct, batch);
@@ -1094,6 +1123,8 @@ static int rotate_hoisted_grouped_impl(dpfhe_ctx *ctx, unsigned n_special, const
     rc = check_rotations(ctx, n_rot, galois_elts, d_gks);
     if (rc) return rc;
     if (overlaps(d_out, n_rot * batch * 2 * Pq * 8, d_ct, batch * 2 * Pq * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    rc = check_keys_apart(d_out, n_rot * batch * 2 * Pq * 8, n_rot, d_gks, grouped_key_bytes(ctx, n_special));
+    if (rc) return rc;
     cudaStream_t st = pick(ctx, stream);
     // scratch per ciphertext of a chunk: lifted digits [dnum][L][N], accumulators [2][L][N], tau' rows [2][K][N]
     const size_t u_words = dnum * L * N, acc_words = 2 * L * N, tau_words = 2 * (size_t)n_special * N;
@@ -1150,6 +1181,8 @@ int dpfhe_rotate_hoisted_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsig
     if (rc) return rc;
     const size_t ct_bytes = batch * 2 * (size_t)level * ctx->N() * 8;
     if (overlaps(d_out, n_rot * ct_bytes, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "level %u: output must not overlap the input", level);
+    rc = check_keys_apart(d_out, n_rot * ct_bytes, n_rot, d_gks, grouped_key_bytes(ctx, n_special));
+    if (rc) return rc;
     const KsLevel *lv = nullptr;
     if (level < ctx->hp.L - n_special) rc = level_state(ctx, n_special, level, lv);
     if (rc) return rc;
@@ -1250,6 +1283,8 @@ int dpfhe_rotate_sum_grouped(dpfhe_ctx *ctx, unsigned n_special, const uint64_t 
     if (rc) return rc;
     const size_t ct_bytes = batch * 2 * (ctx->hp.L - n_special) * ctx->N() * 8;
     if (overlaps(d_out, ct_bytes, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    rc = check_keys_apart(d_out, ct_bytes, n_rot, d_gks, grouped_key_bytes(ctx, n_special));
+    if (rc) return rc;
     cudaStream_t st = pick(ctx, stream);
     RotSumPrep pr;
     rc = rotate_sum_prepare(ctx, n_special, n_rot, galois_elts, d_gks, t_plain, batch, st, pr);
@@ -1273,6 +1308,8 @@ int dpfhe_rotate_sum_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned 
     if (level == ctx->hp.L - n_special) return dpfhe_rotate_sum_grouped(ctx, n_special, d_ct, n_rot, galois_elts, d_gks, d_out, batch, t_plain, stream);
     const size_t ct_bytes = batch * 2 * (size_t)level * ctx->N() * 8;
     if (overlaps(d_out, ct_bytes, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    rc = check_keys_apart(d_out, ct_bytes, n_rot, d_gks, grouped_key_bytes(ctx, n_special));
+    if (rc) return rc;
     const KsLevel *lv = nullptr;
     rc = level_state(ctx, n_special, level, lv);
     if (rc) return rc;
@@ -1310,6 +1347,9 @@ int dpfhe_ct_mul_plain(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_p
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
     CHECK_PTR(d_ct); CHECK_PTR(d_pt); CHECK_PTR(d_out);
+    const size_t ct_bytes = batch * 2 * ctx->P() * 8;
+    if (overlaps_shifted(d_out, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "output must be the input or not overlap it");
+    if (overlaps(d_out, ct_bytes, d_pt, ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the plaintext");
     CU_TRY(VCALL(launch_ct_mul_plain, ctx->lc, d_ct, d_pt, d_out, batch, pick(ctx, stream)));
     note_launch(ctx, 1);
     return DPFHE_OK;
@@ -1320,6 +1360,9 @@ int dpfhe_ct_mul_plain_acc(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t 
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
     CHECK_PTR(d_ct); CHECK_PTR(d_pt); CHECK_PTR(d_acc);
+    const size_t ct_bytes = batch * 2 * ctx->P() * 8;
+    if (overlaps(d_acc, ct_bytes, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "accumulator must not overlap the input");
+    if (overlaps(d_acc, ct_bytes, d_pt, ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "accumulator must not overlap the plaintext");
     CU_TRY(VCALL(launch_ct_mul_plain_acc, ctx->lc, d_ct, d_pt, d_acc, batch, pick(ctx, stream)));
     note_launch(ctx, 1);
     return DPFHE_OK;
@@ -1335,6 +1378,8 @@ int dpfhe_ct_mul_plain_inner(dpfhe_ctx *ctx, const uint64_t *d_steps, size_t n_s
     if (n_groups > 65535) return fail(DPFHE_ERR_INVALID, "n_groups must be below 65536");
     if (overlaps(d_out, n_groups * batch * 2 * ctx->P() * 8, d_steps, n_steps * batch * 2 * ctx->P() * 8))
         return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+    if (overlaps(d_out, n_groups * batch * 2 * ctx->P() * 8, d_pts, n_groups * n_steps * ctx->P() * 8))
+        return fail(DPFHE_ERR_INVALID, "output must not overlap the plaintexts");
     unsigned launches = 0;
     CU_TRY(VCALL(launch_pt_inner, ctx->lc, d_steps, (u32)n_steps, d_pts, (u32)n_groups, d_out, batch, pick(ctx, stream), &launches));
     note_launch(ctx, launches);
@@ -1629,6 +1674,7 @@ int dpfhe_ckks_encode(dpfhe_ctx *ctx, const double *d_slots, uint64_t *d_pt, siz
     if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
     if (n_vec == 0) return DPFHE_OK;
     CHECK_PTR(d_slots); CHECK_PTR(d_pt);
+    if (overlaps(d_pt, n_vec * ctx->P() * 8, d_slots, n_vec * ctx->N() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
     cudaStream_t st = pick(ctx, stream);
     rc = ckks_prepare(ctx, n_vec * ctx->N() * sizeof(double));
     if (rc) return rc;
@@ -1644,6 +1690,7 @@ int dpfhe_ckks_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, double *d_slots, siz
     if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
     if (n_vec == 0) return DPFHE_OK;
     CHECK_PTR(d_pt); CHECK_PTR(d_slots);
+    if (overlaps(d_slots, n_vec * ctx->N() * 8, d_pt, n_vec * ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
     cudaStream_t st = pick(ctx, stream);
     const size_t bytes = n_vec * ctx->P() * 8;
     rc = ckks_prepare(ctx, bytes);
@@ -1723,6 +1770,7 @@ int dpfhe_bgv_encode(dpfhe_ctx *ctx, const int64_t *d_slots, uint64_t *d_pt, siz
     CHECK_T(t_plain);
     if (n_vec == 0) return DPFHE_OK;
     CHECK_PTR(d_slots); CHECK_PTR(d_pt);
+    if (overlaps(d_pt, n_vec * ctx->P() * 8, d_slots, n_vec * ctx->N() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
     cudaStream_t st = pick(ctx, stream);
     rc = bgv_prepare(ctx, t_plain, n_vec * ctx->N() * sizeof(u32));
     if (rc) return rc;
@@ -1737,6 +1785,7 @@ int dpfhe_bgv_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, uint64_t *d_slots, si
     CHECK_T(t_plain);
     if (n_vec == 0) return DPFHE_OK;
     CHECK_PTR(d_pt); CHECK_PTR(d_slots);
+    if (overlaps(d_slots, n_vec * ctx->N() * 8, d_pt, n_vec * ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
     cudaStream_t st = pick(ctx, stream);
     const size_t bytes = n_vec * ctx->P() * 8;
     rc = bgv_prepare(ctx, t_plain, bytes);
@@ -1916,6 +1965,8 @@ int dpfhe_decrypt(dpfhe_ctx *ctx, const uint64_t *d_sk, const uint64_t *d_ct, un
     if (n_comp != 2 && n_comp != 3) return fail(DPFHE_ERR_INVALID, "n_comp must be 2 or 3");
     if (n == 0) return DPFHE_OK;
     CHECK_PTR(d_sk); CHECK_PTR(d_ct); CHECK_PTR(d_pt);
+    if (overlaps(d_pt, n * ctx->P() * 8, d_sk, ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the secret");
+    if (overlaps(d_pt, n * ctx->P() * 8, d_ct, n * n_comp * ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
     CU_TRY(VCALL(launch_decrypt, ctx->lc, d_ct, d_sk, d_pt, n_comp, n, pick(ctx, stream)));
     note_launch(ctx, 1);
     return DPFHE_OK;
@@ -2432,6 +2483,7 @@ int dpfhe_ct_add_plain(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_p
     CHECK_PTR(d_ct); CHECK_PTR(d_pt); CHECK_PTR(d_out);
     if (batch == 0) return DPFHE_OK;
     if (overlaps(d_out, batch * 2 * ctx->P() * 8, d_pt, ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the plaintext");
+    if (overlaps_shifted(d_out, d_ct, batch * 2 * ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must be the input or not overlap it");
     const int64_t one = 1;
     CU_TRY(VCALL(launch_lincomb, ctx->lc, &d_ct, &one, 1u, (int64_t)0, d_pt, d_out, batch, pick(ctx, stream)));
     note_launch(ctx, 1);

@@ -96,27 +96,30 @@ int dpfhe_ntt_fwd(dpfhe_ctx *ctx, uint64_t *d_data, size_t n_polys, void *stream
 int dpfhe_ntt_inv(dpfhe_ctx *ctx, uint64_t *d_data, size_t n_polys, void *stream);
 
 /* ---- pointwise ---- */
-/* out[p][l][n] = a*b mod q_l, [n_polys][L][N]; out may alias a or b */
+/* out[p][l][n] = a*b mod q_l, [n_polys][L][N]; out may BE a or b (or both), any other overlap is rejected */
 int dpfhe_poly_mul_pointwise(dpfhe_ctx *ctx, const uint64_t *d_a, const uint64_t *d_b, uint64_t *d_out,
                              size_t n_polys, void *stream);
-/* out = a + b mod q_l, [n_polys][L][N] (a ciphertext is two polynomials); out may alias a or b */
+/* out = a + b mod q_l, [n_polys][L][N] (a ciphertext is two polynomials); out may BE a or b (or both), any other overlap is rejected */
 int dpfhe_poly_add(dpfhe_ctx *ctx, const uint64_t *d_a, const uint64_t *d_b, uint64_t *d_out,
                    size_t n_polys, void *stream);
-/* a,b: [batch][2][L][N] -> d: [batch][3][L][N] (d0,d1,d2) */
+/* a,b: [batch][2][L][N] -> d: [batch][3][L][N] (d0,d1,d2); d must not overlap a or b */
 int dpfhe_ct_tensor(dpfhe_ctx *ctx, const uint64_t *d_a, const uint64_t *d_b, uint64_t *d_d,
                     size_t batch, void *stream);
 
-/* ---- key switching ---- */
+/* ---- key switching: every work item reads the key for the whole launch, so the output must overlap neither the operands nor
+ *      the key (DPFHE_ERR_INVALID); this holds for every key-switching call below, Galois keys of hoisted and summed rotations
+ *      included ---- */
 /* d: [batch][L][N] (evaluation form) -> out: [batch][2][L][N] = sum_j NTT(INTT(d[j])) o key[j] */
 int dpfhe_keyswitch(dpfhe_ctx *ctx, const uint64_t *d_d, const uint64_t *d_key, uint64_t *d_out,
                     size_t batch, void *stream);
 /* out = relinearise(a (x) b); a,b,out: [batch][2][L][N]; out must not alias a or b */
 int dpfhe_ct_mul_relin(dpfhe_ctx *ctx, const uint64_t *d_a, const uint64_t *d_b, const uint64_t *d_evk,
                        uint64_t *d_out, size_t batch, void *stream);
-/* out = (c0 o pt, c1 o pt); pt [L][N] shared by the batch; out may alias ct */
+/* out = (c0 o pt, c1 o pt); pt [L][N] shared by the batch; out may BE ct, must not otherwise overlap it and must not overlap pt */
 int dpfhe_ct_mul_plain(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out,
                        size_t batch, void *stream);
-/* acc += (c0 o pt, c1 o pt): fused multiply-accumulate for diagonal-method linear layers; acc [batch][2][L][N] */
+/* acc += (c0 o pt, c1 o pt): fused multiply-accumulate for diagonal-method linear layers; acc [batch][2][L][N], overlapping neither
+ * ct nor pt */
 int dpfhe_ct_mul_plain_acc(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_acc,
                            size_t batch, void *stream);
 /* out = (sigma_g(c0) + ks0, ks1), ks = keyswitch(sigma_g(c1), gk); galois_elt odd in [1,2N);
@@ -142,7 +145,8 @@ int dpfhe_rotate_hoisted(dpfhe_ctx *ctx, const uint64_t *d_ct, size_t n_rot, con
  *      out[g][k] = sum_{b < n_steps} steps[b][k] o pts[g][b]   for g < n_groups, k < batch
  *      steps [n_steps][batch][2][L][N] ciphertext batches, pts [n_groups][n_steps][L][N] plaintexts (evaluation form,
  *      shared by the batch), out [n_groups][batch][2][L][N].  Bit-identical to dpfhe_ct_mul_plain followed by
- *      n_steps-1 dpfhe_ct_mul_plain_acc per group, but every ciphertext row is read once. n_steps <= 128. ---- */
+ *      n_steps-1 dpfhe_ct_mul_plain_acc per group, but every ciphertext row is read once. n_steps <= 128.  out must overlap neither
+ *      steps nor pts. ---- */
 int dpfhe_ct_mul_plain_inner(dpfhe_ctx *ctx, const uint64_t *d_steps, size_t n_steps, const uint64_t *d_pts, size_t n_groups,
                              uint64_t *d_out, size_t batch, void *stream);
 
@@ -172,7 +176,8 @@ int dpfhe_linear_apply_host(dpfhe_linear *layer, const uint64_t *h_ct, uint64_t 
 /* ---- scalar linear combinations (DESIGN.md §2.15): d_out = sum_i (coeffs[i] mod q_l) d_cts[i], plus (constant mod q_l) at every
  *      position of every c0 row; coefficients reduced by floor-mod, results canonical.  d_cts: a HOST array of n_terms (1 .. 64)
  *      device pointers, each [batch][2][L][N] over all L limbs of the context; d_out may be any of them.  One launch.
- *      dpfhe_ct_add_plain: d_out = (c0 + d_pt, c1), d_pt [L][N] shared by the batch (it must not overlap d_out). ---- */
+ *      dpfhe_ct_add_plain: d_out = (c0 + d_pt, c1), d_pt [L][N] shared by the batch (it must not overlap d_out); d_out may BE d_ct,
+ *      any other overlap is rejected. ---- */
 int dpfhe_ct_lincomb(dpfhe_ctx *ctx, size_t n_terms, const uint64_t *const *d_cts, const int64_t *coeffs, int64_t constant, uint64_t *d_out,
                      size_t batch, void *stream);
 int dpfhe_ct_add_plain(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch, void *stream);
@@ -388,7 +393,7 @@ int dpfhe_rotate_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint64_t
  *      The results are bit-exact: the floating-point operation order is fixed by the specification.  `scale` must be finite and
  *      positive; non-finite slots, or coefficients beyond the double range, give unspecified (but memory-safe) results.
  *      A plaintext for ciphertexts under a context with special primes is encoded with the context over the ciphertext moduli.
- *      The *_host forms take host buffers and pipeline them in chunks (synchronous). ---- */
+ *      The *_host forms take host buffers and pipeline them in chunks (synchronous).  Outputs must not overlap inputs. ---- */
 int dpfhe_ckks_encode(dpfhe_ctx *ctx, const double *d_slots, uint64_t *d_pt, size_t n_vec, double scale, void *stream);
 int dpfhe_ckks_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, double *d_slots, size_t n_vec, double scale, void *stream);
 int dpfhe_ckks_encode_host(dpfhe_ctx *ctx, const double *h_slots, uint64_t *h_pt, size_t n_vec, double scale);
@@ -403,7 +408,8 @@ int dpfhe_ckks_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, double *h_slots
  *      decode: inverse transform (into scratch: d_pt is not modified), the centred CRT value mod t, its slots in [0, t).
  *      The results are exact.  The context keeps the tables of the last t_plain used; a call with another t replaces them after
  *      the earlier calls have finished.  A plaintext for ciphertexts under a context with special primes is encoded with the
- *      context over the ciphertext moduli.  The *_host forms take host buffers and pipeline them in chunks (synchronous). ---- */
+ *      context over the ciphertext moduli.  The *_host forms take host buffers and pipeline them in chunks (synchronous).  Outputs
+ *      must not overlap inputs. ---- */
 int dpfhe_bgv_encode(dpfhe_ctx *ctx, const int64_t *d_slots, uint64_t *d_pt, size_t n_vec, uint64_t t_plain, void *stream);
 int dpfhe_bgv_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, uint64_t *d_slots, size_t n_vec, uint64_t t_plain, void *stream);
 int dpfhe_bgv_encode_host(dpfhe_ctx *ctx, const int64_t *h_slots, uint64_t *h_pt, size_t n_vec, uint64_t t_plain);
@@ -432,7 +438,8 @@ int dpfhe_bgv_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, uint64_t *h_slot
  *        Use a public key with the t_plain it was made with.
  *      The *_host forms take host buffers (encrypt / decrypt pipelined in chunks; synchronous).
  *      dpfhe_random_seed fills 32 bytes from the operating system (getrandom; DPFHE_ERR_OS if that fails).
- *      Outputs must not overlap the secret, the public key, the plaintexts or each other's inputs. ---- */
+ *      Outputs must not overlap the secret, the public key, the plaintexts or each other's inputs (decrypt: d_pt neither d_sk nor
+ *      d_ct); an overlap is rejected with DPFHE_ERR_INVALID. ---- */
 int dpfhe_random_seed(uint8_t seed[32]);
 int dpfhe_secret_keygen(dpfhe_ctx *ctx, const uint8_t seed[32], uint64_t *d_sk, void *stream);
 int dpfhe_relin_keygen(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32],
