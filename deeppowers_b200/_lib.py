@@ -168,6 +168,32 @@ SYMBOLS = {
 }
 
 
+# the entry points of include/dpfhe_level.h (DESIGN.md section 2.22), which dpfhe.h includes
+LEVEL_SYMBOLS = {
+    "dpfhe_ckks_encode_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_size_t, C.c_double, C.c_void_p]),
+    "dpfhe_ckks_decode_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_size_t, C.c_double, C.c_void_p]),
+    "dpfhe_ckks_encode_level_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_size_t, C.c_double]),
+    "dpfhe_ckks_decode_level_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_size_t, C.c_double]),
+    "dpfhe_bgv_encode_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p]),
+    "dpfhe_bgv_decode_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p]),
+    "dpfhe_bgv_encode_level_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64]),
+    "dpfhe_bgv_decode_level_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64]),
+    "dpfhe_encrypt_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_encrypt_level_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "dpfhe_encrypt_public_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_encrypt_public_level_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "dpfhe_decrypt_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_uint, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_decrypt_level_host": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_uint, C.c_void_p, C.c_size_t]),
+    "dpfhe_ct_add_plain_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_ct_mul_plain_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_ct_lincomb_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_size_t, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dpfhe_mod_switch_down_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p]),
+    "dpfhe_polyeval_create_grouped_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_uint64, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                      C.POINTER(C.c_void_p)]),
+    "dpfhe_polyeval_create_ckks_level": (C.c_int, [C.c_void_p, C.c_uint, C.c_uint, C.c_void_p, C.c_size_t, C.c_double, C.c_double, C.c_void_p,
+                                                   C.POINTER(C.c_void_p)]),
+}
+
 class dpfhe_params(C.Structure):
     _fields_ = [("log_n", C.c_uint32), ("n_limbs", C.c_uint32), ("moduli", C.POINTER(C.c_uint64))]
 
@@ -184,8 +210,8 @@ def load():
     if not os.path.exists(path):
         _build.build()          # raises if nvcc is unavailable: no fallback
     lib = C.CDLL(path)
-    for name, (res, args) in SYMBOLS.items():
-        fn = getattr(lib, name)   # AttributeError if the library does not export what include/dpfhe.h declares
+    for name, (res, args) in list(SYMBOLS.items()) + list(LEVEL_SYMBOLS.items()):
+        fn = getattr(lib, name)   # AttributeError if the library does not export what include/dpfhe.h (with dpfhe_level.h) declares
         fn.restype = res
         fn.argtypes = args
     _lib = lib

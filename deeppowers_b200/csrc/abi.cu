@@ -271,6 +271,49 @@ LaunchCtx level_view(const dpfhe_ctx *ctx, unsigned l) {
     return lc;
 }
 
+// The host parameters of the prefix basis {q_0 .. q_{l-1}}: the context's own at l = L, else built once at the first call and kept on
+// the context.  Only the limb parameters are copied; the twiddles are the context's rows, read through level_view.  nullptr: out of
+// host memory.
+const HostParams *prefix_params(dpfhe_ctx *ctx, unsigned l) {
+    if (l == ctx->hp.L) return &ctx->hp;
+    if (ctx->prefix.size() < ctx->hp.L) ctx->prefix.resize(ctx->hp.L);
+    auto &p = ctx->prefix[l];
+    if (!p) {
+        p.reset(new (std::nothrow) HostParams());
+        if (!p) return nullptr;
+        p->log_n = ctx->hp.log_n;
+        p->L = l;
+        p->limbs.resize(l);
+        for (unsigned i = 0; i < l; ++i) {
+            p->limbs[i].lp = ctx->hp.limbs[i].lp;
+            p->limbs[i].psi = ctx->hp.limbs[i].psi;
+        }
+    }
+    return p.get();
+}
+
+// the level of a keyless level call (DESIGN.md §2.22): 1 <= level <= L
+int check_prefix_level(const dpfhe_ctx *ctx, unsigned level) {
+    if (level < 1 || level > ctx->hp.L) return fail(DPFHE_ERR_INVALID, "level %u is outside [1, %u], the context's limbs", level, ctx->hp.L);
+    return DPFHE_OK;
+}
+
+// rc, the result of a call at `level`; a failure's message is made to name the level
+int level_failure(unsigned level, int rc) {
+    if (rc != DPFHE_OK && g_err.compare(0, 6, "level ") != 0) g_err = "level " + std::to_string(level) + ": " + g_err;
+    return rc;
+}
+
+// A keyless level call: the context and the level checked, then call(), the body on the prefix of `level` limbs, whose failures
+// name the level
+template <class Call>
+int prefix_call(dpfhe_ctx *ctx, unsigned level, Call call) {
+    int rc = enter(ctx);
+    if (!rc) rc = check_prefix_level(ctx, level);
+    if (rc) return rc;
+    return level_failure(level, call());
+}
+
 // n grouped keys [n][dnum][2][L][N] on the device, back to back, and their Shoup companions in a second allocation of the same
 // layout; keys[k] / key_s[k] point at key k.  Copyable: whoever holds it calls release().
 struct PreparedKeys {
@@ -1342,17 +1385,21 @@ int dpfhe_rotate_sum_grouped_host(dpfhe_ctx *ctx, unsigned n_special, const uint
     });
 }
 
-int dpfhe_ct_mul_plain(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch, void *stream) {
+// on the prefix of L limbs (DESIGN.md §2.22); L = hp.L is dpfhe_ct_mul_plain
+static int ct_mul_plain_at(dpfhe_ctx *ctx, unsigned L, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (batch == 0) return DPFHE_OK;
     CHECK_PTR(d_ct); CHECK_PTR(d_pt); CHECK_PTR(d_out);
-    const size_t ct_bytes = batch * 2 * ctx->P() * 8;
+    const size_t P = L * ctx->N(), ct_bytes = batch * 2 * P * 8;
     if (overlaps_shifted(d_out, d_ct, ct_bytes)) return fail(DPFHE_ERR_INVALID, "output must be the input or not overlap it");
-    if (overlaps(d_out, ct_bytes, d_pt, ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the plaintext");
-    CU_TRY(VCALL(launch_ct_mul_plain, ctx->lc, d_ct, d_pt, d_out, batch, pick(ctx, stream)));
+    if (overlaps(d_out, ct_bytes, d_pt, P * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the plaintext");
+    CU_TRY(VCALL(launch_ct_mul_plain, level_view(ctx, L), d_ct, d_pt, d_out, batch, pick(ctx, stream)));
     note_launch(ctx, 1);
     return DPFHE_OK;
+}
+int dpfhe_ct_mul_plain(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch, void *stream) {
+    return ct_mul_plain_at(ctx, ctx ? ctx->hp.L : 0, d_ct, d_pt, d_out, batch, stream);
 }
 
 int dpfhe_ct_mul_plain_acc(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_acc, size_t batch, void *stream) {
@@ -1386,24 +1433,32 @@ int dpfhe_ct_mul_plain_inner(dpfhe_ctx *ctx, const uint64_t *d_steps, size_t n_s
     return DPFHE_OK;
 }
 
-int dpfhe_mod_switch_down(dpfhe_ctx *ctx, const uint64_t *d_in, uint64_t *d_out, size_t n_polys, uint64_t t_plain, void *stream) {
+// The modulus switch of [n_polys][L][N] on the prefix of L = level limbs (DESIGN.md §2.22): its view and host parameters; L = hp.L is
+// dpfhe_mod_switch_down
+static int mod_switch_down_at(dpfhe_ctx *ctx, unsigned L, const uint64_t *d_in, uint64_t *d_out, size_t n_polys, uint64_t t_plain, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (n_polys == 0) return DPFHE_OK;
     CHECK_PTR(d_in); CHECK_PTR(d_out);
-    const unsigned L = ctx->hp.L;
     if (L < 2) return fail(DPFHE_ERR_INVALID, "mod_switch_down needs at least two limbs");
-    if (overlaps(d_out, n_polys * (size_t)(L - 1) * ctx->N() * 8, d_in, n_polys * ctx->P() * 8))
+    const size_t N = ctx->N();
+    if (overlaps(d_out, n_polys * (size_t)(L - 1) * N * 8, d_in, n_polys * L * N * 8))
         return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
     const uint64_t ql = ctx->hp.limbs[L - 1].lp.q;
     if (t_plain >= ql || (t_plain && t_plain % ql == 0)) return fail(DPFHE_ERR_INVALID, "plaintext modulus must be below the dropped modulus");
-    rc = ctx->ms_tau.reserve(ctx, n_polys * ctx->N() * 8);
+    const HostParams *hp = prefix_params(ctx, L);
+    if (!hp) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    rc = ctx->ms_tau.reserve(ctx, n_polys * N * 8);
     if (rc) return rc;
     MsConsts K;
-    build_ms_consts(ctx->hp, t_plain, K);
-    CU_TRY(VCALL(launch_mod_switch, ctx->lc, d_in, ctx->ms_tau.get(), d_out, K, n_polys, pick(ctx, stream)));
+    build_ms_consts(*hp, t_plain, K);
+    CU_TRY(VCALL(launch_mod_switch, level_view(ctx, L), d_in, ctx->ms_tau.get(), d_out, K, n_polys, pick(ctx, stream)));
     note_launch(ctx, 2);
     return DPFHE_OK;
+}
+
+int dpfhe_mod_switch_down(dpfhe_ctx *ctx, const uint64_t *d_in, uint64_t *d_out, size_t n_polys, uint64_t t_plain, void *stream) {
+    return mod_switch_down_at(ctx, ctx ? ctx->hp.L : 0, d_in, d_out, n_polys, t_plain, stream);
 }
 
 // division by the product of the last n_special limbs (DESIGN.md §2.11); n_special = 1 is dpfhe_mod_switch_down
@@ -1668,65 +1723,82 @@ static int ckks_prepare(dpfhe_ctx *ctx, size_t need) {
 
 static bool valid_scale(double scale) { return scale > 0.0 && scale <= 1.7976931348623157e308; }   // finite and positive (NaN fails both)
 
-int dpfhe_ckks_encode(dpfhe_ctx *ctx, const double *d_slots, uint64_t *d_pt, size_t n_vec, double scale, void *stream) {
+// The bodies below take L, the limbs of the prefix basis they run on (DESIGN.md §2.22): its view of the context, its host parameters,
+// buffers and checks sized by it.  L = hp.L is the top-level call.
+static int ckks_encode_at(dpfhe_ctx *ctx, unsigned L, const double *d_slots, uint64_t *d_pt, size_t n_vec, double scale, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
     if (n_vec == 0) return DPFHE_OK;
     CHECK_PTR(d_slots); CHECK_PTR(d_pt);
-    if (overlaps(d_pt, n_vec * ctx->P() * 8, d_slots, n_vec * ctx->N() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    if (overlaps(d_pt, n_vec * L * ctx->N() * 8, d_slots, n_vec * ctx->N() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
     cudaStream_t st = pick(ctx, stream);
     rc = ckks_prepare(ctx, n_vec * ctx->N() * sizeof(double));
     if (rc) return rc;
     const double sc = scale * (2.0 / (double)ctx->N());
-    CU_TRY(VCALL(launch_ckks_encode, ctx->lc, (const Cplx *)d_slots, ctx->enc_work.get<double>(), d_pt, ctx->ckks, sc, n_vec, st));
+    CU_TRY(VCALL(launch_ckks_encode, level_view(ctx, L), (const Cplx *)d_slots, ctx->enc_work.get<double>(), d_pt, ctx->ckks, sc, n_vec, st));
     note_launch(ctx, 2);   // ckks_enc_fft_kernel + ckks_enc_ntt(_pair)_kernel
     return DPFHE_OK;
 }
+int dpfhe_ckks_encode(dpfhe_ctx *ctx, const double *d_slots, uint64_t *d_pt, size_t n_vec, double scale, void *stream) {
+    return ckks_encode_at(ctx, ctx ? ctx->hp.L : 0, d_slots, d_pt, n_vec, scale, stream);
+}
 
-int dpfhe_ckks_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, double *d_slots, size_t n_vec, double scale, void *stream) {
+static int ckks_decode_at(dpfhe_ctx *ctx, unsigned L, const uint64_t *d_pt, double *d_slots, size_t n_vec, double scale, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
     if (n_vec == 0) return DPFHE_OK;
     CHECK_PTR(d_pt); CHECK_PTR(d_slots);
-    if (overlaps(d_slots, n_vec * ctx->N() * 8, d_pt, n_vec * ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    const size_t bytes = n_vec * L * ctx->N() * 8;
+    if (overlaps(d_slots, n_vec * ctx->N() * 8, d_pt, bytes)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    const HostParams *hp = prefix_params(ctx, L);
+    if (!hp) return fail(DPFHE_ERR_NOMEM, "out of host memory");
     cudaStream_t st = pick(ctx, stream);
-    const size_t bytes = n_vec * ctx->P() * 8;
     rc = ckks_prepare(ctx, bytes);
     if (rc) return rc;
+    const LaunchCtx lc = level_view(ctx, L);
     u64 *work = ctx->enc_work.get();
     CU_TRY(cudaMemcpyAsync(work, d_pt, bytes, cudaMemcpyDeviceToDevice, st));   // the caller's plaintexts stay unchanged
-    CU_TRY(VCALL(launch_ntt, ctx->lc, work, n_vec, true, st));
+    CU_TRY(VCALL(launch_ntt, lc, work, n_vec, true, st));
     CkksConsts K;
-    build_ckks_consts(ctx->hp, scale, K);
-    CU_TRY(VCALL(launch_ckks_decode, ctx->lc, work, (Cplx *)d_slots, ctx->ckks, K, n_vec, st));
+    build_ckks_consts(*hp, scale, K);
+    CU_TRY(VCALL(launch_ckks_decode, lc, work, (Cplx *)d_slots, ctx->ckks, K, n_vec, st));
     note_launch(ctx, 2);   // inverse transform + ckks_dec_kernel
     return DPFHE_OK;
 }
-
-int dpfhe_ckks_encode_host(dpfhe_ctx *ctx, const double *h_slots, uint64_t *h_pt, size_t n_vec, double scale) {
-    int rc = enter(ctx);
-    if (rc) return rc;
-    if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
-    if (n_vec == 0) return DPFHE_OK;
-    const size_t P = ctx->P(), S = ctx->N();   // words of a plaintext, and of a slot vector (N/2 complex doubles)
-    return host_call(ctx, {h_slots, h_pt}, nullptr, 0, (const u64 *)h_slots, nullptr, h_pt, n_vec, S, P,
-                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
-                         return dpfhe_ckks_encode(ctx, (const double *)din, dout, cnt, scale, st);
-                     });
+int dpfhe_ckks_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, double *d_slots, size_t n_vec, double scale, void *stream) {
+    return ckks_decode_at(ctx, ctx ? ctx->hp.L : 0, d_pt, d_slots, n_vec, scale, stream);
 }
 
-int dpfhe_ckks_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, double *h_slots, size_t n_vec, double scale) {
+static int ckks_encode_host_at(dpfhe_ctx *ctx, unsigned L, const double *h_slots, uint64_t *h_pt, size_t n_vec, double scale) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
     if (n_vec == 0) return DPFHE_OK;
-    const size_t P = ctx->P(), S = ctx->N();
+    const size_t P = L * ctx->N(), S = ctx->N();   // words of a plaintext, and of a slot vector (N/2 complex doubles)
+    return host_call(ctx, {h_slots, h_pt}, nullptr, 0, (const u64 *)h_slots, nullptr, h_pt, n_vec, S, P,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return ckks_encode_at(ctx, L, (const double *)din, dout, cnt, scale, st);
+                     });
+}
+int dpfhe_ckks_encode_host(dpfhe_ctx *ctx, const double *h_slots, uint64_t *h_pt, size_t n_vec, double scale) {
+    return ckks_encode_host_at(ctx, ctx ? ctx->hp.L : 0, h_slots, h_pt, n_vec, scale);
+}
+
+static int ckks_decode_host_at(dpfhe_ctx *ctx, unsigned L, const uint64_t *h_pt, double *h_slots, size_t n_vec, double scale) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    if (!valid_scale(scale)) return fail(DPFHE_ERR_INVALID, "scale must be finite and positive");
+    if (n_vec == 0) return DPFHE_OK;
+    const size_t P = L * ctx->N(), S = ctx->N();
     return host_call(ctx, {h_slots, h_pt}, nullptr, 0, h_pt, nullptr, (u64 *)h_slots, n_vec, P, S,
                      [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
-                         return dpfhe_ckks_decode(ctx, din, (double *)dout, cnt, scale, st);
+                         return ckks_decode_at(ctx, L, din, (double *)dout, cnt, scale, st);
                      });
+}
+int dpfhe_ckks_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, double *h_slots, size_t n_vec, double scale) {
+    return ckks_decode_host_at(ctx, ctx ? ctx->hp.L : 0, h_pt, h_slots, n_vec, scale);
 }
 
 // ---------------------------------------------------------------- BGV slot encoding (DESIGN.md §2.13)
@@ -1764,64 +1836,80 @@ static int bgv_prepare(dpfhe_ctx *ctx, uint64_t t, size_t need) {
     return ctx->enc_work.reserve(ctx, need);
 }
 
-int dpfhe_bgv_encode(dpfhe_ctx *ctx, const int64_t *d_slots, uint64_t *d_pt, size_t n_vec, uint64_t t_plain, void *stream) {
+// on the prefix of L limbs (DESIGN.md §2.22), as the CKKS bodies above
+static int bgv_encode_at(dpfhe_ctx *ctx, unsigned L, const int64_t *d_slots, uint64_t *d_pt, size_t n_vec, uint64_t t_plain, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     CHECK_T(t_plain);
     if (n_vec == 0) return DPFHE_OK;
     CHECK_PTR(d_slots); CHECK_PTR(d_pt);
-    if (overlaps(d_pt, n_vec * ctx->P() * 8, d_slots, n_vec * ctx->N() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    if (overlaps(d_pt, n_vec * L * ctx->N() * 8, d_slots, n_vec * ctx->N() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
     cudaStream_t st = pick(ctx, stream);
     rc = bgv_prepare(ctx, t_plain, n_vec * ctx->N() * sizeof(u32));
     if (rc) return rc;
-    CU_TRY(VCALL(launch_bgv_encode, ctx->lc, d_slots, ctx->enc_work.get<u32>(), d_pt, ctx->bgv, n_vec, st));
+    CU_TRY(VCALL(launch_bgv_encode, level_view(ctx, L), d_slots, ctx->enc_work.get<u32>(), d_pt, ctx->bgv, n_vec, st));
     note_launch(ctx, 2);   // bgv_enc_kernel + bgv_enc_ntt(_pair)_kernel
     return DPFHE_OK;
 }
+int dpfhe_bgv_encode(dpfhe_ctx *ctx, const int64_t *d_slots, uint64_t *d_pt, size_t n_vec, uint64_t t_plain, void *stream) {
+    return bgv_encode_at(ctx, ctx ? ctx->hp.L : 0, d_slots, d_pt, n_vec, t_plain, stream);
+}
 
-int dpfhe_bgv_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, uint64_t *d_slots, size_t n_vec, uint64_t t_plain, void *stream) {
+static int bgv_decode_at(dpfhe_ctx *ctx, unsigned L, const uint64_t *d_pt, uint64_t *d_slots, size_t n_vec, uint64_t t_plain, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     CHECK_T(t_plain);
     if (n_vec == 0) return DPFHE_OK;
     CHECK_PTR(d_pt); CHECK_PTR(d_slots);
-    if (overlaps(d_slots, n_vec * ctx->N() * 8, d_pt, n_vec * ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    const size_t bytes = n_vec * L * ctx->N() * 8;
+    if (overlaps(d_slots, n_vec * ctx->N() * 8, d_pt, bytes)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    const HostParams *hp = prefix_params(ctx, L);
+    if (!hp) return fail(DPFHE_ERR_NOMEM, "out of host memory");
     cudaStream_t st = pick(ctx, stream);
-    const size_t bytes = n_vec * ctx->P() * 8;
     rc = bgv_prepare(ctx, t_plain, bytes);
     if (rc) return rc;
+    const LaunchCtx lc = level_view(ctx, L);
     u64 *work = ctx->enc_work.get();
     CU_TRY(cudaMemcpyAsync(work, d_pt, bytes, cudaMemcpyDeviceToDevice, st));   // the caller's plaintexts stay unchanged
-    CU_TRY(VCALL(launch_ntt, ctx->lc, work, n_vec, true, st));
+    CU_TRY(VCALL(launch_ntt, lc, work, n_vec, true, st));
     BgvConsts K;
-    build_bgv_consts(ctx->hp, t_plain, K);
-    CU_TRY(VCALL(launch_bgv_decode, ctx->lc, work, d_slots, ctx->bgv, K, n_vec, st));
+    build_bgv_consts(*hp, t_plain, K);
+    CU_TRY(VCALL(launch_bgv_decode, lc, work, d_slots, ctx->bgv, K, n_vec, st));
     note_launch(ctx, 2);   // inverse transform + bgv_dec_kernel
     return DPFHE_OK;
 }
-
-int dpfhe_bgv_encode_host(dpfhe_ctx *ctx, const int64_t *h_slots, uint64_t *h_pt, size_t n_vec, uint64_t t_plain) {
-    int rc = enter(ctx);
-    if (rc) return rc;
-    CHECK_T(t_plain);
-    if (n_vec == 0) return DPFHE_OK;
-    const size_t P = ctx->P(), S = ctx->N();   // words of a plaintext, and of a slot vector
-    return host_call(ctx, {h_slots, h_pt}, nullptr, 0, (const u64 *)h_slots, nullptr, h_pt, n_vec, S, P,
-                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
-                         return dpfhe_bgv_encode(ctx, (const int64_t *)din, dout, cnt, t_plain, st);
-                     });
+int dpfhe_bgv_decode(dpfhe_ctx *ctx, const uint64_t *d_pt, uint64_t *d_slots, size_t n_vec, uint64_t t_plain, void *stream) {
+    return bgv_decode_at(ctx, ctx ? ctx->hp.L : 0, d_pt, d_slots, n_vec, t_plain, stream);
 }
 
-int dpfhe_bgv_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, uint64_t *h_slots, size_t n_vec, uint64_t t_plain) {
+static int bgv_encode_host_at(dpfhe_ctx *ctx, unsigned L, const int64_t *h_slots, uint64_t *h_pt, size_t n_vec, uint64_t t_plain) {
     int rc = enter(ctx);
     if (rc) return rc;
     CHECK_T(t_plain);
     if (n_vec == 0) return DPFHE_OK;
-    const size_t P = ctx->P(), S = ctx->N();
+    const size_t P = L * ctx->N(), S = ctx->N();   // words of a plaintext, and of a slot vector
+    return host_call(ctx, {h_slots, h_pt}, nullptr, 0, (const u64 *)h_slots, nullptr, h_pt, n_vec, S, P,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return bgv_encode_at(ctx, L, (const int64_t *)din, dout, cnt, t_plain, st);
+                     });
+}
+int dpfhe_bgv_encode_host(dpfhe_ctx *ctx, const int64_t *h_slots, uint64_t *h_pt, size_t n_vec, uint64_t t_plain) {
+    return bgv_encode_host_at(ctx, ctx ? ctx->hp.L : 0, h_slots, h_pt, n_vec, t_plain);
+}
+
+static int bgv_decode_host_at(dpfhe_ctx *ctx, unsigned L, const uint64_t *h_pt, uint64_t *h_slots, size_t n_vec, uint64_t t_plain) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_T(t_plain);
+    if (n_vec == 0) return DPFHE_OK;
+    const size_t P = L * ctx->N(), S = ctx->N();
     return host_call(ctx, {h_slots, h_pt}, nullptr, 0, h_pt, nullptr, h_slots, n_vec, P, S,
                      [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
-                         return dpfhe_bgv_decode(ctx, din, dout, cnt, t_plain, st);
+                         return bgv_decode_at(ctx, L, din, dout, cnt, t_plain, st);
                      });
+}
+int dpfhe_bgv_decode_host(dpfhe_ctx *ctx, const uint64_t *h_pt, uint64_t *h_slots, size_t n_vec, uint64_t t_plain) {
+    return bgv_decode_host_at(ctx, ctx ? ctx->hp.L : 0, h_pt, h_slots, n_vec, t_plain);
 }
 #undef CHECK_T
 
@@ -1906,23 +1994,32 @@ int dpfhe_galois_keygen(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, co
     return DPFHE_OK;
 }
 
-int dpfhe_encrypt(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32], uint64_t first_index, const uint64_t *d_pt,
-                  uint64_t *d_ct, size_t n, void *stream) {
+// encryption and decryption on the prefix of L limbs (DESIGN.md §2.22): the first L rows of the secret, which are the prefix basis's
+// own secret; L = hp.L is the top-level call
+static int encrypt_at(dpfhe_ctx *ctx, unsigned L, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32], uint64_t first_index,
+                      const uint64_t *d_pt, uint64_t *d_ct, size_t n, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     CHECK_SEED(seed);
     if (n == 0) return DPFHE_OK;
     CHECK_PTR(d_sk); CHECK_PTR(d_pt); CHECK_PTR(d_ct);
-    if (overlaps(d_ct, n * 2 * ctx->P() * 8, d_pt, n * ctx->P() * 8) || overlaps(d_ct, n * 2 * ctx->P() * 8, d_sk, ctx->P() * 8))
+    const size_t P = L * ctx->N();
+    if (overlaps(d_ct, n * 2 * P * 8, d_pt, n * P * 8) || overlaps(d_ct, n * 2 * P * 8, d_sk, P * 8))
         return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
-    KeyArgs A = build_key_args(ctx->hp, seed, 0, t_plain);
+    const HostParams *hp = prefix_params(ctx, L);
+    if (!hp) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    KeyArgs A = build_key_args(*hp, seed, 0, t_plain);
     A.s = d_sk;
     A.pt = d_pt;
     A.out = d_ct;
     A.item0 = first_index;
-    CU_TRY(VCALL(launch_keys, ctx->lc, KM_ENC, A, n, pick(ctx, stream)));
+    CU_TRY(VCALL(launch_keys, level_view(ctx, L), KM_ENC, A, n, pick(ctx, stream)));
     note_launch(ctx, 1);
     return DPFHE_OK;
+}
+int dpfhe_encrypt(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32], uint64_t first_index, const uint64_t *d_pt,
+                  uint64_t *d_ct, size_t n, void *stream) {
+    return encrypt_at(ctx, ctx ? ctx->hp.L : 0, t_plain, d_sk, seed, first_index, d_pt, d_ct, n, stream);
 }
 
 // the public key (b, a) = (-a s + t NTT(e), a): the encryption of zero with its own nonce domains and item 0
@@ -1940,36 +2037,49 @@ int dpfhe_public_keygen(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_sk, 
     return DPFHE_OK;
 }
 
-int dpfhe_encrypt_public(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_pk, const uint8_t seed[32], uint64_t first_index,
-                         const uint64_t *d_pt, uint64_t *d_ct, size_t n, void *stream) {
+// d_pk is the context's public key [2][hp.L][N] at every L: the prefix reads the first L rows of each component
+static int encrypt_public_at(dpfhe_ctx *ctx, unsigned L, uint64_t t_plain, const uint64_t *d_pk, const uint8_t seed[32], uint64_t first_index,
+                             const uint64_t *d_pt, uint64_t *d_ct, size_t n, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     CHECK_SEED(seed);
     if (n == 0) return DPFHE_OK;
     CHECK_PTR(d_pk); CHECK_PTR(d_pt); CHECK_PTR(d_ct);
-    if (overlaps(d_ct, n * 2 * ctx->P() * 8, d_pt, n * ctx->P() * 8) || overlaps(d_ct, n * 2 * ctx->P() * 8, d_pk, 2 * ctx->P() * 8))
+    const size_t P = L * ctx->N();
+    if (overlaps(d_ct, n * 2 * P * 8, d_pt, n * P * 8) || overlaps(d_ct, n * 2 * P * 8, d_pk, 2 * ctx->P() * 8))
         return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
-    KeyArgs A = build_key_args(ctx->hp, seed, 0, t_plain);
-    A.s = d_pk;   // b at s, a at s + L N
+    const HostParams *hp = prefix_params(ctx, L);
+    if (!hp) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    KeyArgs A = build_key_args(*hp, seed, 0, t_plain);
+    A.s = d_pk;   // b at s, a at s + pk_a
+    A.pk_a = (u32)ctx->P();
     A.pt = d_pt;
     A.out = d_ct;
     A.item0 = first_index;
-    CU_TRY(VCALL(launch_keys, ctx->lc, KM_ENC_PUBLIC, A, n, pick(ctx, stream)));
+    CU_TRY(VCALL(launch_keys, level_view(ctx, L), KM_ENC_PUBLIC, A, n, pick(ctx, stream)));
     note_launch(ctx, 1);
     return DPFHE_OK;
 }
+int dpfhe_encrypt_public(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_pk, const uint8_t seed[32], uint64_t first_index,
+                         const uint64_t *d_pt, uint64_t *d_ct, size_t n, void *stream) {
+    return encrypt_public_at(ctx, ctx ? ctx->hp.L : 0, t_plain, d_pk, seed, first_index, d_pt, d_ct, n, stream);
+}
 
-int dpfhe_decrypt(dpfhe_ctx *ctx, const uint64_t *d_sk, const uint64_t *d_ct, unsigned n_comp, uint64_t *d_pt, size_t n, void *stream) {
+static int decrypt_at(dpfhe_ctx *ctx, unsigned L, const uint64_t *d_sk, const uint64_t *d_ct, unsigned n_comp, uint64_t *d_pt, size_t n, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (n_comp != 2 && n_comp != 3) return fail(DPFHE_ERR_INVALID, "n_comp must be 2 or 3");
     if (n == 0) return DPFHE_OK;
     CHECK_PTR(d_sk); CHECK_PTR(d_ct); CHECK_PTR(d_pt);
-    if (overlaps(d_pt, n * ctx->P() * 8, d_sk, ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the secret");
-    if (overlaps(d_pt, n * ctx->P() * 8, d_ct, n * n_comp * ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
-    CU_TRY(VCALL(launch_decrypt, ctx->lc, d_ct, d_sk, d_pt, n_comp, n, pick(ctx, stream)));
+    const size_t P = L * ctx->N();
+    if (overlaps(d_pt, n * P * 8, d_sk, P * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the secret");
+    if (overlaps(d_pt, n * P * 8, d_ct, n * n_comp * P * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+    CU_TRY(VCALL(launch_decrypt, level_view(ctx, L), d_ct, d_sk, d_pt, n_comp, n, pick(ctx, stream)));
     note_launch(ctx, 1);
     return DPFHE_OK;
+}
+int dpfhe_decrypt(dpfhe_ctx *ctx, const uint64_t *d_sk, const uint64_t *d_ct, unsigned n_comp, uint64_t *d_pt, size_t n, void *stream) {
+    return decrypt_at(ctx, ctx ? ctx->hp.L : 0, d_sk, d_ct, n_comp, d_pt, n, stream);
 }
 
 // host forms of the key generators: a device buffer of their own, the call, a copy out (synchronous)
@@ -2042,20 +2152,25 @@ int dpfhe_galois_keygen_host(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plai
                        }, &args);
 }
 
-int dpfhe_encrypt_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t first_index, const uint64_t *h_pt,
-                       uint64_t *h_ct, size_t n) {
+// host forms on the prefix of L limbs: the secret's first L rows staged once
+static int encrypt_host_at(dpfhe_ctx *ctx, unsigned L, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t first_index,
+                           const uint64_t *h_pt, uint64_t *h_ct, size_t n) {
     int rc = enter(ctx);
     if (rc) return rc;
     CHECK_SEED(seed);
     if (n == 0) return DPFHE_OK;
-    const size_t P = ctx->P();
+    const size_t P = L * ctx->N();
     uint64_t next = first_index;   // the chunks run in order: ciphertext k keeps item number first_index + k
     return host_call(ctx, {h_sk, h_pt, h_ct}, h_sk, P, h_pt, nullptr, h_ct, n, P, 2 * P,
                      [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
-                         const int r = dpfhe_encrypt(ctx, t_plain, ctx->stage_key.get(), seed, next, din, dout, cnt, st);
+                         const int r = encrypt_at(ctx, L, t_plain, ctx->stage_key.get(), seed, next, din, dout, cnt, st);
                          next += cnt;
                          return r;
                      });
+}
+int dpfhe_encrypt_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t first_index, const uint64_t *h_pt,
+                       uint64_t *h_ct, size_t n) {
+    return encrypt_host_at(ctx, ctx ? ctx->hp.L : 0, t_plain, h_sk, seed, first_index, h_pt, h_ct, n);
 }
 
 int dpfhe_public_keygen_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t *h_pk) {
@@ -2071,33 +2186,100 @@ int dpfhe_public_keygen_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h
                        }, &args);
 }
 
-// the public key (2P words) is the staged shared operand; item numbers continue across chunks as in dpfhe_encrypt_host
-int dpfhe_encrypt_public_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_pk, const uint8_t seed[32], uint64_t first_index,
-                              const uint64_t *h_pt, uint64_t *h_ct, size_t n) {
+// the public key (2P words of the top level, whatever L) is the staged shared operand; item numbers continue across chunks as in
+// dpfhe_encrypt_host
+static int encrypt_public_host_at(dpfhe_ctx *ctx, unsigned L, uint64_t t_plain, const uint64_t *h_pk, const uint8_t seed[32], uint64_t first_index,
+                                  const uint64_t *h_pt, uint64_t *h_ct, size_t n) {
     int rc = enter(ctx);
     if (rc) return rc;
     CHECK_SEED(seed);
     if (n == 0) return DPFHE_OK;
-    const size_t P = ctx->P();
+    const size_t P = L * ctx->N();
     uint64_t next = first_index;
-    return host_call(ctx, {h_pk, h_pt, h_ct}, h_pk, 2 * P, h_pt, nullptr, h_ct, n, P, 2 * P,
+    return host_call(ctx, {h_pk, h_pt, h_ct}, h_pk, 2 * ctx->P(), h_pt, nullptr, h_ct, n, P, 2 * P,
                      [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
-                         const int r = dpfhe_encrypt_public(ctx, t_plain, ctx->stage_key.get(), seed, next, din, dout, cnt, st);
+                         const int r = encrypt_public_at(ctx, L, t_plain, ctx->stage_key.get(), seed, next, din, dout, cnt, st);
                          next += cnt;
                          return r;
                      });
 }
+int dpfhe_encrypt_public_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_pk, const uint8_t seed[32], uint64_t first_index,
+                              const uint64_t *h_pt, uint64_t *h_ct, size_t n) {
+    return encrypt_public_host_at(ctx, ctx ? ctx->hp.L : 0, t_plain, h_pk, seed, first_index, h_pt, h_ct, n);
+}
 
-int dpfhe_decrypt_host(dpfhe_ctx *ctx, const uint64_t *h_sk, const uint64_t *h_ct, unsigned n_comp, uint64_t *h_pt, size_t n) {
+static int decrypt_host_at(dpfhe_ctx *ctx, unsigned L, const uint64_t *h_sk, const uint64_t *h_ct, unsigned n_comp, uint64_t *h_pt, size_t n) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (n_comp != 2 && n_comp != 3) return fail(DPFHE_ERR_INVALID, "n_comp must be 2 or 3");
     if (n == 0) return DPFHE_OK;
-    const size_t P = ctx->P();
+    const size_t P = L * ctx->N();
     return host_call(ctx, {h_sk, h_ct, h_pt}, h_sk, P, h_ct, nullptr, h_pt, n, n_comp * P, P,
                      [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
-                         return dpfhe_decrypt(ctx, ctx->stage_key.get(), din, n_comp, dout, cnt, st);
+                         return decrypt_at(ctx, L, ctx->stage_key.get(), din, n_comp, dout, cnt, st);
                      });
+}
+int dpfhe_decrypt_host(dpfhe_ctx *ctx, const uint64_t *h_sk, const uint64_t *h_ct, unsigned n_comp, uint64_t *h_pt, size_t n) {
+    return decrypt_host_at(ctx, ctx ? ctx->hp.L : 0, h_sk, h_ct, n_comp, h_pt, n);
+}
+
+// ---- the keyless calls at level l (DESIGN.md §2.22): each is, bit for bit, the call it is named after on a context over the prefix
+// basis {q_0 .. q_{l-1}}, run on this context's view of that prefix.  1 <= level <= L.
+int dpfhe_ckks_encode_level(dpfhe_ctx *ctx, unsigned level, const double *d_slots, uint64_t *d_pt, size_t n_vec, double scale, void *stream) {
+    return prefix_call(ctx, level, [&] { return ckks_encode_at(ctx, level, d_slots, d_pt, n_vec, scale, stream); });
+}
+int dpfhe_ckks_decode_level(dpfhe_ctx *ctx, unsigned level, const uint64_t *d_pt, double *d_slots, size_t n_vec, double scale, void *stream) {
+    return prefix_call(ctx, level, [&] { return ckks_decode_at(ctx, level, d_pt, d_slots, n_vec, scale, stream); });
+}
+int dpfhe_ckks_encode_level_host(dpfhe_ctx *ctx, unsigned level, const double *h_slots, uint64_t *h_pt, size_t n_vec, double scale) {
+    return prefix_call(ctx, level, [&] { return ckks_encode_host_at(ctx, level, h_slots, h_pt, n_vec, scale); });
+}
+int dpfhe_ckks_decode_level_host(dpfhe_ctx *ctx, unsigned level, const uint64_t *h_pt, double *h_slots, size_t n_vec, double scale) {
+    return prefix_call(ctx, level, [&] { return ckks_decode_host_at(ctx, level, h_pt, h_slots, n_vec, scale); });
+}
+int dpfhe_bgv_encode_level(dpfhe_ctx *ctx, unsigned level, const int64_t *d_slots, uint64_t *d_pt, size_t n_vec, uint64_t t_plain, void *stream) {
+    return prefix_call(ctx, level, [&] { return bgv_encode_at(ctx, level, d_slots, d_pt, n_vec, t_plain, stream); });
+}
+int dpfhe_bgv_decode_level(dpfhe_ctx *ctx, unsigned level, const uint64_t *d_pt, uint64_t *d_slots, size_t n_vec, uint64_t t_plain, void *stream) {
+    return prefix_call(ctx, level, [&] { return bgv_decode_at(ctx, level, d_pt, d_slots, n_vec, t_plain, stream); });
+}
+int dpfhe_bgv_encode_level_host(dpfhe_ctx *ctx, unsigned level, const int64_t *h_slots, uint64_t *h_pt, size_t n_vec, uint64_t t_plain) {
+    return prefix_call(ctx, level, [&] { return bgv_encode_host_at(ctx, level, h_slots, h_pt, n_vec, t_plain); });
+}
+int dpfhe_bgv_decode_level_host(dpfhe_ctx *ctx, unsigned level, const uint64_t *h_pt, uint64_t *h_slots, size_t n_vec, uint64_t t_plain) {
+    return prefix_call(ctx, level, [&] { return bgv_decode_host_at(ctx, level, h_pt, h_slots, n_vec, t_plain); });
+}
+int dpfhe_encrypt_level(dpfhe_ctx *ctx, unsigned level, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32], uint64_t first_index,
+                        const uint64_t *d_pt, uint64_t *d_ct, size_t n, void *stream) {
+    return prefix_call(ctx, level, [&] { return encrypt_at(ctx, level, t_plain, d_sk, seed, first_index, d_pt, d_ct, n, stream); });
+}
+int dpfhe_encrypt_level_host(dpfhe_ctx *ctx, unsigned level, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t first_index,
+                             const uint64_t *h_pt, uint64_t *h_ct, size_t n) {
+    return prefix_call(ctx, level, [&] { return encrypt_host_at(ctx, level, t_plain, h_sk, seed, first_index, h_pt, h_ct, n); });
+}
+int dpfhe_encrypt_public_level(dpfhe_ctx *ctx, unsigned level, uint64_t t_plain, const uint64_t *d_pk, const uint8_t seed[32], uint64_t first_index,
+                               const uint64_t *d_pt, uint64_t *d_ct, size_t n, void *stream) {
+    return prefix_call(ctx, level, [&] { return encrypt_public_at(ctx, level, t_plain, d_pk, seed, first_index, d_pt, d_ct, n, stream); });
+}
+int dpfhe_encrypt_public_level_host(dpfhe_ctx *ctx, unsigned level, uint64_t t_plain, const uint64_t *h_pk, const uint8_t seed[32],
+                                    uint64_t first_index, const uint64_t *h_pt, uint64_t *h_ct, size_t n) {
+    return prefix_call(ctx, level, [&] { return encrypt_public_host_at(ctx, level, t_plain, h_pk, seed, first_index, h_pt, h_ct, n); });
+}
+int dpfhe_decrypt_level(dpfhe_ctx *ctx, unsigned level, const uint64_t *d_sk, const uint64_t *d_ct, unsigned n_comp, uint64_t *d_pt, size_t n,
+                        void *stream) {
+    return prefix_call(ctx, level, [&] { return decrypt_at(ctx, level, d_sk, d_ct, n_comp, d_pt, n, stream); });
+}
+int dpfhe_decrypt_level_host(dpfhe_ctx *ctx, unsigned level, const uint64_t *h_sk, const uint64_t *h_ct, unsigned n_comp, uint64_t *h_pt,
+                             size_t n) {
+    return prefix_call(ctx, level, [&] { return decrypt_host_at(ctx, level, h_sk, h_ct, n_comp, h_pt, n); });
+}
+int dpfhe_ct_mul_plain_level(dpfhe_ctx *ctx, unsigned level, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch,
+                             void *stream) {
+    return prefix_call(ctx, level, [&] { return ct_mul_plain_at(ctx, level, d_ct, d_pt, d_out, batch, stream); });
+}
+int dpfhe_mod_switch_down_level(dpfhe_ctx *ctx, unsigned level, const uint64_t *d_in, uint64_t *d_out, size_t n_polys, uint64_t t_plain,
+                                void *stream) {
+    return prefix_call(ctx, level, [&] { return mod_switch_down_at(ctx, level, d_in, d_out, n_polys, t_plain, stream); });
 }
 #undef CHECK_SEED
 
@@ -2456,8 +2638,9 @@ int dpfhe_linear_apply(dpfhe_linear *lin, const uint64_t *d_ct, uint64_t *d_out,
 int dpfhe_linear_apply_host(dpfhe_linear *lin, const uint64_t *h_ct, uint64_t *h_out, size_t batch) { return object_apply_host(lin, h_ct, h_out, batch); }
 
 // ---------------------------------------------------------------- scalar linear combinations, BGV polynomial evaluation (DESIGN.md §2.15)
-int dpfhe_ct_lincomb(dpfhe_ctx *ctx, size_t n_terms, const uint64_t *const *d_cts, const int64_t *coeffs, int64_t constant, uint64_t *d_out,
-                     size_t batch, void *stream) {
+// on the prefix of L limbs (DESIGN.md §2.22); L = hp.L is dpfhe_ct_lincomb
+static int ct_lincomb_at(dpfhe_ctx *ctx, unsigned L, size_t n_terms, const uint64_t *const *d_cts, const int64_t *coeffs, int64_t constant,
+                         uint64_t *d_out, size_t batch, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (n_terms < 1 || n_terms > (size_t)LINCOMB_MAX_TERMS) return fail(DPFHE_ERR_INVALID, "n_terms must be in [1, %d]", LINCOMB_MAX_TERMS);
@@ -2467,27 +2650,46 @@ int dpfhe_ct_lincomb(dpfhe_ctx *ctx, size_t n_terms, const uint64_t *const *d_ct
     CHECK_PTR(d_out);
     if (batch == 0) return DPFHE_OK;
     // the output may BE an input (a thread reads chunk c of every input, then writes chunk c), but not overlap one at another offset
-    const size_t ct_bytes = batch * 2 * ctx->P() * 8;
+    const size_t ct_bytes = batch * 2 * L * ctx->N() * 8;
     for (size_t i = 0; i < n_terms; ++i)
         if (d_out != d_cts[i] && overlaps(d_out, ct_bytes, d_cts[i], ct_bytes))
             return fail(DPFHE_ERR_INVALID, "output must be an input or not overlap it (input %zu)", i);
-    CU_TRY(VCALL(launch_lincomb, ctx->lc, d_cts, coeffs, (u32)n_terms, constant, nullptr, d_out, batch, pick(ctx, stream)));
+    CU_TRY(VCALL(launch_lincomb, level_view(ctx, L), d_cts, coeffs, (u32)n_terms, constant, nullptr, d_out, batch, pick(ctx, stream)));
     note_launch(ctx, 1);
     return DPFHE_OK;
 }
+int dpfhe_ct_lincomb(dpfhe_ctx *ctx, size_t n_terms, const uint64_t *const *d_cts, const int64_t *coeffs, int64_t constant, uint64_t *d_out,
+                     size_t batch, void *stream) {
+    return ct_lincomb_at(ctx, ctx ? ctx->hp.L : 0, n_terms, d_cts, coeffs, constant, d_out, batch, stream);
+}
 
-// the linear-combination body with one term of coefficient 1 and the plaintext as the c0 addend
-int dpfhe_ct_add_plain(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch, void *stream) {
+// the linear-combination body with one term of coefficient 1 and the plaintext as the c0 addend; on the prefix of L limbs
+// (DESIGN.md §2.22), L = hp.L is dpfhe_ct_add_plain
+static int ct_add_plain_at(dpfhe_ctx *ctx, unsigned L, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch, void *stream) {
     int rc = enter(ctx);
     if (rc) return rc;
     CHECK_PTR(d_ct); CHECK_PTR(d_pt); CHECK_PTR(d_out);
     if (batch == 0) return DPFHE_OK;
-    if (overlaps(d_out, batch * 2 * ctx->P() * 8, d_pt, ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the plaintext");
-    if (overlaps_shifted(d_out, d_ct, batch * 2 * ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must be the input or not overlap it");
+    const size_t P = L * ctx->N();
+    if (overlaps(d_out, batch * 2 * P * 8, d_pt, P * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the plaintext");
+    if (overlaps_shifted(d_out, d_ct, batch * 2 * P * 8)) return fail(DPFHE_ERR_INVALID, "output must be the input or not overlap it");
     const int64_t one = 1;
-    CU_TRY(VCALL(launch_lincomb, ctx->lc, &d_ct, &one, 1u, (int64_t)0, d_pt, d_out, batch, pick(ctx, stream)));
+    CU_TRY(VCALL(launch_lincomb, level_view(ctx, L), &d_ct, &one, 1u, (int64_t)0, d_pt, d_out, batch, pick(ctx, stream)));
     note_launch(ctx, 1);
     return DPFHE_OK;
+}
+int dpfhe_ct_add_plain(dpfhe_ctx *ctx, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch, void *stream) {
+    return ct_add_plain_at(ctx, ctx ? ctx->hp.L : 0, d_ct, d_pt, d_out, batch, stream);
+}
+
+// at level l (DESIGN.md §2.22), as the keyless level calls above
+int dpfhe_ct_lincomb_level(dpfhe_ctx *ctx, unsigned level, size_t n_terms, const uint64_t *const *d_cts, const int64_t *coeffs, int64_t constant,
+                           uint64_t *d_out, size_t batch, void *stream) {
+    return prefix_call(ctx, level, [&] { return ct_lincomb_at(ctx, level, n_terms, d_cts, coeffs, constant, d_out, batch, stream); });
+}
+int dpfhe_ct_add_plain_level(dpfhe_ctx *ctx, unsigned level, const uint64_t *d_ct, const uint64_t *d_pt, uint64_t *d_out, size_t batch,
+                             void *stream) {
+    return prefix_call(ctx, level, [&] { return ct_add_plain_at(ctx, level, d_ct, d_pt, d_out, batch, stream); });
 }
 
 // host buffers: the plaintext uploaded once, the batch pipelined in chunks (as dpfhe_ct_mul_plain_host)
@@ -2560,7 +2762,9 @@ struct PeOp {
 struct dpfhe_polyeval {
     static constexpr const char *what = "null evaluator";
     dpfhe_ctx *const ctx;
-    unsigned K = 0, Lq = 0, Lf = 0;
+    unsigned K = 0, Lq = 0, Lf = 0;      // Lq: the level the evaluator starts from (its input's limbs; DESIGN.md §2.22), Lf: the result's
+    unsigned Lk = 0;                     // the context's L - K: the row of the first special prime in the top-level key, and the level
+                                         //   whose tables are the context's own
     uint64_t t = 0;
     std::vector<PeLevel> lev;            // by level: lev[l - lev_lo]
     unsigned lev_lo = 0;
@@ -2575,7 +2779,7 @@ struct dpfhe_polyeval {
     explicit dpfhe_polyeval(dpfhe_ctx *c) : ctx(c), mem(c) {}
     ~dpfhe_polyeval() {
         for (auto &v : lev) {
-            if (v.l != Lq) {   // the top level's tables are the context's
+            if (v.l != Lk) {   // the top level's tables are the context's
                 cudaFree(v.d_lp);
                 cudaFree(v.d_tw);
                 cudaFree(v.d_itw);
@@ -2776,16 +2980,16 @@ LaunchCtx pe_view(const dpfhe_polyeval *pe, const PeLevel &v) {
 // builds level l's tables, key and companions (st: the context's stream)
 int pe_level(dpfhe_polyeval *pe, PeLevel &v, unsigned l, const uint64_t *h_key, cudaStream_t st) {
     dpfhe_ctx *ctx = pe->ctx;
-    const unsigned K = pe->K, Lq = pe->Lq, L = ctx->hp.L, Ll = l + K;
+    const unsigned K = pe->K, Lk = pe->Lk, L = ctx->hp.L, Ll = l + K;
     const size_t N = ctx->N(), dl = (l + K - 1) / K;
     v.l = l;
     std::vector<uint64_t> mod(Ll);
     for (unsigned i = 0; i < l; ++i) mod[i] = ctx->hp.limbs[i].lp.q;
-    for (unsigned k = 0; k < K; ++k) mod[l + k] = ctx->hp.limbs[Lq + k].lp.q;
+    for (unsigned k = 0; k < K; ++k) mod[l + k] = ctx->hp.limbs[Lk + k].lp.q;
     std::string msg = build_host_params(ctx->hp.log_n, Ll, mod.data(), v.hp);
     if (!msg.empty()) return fail(DPFHE_ERR_INVALID, "%s", msg.c_str());
     build_group_consts(v.hp, K, pe->t, v.G, v.K);
-    if (l == Lq) {   // the context's own basis
+    if (l == Lk) {   // the context's own basis
         v.d_lp = ctx->d_lp;
         v.d_tw = ctx->d_tw;
         v.d_itw = ctx->d_itw;
@@ -2797,14 +3001,14 @@ int pe_level(dpfhe_polyeval *pe, PeLevel &v, unsigned l, const uint64_t *h_key, 
         if (rc) return rc;
         pe->mem.count_fixed(bytes);
     }
-    // the key of level l: digits g < ceil(l / K), limb rows 0 .. l-1 and the special rows Lq .. Lq+K-1 of the top-level key
+    // the key of level l: digits g < ceil(l / K), limb rows 0 .. l-1 and the special rows Lk .. Lk+K-1 of the top-level key
     const int rc = prepare_keys(ctx, pe_view(pe, v), 1, dl, st, "polynomial evaluator keys", [&](u64 *d_key) {
         cudaError_t e = cudaSuccess;
         for (size_t gc = 0; gc < 2 * dl && e == cudaSuccess; ++gc) {   // (digit, component) rows
             const uint64_t *src = h_key + gc * L * N;
             u64 *dst = d_key + gc * Ll * N;
             e = cudaMemcpy(dst, src, l * N * 8, cudaMemcpyHostToDevice);
-            if (e == cudaSuccess) e = cudaMemcpy(dst + l * N, src + Lq * N, K * N * 8, cudaMemcpyHostToDevice);
+            if (e == cudaSuccess) e = cudaMemcpy(dst + l * N, src + Lk * N, K * N * 8, cudaMemcpyHostToDevice);
         }
         return e;
     }, v.key);
@@ -2891,50 +3095,77 @@ int dpfhe_polyeval::apply_on(const uint64_t *d_ct, uint64_t *d_out, size_t batch
     return DPFHE_OK;
 }
 
-int dpfhe_polyeval_create_grouped(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const int64_t *coeffs, size_t degree,
-                                  const uint64_t *h_relin_key, dpfhe_polyeval **out) {
+// level: the start level (DESIGN.md §2.22), nullptr for the top level Lq = L - K
+static int polyeval_grouped_new(dpfhe_ctx *ctx, unsigned n_special, const unsigned *level, uint64_t t_plain, const int64_t *coeffs, size_t degree,
+                                const uint64_t *h_relin_key, dpfhe_polyeval **out) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (!out || !coeffs || !h_relin_key) return fail(DPFHE_ERR_INVALID, "null argument");
     *out = nullptr;
     rc = check_special(ctx, n_special);
+    if (!rc && level) rc = check_level(ctx, n_special, *level, false, 0);
     if (rc) return rc;
     if (t_plain < 2 || t_plain >= ((uint64_t)1 << 31)) return fail(DPFHE_ERR_INVALID, "the plaintext modulus must be in [2, 2^31)");
     if (degree < 1 || degree > 64) return fail(DPFHE_ERR_INVALID, "the degree must be in [1, 64]");
-    const unsigned L = ctx->hp.L, K = n_special, Lq = L - K, D = ceil_log2(degree);
+    const unsigned L = ctx->hp.L, K = n_special, Lk = L - K, Lq = level ? *level : Lk, D = ceil_log2(degree);
     if (D > Lq - 1 || D > Lq - K + 1)
         return fail(DPFHE_ERR_INVALID, "degree %zu needs %u levels: at most min(Lq - 1, Lq - K + 1) = %u with Lq = %u, K = %u", degree, D,
                     std::min(Lq - 1, Lq - K + 1), Lq, K);
     dpfhe_polyeval *pe = new (std::nothrow) dpfhe_polyeval(ctx);
     if (!pe) return fail(DPFHE_ERR_NOMEM, "out of host memory");
-    pe->K = K; pe->Lq = Lq; pe->Lf = Lq - D; pe->t = t_plain;
+    pe->K = K; pe->Lq = Lq; pe->Lk = Lk; pe->Lf = Lq - D; pe->t = t_plain;
     rc = pe_plan(pe, coeffs, degree);
     return pe_finish(pe, rc, D > 0 ? pe->Lf + 1 : Lq + 1, h_relin_key, out);
 }
 
-int dpfhe_polyeval_create_ckks(dpfhe_ctx *ctx, unsigned n_special, const double *coeffs, size_t degree, double scale_in, double scale_out,
-                               const uint64_t *h_relin_key, dpfhe_polyeval **out) {
+static int polyeval_ckks_new(dpfhe_ctx *ctx, unsigned n_special, const unsigned *level, const double *coeffs, size_t degree, double scale_in,
+                             double scale_out, const uint64_t *h_relin_key, dpfhe_polyeval **out) {
     int rc = enter(ctx);
     if (rc) return rc;
     if (!out || !coeffs || !h_relin_key) return fail(DPFHE_ERR_INVALID, "null argument");
     *out = nullptr;
     rc = check_special(ctx, n_special);
+    if (!rc && level) rc = check_level(ctx, n_special, *level, false, 0);
     if (rc) return rc;
     if (degree < 1 || degree > 64) return fail(DPFHE_ERR_INVALID, "the degree must be in [1, 64]");
     for (size_t k = 0; k <= degree; ++k)
         if (!std::isfinite(coeffs[k])) return fail(DPFHE_ERR_INVALID, "coefficient %zu is not finite", k);
     if (!(std::isfinite(scale_in) && scale_in > 0) || !(std::isfinite(scale_out) && scale_out > 0))
         return fail(DPFHE_ERR_INVALID, "the scales must be finite and positive");
-    const unsigned L = ctx->hp.L, K = n_special, Lq = L - K, D = ceil_log2(degree);
+    const unsigned L = ctx->hp.L, K = n_special, Lk = L - K, Lq = level ? *level : Lk, D = ceil_log2(degree);
     if (D + 2 > Lq || D > Lq - K + 1)
         return fail(DPFHE_ERR_INVALID, "degree %zu needs %u levels: at most min(Lq - 2, Lq - K + 1) with Lq = %u, K = %u", degree, D, Lq, K);
     dpfhe_polyeval *pe = new (std::nothrow) dpfhe_polyeval(ctx);
     if (!pe) return fail(DPFHE_ERR_NOMEM, "out of host memory");
-    pe->K = K; pe->Lq = Lq; pe->Lf = Lq - D - 1; pe->t = 0;
+    pe->K = K; pe->Lq = Lq; pe->Lk = Lk; pe->Lf = Lq - D - 1; pe->t = 0;
     pe->ckks = true;
     pe->scale_out = scale_out;
     rc = pe_plan_ckks(pe, coeffs, degree, scale_in);
     return pe_finish(pe, rc, Lq - D, h_relin_key, out);
+}
+
+int dpfhe_polyeval_create_grouped(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const int64_t *coeffs, size_t degree,
+                                  const uint64_t *h_relin_key, dpfhe_polyeval **out) {
+    return polyeval_grouped_new(ctx, n_special, nullptr, t_plain, coeffs, degree, h_relin_key, out);
+}
+
+int dpfhe_polyeval_create_ckks(dpfhe_ctx *ctx, unsigned n_special, const double *coeffs, size_t degree, double scale_in, double scale_out,
+                               const uint64_t *h_relin_key, dpfhe_polyeval **out) {
+    return polyeval_ckks_new(ctx, n_special, nullptr, coeffs, degree, scale_in, scale_out, h_relin_key, out);
+}
+
+// the evaluators at level l (DESIGN.md §2.22): the top-level objects of a context over {q_0 .. q_{l-1}, p_0 .. p_{K-1}} with the top-level
+// key restricted to it; a failure names the level
+int dpfhe_polyeval_create_grouped_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, uint64_t t_plain, const int64_t *coeffs, size_t degree,
+                                        const uint64_t *h_relin_key, dpfhe_polyeval **out) {
+    const int rc = polyeval_grouped_new(ctx, n_special, &level, t_plain, coeffs, degree, h_relin_key, out);
+    return level_failure(level, rc);
+}
+
+int dpfhe_polyeval_create_ckks_level(dpfhe_ctx *ctx, unsigned n_special, unsigned level, const double *coeffs, size_t degree, double scale_in,
+                                     double scale_out, const uint64_t *h_relin_key, dpfhe_polyeval **out) {
+    const int rc = polyeval_ckks_new(ctx, n_special, &level, coeffs, degree, scale_in, scale_out, h_relin_key, out);
+    return level_failure(level, rc);
 }
 
 unsigned dpfhe_polyeval_result_limbs(const dpfhe_polyeval *pe) { return pe ? pe->Lf : 0; }

@@ -93,6 +93,10 @@ struct dpfhe_ctx {
     DeviceScratch hoist_M, hoist_kprime, hoist_delta;
     // the level bases of the level calls, built at the first call at (K, l), counted in device_bytes, released by dpfhe_context_trim
     std::vector<std::unique_ptr<KsLevel>> ks_levels;
+    // the prefix bases {q_0 .. q_{l-1}} of the keyless level calls (DESIGN.md §2.22), by l < L, built at the first call at l: the
+    // limb parameters only (no twiddles), from which each call builds its host constants.  Host memory; the device tables are the
+    // context's own, read through level_view.
+    std::vector<std::unique_ptr<dpfhe::HostParams>> prefix;
     cudaEvent_t ev_h2d[DPFHE_PIPE_DEPTH] = {}, ev_comp[DPFHE_PIPE_DEPTH] = {}, ev_d2h[DPFHE_PIPE_DEPTH] = {};
     size_t N() const { return (size_t)1 << hp.log_n; }
     size_t P() const { return N() * hp.L; }

@@ -17,6 +17,7 @@ KeyArgs build_key_args(const HostParams &hp, const uint8_t seed[32], unsigned K,
     A.K = K;
     A.Lq = L - K;
     A.ndig = K ? (A.Lq + K - 1) / K : L;
+    A.pk_a = L << hp.log_n;
     for (unsigned l = 0; l < L; ++l) {
         const uint64_t q = hp.limbs[l].lp.q;
         const uint64_t r64 = (uint64_t)(((u128)1 << 64) % q);

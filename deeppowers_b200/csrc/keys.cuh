@@ -233,7 +233,7 @@ DPFHE_HD void keys_half_body(CTA &cta, u64 *buf, signed char *small, const KeyAr
 }
 
 // Public-key encryption (KM_ENC_PUBLIC): ct = (b U + t E0 + pt, a U + t E1) with U = NTT(u), E0 = NTT(e0), E1 = NTT(e1) and the
-// public key (b, a) at A.s / A.s + L N.  One limb buffer: pass 0 (buf = U) writes c0 = b U + pt and c1 = a U, pass 1 (buf = t E0)
+// public key (b, a) at A.s / A.s + A.pk_a.  One limb buffer: pass 0 (buf = U) writes c0 = b U + pt and c1 = a U, pass 1 (buf = t E0)
 // adds into c0, pass 2 (buf = t E1) into c1.  A thread owns the same chunks in every pass, so it reads back only its own stores
 // (through L2: .cg); the rows it finishes in a pass are written with st_stream.
 template <int LOGN, int NT, int PASS>
@@ -243,7 +243,7 @@ DPFHE_HD void pub_enc_store(const u64 *buf, const KeyArgs &A, const LimbParams &
     U64x2 *o0 = reinterpret_cast<U64x2 *>(A.out + (item * 2 + 0) * L * N + (size_t)l * N);
     U64x2 *o1 = reinterpret_cast<U64x2 *>(A.out + (item * 2 + 1) * L * N + (size_t)l * N);
     const U64x2 *pkb = reinterpret_cast<const U64x2 *>(A.s + (size_t)l * N);
-    const U64x2 *pka = reinterpret_cast<const U64x2 *>(A.s + ((size_t)L + l) * N);
+    const U64x2 *pka = reinterpret_cast<const U64x2 *>(A.s + A.pk_a + (size_t)l * N);
     const U64x2 *pt = reinterpret_cast<const U64x2 *>(A.pt + (item * L + l) * N);
     for (int c = c_lo + tid; c < c_hi; c += NT) {
         const U64x2 v = sb[swz_chunk(c - c_lo)];

@@ -175,13 +175,13 @@ constexpr int KEYS_MAX_ELTS = 64;   // Galois elements per launch (abi.cu splits
 struct KeyArgs {
     u32 seed[8];                  // the 32-byte seed as little-endian words (the ChaCha20 key)
     u32 K, Lq, ndig;              // special primes (0: per-limb digits), limbs the digits cover, digits per key
-    u32 pad_;
+    u32 pk_a;                     // public-key encryption: the words from the public key's b to its a (L N of the key's context)
     u64 item0;                    // item number of the first item (encryption: first_index)
     u64 galois[KEYS_MAX_ELTS];    // item number and automorphism of Galois key e of the launch
     u64 r64[16], r64_s[16];       // 2^64 mod q_l and its Shoup companion (exact uniform reduction)
     u64 tq[16];                   // t mod q_l (1 for t = 0, and for the secret): the factor of the small row
     u64 fac[16];                  // gadget factor on the limbs of a digit: 1 (K = 0) or P mod q_l
-    const u64 *s;                 // secret [L][N], evaluation form (public-key encryption: the public key [2][L][N])
+    const u64 *s;                 // secret [L][N], evaluation form (public-key encryption: the public key, b at s, a at s + pk_a)
     const u64 *pt;                // encryption: plaintexts [n][L][N]
     u64 *out;                     // secret [L][N], keys [n_elts][ndig][2][L][N], public key [2][L][N], ciphertexts [n][2][L][N]
 };

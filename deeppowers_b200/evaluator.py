@@ -624,6 +624,77 @@ class Context:
     def mod_switch_down_host(self, polys, out, t_plain=0):
         self._chk(self._l.dpfhe_mod_switch_down_host(self._h, _hptr(polys), _hptr(out, True), polys.size // self.P, int(t_plain)))
 
+    # the keyless calls at level `level` on this context (DESIGN.md section 2.22): bit for bit the call of the same name on a context
+    # over the first `level` moduli q_0 .. q_{level-1}; every buffer over the limbs has `level` rows ([..][level][N]).  The secret and
+    # the public key are this context's top-level ones ([L][N], [2][L][N]).  1 <= level <= L (mod_switch_down_level: 2 <= level).
+    def ckks_encode_level(self, level, slots, pt, n_vec, scale, stream=None):
+        self._chk(self._l.dpfhe_ckks_encode_level(self._h, int(level), _cptr(slots), _ptr(pt), n_vec, float(scale), _stream(stream)))
+
+    def ckks_decode_level(self, level, pt, slots, n_vec, scale, stream=None):
+        self._chk(self._l.dpfhe_ckks_decode_level(self._h, int(level), _ptr(pt), _cptr(slots), n_vec, float(scale), _stream(stream)))
+
+    def ckks_encode_level_host(self, level, slots, pt, scale):
+        self._chk(self._l.dpfhe_ckks_encode_level_host(self._h, int(level), _chptr(slots), _hptr(pt, True), slots.size // (self.N // 2),
+                                                       float(scale)))
+
+    def ckks_decode_level_host(self, level, pt, slots, scale):
+        self._chk(self._l.dpfhe_ckks_decode_level_host(self._h, int(level), _hptr(pt), _chptr(slots, True), pt.size // (int(level) * self.N),
+                                                       float(scale)))
+
+    def bgv_encode_level(self, level, slots, pt, n_vec, t_plain, stream=None):
+        self._chk(self._l.dpfhe_bgv_encode_level(self._h, int(level), _ptr(slots), _ptr(pt), n_vec, int(t_plain), _stream(stream)))
+
+    def bgv_decode_level(self, level, pt, slots, n_vec, t_plain, stream=None):
+        self._chk(self._l.dpfhe_bgv_decode_level(self._h, int(level), _ptr(pt), _ptr(slots), n_vec, int(t_plain), _stream(stream)))
+
+    def bgv_encode_level_host(self, level, slots, pt, t_plain):
+        self._chk(self._l.dpfhe_bgv_encode_level_host(self._h, int(level), _ihptr(slots), _hptr(pt, True), slots.size // self.N, int(t_plain)))
+
+    def bgv_decode_level_host(self, level, pt, slots, t_plain):
+        self._chk(self._l.dpfhe_bgv_decode_level_host(self._h, int(level), _hptr(pt), _ihptr(slots, True), pt.size // (int(level) * self.N),
+                                                      int(t_plain)))
+
+    def encrypt_level(self, level, t_plain, sk, seed, first_index, pt, ct, n, stream=None):
+        self._chk(self._l.dpfhe_encrypt_level(self._h, int(level), int(t_plain), _ptr(sk), _seed(seed), int(first_index), _ptr(pt), _ptr(ct), n,
+                                              _stream(stream)))
+
+    def encrypt_level_host(self, level, t_plain, sk, seed, first_index, pt, ct):
+        self._chk(self._l.dpfhe_encrypt_level_host(self._h, int(level), int(t_plain), _hptr(sk), _seed(seed), int(first_index), _hptr(pt),
+                                                   _hptr(ct, True), pt.size // (int(level) * self.N)))
+
+    def encrypt_public_level(self, level, t_plain, pk, seed, first_index, pt, ct, n, stream=None):
+        self._chk(self._l.dpfhe_encrypt_public_level(self._h, int(level), int(t_plain), _ptr(pk), _seed(seed), int(first_index), _ptr(pt),
+                                                     _ptr(ct), n, _stream(stream)))
+
+    def encrypt_public_level_host(self, level, t_plain, pk, seed, first_index, pt, ct):
+        self._chk(self._l.dpfhe_encrypt_public_level_host(self._h, int(level), int(t_plain), _hptr(pk), _seed(seed), int(first_index), _hptr(pt),
+                                                          _hptr(ct, True), pt.size // (int(level) * self.N)))
+
+    def decrypt_level(self, level, sk, ct, n_comp, pt, n, stream=None):
+        self._chk(self._l.dpfhe_decrypt_level(self._h, int(level), _ptr(sk), _ptr(ct), int(n_comp), _ptr(pt), n, _stream(stream)))
+
+    def decrypt_level_host(self, level, sk, ct, n_comp, pt):
+        self._chk(self._l.dpfhe_decrypt_level_host(self._h, int(level), _hptr(sk), _hptr(ct), int(n_comp), _hptr(pt, True),
+                                                   pt.size // (int(level) * self.N)))
+
+    def ct_add_plain_level(self, level, ct, pt, out, batch, stream=None):
+        self._chk(self._l.dpfhe_ct_add_plain_level(self._h, int(level), _ptr(ct), _ptr(pt), _ptr(out), batch, _stream(stream)))
+
+    def ct_mul_plain_level(self, level, ct, pt, out, batch, stream=None):
+        self._chk(self._l.dpfhe_ct_mul_plain_level(self._h, int(level), _ptr(ct), _ptr(pt), _ptr(out), batch, _stream(stream)))
+
+    def ct_lincomb_level(self, level, cts, coeffs, constant, out, batch, stream=None):
+        n = len(cts)
+        if len(coeffs) != n:
+            raise ValueError("need one coefficient per ciphertext")
+        ptrs = (C.c_void_p * max(n, 1))(*[_ptr(c) for c in cts])
+        cs = (C.c_int64 * max(n, 1))(*[int(c) for c in coeffs])
+        self._chk(self._l.dpfhe_ct_lincomb_level(self._h, int(level), n, ptrs, cs, int(constant), _ptr(out), batch, _stream(stream)))
+
+    def mod_switch_down_level(self, level, polys, out, n_polys, t_plain=0, stream=None):
+        """[n_polys][level][N] -> [n_polys][level-1][N]"""
+        self._chk(self._l.dpfhe_mod_switch_down_level(self._h, int(level), _ptr(polys), _ptr(out), n_polys, int(t_plain), _stream(stream)))
+
     def galois_elt(self, k):
         """Galois element 5^k mod 2N of a rotation by k slots (k may be negative)."""
         return pow(5, k % (self.N // 2), 2 * self.N)
@@ -768,24 +839,37 @@ class PolyEval(_ContextObject):
 
     _prefix = "dpfhe_polyeval"
 
-    def __init__(self, ctx, n_special, t_plain, coeffs, relin_key):
+    def __init__(self, ctx, n_special, t_plain, coeffs, relin_key, level=None):
+        """level: the evaluator at that level of the chain (dpfhe_polyeval_create_grouped_level, DESIGN.md section 2.22) with the same
+        top-level key, ciphertexts [batch][2][level][N]; None: the top."""
         super().__init__(ctx, n_special)
         cs = np.ascontiguousarray([int(c) for c in coeffs], dtype=np.int64)
-        self._adopt(self._l.dpfhe_polyeval_create_grouped(ctx._h, self.n_special, int(t_plain), C.c_void_p(cs.ctypes.data), len(cs) - 1,
-                                                          _hptr(relin_key), C.byref(self._h)))
+        if level is None:
+            self._adopt(self._l.dpfhe_polyeval_create_grouped(ctx._h, self.n_special, int(t_plain), C.c_void_p(cs.ctypes.data), len(cs) - 1,
+                                                              _hptr(relin_key), C.byref(self._h)))
+        else:
+            self.Lq = int(level)
+            self._adopt(self._l.dpfhe_polyeval_create_grouped_level(ctx._h, self.n_special, self.Lq, int(t_plain), C.c_void_p(cs.ctypes.data),
+                                                                    len(cs) - 1, _hptr(relin_key), C.byref(self._h)))
 
     @classmethod
-    def ckks(cls, ctx, n_special, coeffs, scale_in, relin_key, scale_out=None):
+    def ckks(cls, ctx, n_special, coeffs, scale_in, relin_key, scale_out=None, level=None):
         """CKKS polynomial evaluation down the rescaling chain (dpfhe_polyeval_create_ckks, DESIGN.md section 2.16): slot-wise
         p(z) = sum_k coeffs[k] z^k with real coefficients, inputs at scale scale_in, the result at scale_out (default scale_in),
         which result_scale reports.  relin_key: the grouped key of the top level generated with t_plain = 0.  The result has
-        result_limbs = Lq - ceil(log2 d) - 1 limbs and decodes with ckks_decode at result_scale."""
+        result_limbs = Lq - ceil(log2 d) - 1 limbs and decodes with ckks_decode at result_scale.  level: as PolyEval's (Lq is then
+        the level)."""
         self = cls.__new__(cls)
         _ContextObject.__init__(self, ctx, n_special)
         cs = np.ascontiguousarray([float(c) for c in coeffs], dtype=np.float64)
         so = float(scale_in if scale_out is None else scale_out)
-        self._adopt(self._l.dpfhe_polyeval_create_ckks(ctx._h, self.n_special, C.c_void_p(cs.ctypes.data), len(cs) - 1, float(scale_in), so,
-                                                       _hptr(relin_key), C.byref(self._h)))
+        if level is None:
+            self._adopt(self._l.dpfhe_polyeval_create_ckks(ctx._h, self.n_special, C.c_void_p(cs.ctypes.data), len(cs) - 1, float(scale_in), so,
+                                                           _hptr(relin_key), C.byref(self._h)))
+        else:
+            self.Lq = int(level)
+            self._adopt(self._l.dpfhe_polyeval_create_ckks_level(ctx._h, self.n_special, self.Lq, C.c_void_p(cs.ctypes.data), len(cs) - 1,
+                                                                 float(scale_in), so, _hptr(relin_key), C.byref(self._h)))
         return self
 
     def _adopt(self, rc):

@@ -181,6 +181,46 @@ public:
                                const std::uint64_t *plain_eval, CiphertextBatch out, void *stream = nullptr) {
         check(dpfhe_encrypt_public(ctx_, plain_modulus, public_key, seed.data(), first_index, plain_eval, out.data, out.count, stream));
     }
+    // ---- the keyless calls at level `level` of the chain (DESIGN.md §2.22): bit for bit the call of the same name on an evaluator over
+    //      the first `level` limbs; plaintexts carry level * poly_degree() words, ciphertexts twice that.  The secret and the public key
+    //      are this evaluator's top-level ones.  1 <= level <= limbs().  Under special primes these encode, encrypt, decrypt and decode
+    //      the ciphertexts of every level on this one evaluator. ----
+    void encode_ckks(unsigned level, const std::complex<double> *slots, std::size_t count, double scale, std::uint64_t *plain_eval) {
+        check(dpfhe_ckks_encode_level_host(ctx_, level, reinterpret_cast<const double *>(slots), plain_eval, count, scale));
+    }
+    void decode_ckks(unsigned level, const std::uint64_t *plain_eval, std::size_t count, double scale, std::complex<double> *slots) {
+        check(dpfhe_ckks_decode_level_host(ctx_, level, plain_eval, reinterpret_cast<double *>(slots), count, scale));
+    }
+    void encode_bgv(unsigned level, const std::int64_t *slots, std::size_t count, std::uint64_t plain_modulus, std::uint64_t *plain_eval) {
+        check(dpfhe_bgv_encode_level_host(ctx_, level, slots, plain_eval, count, plain_modulus));
+    }
+    void decode_bgv(unsigned level, const std::uint64_t *plain_eval, std::size_t count, std::uint64_t plain_modulus, std::uint64_t *slots) {
+        check(dpfhe_bgv_decode_level_host(ctx_, level, plain_eval, slots, count, plain_modulus));
+    }
+    void encrypt(unsigned level, std::uint64_t plain_modulus, const std::uint64_t *secret, const Seed &seed, std::uint64_t first_index,
+                 const std::uint64_t *plain_eval, CiphertextBatch out) {
+        check(dpfhe_encrypt_level_host(ctx_, level, plain_modulus, secret, seed.data(), first_index, plain_eval, out.data, out.count));
+    }
+    void decrypt(unsigned level, const std::uint64_t *secret, ConstCiphertextBatch ct, std::uint64_t *plain_eval, unsigned n_comp = 2) {
+        check(dpfhe_decrypt_level_host(ctx_, level, secret, ct.data, n_comp, plain_eval, ct.count));
+    }
+    void encrypt_device(unsigned level, std::uint64_t plain_modulus, const std::uint64_t *secret, const Seed &seed, std::uint64_t first_index,
+                        const std::uint64_t *plain_eval, CiphertextBatch out, void *stream = nullptr) {
+        check(dpfhe_encrypt_level(ctx_, level, plain_modulus, secret, seed.data(), first_index, plain_eval, out.data, out.count, stream));
+    }
+    void decrypt_device(unsigned level, const std::uint64_t *secret, ConstCiphertextBatch ct, std::uint64_t *plain_eval, unsigned n_comp = 2,
+                        void *stream = nullptr) {
+        check(dpfhe_decrypt_level(ctx_, level, secret, ct.data, n_comp, plain_eval, ct.count, stream));
+    }
+    void encrypt_public(unsigned level, std::uint64_t plain_modulus, const std::uint64_t *public_key, const Seed &seed, std::uint64_t first_index,
+                        const std::uint64_t *plain_eval, CiphertextBatch out) {
+        check(dpfhe_encrypt_public_level_host(ctx_, level, plain_modulus, public_key, seed.data(), first_index, plain_eval, out.data, out.count));
+    }
+    void encrypt_public_device(unsigned level, std::uint64_t plain_modulus, const std::uint64_t *public_key, const Seed &seed,
+                               std::uint64_t first_index, const std::uint64_t *plain_eval, CiphertextBatch out, void *stream = nullptr) {
+        check(dpfhe_encrypt_public_level(ctx_, level, plain_modulus, public_key, seed.data(), first_index, plain_eval, out.data, out.count,
+                                         stream));
+    }
     std::vector<std::uint64_t> galois_elements(const std::vector<long> &steps) const {
         std::vector<std::uint64_t> elts;
         for (long k : steps) elts.push_back(galois_element(k));
@@ -400,6 +440,25 @@ public:
         if (cts.size() != coeffs.size()) throw std::runtime_error("one coefficient per ciphertext batch");
         check(dpfhe_ct_lincomb(ctx_, cts.size(), cts.data(), coeffs.data(), constant, out, count, stream));
     }
+    // the three calls above and mod_switch_to_next_device at level `level` (DESIGN.md §2.22): ciphertexts and plaintexts carry `level`
+    // limbs (mod_switch_to_next_device: out level-1); 1 <= level <= limbs()
+    void add_plain_device(unsigned level, const std::uint64_t *ct, const std::uint64_t *plain_eval, std::uint64_t *out, std::size_t count,
+                          void *stream = nullptr) {
+        check(dpfhe_ct_add_plain_level(ctx_, level, ct, plain_eval, out, count, stream));
+    }
+    void multiply_plain_device(unsigned level, const std::uint64_t *ct, const std::uint64_t *plain_eval, std::uint64_t *out, std::size_t count,
+                               void *stream = nullptr) {
+        check(dpfhe_ct_mul_plain_level(ctx_, level, ct, plain_eval, out, count, stream));
+    }
+    void lincomb_device(unsigned level, const std::vector<const std::uint64_t *> &cts, const std::vector<std::int64_t> &coeffs,
+                        std::int64_t constant, std::uint64_t *out, std::size_t count, void *stream = nullptr) {
+        if (cts.size() != coeffs.size()) throw std::runtime_error("one coefficient per ciphertext batch");
+        check(dpfhe_ct_lincomb_level(ctx_, level, cts.size(), cts.data(), coeffs.data(), constant, out, count, stream));
+    }
+    void mod_switch_to_next_device(unsigned level, const std::uint64_t *ct, std::uint64_t *out, std::size_t count, std::uint64_t plain_modulus = 0,
+                                   void *stream = nullptr) {
+        check(dpfhe_mod_switch_down_level(ctx_, level, ct, out, 2 * count, plain_modulus, stream));
+    }
     void multiply_plain_accumulate_device(const std::uint64_t *ct, const std::uint64_t *plain_eval, std::uint64_t *acc, std::size_t count,
                                           void *stream = nullptr) {
         check(dpfhe_ct_mul_plain_acc(ctx_, ct, plain_eval, acc, count, stream));
@@ -566,6 +625,13 @@ public:
         if (coeffs.size() < 2) throw std::runtime_error("a polynomial of degree at least 1");
         check(dpfhe_polyeval_create_grouped(ev.native_handle(), special, plain_modulus, coeffs.data(), coeffs.size() - 1, relin_key, &h_));
     }
+    // the evaluator at level `level` of the chain (DESIGN.md §2.22): inputs carry `level` limbs, the key is the top-level one
+    PolyEval(Evaluator &ev, unsigned special, unsigned level, std::uint64_t plain_modulus, const std::vector<std::int64_t> &coeffs,
+             const std::uint64_t *relin_key) {
+        if (coeffs.size() < 2) throw std::runtime_error("a polynomial of degree at least 1");
+        check(dpfhe_polyeval_create_grouped_level(ev.native_handle(), special, level, plain_modulus, coeffs.data(), coeffs.size() - 1, relin_key,
+                                                  &h_));
+    }
     unsigned result_limbs() const { return dpfhe_polyeval_result_limbs(h_); }
 };
 
@@ -606,6 +672,13 @@ public:
         if (coeffs.size() < 2) throw std::runtime_error("a polynomial of degree at least 1");
         check(dpfhe_polyeval_create_ckks(ev.native_handle(), special, coeffs.data(), coeffs.size() - 1, scale_in,
                                                     scale_out == 0 ? scale_in : scale_out, relin_key, &h_));
+    }
+    // the evaluator at level `level` of the chain (DESIGN.md §2.22): inputs carry `level` limbs, the key is the top-level one
+    CkksPolyEval(Evaluator &ev, unsigned special, unsigned level, const std::vector<double> &coeffs, double scale_in, const std::uint64_t *relin_key,
+                 double scale_out = 0) {
+        if (coeffs.size() < 2) throw std::runtime_error("a polynomial of degree at least 1");
+        check(dpfhe_polyeval_create_ckks_level(ev.native_handle(), special, level, coeffs.data(), coeffs.size() - 1, scale_in,
+                                               scale_out == 0 ? scale_in : scale_out, relin_key, &h_));
     }
     unsigned result_limbs() const { return dpfhe_polyeval_result_limbs(h_); }
     double result_scale() const { return dpfhe_polyeval_result_scale(h_); }

@@ -538,4 +538,8 @@ int dpfhe_describe(const dpfhe_ctx *ctx, char *buf, size_t buf_len);
 #ifdef __cplusplus
 }
 #endif
+
+/* the polynomial evaluators and the keyless calls at any level of the modulus chain (DESIGN.md §2.22) */
+#include "dpfhe_level.h"
+
 #endif /* DPFHE_H */
