@@ -194,6 +194,28 @@ LEVEL_SYMBOLS = {
                                                    C.POINTER(C.c_void_p)]),
 }
 
+# the entry points of include/dpfhe_seeded.h (DESIGN.md section 2.23), which dpfhe.h includes
+_V, _U, _U64, _SZ = C.c_void_p, C.c_uint, C.c_uint64, C.c_size_t
+SEEDED_SYMBOLS = {
+    "dpfhe_seeded_public_seed": (C.c_int, [_V, _V]),
+    "dpfhe_encrypt_seeded": (C.c_int, [_V, _U64, _V, _V, _U64, _V, _V, _SZ, _V]),
+    "dpfhe_encrypt_seeded_host": (C.c_int, [_V, _U64, _V, _V, _U64, _V, _V, _SZ]),
+    "dpfhe_encrypt_seeded_level": (C.c_int, [_V, _U, _U64, _V, _V, _U64, _V, _V, _SZ, _V]),
+    "dpfhe_encrypt_seeded_level_host": (C.c_int, [_V, _U, _U64, _V, _V, _U64, _V, _V, _SZ]),
+    "dpfhe_expand_ciphertexts": (C.c_int, [_V, _V, _U64, _V, _V, _SZ, _V]),
+    "dpfhe_expand_ciphertexts_level": (C.c_int, [_V, _U, _V, _U64, _V, _V, _SZ, _V]),
+    "dpfhe_upload_seeded_ciphertexts": (C.c_int, [_V, _V, _U64, _V, _V, _SZ]),
+    "dpfhe_upload_seeded_ciphertexts_level": (C.c_int, [_V, _U, _V, _U64, _V, _V, _SZ]),
+    "dpfhe_relin_keygen_seeded": (C.c_int, [_V, _U, _U64, _V, _V, _V, _V]),
+    "dpfhe_relin_keygen_seeded_host": (C.c_int, [_V, _U, _U64, _V, _V, _V]),
+    "dpfhe_galois_keygen_seeded": (C.c_int, [_V, _U, _U64, _V, _SZ, _V, _V, _V, _V]),
+    "dpfhe_galois_keygen_seeded_host": (C.c_int, [_V, _U, _U64, _V, _SZ, _V, _V, _V]),
+    "dpfhe_expand_switch_keys": (C.c_int, [_V, _U, _V, _SZ, _V, _V, _V, _V]),
+    "dpfhe_upload_seeded_switch_keys": (C.c_int, [_V, _U, _V, _SZ, _V, _V, _V]),
+    "dpfhe_expand_switch_keys_host": (C.c_int, [_V, _U, _V, _SZ, _V, _V, _V]),
+}
+
+
 class dpfhe_params(C.Structure):
     _fields_ = [("log_n", C.c_uint32), ("n_limbs", C.c_uint32), ("moduli", C.POINTER(C.c_uint64))]
 
@@ -210,8 +232,8 @@ def load():
     if not os.path.exists(path):
         _build.build()          # raises if nvcc is unavailable: no fallback
     lib = C.CDLL(path)
-    for name, (res, args) in list(SYMBOLS.items()) + list(LEVEL_SYMBOLS.items()):
-        fn = getattr(lib, name)   # AttributeError if the library does not export what include/dpfhe.h (with dpfhe_level.h) declares
+    for name, (res, args) in list(SYMBOLS.items()) + list(LEVEL_SYMBOLS.items()) + list(SEEDED_SYMBOLS.items()):
+        fn = getattr(lib, name)   # AttributeError if the library does not export what include/dpfhe.h (with its included headers) declares
         fn.restype = res
         fn.argtypes = args
     _lib = lib

@@ -18,7 +18,7 @@ UNITS = [("kernels.cu", "kernels_%s_%s" % (v, n), ["-DDPFHE_FAST=%d" % f, "-DDPF
 SOURCES = sorted({u[0] for u in UNITS})
 HEADERS = ["types.hpp", "modarith.cuh", "ntt_core.cuh", "kernel_bodies.cuh", "keys.cuh", "eval.cuh", "launch.hpp", "launch_util.hpp", "host_params.hpp", "ctx.hpp",
            os.path.join("..", "..", "include", "dpfhe.h"),
-           os.path.join("..", "..", "include", "dpfhe_level.h")]
+           os.path.join("..", "..", "include", "dpfhe_level.h"), os.path.join("..", "..", "include", "dpfhe_seeded.h")]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + [
     "-std=c++17", "-O3", "-lineinfo",

@@ -21,6 +21,7 @@
 #include "../../include/dpfhe.h"
 #include "ctx.hpp"
 #include "eval.cuh"
+#include "keys.cuh"
 
 using namespace dpfhe;
 
@@ -108,14 +109,47 @@ int DeviceScratch::reserve(dpfhe_ctx *ctx, size_t bytes) {
 
 namespace {
 
+// A device-resident output of the pipeline (dpfhe_seeded.h's uploads): every item of the input is rows of `row_words` words, which
+// are copied straight into the output's items (out_item_words each), one row every 2 * row_words words: the c0 / b rows of
+// [..][2][L][N] items.  The chunk's compute then runs in place on its items of d, and nothing is staged or downloaded.
+struct DeviceOut {
+    u64 *d = nullptr;
+    size_t row_words = 0;
+};
+
 // Generic three-stage pipeline over `n_items` items split into chunks:
 //   upload(chunk -> stage_in[slot]) on s_h2d, compute on ctx->stream, download(stage_out[slot]) on s_d2h.
 // in_item_bytes / out_item_bytes are per item; h_in may be two arrays (a and b) laid out back to back in the stage.
 // n_slices > 1: each input is n_slices arrays of n_items items, slice_stride words apart (the operands of an inner product,
 // [n_terms][batch] ciphertexts); a chunk stages its items of every slice, [input][slice][chunk_items], slice after slice.
+// dev.d: a device-resident output (DeviceOut): upload(chunk -> its items of dev.d) on s_h2d, compute in place on ctx->stream.
 template <class Compute>
 int run_pipeline_body(dpfhe_ctx *ctx, const u64 *h_in0, const u64 *h_in1, u64 *h_out, size_t n_items, size_t in_item_words,
-                      size_t out_item_words, size_t chunk_items, Compute compute, size_t n_slices, size_t slice_stride) {
+                      size_t out_item_words, size_t chunk_items, Compute compute, size_t n_slices, size_t slice_stride, DeviceOut dev) {
+    if (dev.d) {
+        // the output is the caller's memory: the first copy waits for the context's previous call (whatever stream it ran on) and for
+        // the work issued before this call on the legacy default stream, which the non-blocking s_h2d does not wait for by itself
+        if (ctx->have_last) CU_TRY(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_last, 0));
+        CU_TRY(cudaEventRecord(ctx->ev_h2d[0], cudaStreamLegacy));
+        CU_TRY(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_h2d[0], 0));
+        // each chunk's copy is recorded in its slot's event and waited on by the compute stream at once (a wait takes the event's
+        // state when it is issued), so a slot's event can be recorded again for a later chunk; no staging buffer is used
+        const size_t row = dev.row_words, rows_per_item = in_item_words / row;
+        size_t k = 0;
+        for (size_t first = 0; first < n_items; first += chunk_items, ++k) {
+            const size_t cnt = n_items - first < chunk_items ? n_items - first : chunk_items;
+            const int slot = (int)(k % PIPE_DEPTH);
+            u64 *dout = dev.d + first * out_item_words;
+            CU_TRY(cudaMemcpy2DAsync(dout, 2 * row * 8, h_in0 + first * in_item_words, row * 8, row * 8, cnt * rows_per_item,
+                                     cudaMemcpyHostToDevice, ctx->s_h2d));
+            CU_TRY(cudaEventRecord(ctx->ev_h2d[slot], ctx->s_h2d));
+            CU_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ev_h2d[slot], 0));
+            const int rc = compute(dout, nullptr, dout, cnt, ctx->stream);
+            if (rc) return rc;
+        }
+        CU_TRY(cudaStreamSynchronize(ctx->stream));
+        return DPFHE_OK;
+    }
     const size_t n_in = (h_in1 ? 2 : 1) * n_slices;
     int rc = DPFHE_OK;
     for (int k = 0; k < PIPE_DEPTH && !rc; ++k) rc = ctx->stage_in[k].reserve(ctx, n_in * chunk_items * in_item_words * 8);
@@ -151,8 +185,9 @@ int run_pipeline_body(dpfhe_ctx *ctx, const u64 *h_in0, const u64 *h_in1, u64 *h
 // the caller's host buffers (or the staging slots) when the error is reported
 template <class Compute>
 int run_pipeline(dpfhe_ctx *ctx, const u64 *h_in0, const u64 *h_in1, u64 *h_out, size_t n_items, size_t in_item_words,
-                 size_t out_item_words, size_t chunk_items, Compute compute, size_t n_slices = 1, size_t slice_stride = 0) {
-    const int rc = run_pipeline_body(ctx, h_in0, h_in1, h_out, n_items, in_item_words, out_item_words, chunk_items, compute, n_slices, slice_stride);
+                 size_t out_item_words, size_t chunk_items, Compute compute, size_t n_slices = 1, size_t slice_stride = 0, DeviceOut dev = {}) {
+    const int rc = run_pipeline_body(ctx, h_in0, h_in1, h_out, n_items, in_item_words, out_item_words, chunk_items, compute, n_slices, slice_stride,
+                                     dev);
     if (rc != DPFHE_OK) {
         const std::string why = g_err;   // the drains below must not replace the message of the failure
         cudaStreamSynchronize(ctx->s_h2d);
@@ -187,9 +222,11 @@ int no_check() { return DPFHE_OK; }
 // The host-buffer form of an entry point: the host pointers `ptrs` must not be null, then `check()` runs the call's remaining
 // argument checks.  The operand every item shares (a key, a plaintext or a secret of `shared_words` words; none when
 // shared_words is 0) is uploaded once into the key staging buffer, and the items are pipelined through `compute` in chunks.
+// dev.d: the output is that device buffer instead of h_out (DeviceOut).
 template <class Compute, class Check = int (*)()>
 int host_call(dpfhe_ctx *ctx, std::initializer_list<const void *> ptrs, const uint64_t *h_shared, size_t shared_words, const u64 *h_in0,
-              const u64 *h_in1, u64 *h_out, size_t n_items, size_t in_item_words, size_t out_item_words, Compute compute, Check check = no_check) {
+              const u64 *h_in1, u64 *h_out, size_t n_items, size_t in_item_words, size_t out_item_words, Compute compute, Check check = no_check,
+              DeviceOut dev = {}) {
     for (const void *p : ptrs)
         if (!p) return fail(DPFHE_ERR_INVALID, "null host pointer");
     int rc = check();
@@ -199,7 +236,7 @@ int host_call(dpfhe_ctx *ctx, std::initializer_list<const void *> ptrs, const ui
         if (rc) return rc;
     }
     const size_t chunk = pick_chunk(ctx, std::max(in_item_words, out_item_words) * 8, n_items);
-    return run_pipeline(ctx, h_in0, h_in1, h_out, n_items, in_item_words, out_item_words, chunk, compute);
+    return run_pipeline(ctx, h_in0, h_in1, h_out, n_items, in_item_words, out_item_words, chunk, compute, 1, 0, dev);
 }
 
 int check_galois(const dpfhe_ctx *ctx, uint64_t galois) {
@@ -2281,6 +2318,321 @@ int dpfhe_mod_switch_down_level(dpfhe_ctx *ctx, unsigned level, const uint64_t *
                                 void *stream) {
     return prefix_call(ctx, level, [&] { return mod_switch_down_at(ctx, level, d_in, d_out, n_polys, t_plain, stream); });
 }
+// ---------------------------------------------------------------- seeded ciphertexts and switch keys (DESIGN.md §2.23)
+
+static void seed_words(const uint8_t b[32], u32 w[8]) {
+    for (int i = 0; i < 8; ++i) w[i] = (u32)b[4 * i] | (u32)b[4 * i + 1] << 8 | (u32)b[4 * i + 2] << 16 | (u32)b[4 * i + 3] << 24;
+}
+
+// a_seed of the key owner's seed: words 0..7 of its ChaCha20 block at counter 0, nonce (KD_PUBLIC_SEED, 0, 0)
+static void public_seed_words(const uint8_t seed[32], u32 a_seed[8]) {
+    u32 key[8], w[16];
+    seed_words(seed, key);
+    gen::chacha20_block(key, 0, key_nonce0(KD_PUBLIC_SEED, 0, 0, 0), 0, 0, w);
+    for (int i = 0; i < 8; ++i) a_seed[i] = w[i];
+}
+
+int dpfhe_seeded_public_seed(const uint8_t seed[32], uint8_t a_seed[32]) {
+    if (!seed || !a_seed) return fail(DPFHE_ERR_INVALID, "null seed");
+    u32 w[8];
+    public_seed_words(seed, w);
+    for (int i = 0; i < 32; ++i) a_seed[i] = (uint8_t)(w[i / 4] >> (8 * (i % 4)));
+    return DPFHE_OK;
+}
+
+// the key arguments of a seeded launch: build_key_args' with the public seed a_seed (words) of the `a` rows
+static SeededKeyArgs seeded_args(const HostParams &hp, const uint8_t seed[32], unsigned K, uint64_t t_plain, const u32 a_seed[8]) {
+    SeededKeyArgs A;
+    static_cast<KeyArgs &>(A) = build_key_args(hp, seed, K, t_plain);
+    for (int i = 0; i < 8; ++i) A.a_seed[i] = a_seed[i];
+    return A;
+}
+
+// the key arguments of an expansion over the first L limbs: only a_seed, K, ndig and the uniform reduction's constants are read
+static SeededKeyArgs expand_args(const HostParams &hp, const uint8_t a_seed[32], unsigned K) {
+    u32 w[8];
+    seed_words(a_seed, w);
+    return seeded_args(hp, a_seed, K, 0, w);
+}
+
+static int encrypt_seeded_at(dpfhe_ctx *ctx, unsigned L, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32], uint64_t first_index,
+                             const uint64_t *d_pt, uint64_t *d_c0, size_t n, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    if (n == 0) return DPFHE_OK;
+    CHECK_PTR(d_sk); CHECK_PTR(d_pt); CHECK_PTR(d_c0);
+    const size_t P = L * ctx->N();
+    if (overlaps(d_c0, n * P * 8, d_pt, n * P * 8) || overlaps(d_c0, n * P * 8, d_sk, P * 8))
+        return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+    const HostParams *hp = prefix_params(ctx, L);
+    if (!hp) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    u32 a_seed[8];
+    public_seed_words(seed, a_seed);
+    SeededKeyArgs A = seeded_args(*hp, seed, 0, t_plain, a_seed);
+    A.s = d_sk;
+    A.pt = d_pt;
+    A.out = d_c0;
+    A.item0 = first_index;
+    CU_TRY(VCALL(launch_keys, level_view(ctx, L), KM_ENC_SEEDED, A, n, pick(ctx, stream)));
+    note_launch(ctx, 1);
+    return DPFHE_OK;
+}
+
+static int encrypt_seeded_host_at(dpfhe_ctx *ctx, unsigned L, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t first_index,
+                                  const uint64_t *h_pt, uint64_t *h_c0, size_t n) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    if (n == 0) return DPFHE_OK;
+    const size_t P = L * ctx->N();
+    uint64_t next = first_index;   // as dpfhe_encrypt_host: ciphertext k keeps item number first_index + k across chunks
+    return host_call(ctx, {h_sk, h_pt, h_c0}, h_sk, P, h_pt, nullptr, h_c0, n, P, P,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         const int r = encrypt_seeded_at(ctx, L, t_plain, ctx->stage_key.get(), seed, next, din, dout, cnt, st);
+                         next += cnt;
+                         return r;
+                     });
+}
+
+static int expand_ciphertexts_at(dpfhe_ctx *ctx, unsigned L, const uint8_t a_seed[32], uint64_t first_index, const uint64_t *d_c0, uint64_t *d_ct,
+                                 size_t n, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(a_seed);
+    if (n == 0) return DPFHE_OK;
+    CHECK_PTR(d_c0); CHECK_PTR(d_ct);
+    const size_t P = L * ctx->N();
+    if (overlaps(d_ct, n * 2 * P * 8, d_c0, n * P * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+    const HostParams *hp = prefix_params(ctx, L);
+    if (!hp) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    SeededKeyArgs A = expand_args(*hp, a_seed, 0);
+    A.item0 = first_index;
+    CU_TRY(VCALL(launch_expand_seeded, level_view(ctx, L), false, A, d_c0, d_ct, n, pick(ctx, stream)));
+    note_launch(ctx, 1);
+    return DPFHE_OK;
+}
+
+// host c0 rows straight into d_ct's c0 rows, chunk by chunk, each chunk's c1 rows expanded in place behind its copy
+static int upload_seeded_ciphertexts_at(dpfhe_ctx *ctx, unsigned L, const uint8_t a_seed[32], uint64_t first_index, const uint64_t *h_c0,
+                                        uint64_t *d_ct, size_t n) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(a_seed);
+    if (n == 0) return DPFHE_OK;
+    CHECK_PTR(d_ct);
+    const HostParams *hp = prefix_params(ctx, L);
+    if (!hp) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+    const size_t P = L * ctx->N();
+    SeededKeyArgs A = expand_args(*hp, a_seed, 0);
+    A.item0 = first_index;
+    const LaunchCtx lc = level_view(ctx, L);
+    return host_call(ctx, {h_c0}, nullptr, 0, h_c0, nullptr, nullptr, n, P, 2 * P,
+                     [&](u64 *, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                         CU_TRY(VCALL(launch_expand_seeded, lc, false, A, nullptr, dout, cnt, pick(ctx, st)));
+                         A.item0 += cnt;
+                         note_launch(ctx, 1);
+                         return DPFHE_OK;
+                     }, no_check, DeviceOut{d_ct, P});
+}
+
+int dpfhe_encrypt_seeded(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32], uint64_t first_index, const uint64_t *d_pt,
+                         uint64_t *d_c0, size_t n, void *stream) {
+    return encrypt_seeded_at(ctx, ctx ? ctx->hp.L : 0, t_plain, d_sk, seed, first_index, d_pt, d_c0, n, stream);
+}
+int dpfhe_encrypt_seeded_host(dpfhe_ctx *ctx, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32], uint64_t first_index,
+                              const uint64_t *h_pt, uint64_t *h_c0, size_t n) {
+    return encrypt_seeded_host_at(ctx, ctx ? ctx->hp.L : 0, t_plain, h_sk, seed, first_index, h_pt, h_c0, n);
+}
+int dpfhe_encrypt_seeded_level(dpfhe_ctx *ctx, unsigned level, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32],
+                               uint64_t first_index, const uint64_t *d_pt, uint64_t *d_c0, size_t n, void *stream) {
+    return prefix_call(ctx, level, [&] { return encrypt_seeded_at(ctx, level, t_plain, d_sk, seed, first_index, d_pt, d_c0, n, stream); });
+}
+int dpfhe_encrypt_seeded_level_host(dpfhe_ctx *ctx, unsigned level, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32],
+                                    uint64_t first_index, const uint64_t *h_pt, uint64_t *h_c0, size_t n) {
+    return prefix_call(ctx, level, [&] { return encrypt_seeded_host_at(ctx, level, t_plain, h_sk, seed, first_index, h_pt, h_c0, n); });
+}
+int dpfhe_expand_ciphertexts(dpfhe_ctx *ctx, const uint8_t a_seed[32], uint64_t first_index, const uint64_t *d_c0, uint64_t *d_ct, size_t n,
+                             void *stream) {
+    return expand_ciphertexts_at(ctx, ctx ? ctx->hp.L : 0, a_seed, first_index, d_c0, d_ct, n, stream);
+}
+int dpfhe_expand_ciphertexts_level(dpfhe_ctx *ctx, unsigned level, const uint8_t a_seed[32], uint64_t first_index, const uint64_t *d_c0,
+                                   uint64_t *d_ct, size_t n, void *stream) {
+    return prefix_call(ctx, level, [&] { return expand_ciphertexts_at(ctx, level, a_seed, first_index, d_c0, d_ct, n, stream); });
+}
+int dpfhe_upload_seeded_ciphertexts(dpfhe_ctx *ctx, const uint8_t a_seed[32], uint64_t first_index, const uint64_t *h_c0, uint64_t *d_ct,
+                                    size_t n) {
+    return upload_seeded_ciphertexts_at(ctx, ctx ? ctx->hp.L : 0, a_seed, first_index, h_c0, d_ct, n);
+}
+int dpfhe_upload_seeded_ciphertexts_level(dpfhe_ctx *ctx, unsigned level, const uint8_t a_seed[32], uint64_t first_index,
+                                          const uint64_t *h_c0, uint64_t *d_ct, size_t n) {
+    return prefix_call(ctx, level, [&] { return upload_seeded_ciphertexts_at(ctx, level, a_seed, first_index, h_c0, d_ct, n); });
+}
+
+// seeded relinearisation key (galois_elts = nullptr, n_elts = 1) or Galois keys: the b rows [n_elts][dnum][L][N]
+static int switch_keygen_seeded(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *d_sk, size_t n_elts,
+                                const uint64_t *galois_elts, const uint8_t seed[32], uint64_t *d_b, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    rc = check_key_special(ctx, n_special);
+    if (rc) return rc;
+    if (n_elts == 0) return DPFHE_OK;
+    for (size_t e = 0; galois_elts && e < n_elts; ++e) {
+        rc = check_galois(ctx, galois_elts[e]);
+        if (rc) return rc;
+    }
+    CHECK_PTR(d_sk); CHECK_PTR(d_b);
+    u32 a_seed[8];
+    public_seed_words(seed, a_seed);
+    SeededKeyArgs A = seeded_args(ctx->hp, seed, n_special, t_plain, a_seed);
+    A.s = d_sk;
+    const size_t key_words = (size_t)A.ndig * ctx->P();
+    if (overlaps(d_b, n_elts * key_words * 8, d_sk, ctx->P() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the secret");
+    cudaStream_t st = pick(ctx, stream);
+    uint64_t launches = 0;
+    for (size_t e0 = 0; e0 < n_elts; e0 += KEYS_MAX_ELTS) {
+        const size_t cnt = std::min<size_t>(KEYS_MAX_ELTS, n_elts - e0);
+        for (size_t e = 0; galois_elts && e < cnt; ++e) A.galois[e] = galois_elts[e0 + e];
+        A.out = d_b + e0 * key_words;
+        CU_TRY(VCALL(launch_keys, ctx->lc, galois_elts ? KM_GALOIS_SEEDED : KM_RELIN_SEEDED, A, cnt * A.ndig, st));
+        ++launches;
+    }
+    note_launch(ctx, launches);
+    return DPFHE_OK;
+}
+
+int dpfhe_relin_keygen_seeded(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *d_sk, const uint8_t seed[32], uint64_t *d_b,
+                              void *stream) {
+    return switch_keygen_seeded(ctx, n_special, t_plain, d_sk, 1, nullptr, seed, d_b, stream);
+}
+int dpfhe_galois_keygen_seeded(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *d_sk, size_t n_elts,
+                               const uint64_t *galois_elts, const uint8_t seed[32], uint64_t *d_b, void *stream) {
+    if (ctx && n_elts && !galois_elts) return fail(DPFHE_ERR_INVALID, "null galois_elts");
+    return switch_keygen_seeded(ctx, n_special, t_plain, d_sk, n_elts, galois_elts, seed, d_b, stream);
+}
+int dpfhe_relin_keygen_seeded_host(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *h_sk, const uint8_t seed[32],
+                                   uint64_t *h_b) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    rc = check_key_special(ctx, n_special);
+    if (rc) return rc;
+    if (!h_sk) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const KeygenHostArgs args{n_special, t_plain, seed, 0, nullptr};
+    return keygen_host(ctx, h_sk, key_digits(ctx, n_special) * ctx->P(), h_b,
+                       [](dpfhe_ctx *c, const uint64_t *sk, uint64_t *out, const void *a) {
+                           const KeygenHostArgs &k = *(const KeygenHostArgs *)a;
+                           return dpfhe_relin_keygen_seeded(c, k.n_special, k.t_plain, sk, k.seed, out, nullptr);
+                       }, &args);
+}
+int dpfhe_galois_keygen_seeded_host(dpfhe_ctx *ctx, unsigned n_special, uint64_t t_plain, const uint64_t *h_sk, size_t n_elts,
+                                    const uint64_t *galois_elts, const uint8_t seed[32], uint64_t *h_b) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(seed);
+    rc = check_key_special(ctx, n_special);
+    if (rc) return rc;
+    if (n_elts == 0) return DPFHE_OK;
+    if (!galois_elts) return fail(DPFHE_ERR_INVALID, "null galois_elts");
+    for (size_t e = 0; e < n_elts; ++e) {
+        rc = check_galois(ctx, galois_elts[e]);
+        if (rc) return rc;
+    }
+    if (!h_sk) return fail(DPFHE_ERR_INVALID, "null host pointer");
+    const KeygenHostArgs args{n_special, t_plain, seed, n_elts, galois_elts};
+    return keygen_host(ctx, h_sk, n_elts * key_digits(ctx, n_special) * ctx->P(), h_b,
+                       [](dpfhe_ctx *c, const uint64_t *sk, uint64_t *out, const void *a) {
+                           const KeygenHostArgs &k = *(const KeygenHostArgs *)a;
+                           return dpfhe_galois_keygen_seeded(c, k.n_special, k.t_plain, sk, k.n_elts, k.galois_elts, k.seed, out, nullptr);
+                       }, &args);
+}
+
+// the checks every expansion of switch keys makes before its first copy or launch: K and the item numbers
+static int check_key_items(const dpfhe_ctx *ctx, unsigned n_special, size_t n_keys, const uint64_t *items) {
+    int rc = check_key_special(ctx, n_special);
+    if (rc) return rc;
+    if (n_keys && !items) return fail(DPFHE_ERR_INVALID, "null items");
+    for (size_t e = 0; e < n_keys; ++e)
+        if (items[e] && (rc = check_galois(ctx, items[e]))) return rc;
+    return DPFHE_OK;
+}
+
+// n_keys seeded keys' b rows (src, [n_keys][dnum][L][N]; nullptr: already in place in dst) -> dst [n_keys][dnum][2][L][N], one launch per
+// KEYS_MAX_ELTS keys; returns the launches
+static cudaError_t launch_expand_keys(dpfhe_ctx *ctx, SeededKeyArgs &A, size_t n_keys, const uint64_t *items, const u64 *src, u64 *dst, cudaStream_t st,
+                                      uint64_t &launches) {
+    const size_t key_words = (size_t)A.ndig * ctx->P();
+    for (size_t e0 = 0; e0 < n_keys; e0 += KEYS_MAX_ELTS) {
+        const size_t cnt = std::min<size_t>(KEYS_MAX_ELTS, n_keys - e0);
+        for (size_t e = 0; e < cnt; ++e) A.galois[e] = items[e0 + e];
+        const cudaError_t err = VCALL(launch_expand_seeded, ctx->lc, true, A, src ? src + e0 * key_words : nullptr, dst + e0 * 2 * key_words,
+                                      cnt * A.ndig, st);
+        if (err != cudaSuccess) return err;
+        ++launches;
+    }
+    return cudaSuccess;
+}
+
+int dpfhe_expand_switch_keys(dpfhe_ctx *ctx, unsigned n_special, const uint8_t a_seed[32], size_t n_keys, const uint64_t *items,
+                             const uint64_t *d_b, uint64_t *d_keys, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(a_seed);
+    rc = check_key_items(ctx, n_special, n_keys, items);
+    if (rc || n_keys == 0) return rc;
+    CHECK_PTR(d_b); CHECK_PTR(d_keys);
+    const size_t key_words = key_digits(ctx, n_special) * ctx->P();
+    if (overlaps(d_keys, n_keys * 2 * key_words * 8, d_b, n_keys * key_words * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+    SeededKeyArgs A = expand_args(ctx->hp, a_seed, n_special);
+    uint64_t launches = 0;
+    CU_TRY(launch_expand_keys(ctx, A, n_keys, items, d_b, d_keys, pick(ctx, stream), launches));
+    note_launch(ctx, launches);
+    return DPFHE_OK;
+}
+
+int dpfhe_upload_seeded_switch_keys(dpfhe_ctx *ctx, unsigned n_special, const uint8_t a_seed[32], size_t n_keys, const uint64_t *items,
+                                    const uint64_t *h_b, uint64_t *d_keys) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(a_seed);
+    rc = check_key_items(ctx, n_special, n_keys, items);
+    if (rc || n_keys == 0) return rc;
+    CHECK_PTR(d_keys);
+    const size_t key_words = key_digits(ctx, n_special) * ctx->P();
+    SeededKeyArgs A = expand_args(ctx->hp, a_seed, n_special);
+    size_t next = 0;
+    return host_call(ctx, {h_b}, nullptr, 0, h_b, nullptr, nullptr, n_keys, key_words, 2 * key_words,
+                     [&](u64 *, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                         uint64_t launches = 0;
+                         CU_TRY(launch_expand_keys(ctx, A, cnt, items + next, nullptr, dout, pick(ctx, st), launches));
+                         note_launch(ctx, launches);
+                         next += cnt;
+                         return DPFHE_OK;
+                     }, no_check, DeviceOut{d_keys, ctx->P()});
+}
+
+int dpfhe_expand_switch_keys_host(dpfhe_ctx *ctx, unsigned n_special, const uint8_t a_seed[32], size_t n_keys, const uint64_t *items,
+                                  const uint64_t *h_b, uint64_t *h_keys) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CHECK_SEED(a_seed);
+    rc = check_key_items(ctx, n_special, n_keys, items);
+    if (rc || n_keys == 0) return rc;
+    const size_t key_words = key_digits(ctx, n_special) * ctx->P();
+    if (overlaps(h_keys, n_keys * 2 * key_words * 8, h_b, n_keys * key_words * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+    SeededKeyArgs A = expand_args(ctx->hp, a_seed, n_special);
+    size_t next = 0;
+    return host_call(ctx, {h_b, h_keys}, nullptr, 0, h_b, nullptr, h_keys, n_keys, key_words, 2 * key_words,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) -> int {
+                         uint64_t launches = 0;
+                         CU_TRY(launch_expand_keys(ctx, A, cnt, items + next, din, dout, pick(ctx, st), launches));
+                         note_launch(ctx, launches);
+                         next += cnt;
+                         return DPFHE_OK;
+                     });
+}
+
 #undef CHECK_SEED
 
 // waits for everything this context has in flight, whatever stream it was issued on

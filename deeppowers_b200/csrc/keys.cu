@@ -4,6 +4,8 @@
 // compilation unit: no kernel of kernels.cu shares a body with these.
 #include <cuda_runtime.h>
 
+#include <type_traits>
+
 #include "keys.cuh"
 #include "launch_util.hpp"
 
@@ -61,6 +63,35 @@ __global__ void __launch_bounds__(NT, MINB) keys_ntt_pair_kernel(const __grid_co
     else keys_half_body<NT, MODE>(cta, buf, small, A, tw + (size_t)l * N, lt.lp[l], l, L, w / L, h);
 }
 
+// the seeded modes (DESIGN.md §2.23) of keys_ntt_kernel and keys_ntt_pair_kernel: kernels of their own, whose parameter block carries
+// the public seed after the KeyArgs, so that the unseeded instances keep theirs
+template <int LOGN, int NT, int MINB, int MODE>
+__global__ void __launch_bounds__(NT, MINB) keys_seeded_ntt_kernel(const __grid_constant__ SeededKeyArgs A, const Twiddle *__restrict__ tw,
+                                                                   const __grid_constant__ LimbTable lt, u32 L) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    constexpr size_t N = (size_t)1 << LOGN;
+    u64 *buf = reinterpret_cast<u64 *>(smem_raw);
+    signed char *small = reinterpret_cast<signed char *>(smem_raw + N * 8);
+    KeyCta<NT> cta;
+    const size_t w = blockIdx.x;
+    const u32 l = (u32)(w % L);
+    keys_limb_body<LOGN, NT, MODE>(cta, buf, small, A, tw + (size_t)l * N, lt.lp[l], l, L, w / L);
+}
+
+template <int NT, int MINB, int MODE>
+__global__ void __launch_bounds__(NT, MINB) keys_seeded_ntt_pair_kernel(const __grid_constant__ SeededKeyArgs A, const Twiddle *__restrict__ tw,
+                                                                        const __grid_constant__ LimbTable lt, u32 L) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    constexpr size_t N = (size_t)1 << NTT_PAIR_LOGN;
+    u64 *buf = reinterpret_cast<u64 *>(smem_raw);
+    signed char *small = reinterpret_cast<signed char *>(smem_raw + N * 4);
+    KeyCta<NT> cta;
+    const size_t w = blockIdx.x / 2;
+    const int h = (int)(blockIdx.x & 1);
+    const u32 l = (u32)(w % L);
+    keys_half_body<NT, MODE>(cta, buf, small, A, tw + (size_t)l * N, lt.lp[l], l, L, w / L, h);
+}
+
 // pt [n][L][N] = c0 + c1 s (+ c2 s^2), ct [n][n_comp][L][N], s [L][N]
 template <int LOGN>
 __global__ void __launch_bounds__(256) decrypt_kernel(const U64x2 *__restrict__ ct, const U64x2 *__restrict__ s, U64x2 *__restrict__ pt,
@@ -73,27 +104,39 @@ __global__ void __launch_bounds__(256) decrypt_kernel(const U64x2 *__restrict__ 
     }
 }
 
+// seeded rows [n][L][N] (src; nullptr: already in place in dst) -> [n][2][L][N] (dst): one ChaCha20 block per thread
+template <int LOGN, bool KEYS>
+__global__ void __launch_bounds__(256) expand_seeded_kernel(const __grid_constant__ SeededKeyArgs A, const U64x2 *__restrict__ src, U64x2 *__restrict__ dst,
+                                                            const __grid_constant__ LimbTable lt, u32 L, size_t n_blocks) {
+    for (size_t w = (size_t)blockIdx.x * blockDim.x + threadIdx.x; w < n_blocks; w += (size_t)gridDim.x * blockDim.x)
+        expand_block<LOGN, KEYS>(src, dst, A, lt.lp[(w >> (LOGN - 2)) % L], L, w);
+}
+
 namespace {
 
 template <int LOGN, int MODE>
-cudaError_t launch_keys_mode(const LaunchCtx &lc, const KeyArgs &A, size_t n_items, cudaStream_t st) {
+cudaError_t launch_keys_mode(const LaunchCtx &lc, const KeyArgs &A_, size_t n_items, cudaStream_t st) {
     constexpr size_t N = (size_t)1 << LOGN;
+    constexpr bool SEEDED = key_mode_seeded(MODE);
+    using Args = std::conditional_t<SEEDED, SeededKeyArgs, KeyArgs>;
+    const Args &A = static_cast<const Args &>(A_);   // a seeded mode is launched with SeededKeyArgs
     const size_t n_limbs = n_items * lc.L;
     static ConfiguredMask conf;
+    auto launch = [&](auto k, size_t grid, size_t smem) {
+        cudaError_t e = set_smem_once(conf, lc.device, smem, k);
+        if (e != cudaSuccess) return e;
+        k<<<(unsigned)grid, 256, smem, st>>>(A, lc.tw, lc.lt, lc.L);
+        return cudaGetLastError();
+    };
+    // half a limb + the small row per CTA of a pair at N = 16384, else the limb + the small row.  At 3 CTAs per SM (80 registers)
+    // the generic variant's store stage spills: 2 per SM
     if constexpr (LOGN == NTT_PAIR_LOGN) {
-        auto k = keys_ntt_pair_kernel<256, 2, MODE>;
-        const size_t smem = N * 4 + N;   // half a limb + the small row
-        cudaError_t e = set_smem_once(conf, lc.device, smem, k);
-        if (e != cudaSuccess) return e;
-        k<<<(unsigned)(2 * n_limbs), 256, smem, st>>>(A, lc.tw, lc.lt, lc.L);
+        if constexpr (SEEDED) return launch(keys_seeded_ntt_pair_kernel<256, 2, MODE>, 2 * n_limbs, N * 4 + N);
+        else return launch(keys_ntt_pair_kernel<256, 2, MODE>, 2 * n_limbs, N * 4 + N);
     } else {
-        auto k = keys_ntt_kernel<LOGN, 256, 2, MODE>;   // at 3 CTAs per SM (80 registers) the generic variant's store stage spills
-        const size_t smem = N * 8 + N;
-        cudaError_t e = set_smem_once(conf, lc.device, smem, k);
-        if (e != cudaSuccess) return e;
-        k<<<(unsigned)n_limbs, 256, smem, st>>>(A, lc.tw, lc.lt, lc.L);
+        if constexpr (SEEDED) return launch(keys_seeded_ntt_kernel<LOGN, 256, 2, MODE>, n_limbs, N * 8 + N);
+        else return launch(keys_ntt_kernel<LOGN, 256, 2, MODE>, n_limbs, N * 8 + N);
     }
-    return cudaGetLastError();
 }
 
 template <int LOGN>
@@ -105,17 +148,35 @@ cudaError_t launch_keys_n(const LaunchCtx &lc, int mode, const KeyArgs &A, size_
         case KM_GALOIS: return launch_keys_mode<LOGN, KM_GALOIS>(lc, A, n_items, st);
         case KM_PUBLIC_KEY: return launch_keys_mode<LOGN, KM_PUBLIC_KEY>(lc, A, n_items, st);
         case KM_ENC_PUBLIC: return launch_keys_mode<LOGN, KM_ENC_PUBLIC>(lc, A, n_items, st);
+        case KM_ENC_SEEDED: return launch_keys_mode<LOGN, KM_ENC_SEEDED>(lc, A, n_items, st);
+        case KM_RELIN_SEEDED: return launch_keys_mode<LOGN, KM_RELIN_SEEDED>(lc, A, n_items, st);
+        case KM_GALOIS_SEEDED: return launch_keys_mode<LOGN, KM_GALOIS_SEEDED>(lc, A, n_items, st);
     }
     return cudaErrorInvalidValue;
 }
 
 }  // namespace
 
-// n_items: 1 (secret, public key), ciphertexts (encryption, public-key encryption), n_elts * ndig (switch keys); one launch
+// n_items: 1 (secret, public key), ciphertexts (encryption, public-key encryption), n_elts * ndig (switch keys); one launch.  A seeded
+// mode's A is a SeededKeyArgs.
 cudaError_t launch_keys(const LaunchCtx &lc, int mode, const KeyArgs &A, size_t n_items, cudaStream_t st) {
     if (n_items == 0) return cudaSuccess;
     if (n_items * lc.L * 2 > 0x7fffffffull) return cudaErrorInvalidValue;
     return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) { return launch_keys_n<decltype(lg)::value>(lc, mode, A, n_items, st); });
+}
+
+// n_rows seeded rows of lc.L limbs (ciphertexts, or n_keys * ndig key digits when keys) expanded into [n_rows][2][L][N]; one launch
+cudaError_t launch_expand_seeded(const LaunchCtx &lc, bool keys, const SeededKeyArgs &A, const u64 *src, u64 *dst, size_t n_rows, cudaStream_t st) {
+    const size_t n_blocks = n_rows * lc.L << (lc.log_n - 2);
+    if (!n_blocks) return cudaSuccess;
+    auto S = reinterpret_cast<const U64x2 *>(src);
+    auto D = reinterpret_cast<U64x2 *>(dst);
+    return with_log_n(lc.log_n, cudaErrorInvalidValue, [&](auto lg) {
+        constexpr int LOGN = decltype(lg)::value;
+        auto k = keys ? expand_seeded_kernel<LOGN, true> : expand_seeded_kernel<LOGN, false>;
+        k<<<ew_grid(lc, n_blocks), 256, 0, st>>>(A, S, D, lc.lt, lc.L, n_blocks);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t launch_decrypt(const LaunchCtx &lc, const u64 *ct, const u64 *s, u64 *pt, u32 n_comp, size_t n, cudaStream_t st) {

@@ -11,9 +11,20 @@ namespace dpfhe {
 enum KeyDomain : u32 {
     KD_SECRET = 1, KD_KEY_A = 2, KD_KEY_E = 3, KD_ENC_A = 4, KD_ENC_E = 5,
     KD_PK_A = 6, KD_PK_E = 7,                          // public key (the key owner's seed)
-    KD_PENC_U = 8, KD_PENC_E0 = 9, KD_PENC_E1 = 10     // public-key encryption (the encryptor's seed)
+    KD_PENC_U = 8, KD_PENC_E0 = 9, KD_PENC_E1 = 10,    // public-key encryption (the encryptor's seed)
+    KD_PUBLIC_SEED = 11,                               // the public seed a_seed (the key owner's seed; DESIGN.md §2.23)
+    KD_SENC_A = 12, KD_SENC_E = 13,                    // seeded encryption: a from a_seed, e from the key owner's seed
+    KD_SKEY_A = 14, KD_SKEY_E = 15                     // seeded switch keys: likewise
 };
 DPFHE_HD u32 key_nonce0(u32 domain, u32 K, u32 digit, u32 limb) { return domain | K << 8 | digit << 16 | limb << 24; }
+// the ChaCha20 key of the `a` rows: the public seed of a seeded mode (whose launch passes SeededKeyArgs), else the seed
+template <bool SEEDED>
+DPFHE_HD const u32 *key_a_seed(const KeyArgs &A) {
+    if constexpr (SEEDED) return static_cast<const SeededKeyArgs &>(A).a_seed;
+    else return A.seed;
+}
+// the unseeded mode whose formula a seeded mode shares
+DPFHE_HD constexpr int key_base_mode(int mode) { return mode == KM_ENC_SEEDED ? KM_ENC : mode == KM_RELIN_SEEDED ? KM_RELIN : mode == KM_GALOIS_SEEDED ? KM_GALOIS : mode; }
 
 namespace DPFHE_VNS {
 
@@ -91,9 +102,12 @@ DPFHE_HD void sample_small(signed char *small, const u32 seed[8], bool ternary, 
 // [c_lo, c_hi) of the limb, two chunks (one ChaCha20 block of uniform values) per step; buf chunk = chunk - c_lo.
 //   SECRET: out row = the transform.
 //   ENC / KEY / PUBLIC_KEY: a from its stream, c0 / b = transform - a s + (plaintext | gadget term | nothing), c1 / a = a.
+//   seeded ENC / KEY: a from the stream of A.a_seed in the seeded domains, only c0 / b stored ([item][L][N]).
 
-template <int LOGN, int NT, int MODE>
+template <int LOGN, int NT, int MODE_>
 DPFHE_HD void keys_store(const u64 *buf, const KeyArgs &A, const LimbParams &p, u32 l, u32 L, size_t item, int c_lo, int c_hi, int tid) {
+    constexpr int MODE = key_base_mode(MODE_);
+    constexpr bool SEEDED = MODE != MODE_;
     constexpr bool SWITCH_KEY = MODE == KM_RELIN || MODE == KM_GALOIS;
     constexpr size_t N = (size_t)1 << LOGN;
     const U64x2 *sb = reinterpret_cast<const U64x2 *>(buf);
@@ -121,16 +135,17 @@ DPFHE_HD void keys_store(const u64 *buf, const KeyArgs &A, const LimbParams &p, 
         item_no = MODE == KM_GALOIS ? A.galois[e] : 0;
         g = (u32)item_no;
     }
-    const u32 n0 = key_nonce0(MODE == KM_ENC ? KD_ENC_A : MODE == KM_PUBLIC_KEY ? KD_PK_A : KD_KEY_A, A.K, digit, l);
+    const u32 n0 = key_nonce0(SEEDED ? (MODE == KM_ENC ? KD_SENC_A : KD_SKEY_A)
+                                     : MODE == KM_ENC ? KD_ENC_A : MODE == KM_PUBLIC_KEY ? KD_PK_A : KD_KEY_A, A.K, digit, l);
     const bool in_digit = SWITCH_KEY && (A.K == 0 ? l == digit : (l < A.Lq && l / A.K == digit));
     const u64 r64 = A.r64[l], r64_s = A.r64_s[l], fac = A.fac[l];
     const u64 *srow = A.s + (size_t)l * N;
-    U64x2 *ob = reinterpret_cast<U64x2 *>(A.out + (item * 2 + 0) * L * N + (size_t)l * N);
+    U64x2 *ob = reinterpret_cast<U64x2 *>(A.out + (item * (SEEDED ? 1 : 2) + 0) * L * N + (size_t)l * N);
     U64x2 *oa = reinterpret_cast<U64x2 *>(A.out + (item * 2 + 1) * L * N + (size_t)l * N);
     const U64x2 *pt = MODE == KM_ENC ? reinterpret_cast<const U64x2 *>(A.pt + (item * L + l) * N) : nullptr;
     for (int c = c_lo + 2 * tid; c < c_hi; c += 2 * NT) {
         u32 w[16];
-        chacha20_block(A.seed, (u32)(c >> 1), n0, (u32)item_no, (u32)(item_no >> 32), w);
+        chacha20_block(key_a_seed<SEEDED>(A), (u32)(c >> 1), n0, (u32)item_no, (u32)(item_no >> 32), w);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int cc = c + h;
@@ -167,26 +182,28 @@ DPFHE_HD void keys_store(const u64 *buf, const KeyArgs &A, const LimbParams &p, 
             b.x = r[0];
             b.y = r[1];
             st_stream(ob + cc, b);
-            st_stream(oa + cc, a);
+            if (!SEEDED) st_stream(oa + cc, a);
         }
     }
 }
 
 // the noise (or ternary) row of an item: nonce and domain
-template <int MODE>
+template <int MODE_>
 DPFHE_HD void keys_small_nonce(const KeyArgs &A, size_t item, u32 &n0, u64 &item_no) {
+    constexpr int MODE = key_base_mode(MODE_);
+    constexpr bool SEEDED = MODE != MODE_;
     if (MODE == KM_SECRET) {
         n0 = key_nonce0(KD_SECRET, 0, 0, 0);
         item_no = 0;
     } else if (MODE == KM_ENC) {
-        n0 = key_nonce0(KD_ENC_E, 0, 0, 0);
+        n0 = key_nonce0(SEEDED ? KD_SENC_E : KD_ENC_E, 0, 0, 0);
         item_no = A.item0 + item;
     } else if (MODE == KM_PUBLIC_KEY) {
         n0 = key_nonce0(KD_PK_E, 0, 0, 0);
         item_no = 0;
     } else {
         const u32 digit = (u32)(item % A.ndig);
-        n0 = key_nonce0(KD_KEY_E, A.K, digit, 0);
+        n0 = key_nonce0(SEEDED ? KD_SKEY_E : KD_KEY_E, A.K, digit, 0);
         item_no = MODE == KM_GALOIS ? A.galois[item / A.ndig] : 0;
     }
 }
@@ -301,6 +318,46 @@ DPFHE_HD void pub_enc_body(CTA &cta, u64 *buf, signed char *small, const KeyArgs
     pub_enc_pass<LOGN, NT, 0>(cta, buf, small, A, tw, p, l, L, item, h);
     pub_enc_pass<LOGN, NT, 1>(cta, buf, small, A, tw, p, l, L, item, h);
     pub_enc_pass<LOGN, NT, 2>(cta, buf, small, A, tw, p, l, L, item, h);
+}
+
+// Expansion of seeded rows (DESIGN.md §2.23), one ChaCha20 block w of [n][L][N / 4]: the four `a` values of coefficients 4b .. 4b + 3
+// of limb l of row item, and the matching c0 / b words.  KEYS: row item = e * ndig + digit of [n_keys][ndig], item number
+// A.galois[e] (0 for the relinearisation key); else ciphertext item, item number A.item0 + item.  src = nullptr: the c0 / b words
+// are already in place (the upload writes them straight into dst).  dst [n][2][L][N].
+template <int LOGN, bool KEYS>
+DPFHE_HD void expand_block(const U64x2 *src, U64x2 *dst, const SeededKeyArgs &A, const LimbParams &p, u32 L, size_t w) {
+    constexpr size_t NB = (size_t)1 << (LOGN - 2);
+    const size_t b = w % NB, row = w / NB;
+    const u32 l = (u32)(row % L);
+    const size_t item = row / L;
+    u32 digit = 0;
+    u64 item_no;
+    if (KEYS) {
+        digit = (u32)(item % A.ndig);
+        item_no = A.galois[item / A.ndig];
+    } else {
+        item_no = A.item0 + item;
+    }
+    u32 x[16];
+    chacha20_block(A.a_seed, (u32)b, key_nonce0(KEYS ? KD_SKEY_A : KD_SENC_A, A.K, digit, l), (u32)item_no, (u32)(item_no >> 32), x);
+    const u64 r64 = A.r64[l], r64_s = A.r64_s[l];
+    U64x2 a[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        a[h].x = uniform_reduce((u64)x[8 * h + 0] | (u64)x[8 * h + 1] << 32, (u64)x[8 * h + 2] | (u64)x[8 * h + 3] << 32, r64, r64_s, p);
+        a[h].y = uniform_reduce((u64)x[8 * h + 4] | (u64)x[8 * h + 5] << 32, (u64)x[8 * h + 6] | (u64)x[8 * h + 7] << 32, r64, r64_s, p);
+    }
+    const size_t in_row = (size_t)l << (LOGN - 1), c = 2 * b;   // 16-byte chunks: limb offset, first chunk of the block
+    U64x2 *o0 = dst + item * 2 * L * (NB * 2) + in_row + c;
+    U64x2 *o1 = o0 + L * (NB * 2);
+    if (src) {
+        const U64x2 *s0 = src + row * (NB * 2) + c;
+        const U64x2 v0 = ld_stream(s0), v1 = ld_stream(s0 + 1);
+        st_stream(o0, v0);
+        st_stream(o0 + 1, v1);
+    }
+    st_stream(o1, a[0]);
+    st_stream(o1 + 1, a[1]);
 }
 
 // decryption, one 16-byte chunk c of [n][L][N]: c0 + c1 s (+ c2 s^2)

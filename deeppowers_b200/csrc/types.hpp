@@ -170,7 +170,9 @@ struct BgvConsts {
 
 // Key generation and encryption (DESIGN.md §2.14): what one launch of the key / encryption kernels (keys.cu) produces, built in
 // abi.cu and passed by value in the kernel parameter block
-enum KeyMode { KM_SECRET = 0, KM_ENC = 1, KM_RELIN = 2, KM_GALOIS = 3, KM_PUBLIC_KEY = 4, KM_ENC_PUBLIC = 5 };
+// the seeded modes (DESIGN.md §2.23) are KM_ENC / KM_RELIN / KM_GALOIS with `a` drawn from a_seed and only c0 / b stored
+enum KeyMode { KM_SECRET = 0, KM_ENC = 1, KM_RELIN = 2, KM_GALOIS = 3, KM_PUBLIC_KEY = 4, KM_ENC_PUBLIC = 5,
+               KM_ENC_SEEDED = 6, KM_RELIN_SEEDED = 7, KM_GALOIS_SEEDED = 8 };
 constexpr int KEYS_MAX_ELTS = 64;   // Galois elements per launch (abi.cu splits longer lists)
 struct KeyArgs {
     u32 seed[8];                  // the 32-byte seed as little-endian words (the ChaCha20 key)
@@ -184,7 +186,14 @@ struct KeyArgs {
     const u64 *s;                 // secret [L][N], evaluation form (public-key encryption: the public key, b at s, a at s + pk_a)
     const u64 *pt;                // encryption: plaintexts [n][L][N]
     u64 *out;                     // secret [L][N], keys [n_elts][ndig][2][L][N], public key [2][L][N], ciphertexts [n][2][L][N]
+                                  // (seeded: keys [n_elts][ndig][L][N], ciphertexts [n][L][N])
 };
+// the seeded modes and the expansion of seeded rows (DESIGN.md §2.23): KeyArgs and the public seed of the `a` rows.  A type of its own,
+// so that the parameter block of every unseeded instance keeps its layout (a longer KeyArgs would move the kernel parameters after it)
+struct SeededKeyArgs : KeyArgs {
+    u32 a_seed[8];                // the public seed as little-endian words (the ChaCha20 key of the `a` rows)
+};
+DPFHE_HD constexpr bool key_mode_seeded(int mode) { return mode >= KM_ENC_SEEDED; }
 
 // KS_DOT (grouped keys only, DESIGN.md §2.18): the digit is the third component of a SUM of tensor products
 enum KsMode { KS_MUL_RELIN = 0, KS_PLAIN = 1, KS_ROTATE = 2, KS_DOT = 3 };

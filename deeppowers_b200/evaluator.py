@@ -72,6 +72,22 @@ def _seed(s):
     return bytes(s)
 
 
+def _u64_array(values):
+    """(count, ctypes uint64 array) of a list of item numbers or Galois elements"""
+    n = len(values)
+    return n, (C.c_uint64 * max(n, 1))(*[int(v) for v in values])
+
+
+def public_seed(seed):
+    """the public seed (32 bytes) of a key owner's 32-byte seed: words 0..7 of its ChaCha20 block in nonce domain 11 (DESIGN.md
+    section 2.23).  Needs no context or device."""
+    lib = _lib.load()
+    out = C.create_string_buffer(32)
+    if lib.dpfhe_seeded_public_seed(_seed(seed), out) != 0:
+        raise DpfheError(lib.dpfhe_last_error().decode())
+    return out.raw
+
+
 _CUDA_STREAM_LEGACY = 1   # cudaStreamLegacy: the ABI reserves NULL for "the context's own stream"
 
 
@@ -694,6 +710,71 @@ class Context:
     def mod_switch_down_level(self, level, polys, out, n_polys, t_plain=0, stream=None):
         """[n_polys][level][N] -> [n_polys][level-1][N]"""
         self._chk(self._l.dpfhe_mod_switch_down_level(self._h, int(level), _ptr(polys), _ptr(out), n_polys, int(t_plain), _stream(stream)))
+
+    # seeded ciphertexts and switch keys (DESIGN.md section 2.23): the `a` rows come from the public seed of the key owner's seed
+    # (public_seed), so only c0 [n][L][N] and the b rows [n_keys][digits][L][N] are stored or moved; the expansions give the full
+    # ciphertexts [n][2][L][N] and keys [n_keys][digits][2][L][N].  Key item numbers: 0 (relinearisation key) or the Galois element.
+    def public_seed(self, seed):
+        return public_seed(seed)
+
+    def encrypt_seeded(self, t_plain, sk, seed, first_index, pt, c0, n, stream=None):
+        self._chk(self._l.dpfhe_encrypt_seeded(self._h, int(t_plain), _ptr(sk), _seed(seed), int(first_index), _ptr(pt), _ptr(c0), n,
+                                               _stream(stream)))
+
+    def encrypt_seeded_host(self, t_plain, sk, seed, first_index, pt, c0):
+        self._chk(self._l.dpfhe_encrypt_seeded_host(self._h, int(t_plain), _hptr(sk), _seed(seed), int(first_index), _hptr(pt),
+                                                    _hptr(c0, True), pt.size // self.P))
+
+    def encrypt_seeded_level(self, level, t_plain, sk, seed, first_index, pt, c0, n, stream=None):
+        self._chk(self._l.dpfhe_encrypt_seeded_level(self._h, int(level), int(t_plain), _ptr(sk), _seed(seed), int(first_index), _ptr(pt),
+                                                     _ptr(c0), n, _stream(stream)))
+
+    def encrypt_seeded_level_host(self, level, t_plain, sk, seed, first_index, pt, c0):
+        self._chk(self._l.dpfhe_encrypt_seeded_level_host(self._h, int(level), int(t_plain), _hptr(sk), _seed(seed), int(first_index),
+                                                          _hptr(pt), _hptr(c0, True), pt.size // (int(level) * self.N)))
+
+    def expand_ciphertexts(self, a_seed, first_index, c0, ct, n, stream=None):
+        self._chk(self._l.dpfhe_expand_ciphertexts(self._h, _seed(a_seed), int(first_index), _ptr(c0), _ptr(ct), n, _stream(stream)))
+
+    def expand_ciphertexts_level(self, level, a_seed, first_index, c0, ct, n, stream=None):
+        self._chk(self._l.dpfhe_expand_ciphertexts_level(self._h, int(level), _seed(a_seed), int(first_index), _ptr(c0), _ptr(ct), n,
+                                                         _stream(stream)))
+
+    def upload_seeded_ciphertexts(self, a_seed, first_index, c0, ct):
+        """host c0 [n][L][N] (numpy) -> device ciphertexts [n][2][L][N] (synchronous)"""
+        self._chk(self._l.dpfhe_upload_seeded_ciphertexts(self._h, _seed(a_seed), int(first_index), _hptr(c0), _ptr(ct), c0.size // self.P))
+
+    def upload_seeded_ciphertexts_level(self, level, a_seed, first_index, c0, ct):
+        self._chk(self._l.dpfhe_upload_seeded_ciphertexts_level(self._h, int(level), _seed(a_seed), int(first_index), _hptr(c0), _ptr(ct),
+                                                                c0.size // (int(level) * self.N)))
+
+    def generate_relin_key_seeded(self, n_special, t_plain, sk, seed, b, stream=None):
+        self._chk(self._l.dpfhe_relin_keygen_seeded(self._h, int(n_special), int(t_plain), _ptr(sk), _seed(seed), _ptr(b), _stream(stream)))
+
+    def generate_relin_key_seeded_host(self, n_special, t_plain, sk, seed, b):
+        self._chk(self._l.dpfhe_relin_keygen_seeded_host(self._h, int(n_special), int(t_plain), _hptr(sk), _seed(seed), _hptr(b, True)))
+
+    def generate_galois_keys_seeded(self, n_special, t_plain, sk, galois_elts, seed, b, stream=None):
+        n, ge = _u64_array(galois_elts)
+        self._chk(self._l.dpfhe_galois_keygen_seeded(self._h, int(n_special), int(t_plain), _ptr(sk), n, ge, _seed(seed), _ptr(b),
+                                                     _stream(stream)))
+
+    def generate_galois_keys_seeded_host(self, n_special, t_plain, sk, galois_elts, seed, b):
+        n, ge = _u64_array(galois_elts)
+        self._chk(self._l.dpfhe_galois_keygen_seeded_host(self._h, int(n_special), int(t_plain), _hptr(sk), n, ge, _seed(seed), _hptr(b, True)))
+
+    def expand_switch_keys(self, n_special, a_seed, items, b, keys, stream=None):
+        n, it = _u64_array(items)
+        self._chk(self._l.dpfhe_expand_switch_keys(self._h, int(n_special), _seed(a_seed), n, it, _ptr(b), _ptr(keys), _stream(stream)))
+
+    def upload_seeded_switch_keys(self, n_special, a_seed, items, b, keys):
+        """host b rows (numpy) -> device keys (synchronous)"""
+        n, it = _u64_array(items)
+        self._chk(self._l.dpfhe_upload_seeded_switch_keys(self._h, int(n_special), _seed(a_seed), n, it, _hptr(b), _ptr(keys)))
+
+    def expand_switch_keys_host(self, n_special, a_seed, items, b, keys):
+        n, it = _u64_array(items)
+        self._chk(self._l.dpfhe_expand_switch_keys_host(self._h, int(n_special), _seed(a_seed), n, it, _hptr(b), _hptr(keys, True)))
 
     def galois_elt(self, k):
         """Galois element 5^k mod 2N of a rotation by k slots (k may be negative)."""

@@ -227,6 +227,53 @@ public:
         return elts;
     }
 
+    // ---- seeded ciphertexts and switch keys (DESIGN.md §2.23): only c0 [count][level][N] / the b rows [n][digits][L][N] are made;
+    //      the `a` rows come from the public seed of the key owner's seed (public_seed), and the expand / upload calls give the full
+    //      ciphertexts [count][2][level][N] and keys [n][digits][2][L][N].  Key items: 0 (relinearisation key) or a Galois element. ----
+    static Seed public_seed(const Seed &seed) {
+        Seed a;
+        check(dpfhe_seeded_public_seed(seed.data(), a.data()));
+        return a;
+    }
+    std::size_t seeded_key_words(unsigned special) const { return key_words(special) / 2; }
+    void encrypt_seeded(unsigned level, std::uint64_t plain_modulus, const std::uint64_t *secret, const Seed &seed, std::uint64_t first_index,
+                        const std::uint64_t *plain_eval, std::size_t count, std::uint64_t *c0) {
+        check(dpfhe_encrypt_seeded_level_host(ctx_, level, plain_modulus, secret, seed.data(), first_index, plain_eval, c0, count));
+    }
+    void encrypt_seeded_device(unsigned level, std::uint64_t plain_modulus, const std::uint64_t *secret, const Seed &seed,
+                               std::uint64_t first_index, const std::uint64_t *plain_eval, std::size_t count, std::uint64_t *c0,
+                               void *stream = nullptr) {
+        check(dpfhe_encrypt_seeded_level(ctx_, level, plain_modulus, secret, seed.data(), first_index, plain_eval, c0, count, stream));
+    }
+    void generate_relin_key_seeded(unsigned special, std::uint64_t plain_modulus, const std::uint64_t *secret, const Seed &seed, std::uint64_t *b) {
+        check(dpfhe_relin_keygen_seeded_host(ctx_, special, plain_modulus, secret, seed.data(), b));
+    }
+    void generate_galois_keys_seeded(unsigned special, std::uint64_t plain_modulus, const std::uint64_t *secret, const std::vector<long> &steps,
+                                     const Seed &seed, std::uint64_t *b) {
+        const std::vector<std::uint64_t> elts = galois_elements(steps);
+        check(dpfhe_galois_keygen_seeded_host(ctx_, special, plain_modulus, secret, elts.size(), elts.data(), seed.data(), b));
+    }
+    // device c0 -> device ciphertexts; host c0 -> device ciphertexts (half the bytes over the bus, synchronous)
+    void expand_ciphertexts_device(unsigned level, const Seed &a_seed, std::uint64_t first_index, const std::uint64_t *c0, CiphertextBatch out,
+                                   void *stream = nullptr) {
+        check(dpfhe_expand_ciphertexts_level(ctx_, level, a_seed.data(), first_index, c0, out.data, out.count, stream));
+    }
+    void upload_seeded_ciphertexts(unsigned level, const Seed &a_seed, std::uint64_t first_index, const std::uint64_t *host_c0, CiphertextBatch out) {
+        check(dpfhe_upload_seeded_ciphertexts_level(ctx_, level, a_seed.data(), first_index, host_c0, out.data, out.count));
+    }
+    void expand_switch_keys_device(unsigned special, const Seed &a_seed, const std::vector<std::uint64_t> &items, const std::uint64_t *b,
+                                   std::uint64_t *keys, void *stream = nullptr) {
+        check(dpfhe_expand_switch_keys(ctx_, special, a_seed.data(), items.size(), items.data(), b, keys, stream));
+    }
+    void upload_seeded_switch_keys(unsigned special, const Seed &a_seed, const std::vector<std::uint64_t> &items, const std::uint64_t *host_b,
+                                   std::uint64_t *keys) {
+        check(dpfhe_upload_seeded_switch_keys(ctx_, special, a_seed.data(), items.size(), items.data(), host_b, keys));
+    }
+    void expand_switch_keys(unsigned special, const Seed &a_seed, const std::vector<std::uint64_t> &items, const std::uint64_t *host_b,
+                            std::uint64_t *host_keys) {
+        check(dpfhe_expand_switch_keys_host(ctx_, special, a_seed.data(), items.size(), items.data(), host_b, host_keys));
+    }
+
     // ---- host-buffer calls: synchronous; H2D / compute / D2H are pipelined inside the library ----
     void multiply_relin(ConstCiphertextBatch a, ConstCiphertextBatch b, const std::uint64_t *relin_key, CiphertextBatch out) {
         same(a.count, b.count, out.count);
@@ -534,6 +581,33 @@ private:
     Memory where_;
     const std::uint64_t *secret_;
     Evaluator::Seed seed_;
+    std::uint64_t t_, next_;
+};
+
+// Seeded symmetric encryption at a level (DESIGN.md §2.23), numbering the ciphertexts itself as Encryptor does: it writes c0 only and
+// holds the public seed (public_seed()) that a receiver needs, with next_index(), to expand them.  Host or device memory as Encryptor.
+class SeededEncryptor {
+public:
+    using Memory = Encryptor::Memory;
+    SeededEncryptor(Evaluator &ev, Memory where, unsigned level, const std::uint64_t *secret, const Evaluator::Seed &seed,
+                    std::uint64_t plain_modulus, std::uint64_t first_index = 0)
+        : ev_(ev), where_(where), level_(level), secret_(secret), seed_(seed), a_seed_(Evaluator::public_seed(seed)), t_(plain_modulus),
+          next_(first_index) {}
+    // c0 [count][level][N] of the next `count` item numbers
+    void encrypt(const std::uint64_t *plain_eval, std::size_t count, std::uint64_t *c0, void *stream = nullptr) {
+        if (where_ == Memory::host) ev_.encrypt_seeded(level_, t_, secret_, seed_, next_, plain_eval, count, c0);
+        else ev_.encrypt_seeded_device(level_, t_, secret_, seed_, next_, plain_eval, count, c0, stream);
+        next_ += count;
+    }
+    const Evaluator::Seed &public_seed() const { return a_seed_; }
+    std::uint64_t next_index() const { return next_; }
+
+private:
+    Evaluator &ev_;
+    Memory where_;
+    unsigned level_;
+    const std::uint64_t *secret_;
+    Evaluator::Seed seed_, a_seed_;
     std::uint64_t t_, next_;
 };
 

@@ -541,5 +541,7 @@ int dpfhe_describe(const dpfhe_ctx *ctx, char *buf, size_t buf_len);
 
 /* the polynomial evaluators and the keyless calls at any level of the modulus chain (DESIGN.md §2.22) */
 #include "dpfhe_level.h"
+/* seeded ciphertexts and switch keys, their uniform half regenerated on the device from a public seed (DESIGN.md §2.23) */
+#include "dpfhe_seeded.h"
 
 #endif /* DPFHE_H */

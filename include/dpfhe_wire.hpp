@@ -14,6 +14,11 @@
 //                       4 = hybrid switch key [L-1][2][L][N] (the last modulus is the special prime; count = 1),
 //                       5 = grouped hybrid switch key [ceil((L-K)/K)][2][L][N] with count = K special primes (1 <= K <= 4, 2K <= L)
 //                       6 = public key [2][L][N] (b, a) (count = 1)
+//                       7 = seeded ciphertexts (DESIGN.md §2.23): a 5-word prefix (the public seed as four LE words, then first_index)
+//                           and c0 [count][L][N]
+//                       8 = seeded switch key: a 5-word prefix (the public seed as four LE words, then the item number: 0 for the
+//                           relinearisation key, else the Galois element) and the b rows [digits][L][N], count = K special primes
+//                           (0 <= K <= 4, 2K <= L; digits = L for K = 0, else ceil((L-K)/K))
 //   20      4     form: 1 = evaluation (NTT, bit-reversed order), 0 = coefficient
 //   24      8     count
 //   32      128   moduli[16] (unused entries 0)
@@ -33,7 +38,11 @@ namespace fhe {
 
 // HybridSwitchKey: n_limbs counts the special prime (the last modulus); payload [n_limbs-1][2][n_limbs][N]
 // GroupedSwitchKey: n_limbs counts the K = count special primes at the end of the basis; payload [ceil((n_limbs-K)/K)][2][n_limbs][N]
-enum class WireKind : std::uint32_t { Ciphertexts = 1, SwitchKey = 2, Plaintexts = 3, HybridSwitchKey = 4, GroupedSwitchKey = 5, PublicKey = 6 };
+enum class WireKind : std::uint32_t {
+    Ciphertexts = 1, SwitchKey = 2, Plaintexts = 3, HybridSwitchKey = 4, GroupedSwitchKey = 5, PublicKey = 6, SeededCiphertexts = 7,
+    SeededSwitchKey = 8
+};
+constexpr std::size_t kSeededPrefixWords = 5;   // the public seed (4 words) and first_index / the item number
 
 struct WireHeader {
     char magic[8];
@@ -64,8 +73,26 @@ inline std::size_t wire_payload_words(const WireHeader &h) {
             const std::size_t k = static_cast<std::size_t>(h.count), digits = (h.n_limbs - k + k - 1) / k;
             return std::size_t(2) * digits * poly;
         }
+        case WireKind::SeededCiphertexts:
+            if (h.count < 1) throw std::runtime_error("dpfhe wire: no seeded ciphertexts");
+            return kSeededPrefixWords + checked(h.count, poly);
+        case WireKind::SeededSwitchKey: {
+            if (h.count > 4 || 2 * h.count > h.n_limbs) throw std::runtime_error("dpfhe wire: bad number of special primes");
+            const std::size_t k = static_cast<std::size_t>(h.count), digits = k ? (h.n_limbs - k + k - 1) / k : h.n_limbs;
+            return kSeededPrefixWords + digits * poly;
+        }
     }
     throw std::runtime_error("dpfhe wire: unknown kind");
+}
+
+// the prefix of a seeded kind, which the header does not describe: the item numbers first_index .. first_index + count - 1 of seeded
+// ciphertexts must not wrap, and a seeded key's item number is 0 or a Galois element (odd, < 2N)
+inline void check_wire_prefix(const WireHeader &h, const std::uint64_t *payload) {
+    if (h.kind == static_cast<std::uint32_t>(WireKind::SeededCiphertexts) && payload[4] > ~std::uint64_t(0) - (h.count - 1))
+        throw std::runtime_error("dpfhe wire: item numbers of seeded ciphertexts wrap");
+    if (h.kind == static_cast<std::uint32_t>(WireKind::SeededSwitchKey) && payload[4] != 0 &&
+        (!(payload[4] & 1) || payload[4] >= (std::uint64_t(2) << h.log_n)))
+        throw std::runtime_error("dpfhe wire: item number of a seeded key is neither 0 nor a Galois element");
 }
 
 inline WireHeader make_wire_header(unsigned log_n, unsigned n_limbs, WireKind kind, std::uint64_t count, const std::uint64_t *moduli) {
@@ -85,6 +112,7 @@ inline void write_wire_file(const std::string &path, const WireHeader &h, const 
     std::FILE *f = std::fopen(path.c_str(), "wb");
     if (!f) throw std::runtime_error("dpfhe wire: cannot open " + path + " for writing");
     const std::size_t words = wire_payload_words(h);
+    check_wire_prefix(h, payload);
     const bool ok = std::fwrite(&h, sizeof(h), 1, f) == 1 && std::fwrite(payload, 8, words, f) == words;
     std::fclose(f);
     if (!ok) throw std::runtime_error("dpfhe wire: short write to " + path);
@@ -115,6 +143,11 @@ inline WireHeader read_wire_file(const std::string &path, std::vector<std::uint6
     if (std::fseek(file.f, static_cast<long>(sizeof(h)), SEEK_SET) != 0) throw std::runtime_error("dpfhe wire: cannot seek in " + path);
     payload.resize(words);
     if (std::fread(payload.data(), 8, words, file.f) != words) throw std::runtime_error("dpfhe wire: truncated payload in " + path);
+    try {
+        check_wire_prefix(h, payload.data());
+    } catch (const std::runtime_error &e) {
+        throw std::runtime_error(std::string(e.what()) + " in " + path);
+    }
     return h;
 }
 
