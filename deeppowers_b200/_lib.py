@@ -215,6 +215,14 @@ SEEDED_SYMBOLS = {
     "dpfhe_expand_switch_keys_host": (C.c_int, [_V, _U, _V, _SZ, _V, _V, _V]),
 }
 
+# the entry points of include/dpfhe_compact.h (DESIGN.md section 2.24), which dpfhe.h includes
+COMPACT_SYMBOLS = {
+    "dpfhe_compact_ciphertexts": (C.c_int, [_V, _U, _U, _U64, _V, _V, _SZ, _V]),
+    "dpfhe_download_compact_ciphertexts": (C.c_int, [_V, _U, _U, _U64, _V, _V, _SZ]),
+    "dpfhe_decrypt_compact": (C.c_int, [_V, _U, _U64, _V, _V, _V, _SZ, _V]),
+    "dpfhe_decrypt_compact_host": (C.c_int, [_V, _U, _U64, _V, _V, _V, _SZ]),
+}
+
 
 class dpfhe_params(C.Structure):
     _fields_ = [("log_n", C.c_uint32), ("n_limbs", C.c_uint32), ("moduli", C.POINTER(C.c_uint64))]
@@ -232,7 +240,7 @@ def load():
     if not os.path.exists(path):
         _build.build()          # raises if nvcc is unavailable: no fallback
     lib = C.CDLL(path)
-    for name, (res, args) in list(SYMBOLS.items()) + list(LEVEL_SYMBOLS.items()) + list(SEEDED_SYMBOLS.items()):
+    for name, (res, args) in list(SYMBOLS.items()) + list(LEVEL_SYMBOLS.items()) + list(SEEDED_SYMBOLS.items()) + list(COMPACT_SYMBOLS.items()):
         fn = getattr(lib, name)   # AttributeError if the library does not export what include/dpfhe.h (with its included headers) declares
         fn.restype = res
         fn.argtypes = args

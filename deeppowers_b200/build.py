@@ -14,11 +14,13 @@ UNITS = [("kernels.cu", "kernels_%s_%s" % (v, n), ["-DDPFHE_FAST=%d" % f, "-DDPF
          for v, f in (("gen", 0), ("fast", 1)) for n, part in (("main", 1), ("hybrid", 2), ("grouped", 3))] + [
          ("keys.cu", "keys_%s" % v, ["-DDPFHE_FAST=%d" % f]) for v, f in (("gen", 0), ("fast", 1))] + [
          ("eval.cu", "eval_%s" % v, ["-DDPFHE_FAST=%d" % f]) for v, f in (("gen", 0), ("fast", 1))] + [
+         ("compact.cu", "compact_%s" % v, ["-DDPFHE_FAST=%d" % f]) for v, f in (("gen", 0), ("fast", 1))] + [
          ("abi.cu", "abi", []), ("multi.cu", "multi", []), ("hostmem.cu", "hostmem", []), ("host_params.cpp", "host_params", [])]
 SOURCES = sorted({u[0] for u in UNITS})
-HEADERS = ["types.hpp", "modarith.cuh", "ntt_core.cuh", "kernel_bodies.cuh", "keys.cuh", "eval.cuh", "launch.hpp", "launch_util.hpp", "host_params.hpp", "ctx.hpp",
+HEADERS = ["types.hpp", "modarith.cuh", "ntt_core.cuh", "kernel_bodies.cuh", "keys.cuh", "eval.cuh", "compact.cuh", "launch.hpp", "launch_util.hpp", "host_params.hpp", "ctx.hpp",
            os.path.join("..", "..", "include", "dpfhe.h"),
-           os.path.join("..", "..", "include", "dpfhe_level.h"), os.path.join("..", "..", "include", "dpfhe_seeded.h")]
+           os.path.join("..", "..", "include", "dpfhe_level.h"), os.path.join("..", "..", "include", "dpfhe_seeded.h"),
+           os.path.join("..", "..", "include", "dpfhe_compact.h")]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + [
     "-std=c++17", "-O3", "-lineinfo",

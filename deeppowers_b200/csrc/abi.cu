@@ -117,15 +117,23 @@ struct DeviceOut {
     size_t row_words = 0;
 };
 
+// A device-resident input of the pipeline (dpfhe_compact.h's download): the chunk's compute reads its items of d in place, and nothing
+// is uploaded.  The input is the caller's memory, so the first compute waits as DeviceOut's first copy does.
+struct DeviceIn {
+    const u64 *d = nullptr;
+};
+
 // Generic three-stage pipeline over `n_items` items split into chunks:
 //   upload(chunk -> stage_in[slot]) on s_h2d, compute on ctx->stream, download(stage_out[slot]) on s_d2h.
 // in_item_bytes / out_item_bytes are per item; h_in may be two arrays (a and b) laid out back to back in the stage.
 // n_slices > 1: each input is n_slices arrays of n_items items, slice_stride words apart (the operands of an inner product,
 // [n_terms][batch] ciphertexts); a chunk stages its items of every slice, [input][slice][chunk_items], slice after slice.
 // dev.d: a device-resident output (DeviceOut): upload(chunk -> its items of dev.d) on s_h2d, compute in place on ctx->stream.
+// dev_in.d: a device-resident input (DeviceIn): compute(its items of dev_in.d -> stage_out[slot]) on ctx->stream, then the download.
 template <class Compute>
 int run_pipeline_body(dpfhe_ctx *ctx, const u64 *h_in0, const u64 *h_in1, u64 *h_out, size_t n_items, size_t in_item_words,
-                      size_t out_item_words, size_t chunk_items, Compute compute, size_t n_slices, size_t slice_stride, DeviceOut dev) {
+                      size_t out_item_words, size_t chunk_items, Compute compute, size_t n_slices, size_t slice_stride, DeviceOut dev,
+                      DeviceIn dev_in) {
     if (dev.d) {
         // the output is the caller's memory: the first copy waits for the context's previous call (whatever stream it ran on) and for
         // the work issued before this call on the legacy default stream, which the non-blocking s_h2d does not wait for by itself
@@ -152,22 +160,33 @@ int run_pipeline_body(dpfhe_ctx *ctx, const u64 *h_in0, const u64 *h_in1, u64 *h
     }
     const size_t n_in = (h_in1 ? 2 : 1) * n_slices;
     int rc = DPFHE_OK;
-    for (int k = 0; k < PIPE_DEPTH && !rc; ++k) rc = ctx->stage_in[k].reserve(ctx, n_in * chunk_items * in_item_words * 8);
+    for (int k = 0; k < PIPE_DEPTH && !rc && !dev_in.d; ++k) rc = ctx->stage_in[k].reserve(ctx, n_in * chunk_items * in_item_words * 8);
     for (int k = 0; k < PIPE_DEPTH && !rc; ++k) rc = ctx->stage_out[k].reserve(ctx, chunk_items * out_item_words * 8);
     if (rc) return rc;
+    if (dev_in.d) {
+        if (ctx->have_last) CU_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ev_last, 0));
+        CU_TRY(cudaEventRecord(ctx->ev_h2d[0], cudaStreamLegacy));
+        CU_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ev_h2d[0], 0));
+    }
     size_t k = 0;
     for (size_t first = 0; first < n_items; first += chunk_items, ++k) {
         const size_t cnt = n_items - first < chunk_items ? n_items - first : chunk_items;
         const int slot = (int)(k % PIPE_DEPTH);
-        u64 *din0 = ctx->stage_in[slot].get(), *din1 = din0 + n_slices * chunk_items * in_item_words, *dout = ctx->stage_out[slot].get();
-        if (k >= PIPE_DEPTH) CU_TRY(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_comp[slot], 0));   // stage_in[slot] free again
-        for (size_t s = 0; s < n_slices; ++s) {
-            const size_t src = s * slice_stride + first * in_item_words, dst = s * chunk_items * in_item_words;
-            CU_TRY(cudaMemcpyAsync(din0 + dst, h_in0 + src, cnt * in_item_words * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
-            if (h_in1) CU_TRY(cudaMemcpyAsync(din1 + dst, h_in1 + src, cnt * in_item_words * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
+        u64 *din0 = nullptr, *din1 = nullptr, *dout = ctx->stage_out[slot].get();
+        if (dev_in.d) {
+            din0 = const_cast<u64 *>(dev_in.d) + first * in_item_words;   // read only
+        } else {
+            din0 = ctx->stage_in[slot].get();
+            din1 = din0 + n_slices * chunk_items * in_item_words;
+            if (k >= PIPE_DEPTH) CU_TRY(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_comp[slot], 0));   // stage_in[slot] free again
+            for (size_t s = 0; s < n_slices; ++s) {
+                const size_t src = s * slice_stride + first * in_item_words, dst = s * chunk_items * in_item_words;
+                CU_TRY(cudaMemcpyAsync(din0 + dst, h_in0 + src, cnt * in_item_words * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
+                if (h_in1) CU_TRY(cudaMemcpyAsync(din1 + dst, h_in1 + src, cnt * in_item_words * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
+            }
+            CU_TRY(cudaEventRecord(ctx->ev_h2d[slot], ctx->s_h2d));
+            CU_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ev_h2d[slot], 0));
         }
-        CU_TRY(cudaEventRecord(ctx->ev_h2d[slot], ctx->s_h2d));
-        CU_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ev_h2d[slot], 0));
         if (k >= PIPE_DEPTH) CU_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ev_d2h[slot], 0));   // stage_out[slot] drained
         rc = compute(din0, din1, dout, cnt, ctx->stream);
         if (rc) return rc;
@@ -185,9 +204,10 @@ int run_pipeline_body(dpfhe_ctx *ctx, const u64 *h_in0, const u64 *h_in1, u64 *h
 // the caller's host buffers (or the staging slots) when the error is reported
 template <class Compute>
 int run_pipeline(dpfhe_ctx *ctx, const u64 *h_in0, const u64 *h_in1, u64 *h_out, size_t n_items, size_t in_item_words,
-                 size_t out_item_words, size_t chunk_items, Compute compute, size_t n_slices = 1, size_t slice_stride = 0, DeviceOut dev = {}) {
+                 size_t out_item_words, size_t chunk_items, Compute compute, size_t n_slices = 1, size_t slice_stride = 0, DeviceOut dev = {},
+                 DeviceIn dev_in = {}) {
     const int rc = run_pipeline_body(ctx, h_in0, h_in1, h_out, n_items, in_item_words, out_item_words, chunk_items, compute, n_slices, slice_stride,
-                                     dev);
+                                     dev, dev_in);
     if (rc != DPFHE_OK) {
         const std::string why = g_err;   // the drains below must not replace the message of the failure
         cudaStreamSynchronize(ctx->s_h2d);
@@ -222,11 +242,12 @@ int no_check() { return DPFHE_OK; }
 // The host-buffer form of an entry point: the host pointers `ptrs` must not be null, then `check()` runs the call's remaining
 // argument checks.  The operand every item shares (a key, a plaintext or a secret of `shared_words` words; none when
 // shared_words is 0) is uploaded once into the key staging buffer, and the items are pipelined through `compute` in chunks.
-// dev.d: the output is that device buffer instead of h_out (DeviceOut).
+// dev.d: the output is that device buffer instead of h_out (DeviceOut); dev_in.d: the input is that device buffer instead of h_in0
+// (DeviceIn).
 template <class Compute, class Check = int (*)()>
 int host_call(dpfhe_ctx *ctx, std::initializer_list<const void *> ptrs, const uint64_t *h_shared, size_t shared_words, const u64 *h_in0,
               const u64 *h_in1, u64 *h_out, size_t n_items, size_t in_item_words, size_t out_item_words, Compute compute, Check check = no_check,
-              DeviceOut dev = {}) {
+              DeviceOut dev = {}, DeviceIn dev_in = {}) {
     for (const void *p : ptrs)
         if (!p) return fail(DPFHE_ERR_INVALID, "null host pointer");
     int rc = check();
@@ -236,7 +257,7 @@ int host_call(dpfhe_ctx *ctx, std::initializer_list<const void *> ptrs, const ui
         if (rc) return rc;
     }
     const size_t chunk = pick_chunk(ctx, std::max(in_item_words, out_item_words) * 8, n_items);
-    return run_pipeline(ctx, h_in0, h_in1, h_out, n_items, in_item_words, out_item_words, chunk, compute, 1, 0, dev);
+    return run_pipeline(ctx, h_in0, h_in1, h_out, n_items, in_item_words, out_item_words, chunk, compute, 1, 0, dev, dev_in);
 }
 
 int check_galois(const dpfhe_ctx *ctx, uint64_t galois) {
@@ -2630,6 +2651,150 @@ int dpfhe_expand_switch_keys_host(dpfhe_ctx *ctx, unsigned n_special, const uint
                          note_launch(ctx, launches);
                          next += cnt;
                          return DPFHE_OK;
+                     });
+}
+
+// ---------------------------------------------------------------- compact ciphertexts (DESIGN.md §2.24)
+
+// the checks on bits and t_plain (level 1), and the switch's constants
+static int compact_args(const dpfhe_ctx *ctx, unsigned bits, uint64_t t_plain, CompactArgs &A) {
+    const uint64_t q = ctx->hp.limbs[0].lp.q;
+    // compared without a sum, so that no `bits` wraps past the range check; every shift below is then by less than 64
+    if (bits < 2 || bits >= 64 - ctx->hp.log_n || ((uint64_t)ctx->N() << bits) >= q)
+        return fail(DPFHE_ERR_INVALID, "bits must be at least 2 with N 2^bits below q0");
+    if (t_plain && (!(t_plain & 1) || t_plain < 3 || t_plain >= (uint64_t)1 << (bits - 1)))
+        return fail(DPFHE_ERR_INVALID, "plaintext modulus must be 0 or odd with 3 <= t < 2^(bits-1)");
+    build_compact_args(q, ctx->hp.log_n, bits, t_plain, A);
+    return DPFHE_OK;
+}
+
+// every check of a compaction at `level` (1 <= level <= L checked by the caller) before its first launch
+static int check_compact(const dpfhe_ctx *ctx, unsigned level, unsigned bits, uint64_t t_plain, CompactArgs &A) {
+    int rc = compact_args(ctx, bits, t_plain, A);
+    if (rc || !t_plain) return rc;
+    for (unsigned k = level; k >= 2; --k) {   // the checks of dpfhe_mod_switch_down_level at k
+        const uint64_t ql = ctx->hp.limbs[k - 1].lp.q;
+        if (t_plain >= ql || t_plain % ql == 0) return fail(DPFHE_ERR_INVALID, "plaintext modulus must be below the dropped modulus");
+    }
+    return DPFHE_OK;
+}
+
+// the launches of a checked compaction of n ciphertexts at level l: the level-1 pairs into compact_work, the inverse transform, the pack
+static int compact_run(dpfhe_ctx *ctx, unsigned l, const CompactArgs &A, const uint64_t *d_ct, uint64_t *d_out, size_t n, cudaStream_t st) {
+    const size_t N = ctx->N(), polys = 2 * n;
+    const bool chain = A.t && l >= 2;
+    const size_t words_a = polys * N * (chain ? l - 1 : 1), words_b = chain && l >= 3 ? polys * N * (l - 2) : 0;
+    int rc = ctx->compact_work.reserve(ctx, (words_a + words_b) * 8);
+    if (!rc && chain) rc = ctx->ms_tau.reserve(ctx, polys * N * 8);
+    if (rc) return rc;
+    u64 *bufs[2] = {ctx->compact_work.get(), ctx->compact_work.get() + words_a};
+    u64 *x = bufs[0];
+    uint64_t launches = 2;
+    if (chain) {
+        // BGV: l - 1 modulus switches, alternating between the two buffers
+        const u64 *src = d_ct;
+        for (unsigned k = l, i = 0; k >= 2; --k, ++i) {
+            const HostParams *hp = prefix_params(ctx, k);
+            if (!hp) return fail(DPFHE_ERR_NOMEM, "out of host memory");
+            MsConsts K;
+            build_ms_consts(*hp, A.t, K);
+            x = bufs[i & 1];
+            CU_TRY(VCALL(launch_mod_switch, level_view(ctx, k), src, ctx->ms_tau.get(), x, K, polys, st));
+            src = x;
+            launches += 2;
+        }
+    } else {
+        // CKKS (or level 1): limb 0 of every polynomial
+        CU_TRY(cudaMemcpy2DAsync(x, N * 8, d_ct, l * N * 8, N * 8, polys, cudaMemcpyDeviceToDevice, st));
+    }
+    const LaunchCtx lc1 = level_view(ctx, 1);
+    CU_TRY(VCALL(launch_ntt, lc1, x, polys, true, st));
+    CU_TRY(VCALL(launch_compact_pack, lc1, A, x, d_out, polys, st));
+    note_launch(ctx, launches);
+    return DPFHE_OK;
+}
+
+static int compact_at(dpfhe_ctx *ctx, unsigned level, unsigned bits, uint64_t t_plain, const uint64_t *d_ct, uint64_t *d_out, size_t n,
+                      void *stream) {
+    CompactArgs A;
+    int rc = check_compact(ctx, level, bits, t_plain, A);
+    if (rc) return rc;
+    if (n == 0) return DPFHE_OK;
+    CHECK_PTR(d_ct); CHECK_PTR(d_out);
+    if (overlaps(d_out, n * 2 * A.tiles * bits * 8, d_ct, n * 2 * level * ctx->N() * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the input");
+    return compact_run(ctx, level, A, d_ct, d_out, n, pick(ctx, stream));
+}
+
+int dpfhe_compact_ciphertexts(dpfhe_ctx *ctx, unsigned level, unsigned bits, uint64_t t_plain, const uint64_t *d_ct, uint64_t *d_out,
+                              size_t n, void *stream) {
+    return prefix_call(ctx, level, [&] { return compact_at(ctx, level, bits, t_plain, d_ct, d_out, n, stream); });
+}
+
+// device ciphertexts read in place chunk by chunk (DeviceIn), each chunk compacted into its staging slot, the packed words downloaded
+int dpfhe_download_compact_ciphertexts(dpfhe_ctx *ctx, unsigned level, unsigned bits, uint64_t t_plain, const uint64_t *d_ct,
+                                       uint64_t *h_out, size_t n) {
+    return prefix_call(ctx, level, [&]() -> int {
+        CompactArgs A;
+        int rc = check_compact(ctx, level, bits, t_plain, A);
+        if (rc) return rc;
+        if (n == 0) return DPFHE_OK;
+        CHECK_PTR(d_ct);
+        const size_t in_words = 2 * level * ctx->N(), out_words = 2 * (size_t)A.tiles * bits;
+        return host_call(ctx, {h_out}, nullptr, 0, nullptr, nullptr, h_out, n, in_words, out_words,
+                         [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) { return compact_run(ctx, level, A, din, dout, cnt, pick(ctx, st)); },
+                         no_check, DeviceOut{}, DeviceIn{d_ct});
+    });
+}
+
+// c1' lifted, forward transform, times s_0, inverse transform, c0' added and mapped, forward transform.  The product by s_0 is
+// ct_mul_plain's, whose plaintext is shared by every row: the rows are taken two by two as level-1 ciphertexts, an odd count padded
+// with a zero row.
+static int decrypt_compact_at(dpfhe_ctx *ctx, unsigned bits, uint64_t t_plain, const uint64_t *d_sk, const uint64_t *d_cct, uint64_t *d_pt,
+                              size_t n, void *stream) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CompactArgs A;
+    rc = compact_args(ctx, bits, t_plain, A);
+    if (rc) return rc;
+    if (n == 0) return DPFHE_OK;
+    CHECK_PTR(d_sk); CHECK_PTR(d_cct); CHECK_PTR(d_pt);
+    const size_t N = ctx->N();
+    if (overlaps(d_pt, n * N * 8, d_sk, N * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap the secret");
+    if (overlaps(d_pt, n * N * 8, d_cct, n * 2 * A.tiles * bits * 8)) return fail(DPFHE_ERR_INVALID, "output must not overlap an input");
+    const size_t pairs = (n + 1) / 2;
+    rc = ctx->compact_work.reserve(ctx, 2 * pairs * N * 8);
+    if (rc) return rc;
+    u64 *rows = ctx->compact_work.get();
+    cudaStream_t st = pick(ctx, stream);
+    const LaunchCtx lc1 = level_view(ctx, 1);
+    if (n & 1) CU_TRY(cudaMemsetAsync(rows + n * N, 0, N * 8, st));
+    CU_TRY(VCALL(launch_compact_unpack, lc1, false, A, d_cct, nullptr, rows, n, st));
+    CU_TRY(VCALL(launch_ntt, lc1, rows, n, false, st));
+    CU_TRY(VCALL(launch_ct_mul_plain, lc1, rows, d_sk, rows, pairs, st));
+    CU_TRY(VCALL(launch_ntt, lc1, rows, n, true, st));
+    CU_TRY(VCALL(launch_compact_unpack, lc1, true, A, d_cct, rows, d_pt, n, st));
+    CU_TRY(VCALL(launch_ntt, lc1, d_pt, n, false, st));
+    note_launch(ctx, 6);
+    return DPFHE_OK;
+}
+
+int dpfhe_decrypt_compact(dpfhe_ctx *ctx, unsigned bits, uint64_t t_plain, const uint64_t *d_sk, const uint64_t *d_cct, uint64_t *d_pt,
+                          size_t n, void *stream) {
+    return decrypt_compact_at(ctx, bits, t_plain, d_sk, d_cct, d_pt, n, stream);
+}
+
+// row 0 of the secret is the staged shared operand
+int dpfhe_decrypt_compact_host(dpfhe_ctx *ctx, unsigned bits, uint64_t t_plain, const uint64_t *h_sk, const uint64_t *h_cct,
+                               uint64_t *h_pt, size_t n) {
+    int rc = enter(ctx);
+    if (rc) return rc;
+    CompactArgs A;
+    rc = compact_args(ctx, bits, t_plain, A);
+    if (rc || n == 0) return rc;
+    const size_t N = ctx->N();
+    return host_call(ctx, {h_sk, h_cct, h_pt}, h_sk, N, h_cct, nullptr, h_pt, n, 2 * (size_t)A.tiles * bits, N,
+                     [&](u64 *din, u64 *, u64 *dout, size_t cnt, cudaStream_t st) {
+                         return decrypt_compact_at(ctx, bits, t_plain, ctx->stage_key.get(), din, dout, cnt, st);
                      });
 }
 

@@ -87,6 +87,7 @@ struct dpfhe_ctx {
     uint64_t bgv_t = 0;                     //   last used (0: none), rewritten when t changes
     dpfhe::BgvTables bgv;
     DeviceScratch enc_work;                 // both slot encoders (encode: [n_vec][N] coefficients; decode: [n_vec][L][N] inverse transforms)
+    DeviceScratch compact_work;             // compact ciphertexts: the level-1 pairs of a compaction, the c1' s rows of a decryption
     DeviceScratch stage_in[DPFHE_PIPE_DEPTH], stage_out[DPFHE_PIPE_DEPTH], stage_key;   // staging of the host-buffer entry points
     // allocated on first use and kept: per-rotation constants of the hoisted rotations, M [L][N] and kprime [2][L][N], and the
     // table delta[j][i] = q_j mod q_i
@@ -103,7 +104,7 @@ struct dpfhe_ctx {
     // calls f on each buffer that dpfhe_context_trim releases (Self: dpfhe_ctx or const dpfhe_ctx)
     template <class Self, class F>
     static void each_trimmed(Self &c, F f) {
-        for (auto *s : {&c.ms_tau, &c.hoist_U, &c.hoist_zero, &c.hoistg, &c.ckks_tab, &c.bgv_tab, &c.enc_work, &c.stage_key}) f(*s);
+        for (auto *s : {&c.ms_tau, &c.hoist_U, &c.hoist_zero, &c.hoistg, &c.ckks_tab, &c.bgv_tab, &c.enc_work, &c.compact_work, &c.stage_key}) f(*s);
         for (auto &s : c.stage_in) f(s);
         for (auto &s : c.stage_out) f(s);
     }

@@ -444,4 +444,37 @@ void build_bgv_consts(const HostParams &hp, uint64_t t, BgvConsts &K) {
     K.m = make_mod32(t);
 }
 
+// a^-1 mod m for gcd(a, m) = 1, m >= 2
+static uint64_t inv_mod(uint64_t a, uint64_t m) {
+    __int128 r0 = m, r1 = a % m, s0 = 0, s1 = 1;
+    while (r1) {
+        const __int128 q = r0 / r1, r2 = r0 - q * r1, s2 = s0 - q * s1;
+        r0 = r1; r1 = r2; s0 = s1; s1 = s2;
+    }
+    return (uint64_t)(s0 < 0 ? s0 + m : s0);
+}
+// floor(w 2^64 / m), w < m
+static uint64_t companion(uint64_t w, uint64_t m) { return (uint64_t)(((unsigned __int128)w << 64) / m); }
+
+void build_compact_args(uint64_t q0, unsigned log_n, unsigned bits, uint64_t t_plain, CompactArgs &A) {
+    A = CompactArgs();
+    A.q = q0;
+    A.r = (uint64_t)(((unsigned __int128)1 << bits) % q0);
+    A.r_s = companion(A.r, q0);
+    uint64_t inv = 1;   // q0^-1 mod 2^64 by Newton's iteration (q0 odd): each step doubles the correct low bits
+    for (int i = 0; i < 6; ++i) inv *= 2 - q0 * inv;
+    A.qinv64 = inv;
+    A.t = t_plain;
+    if (t_plain) {
+        const uint64_t qinv_t = inv_mod(q0 % t_plain, t_plain);
+        A.c = (t_plain - qinv_t) % t_plain;
+        A.c_s = companion(A.c, t_plain);
+        const uint64_t lambda = (uint64_t)((unsigned __int128)(((unsigned __int128)1 << bits) % t_plain) * qinv_t % t_plain);
+        A.mu = inv_mod(lambda, t_plain);
+        A.mu_s = companion(A.mu, t_plain);
+    }
+    A.bits = bits;
+    A.tiles = (uint32_t)(((size_t)1 << log_n) / 64);
+}
+
 }  // namespace dpfhe

@@ -56,6 +56,10 @@ bool build_bgv_tables(const HostParams &hp, uint64_t t, std::vector<uint32_t> &t
 // decoding constants: CKKS's Garner inverses and digits of (Q-1)/2, q_i mod t and Q mod t (requires a valid t)
 void build_bgv_consts(const HostParams &hp, uint64_t t, BgvConsts &K);
 
+// Compact ciphertexts (DESIGN.md §2.24): the constants of the switch between q0 and 2^bits at N = 2^log_n, for arguments the caller has
+// checked (2 <= bits, N 2^bits < q0, t_plain = 0 or odd with 3 <= t_plain < 2^(bits-1))
+void build_compact_args(uint64_t q0, unsigned log_n, unsigned bits, uint64_t t_plain, CompactArgs &A);
+
 // key generation and encryption (DESIGN.md §2.14): the constants of one launch of the key / encryption kernels for the 32-byte seed,
 // K special primes (0: per-limb digits) and the noise factor t (t = 0: unscaled); the pointers and item numbers stay unset
 KeyArgs build_key_args(const HostParams &hp, const uint8_t seed[32], unsigned K, uint64_t t_plain);

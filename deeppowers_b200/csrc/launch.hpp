@@ -98,6 +98,9 @@ struct LaunchCtx {
     cudaError_t launch_keys(const LaunchCtx &lc, int mode, const KeyArgs &A, size_t n_items, cudaStream_t st); \
     cudaError_t launch_decrypt(const LaunchCtx &lc, const u64 *ct, const u64 *s, u64 *pt, u32 n_comp, size_t n, cudaStream_t st); \
     cudaError_t launch_expand_seeded(const LaunchCtx &lc, bool keys, const SeededKeyArgs &A, const u64 *src, u64 *dst, size_t n_rows, cudaStream_t st); \
+    cudaError_t launch_compact_pack(const LaunchCtx &lc, const CompactArgs &A, const u64 *x, u64 *out, size_t n_polys, cudaStream_t st); \
+    cudaError_t launch_compact_unpack(const LaunchCtx &lc, bool finish, const CompactArgs &A, const u64 *cct, const u64 *prod, u64 *dst, size_t n, \
+                                      cudaStream_t st); \
     cudaError_t launch_lincomb(const LaunchCtx &lc, const u64 *const *in, const int64_t *coeffs, u32 n_terms, int64_t constant, const u64 *pt, \
                                u64 *out, size_t batch, cudaStream_t st); \
     cudaError_t launch_ckks_comb(const LaunchCtx &lc, const u64 *const *in, const u32 *levels, const double *coeffs, u32 n_terms, \

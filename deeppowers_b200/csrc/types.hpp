@@ -195,6 +195,19 @@ struct SeededKeyArgs : KeyArgs {
 };
 DPFHE_HD constexpr bool key_mode_seeded(int mode) { return mode >= KM_ENC_SEEDED; }
 
+// Compact ciphertexts (DESIGN.md §2.24): the constants of the switch between q0 and 2^bits, built on the host (abi.cu) and passed by
+// value in the kernel parameter block of compact.cu.  The "companion" of w modulo m is floor(w 2^64 / m).
+struct CompactArgs {
+    u64 q;             // q0
+    u64 r, r_s;        // 2^bits mod q0 and its companion modulo q0
+    u64 qinv64;        // q0^-1 mod 2^64
+    u64 t;             // the plaintext modulus; 0: CKKS
+    u64 c, c_s;        // BGV: -q0^-1 mod t and its companion modulo t (the correction j of the switch)
+    u64 mu, mu_s;      // BGV: lambda^-1 mod t (lambda = 2^bits q0^-1 mod t) and its companion modulo t
+    u32 bits;          // 2 <= bits, N 2^bits < q0
+    u32 tiles;         // 64-coefficient tiles per polynomial, N / 64
+};
+
 // KS_DOT (grouped keys only, DESIGN.md §2.18): the digit is the third component of a SUM of tensor products
 enum KsMode { KS_MUL_RELIN = 0, KS_PLAIN = 1, KS_ROTATE = 2, KS_DOT = 3 };
 constexpr int DOT_MAX_TERMS = 64;   // pairs of one encrypted inner product

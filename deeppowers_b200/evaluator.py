@@ -776,6 +776,27 @@ class Context:
         n, it = _u64_array(items)
         self._chk(self._l.dpfhe_expand_switch_keys_host(self._h, int(n_special), _seed(a_seed), n, it, _hptr(b), _hptr(keys, True)))
 
+    # compact ciphertexts (DESIGN.md section 2.24): level-1 ciphertexts switched to 2^bits and bit-packed, [n][2][N bits / 64] words;
+    # t_plain = 0 for CKKS.  Decryption gives level-1 plaintexts [n][1][N] for the level-1 decoders.
+    def compact_words(self, bits):
+        """u64 words of one compact ciphertext: N bits / 32"""
+        return self.N * int(bits) // 32
+
+    def compact_ciphertexts(self, level, bits, t_plain, ct, out, n, stream=None):
+        """device ciphertexts [n][2][level][N] -> device compact ciphertexts [n][2][N bits / 64]"""
+        self._chk(self._l.dpfhe_compact_ciphertexts(self._h, int(level), int(bits), int(t_plain), _ptr(ct), _ptr(out), n, _stream(stream)))
+
+    def download_compact_ciphertexts(self, level, bits, t_plain, ct, out, n):
+        """device ciphertexts [n][2][level][N] -> host compact words (numpy, n * compact_words(bits)); synchronous"""
+        self._chk(self._l.dpfhe_download_compact_ciphertexts(self._h, int(level), int(bits), int(t_plain), _ptr(ct), _hptr(out, True), n))
+
+    def decrypt_compact(self, bits, t_plain, sk, cct, pt, n, stream=None):
+        self._chk(self._l.dpfhe_decrypt_compact(self._h, int(bits), int(t_plain), _ptr(sk), _ptr(cct), _ptr(pt), n, _stream(stream)))
+
+    def decrypt_compact_host(self, bits, t_plain, sk, cct, pt):
+        self._chk(self._l.dpfhe_decrypt_compact_host(self._h, int(bits), int(t_plain), _hptr(sk), _hptr(cct), _hptr(pt, True),
+                                                     cct.size // self.compact_words(bits)))
+
     def galois_elt(self, k):
         """Galois element 5^k mod 2N of a rotation by k slots (k may be negative)."""
         return pow(5, k % (self.N // 2), 2 * self.N)

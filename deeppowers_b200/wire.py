@@ -11,15 +11,39 @@ PUBLIC_KEY = 6   # (b, a): payload [2][n_limbs][N], count = 1
 # and c0 [count][n_limbs][N] (SEEDED_CIPHERTEXTS) or the b rows [digits][n_limbs][N] (SEEDED_SWITCH_KEY, count = K special primes, 0 .. 4)
 SEEDED_CIPHERTEXTS, SEEDED_SWITCH_KEY = 7, 8
 SEEDED_PREFIX_WORDS = 5
+# compact ciphertexts (DESIGN.md section 2.24): a 2-word prefix (bits, t_plain) and [count][2][N bits / 64] packed words; n_limbs = 1,
+# moduli[0] = q0, form = 0 (coefficient)
+COMPACT_CIPHERTEXTS = 10
+COMPACT_PREFIX_WORDS = 2
 _HDR = struct.Struct("<8sIIIIQ16Q")
 
 
-def payload_words(log_n, n_limbs, kind, count):
+def check_compact_prefix(log_n, n_limbs, form, q0, bits, t_plain):
+    """the prefix (bits, t_plain) of compact ciphertexts against their header"""
+    if n_limbs != 1 or form != 0:
+        raise ValueError("compact ciphertexts are one limb in coefficient form")
+    if not (2 <= bits and bits + log_n < 64 and (1 << (bits + log_n)) < q0):
+        raise ValueError("bits of compact ciphertexts out of range for q0")
+    if t_plain and (not t_plain & 1 or not 3 <= t_plain < 1 << (bits - 1)):
+        raise ValueError("plaintext modulus of compact ciphertexts must be 0 or odd with 3 <= t < 2^(bits-1)")
+
+
+def payload_words(log_n, n_limbs, kind, count, compact=None):
+    """compact: (form, q0, bits, t_plain) of compact ciphertexts, whose payload is sized by its prefix"""
     if not (1 <= log_n <= 17 and 1 <= n_limbs <= 16):
         raise ValueError("bad parameters")
-    if kind not in (CIPHERTEXTS, SWITCH_KEY, PLAINTEXTS, HYBRID_SWITCH_KEY, GROUPED_SWITCH_KEY, PUBLIC_KEY, SEEDED_CIPHERTEXTS, SEEDED_SWITCH_KEY):
+    if kind not in (CIPHERTEXTS, SWITCH_KEY, PLAINTEXTS, HYBRID_SWITCH_KEY, GROUPED_SWITCH_KEY, PUBLIC_KEY, SEEDED_CIPHERTEXTS, SEEDED_SWITCH_KEY,
+                    COMPACT_CIPHERTEXTS):
         raise ValueError("unknown kind")
     poly = (1 << log_n) * n_limbs
+    if kind == COMPACT_CIPHERTEXTS:
+        if compact is None:
+            raise ValueError("compact ciphertexts are sized by their prefix")
+        form, q0, bits, t_plain = compact
+        check_compact_prefix(log_n, n_limbs, form, q0, bits, t_plain)
+        if count < 1:
+            raise ValueError("no compact ciphertexts")
+        return COMPACT_PREFIX_WORDS + count * 2 * (1 << log_n) // 64 * bits
     if kind == SEEDED_CIPHERTEXTS:
         if count < 1:
             raise ValueError("no seeded ciphertexts")
@@ -57,9 +81,15 @@ def _check_prefix(log_n, kind, count, payload):
             raise ValueError("item number of a seeded key is neither 0 nor a Galois element")
 
 
+def compact_prefix(bits, t_plain):
+    """the 2-word prefix of compact ciphertexts"""
+    return np.array([bits, t_plain], dtype=np.uint64)
+
+
 def write(path, log_n, n_limbs, kind, count, moduli, payload, form=1):
     payload = np.ascontiguousarray(payload, dtype="<u8").reshape(-1)
-    if payload.size != payload_words(log_n, n_limbs, kind, count):
+    compact = (form, int(moduli[0]), int(payload[0]), int(payload[1])) if kind == COMPACT_CIPHERTEXTS and payload.size >= 2 else None
+    if payload.size != payload_words(log_n, n_limbs, kind, count, compact):
         raise ValueError("payload size does not match the header")
     _check_prefix(log_n, kind, count, payload)
     mods = list(int(m) for m in moduli) + [0] * (16 - len(moduli))
@@ -76,7 +106,13 @@ def read(path):
         magic, log_n, n_limbs, kind, form, count, *mods = _HDR.unpack(raw)
         if magic != MAGIC:
             raise ValueError("not a DPFHEv1 file")
-        words = payload_words(log_n, n_limbs, kind, count)
+        compact = None
+        if kind == COMPACT_CIPHERTEXTS:
+            prefix = np.frombuffer(f.read(8 * COMPACT_PREFIX_WORDS), dtype="<u8")
+            if prefix.size != COMPACT_PREFIX_WORDS:
+                raise ValueError("truncated payload")
+            compact = (form, mods[0], int(prefix[0]), int(prefix[1]))
+        words = payload_words(log_n, n_limbs, kind, count, compact)
         f.seek(0, 2)
         if f.tell() != _HDR.size + 8 * words:      # the header is untrusted: it must describe exactly this file
             raise ValueError("file size does not match the header")

@@ -274,6 +274,26 @@ public:
         check(dpfhe_expand_switch_keys_host(ctx_, special, a_seed.data(), items.size(), items.data(), host_b, host_keys));
     }
 
+    // ---- compact ciphertexts (DESIGN.md §2.24): level-1 ciphertexts switched to 2^bits and bit-packed, [count][2][N bits / 64] words;
+    //      plain_modulus = 0 for CKKS.  Decryption gives level-1 plaintexts [count][1][N] for the level-1 decoders. ----
+    std::size_t compact_words(unsigned bits) const { return poly_degree() * bits / 32; }
+    void compact_ciphertexts_device(unsigned level, unsigned bits, std::uint64_t plain_modulus, ConstCiphertextBatch ct, std::uint64_t *out,
+                                    void *stream = nullptr) {
+        check(dpfhe_compact_ciphertexts(ctx_, level, bits, plain_modulus, ct.data, out, ct.count, stream));
+    }
+    // device ciphertexts -> host compact words (synchronous)
+    void download_compact_ciphertexts(unsigned level, unsigned bits, std::uint64_t plain_modulus, ConstCiphertextBatch ct, std::uint64_t *host_out) {
+        check(dpfhe_download_compact_ciphertexts(ctx_, level, bits, plain_modulus, ct.data, host_out, ct.count));
+    }
+    void decrypt_compact(unsigned bits, std::uint64_t plain_modulus, const std::uint64_t *secret, const std::uint64_t *compact, std::size_t count,
+                         std::uint64_t *plain_eval) {
+        check(dpfhe_decrypt_compact_host(ctx_, bits, plain_modulus, secret, compact, plain_eval, count));
+    }
+    void decrypt_compact_device(unsigned bits, std::uint64_t plain_modulus, const std::uint64_t *secret, const std::uint64_t *compact,
+                                std::size_t count, std::uint64_t *plain_eval, void *stream = nullptr) {
+        check(dpfhe_decrypt_compact(ctx_, bits, plain_modulus, secret, compact, plain_eval, count, stream));
+    }
+
     // ---- host-buffer calls: synchronous; H2D / compute / D2H are pipelined inside the library ----
     void multiply_relin(ConstCiphertextBatch a, ConstCiphertextBatch b, const std::uint64_t *relin_key, CiphertextBatch out) {
         same(a.count, b.count, out.count);

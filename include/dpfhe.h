@@ -543,5 +543,7 @@ int dpfhe_describe(const dpfhe_ctx *ctx, char *buf, size_t buf_len);
 #include "dpfhe_level.h"
 /* seeded ciphertexts and switch keys, their uniform half regenerated on the device from a public seed (DESIGN.md §2.23) */
 #include "dpfhe_seeded.h"
+/* compact result ciphertexts: switched to a power-of-two modulus and bit-packed on the device (DESIGN.md §2.24) */
+#include "dpfhe_compact.h"
 
 #endif /* DPFHE_H */

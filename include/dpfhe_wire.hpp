@@ -19,6 +19,9 @@
 //                       8 = seeded switch key: a 5-word prefix (the public seed as four LE words, then the item number: 0 for the
 //                           relinearisation key, else the Galois element) and the b rows [digits][L][N], count = K special primes
 //                           (0 <= K <= 4, 2K <= L; digits = L for K = 0, else ceil((L-K)/K))
+//                      10 = compact ciphertexts (DESIGN.md §2.24): a 2-word prefix (bits, t_plain) and [count][2][N bits / 64] packed
+//                           words; n_limbs = 1, moduli[0] = q0, form = 0 (coefficient).  2 <= bits with N 2^bits < q0; t_plain = 0
+//                           (CKKS) or odd with 3 <= t_plain < 2^(bits-1)
 //   20      4     form: 1 = evaluation (NTT, bit-reversed order), 0 = coefficient
 //   24      8     count
 //   32      128   moduli[16] (unused entries 0)
@@ -40,9 +43,10 @@ namespace fhe {
 // GroupedSwitchKey: n_limbs counts the K = count special primes at the end of the basis; payload [ceil((n_limbs-K)/K)][2][n_limbs][N]
 enum class WireKind : std::uint32_t {
     Ciphertexts = 1, SwitchKey = 2, Plaintexts = 3, HybridSwitchKey = 4, GroupedSwitchKey = 5, PublicKey = 6, SeededCiphertexts = 7,
-    SeededSwitchKey = 8
+    SeededSwitchKey = 8, CompactCiphertexts = 10
 };
 constexpr std::size_t kSeededPrefixWords = 5;   // the public seed (4 words) and first_index / the item number
+constexpr std::size_t kCompactPrefixWords = 2;  // bits, t_plain
 
 struct WireHeader {
     char magic[8];
@@ -52,9 +56,22 @@ struct WireHeader {
 };
 static_assert(sizeof(WireHeader) == 160, "wire header must be 160 bytes");
 
+// the prefix (bits, t_plain) of compact ciphertexts against their header, which it completes: one limb, coefficient form,
+// 2 <= bits with N 2^bits < moduli[0], t_plain 0 or odd with 3 <= t_plain < 2^(bits-1)
+inline void check_compact_prefix(const WireHeader &h, const std::uint64_t *prefix) {
+    if (h.n_limbs != 1 || h.form != 0) throw std::runtime_error("dpfhe wire: compact ciphertexts are one limb in coefficient form");
+    const std::uint64_t bits = prefix[0], t = prefix[1];
+    // compared without a sum (log_n <= 17 is checked first), so that no `bits` wraps past the range check
+    if (bits < 2 || bits >= 64 - std::uint64_t(h.log_n) || (std::uint64_t(1) << (bits + h.log_n)) >= h.moduli[0])
+        throw std::runtime_error("dpfhe wire: bits of compact ciphertexts out of range for q0");
+    if (t && (!(t & 1) || t < 3 || t >= (std::uint64_t(1) << (bits - 1))))
+        throw std::runtime_error("dpfhe wire: plaintext modulus of compact ciphertexts must be 0 or odd with 3 <= t < 2^(bits-1)");
+}
+
 // words of payload a header announces; throws on an unknown kind, bad parameters or a count whose byte size does not fit
-// size_t (a header is untrusted input: the count of a file must never be able to wrap the size computation)
-inline std::size_t wire_payload_words(const WireHeader &h) {
+// size_t (a header is untrusted input: the count of a file must never be able to wrap the size computation).  Compact ciphertexts
+// are sized by their prefix, the payload's first two words, which `prefix` points at (checked here).
+inline std::size_t wire_payload_words(const WireHeader &h, const std::uint64_t *prefix = nullptr) {
     if (h.log_n < 1 || h.log_n > 17 || h.n_limbs < 1 || h.n_limbs > 16) throw std::runtime_error("dpfhe wire: bad parameters");
     const std::size_t poly = (std::size_t(1) << h.log_n) * h.n_limbs;   // <= 2^21 words
     const std::size_t max_words = static_cast<std::size_t>(-1) / 8;
@@ -81,6 +98,11 @@ inline std::size_t wire_payload_words(const WireHeader &h) {
             const std::size_t k = static_cast<std::size_t>(h.count), digits = k ? (h.n_limbs - k + k - 1) / k : h.n_limbs;
             return kSeededPrefixWords + digits * poly;
         }
+        case WireKind::CompactCiphertexts:
+            if (!prefix) throw std::runtime_error("dpfhe wire: compact ciphertexts are sized by their prefix");
+            check_compact_prefix(h, prefix);
+            if (h.count < 1) throw std::runtime_error("dpfhe wire: no compact ciphertexts");
+            return kCompactPrefixWords + checked(h.count, 2 * ((std::size_t(1) << h.log_n) / 64) * static_cast<std::size_t>(prefix[0]));
     }
     throw std::runtime_error("dpfhe wire: unknown kind");
 }
@@ -111,7 +133,7 @@ inline WireHeader make_wire_header(unsigned log_n, unsigned n_limbs, WireKind ki
 inline void write_wire_file(const std::string &path, const WireHeader &h, const std::uint64_t *payload) {
     std::FILE *f = std::fopen(path.c_str(), "wb");
     if (!f) throw std::runtime_error("dpfhe wire: cannot open " + path + " for writing");
-    const std::size_t words = wire_payload_words(h);
+    const std::size_t words = wire_payload_words(h, payload);
     check_wire_prefix(h, payload);
     const bool ok = std::fwrite(&h, sizeof(h), 1, f) == 1 && std::fwrite(payload, 8, words, f) == words;
     std::fclose(f);
@@ -130,9 +152,12 @@ inline WireHeader read_wire_file(const std::string &path, std::vector<std::uint6
     WireHeader h;
     if (std::fread(&h, sizeof(h), 1, file.f) != 1 || std::memcmp(h.magic, "DPFHEv1", 8) != 0)
         throw std::runtime_error("dpfhe wire: " + path + " is not a DPFHEv1 file");
+    std::uint64_t prefix[kCompactPrefixWords] = {0, 0};
+    if (h.kind == static_cast<std::uint32_t>(WireKind::CompactCiphertexts) && std::fread(prefix, 8, kCompactPrefixWords, file.f) != kCompactPrefixWords)
+        throw std::runtime_error("dpfhe wire: truncated payload in " + path);
     std::size_t words = 0;
     try {
-        words = wire_payload_words(h);
+        words = wire_payload_words(h, prefix);
     } catch (const std::runtime_error &e) {
         throw std::runtime_error(std::string(e.what()) + " in " + path);
     }
